@@ -1,5 +1,5 @@
 """Drop-in for the reference module ``autoregressive/models/gpt_t2i.py`` (LlamaGen transformer with ControlAR
-conditional decoding) whose inference arithmetic runs in hand-written sm_100a kernels behind the C ABI.
+conditional decoding) whose inference arithmetic runs in hand-written sm_90a kernels behind the C ABI.
 
 What is preserved (SURVEY.md §8b): ``ModelArgs`` fields, ``GPT_models`` factory names, module/parameter names
 (identical state-dict keys: reference gpt_t2i.py:310-389), ``setup_caches`` / ``forward`` / ``get_fsdp_wrap_module_list``

@@ -1,4 +1,4 @@
-"""Build the CUDA libraries in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the snapshot)."""
+"""Build the CUDA library in-tree with nvcc for sm_90a (H100)."""
 from __future__ import annotations
 
 import os
@@ -10,12 +10,12 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libcontrolar_b200.so")
 SOURCES = ["car_api.cu", "car_vision.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC", "-cudart", "static"]
 
 
 def _source_hash(flags) -> str:
-    """Content hash of every source the library is built from (+ flags): mtimes do not survive the copy to a GPU box."""
+    """Content hash of every source the library is built from (+ flags): mtimes do not survive a copy of the tree."""
     import hashlib
     h = hashlib.sha256(" ".join(flags).encode())
     for root in (CSRC, os.path.join(os.path.dirname(HERE), "include")):

@@ -12,7 +12,7 @@
 #include "misc.cuh"
 #include "decode_persistent.cuh"
 #include "gemm_dense.cuh"
-#include "gemm_tc5.cuh"
+#include "gemm_wgmma.cuh"
 #include "train.cuh"
 #include "train_bwd.cuh"
 #include "t5.cuh"
@@ -100,10 +100,9 @@ static int alloc_dev(std::vector<void*>& owned, void** p, size_t bytes) {
     return CAR_OK;
 }
 
-// Device buffers that other SMs POLL (packet tags, barrier counters) are initialised with SM stores, not cudaMemset: on B200 a
+// Device buffers that other SMs POLL (packet tags, barrier counters) are initialised with SM stores, not cudaMemset: a
 // recycled allocation that was zeroed by cudaMemset has been observed to still return the previous owner's packets to strong
-// polling loads (tests/test_ar_gpu.py run as a whole failed deterministically until tags were made unique per state;
-// profiles/r2_stale_tags.md).  Two defences: this fill kernel, and tags that are unique process-wide (pk_alloc_tags).
+// polling loads (tests/test_ar_gpu.py run as a whole failed deterministically until tags were made unique per state).  Two defences: this fill kernel, and tags that are unique process-wide (pk_alloc_tags).
 __global__ void fill_u32_kernel(unsigned int* __restrict__ p, unsigned int v, size_t n) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;
 }
@@ -143,7 +142,7 @@ static int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
-    if (cached[dev] == 0) { int n = 0; cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); cached[dev] = n > 0 ? n : 148; }
+    if (cached[dev] == 0) { int n = 0; cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); cached[dev] = n > 0 ? n : 132; }
     return cached[dev];
 }
 
@@ -205,7 +204,7 @@ static int launch_skinny(cudaStream_t st, int dtype, const void* A, int lda, con
     int NB;
     if (mtiles > 1) NB = 4;                       // M-tiled (prefill): maximise reuse of the activation tile
     else {
-        // one wave: ceil(nblk / NB) <= 148 where possible (register use makes these 1 CTA / SM kernels)
+        // one wave: ceil(nblk / NB) <= SM count where possible (register use makes these 1 CTA / SM kernels)
         const int want = (nblk + sm_count() - 1) / sm_count();
         NB = want > 4 ? 8 : (want > 2 ? 4 : (want > 1 ? 2 : 1));
     }
@@ -508,31 +507,18 @@ static int dense_linear(cudaStream_t st, const void* A, int lda, const void* W, 
     if (M <= 0 || N <= 0) return CAR_OK;
     static const bool use_tc5 = [] { const char* e = getenv("CAR_TC5"); return e ? atoi(e) != 0 : true; }();
     if (use_tc5 && K % 8 == 0 && N % 8 == 0 && lda % 8 == 0 && ldo % 8 == 0 && (resid == nullptr || ldr % 8 == 0) &&
-        ((uintptr_t)A % 16) == 0 && ((uintptr_t)W % 16) == 0 && t5_encoder() != nullptr) {
-        // tcgen05 path (gemm_tc5.cuh): TMA tensor-map loads, accumulator in TMEM, persistent warp-specialised CTAs
+        ((uintptr_t)A % 16) == 0 && ((uintptr_t)W % 16) == 0 && wg_encoder() != nullptr) {
+        // wgmma path (gemm_wgmma.cuh): TMA tensor-map loads, accumulators in registers, persistent warp-specialised CTAs
         static DevOnce once5;
-        if (once5.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_tc5_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T5_SMEM));
+        if (once5.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
         alignas(64) CUtensorMap mapA, mapB;
-        if (!t5_make_map(&mapA, A, M, K, lda) || !t5_make_map(&mapB, W, N, K, K)) CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-        Tc5P q;
+        if (!wg_make_map(&mapA, A, M, K, lda) || !wg_make_map(&mapB, W, N, K, K)) CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
+        WgP q;
         memset(&q, 0, sizeof(q));
         q.M = M; q.N = N; q.K = K;
         q.resid = (const bf16*)resid; q.ldr = ldr; q.C = (bf16*)out; q.ldc = ldo; q.act = act == ACT_GELU_TANH ? 1 : 0;
-        static const bool use_x2 = [] { const char* e = getenv("CAR_TC5X2"); return e ? atoi(e) != 0 : true; }();
-        // 2-CTA tiles (cta_group::2, 256 x 256 per CTA pair): twice the math per operand byte pulled from L2.  Measured (B200,
-        // scripts/bench_gemm.py, TFLOP/s 1-CTA -> 2-CTA): 8192^3 894 -> 1345; 16384 x 1280 x 1280 700 -> 870; 1920 x 3840 x 1280
-        // 503 -> 598; 1920 x 3584 x 1280 546 -> 554; but 1920 x 1280 x 3584 (40 pair tiles on 74 pairs) 375 -> 265: with fewer
-        // pair tiles than ~1.3 waves the coarser tiling idles SMs, so small grids stay on the 128 x 128 kernel.
-        const int ptiles_x2 = ((M + T2_BM - 1) / T2_BM) * ((N + T2_BN - 1) / T2_BN);
-        if (use_x2 && M >= T2_BM && N >= T2_BN && ptiles_x2 >= 100) {
-            static DevOnce once52;
-            if (once52.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_tc5x2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T5_SMEM));
-            const int pairs = std::max(1, std::min(ptiles_x2, sm_count() / 2));
-            CAR_LAUNCH(gemm_tc5x2_kernel, 2 * pairs, T5_THREADS, T5_SMEM, st, mapA, mapB, q);
-            return CAR_OK;
-        }
-        const int ntiles = ((M + T5_BM - 1) / T5_BM) * ((N + T5_BN - 1) / T5_BN);
-        CAR_LAUNCH(gemm_tc5_kernel, std::min(ntiles, sm_count()), T5_THREADS, T5_SMEM, st, mapA, mapB, q);
+        const int ntiles = ((M + WG_BM - 1) / WG_BM) * ((N + WG_BN - 1) / WG_BN);
+        CAR_LAUNCH(gemm_wgmma_kernel, std::min(ntiles, sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
         return CAR_OK;
     }
     DenseP p;
@@ -981,7 +967,7 @@ extern "C" int car_op_linear(int32_t dtype, const void* x, const void* w, const 
 }
 
 // the dense (M >= 64 rows) tensor-core linear of the prefill / MLP path, exposed for unit tests and micro-benchmarks:
-// y[M,N] = act(x[M,K] · w[N,K]^T) (+ resid), bf16, fp32 accumulate (gemm_tc5.cuh; CAR_TC5=0 selects the mma.sync kernel)
+// y[M,N] = act(x[M,K] · w[N,K]^T) (+ resid), bf16, fp32 accumulate (gemm_wgmma.cuh; CAR_TC5=0 selects the mma.sync kernel)
 extern "C" int car_op_dense_linear(const void* x, const void* w, const void* resid, void* y, int32_t M, int32_t N, int32_t K, int32_t act,
                                    void* stream) {
     if (!x || !w || !y) CAR_FAIL(CAR_ERR_ARG, "null argument");
@@ -1026,10 +1012,10 @@ struct CarTrain {
 };
 
 static int tr_cast(cudaStream_t st, const void* src, bf16* dst, long long n) {
-    CAR_LAUNCH(tr_cast_bf16_kernel, (int)std::min<long long>((n + 255) / 256, 148 * 16), 256, 0, st, (const float*)src, dst, n);
+    CAR_LAUNCH(tr_cast_bf16_kernel, (int)std::min<long long>((n + 255) / 256, sm_count() * 16), 256, 0, st, (const float*)src, dst, n);
     return CAR_OK;
 }
-static int tr_grid(long long n) { return (int)std::min<long long>((n + 255) / 256, 148 * 16); }
+static int tr_grid(long long n) { return (int)std::min<long long>((n + 255) / 256, sm_count() * 16); }
 // MLP.forward gpt_t2i.py:177-181 on bf16 operands: out = fc2(gelu_tanh(fc1 x))
 static int tr_mlp(cudaStream_t st, const bf16* x, int rows, int K, const bf16* fc1, const bf16* fc2, int d, bf16* tmp, bf16* out) {
     CAR_TRY(dense_linear(st, x, K, fc1, rows, d, K, ACT_GELU_TANH, nullptr, 0, tmp, d));
@@ -1130,7 +1116,7 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     CAR_TRY(tr_attn_smem((size_t)S, (const void*)tr_attention_kernel, &att_smem));
     CAR_LAUNCH(tr_rmsnorm_kernel, R, 256, 0, st, (const float*)t->h, (const float*)t->attention_norm[l], t->x, dim, d.norm_eps, S, S, 0);
     CAR_TRY(dense_linear(st, t->x, dim, t->b_wqkv[l], R, 3 * dim, dim, ACT_NONE, nullptr, 0, t->qkv, 3 * dim));
-    CAR_LAUNCH(rope_kv_write_kernel, 148 * 8, 256, 0, st, (const bf16*)t->qkv, t->rope, t->q, t->kc, t->vc, R, S, dim, H, S);
+    CAR_LAUNCH(rope_kv_write_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->qkv, t->rope, t->q, t->kc, t->vc, R, S, dim, H, S);
     CAR_LAUNCH(tr_attention_kernel, (unsigned)(((long long)B * H * S + TRA_WARPS - 1) / TRA_WARPS), TRA_WARPS * 32, att_smem, st, (const bf16*)t->q,
                (const bf16*)t->kc, (const bf16*)t->vc, mask, B, H, S, t->att);
     CAR_TRY(dense_linear(st, t->att, dim, t->b_wo[l], R, dim, dim, ACT_NONE, nullptr, 0, t->o, dim));
@@ -1139,7 +1125,7 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     CAR_LAUNCH(tr_rmsnorm_kernel, R, 256, 0, st, (const float*)t->h, (const float*)t->ffn_norm[l], xn, dim, d.norm_eps, S, S, 0);
     CAR_TRY(dense_linear(st, xn, dim, t->b_w1[l], R, F, dim, ACT_NONE, nullptr, 0, t->g, F));
     CAR_TRY(dense_linear(st, xn, dim, t->b_w3[l], R, F, dim, ACT_NONE, nullptr, 0, t->u, F));
-    CAR_LAUNCH(swiglu_kernel, 148 * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, t->act, (long long)R * F);
+    CAR_LAUNCH(swiglu_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, t->act, (long long)R * F);
     if (for_bwd) return CAR_OK;
     CAR_TRY(dense_linear(st, t->act, F, t->b_w2[l], R, dim, F, ACT_NONE, nullptr, 0, t->o, dim));
     CAR_LAUNCH(tr_add_rows_kernel, tr_grid((long long)R * dim), 256, 0, st, t->h, (const bf16*)t->o, B, S, S, 0, dim);
@@ -1282,7 +1268,7 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         CAR_LAUNCH(tr_take_rows_bf16_kernel, tr_grid((long long)R * dim), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim);
         CAR_TRY(tr_wgrad(t, st, t->db, t->act, R, dim, F, g->w.w2 ? (float*)g->w.w2[l] : nullptr));
         CAR_TRY(tr_dgrad(t, st, t->db, t->b_w2[l], R, dim, F, nullptr, t->dact));
-        CAR_LAUNCH(tr_swiglu_bwd_kernel, 148 * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, (const bf16*)t->dact, t->dg, t->du, (long long)R * F);
+        CAR_LAUNCH(tr_swiglu_bwd_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, (const bf16*)t->dact, t->dg, t->du, (long long)R * F);
         CAR_TRY(tr_wgrad(t, st, t->dg, t->x2, R, F, dim, g->w.w1 ? (float*)g->w.w1[l] : nullptr));
         CAR_TRY(tr_wgrad(t, st, t->du, t->x2, R, F, dim, g->w.w3 ? (float*)g->w.w3[l] : nullptr));
         CAR_TRY(tr_dgrad(t, st, t->dg, t->b_w1[l], R, F, dim, nullptr, t->dx));
@@ -1296,7 +1282,7 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
                    (const bf16*)t->datt, B, H, S, t->lse, t->dsum, t->dq);
         CAR_LAUNCH(tr_attn_bwd_kv_kernel, att_grid, TRA_WARPS * 32, smem_kv, st, (const bf16*)t->q, (const bf16*)t->kc, (const bf16*)t->vc, mask,
                    (const bf16*)t->datt, (const float*)t->lse, (const float*)t->dsum, B, H, S, t->dk, t->dv);
-        CAR_LAUNCH(tr_rope_bwd_kernel, 148 * 8, 256, 0, st, (const bf16*)t->dq, (const bf16*)t->dk, (const bf16*)t->dv, t->rope, t->dqkv, R, S, dim, H, S);
+        CAR_LAUNCH(tr_rope_bwd_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->dq, (const bf16*)t->dk, (const bf16*)t->dv, t->rope, t->dqkv, R, S, dim, H, S);
         CAR_TRY(tr_wgrad(t, st, t->dqkv, t->x, R, 3 * dim, dim, g->w.wqkv ? (float*)g->w.wqkv[l] : nullptr));
         CAR_TRY(tr_dgrad(t, st, t->dqkv, t->b_wqkv[l], R, 3 * dim, dim, nullptr, t->dx));
         CAR_TRY(tr_norm_bwd(t, st, t->h0, t->attention_norm[l], t->dx, R, S, S, 0, g->w.attention_norm ? (float*)g->w.attention_norm[l] : nullptr));
@@ -1346,7 +1332,7 @@ extern "C" int car_adamw_step(const void* tensors_dev, const void* chunks_dev, i
 // ---------------------------------------------------------------------------------------------------------
 // T5 text encoder forward (SURVEY.md §8 row f3): language/t5.py:58-79 -> HF T5EncoderModel(...).last_hidden_state, bf16.
 // v1.1 / flan architecture: gated gelu_new feed-forward, no biases, RMS layer norm (eps 1e-6), relative position bias of block 0
-// shared by every block, no 1/sqrt(d) scaling.  GEMMs: dense_linear (tcgen05); glue: t5.cuh.
+// shared by every block, no 1/sqrt(d) scaling.  GEMMs: dense_linear (wgmma); glue: t5.cuh.
 // ---------------------------------------------------------------------------------------------------------
 struct CarT5 {
     CarT5Desc d;
@@ -1409,7 +1395,7 @@ extern "C" int car_t5_forward(CarT5* t, const int32_t* ids, const int32_t* mask,
         CAR_LAUNCH((rmsnorm_rows_kernel<bf16>), R, 256, 0, st, (const bf16*)t->h, (const bf16*)t->ln2[l], t->x, dm, d.eps);
         CAR_TRY(dense_linear(st, t->x, dm, t->wi0[l], R, F, dm, ACT_NONE, nullptr, 0, t->g, F));
         CAR_TRY(dense_linear(st, t->x, dm, t->wi1[l], R, F, dm, ACT_NONE, nullptr, 0, t->u, F));
-        CAR_LAUNCH(t5_geglu_kernel, (int)std::min<long long>(((long long)R * F + 255) / 256, 148 * 16), 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, t->act,
+        CAR_LAUNCH(t5_geglu_kernel, (int)std::min<long long>(((long long)R * F + 255) / 256, sm_count() * 16), 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, t->act,
                    (long long)R * F);
         CAR_TRY(dense_linear(st, t->act, F, t->wo2[l], R, dm, F, ACT_NONE, t->h, dm, t->h, dm));
     }

@@ -5,27 +5,27 @@
 
 #include "common.cuh"
 #include "gemm_dense.cuh"
-#include "gemm_tc5.cuh"
+#include "gemm_wgmma.cuh"
 #include "vision.cuh"
 #include "frontend.cuh"
 
 static int vis_sm_count() {
-    int dev = 0, n = 148;
+    int dev = 0, n = 132;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     return n;
 }
-// tcgen05 path of the vision stages (gemm_tc5.cuh): TMA tensor-map loads, accumulator in TMEM, persistent warp-specialised CTAs.
+// wgmma path of the vision stages (gemm_wgmma.cuh): TMA tensor-map loads, accumulators in registers, persistent warp-specialised CTAs.
 // CAR_TC5=0 sends everything back to the mma.sync kernel (dev A/B).
-static bool tc5_on() {
+static bool wg_on() {
     static const bool on = [] { const char* e = getenv("CAR_TC5"); return e ? atoi(e) != 0 : true; }();
-    return on && t5_encoder() != nullptr;
+    return on && wg_encoder() != nullptr;
 }
-static int tc5_launch(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, const Tc5P& q, int tiles_m) {
+static int wg_launch(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, const WgP& q, int tiles_m) {
     static DevOnce once5;
-    if (once5.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_tc5_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T5_SMEM));
-    const int ntiles = tiles_m * ((q.N + T5_BN - 1) / T5_BN);
-    CAR_LAUNCH(gemm_tc5_kernel, std::min(ntiles, vis_sm_count()), T5_THREADS, T5_SMEM, st, mapA, mapB, q);
+    if (once5.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
+    const int ntiles = tiles_m * ((q.N + WG_BN - 1) / WG_BN);
+    CAR_LAUNCH(gemm_wgmma_kernel, std::min(ntiles, vis_sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
     return CAR_OK;
 }
 
@@ -34,17 +34,17 @@ static int dense(cudaStream_t st, DenseP p, int batch = 1) {
     if (once.first()) CAR_CUDA(cudaFuncSetAttribute(dense_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM));
     if (p.M <= 0 || p.N <= 0) return CAR_OK;
     if (p.alpha == 0.f) p.alpha = 1.f;
-    // plain bf16 -> bf16 GEMMs (DINOv2 linears, 1x1 convolutions) go to the tcgen05 kernel; same epilogue order as below
-    if (batch == 1 && p.amode == A_PLAIN && p.out_mode == 0 && !p.bias_along_m && p.alpha == 1.f && !p.bias_f && !p.resid_f && tc5_on() &&
+    // plain bf16 -> bf16 GEMMs (DINOv2 linears, 1x1 convolutions) go to the wgmma kernel; same epilogue order as below
+    if (batch == 1 && p.amode == A_PLAIN && p.out_mode == 0 && !p.bias_along_m && p.alpha == 1.f && !p.bias_f && !p.resid_f && wg_on() &&
         p.K % 8 == 0 && p.N % 8 == 0 && p.lda % 8 == 0 && p.ldb % 8 == 0 && p.ldc % 8 == 0 && (!p.resid || p.ldr % 8 == 0) &&
         ((uintptr_t)p.A % 16) == 0 && ((uintptr_t)p.B % 16) == 0 && ((uintptr_t)p.C % 16) == 0 && (!p.resid || ((uintptr_t)p.resid % 16) == 0)) {
         alignas(64) CUtensorMap mapA, mapB;
-        if (!t5_make_map(&mapA, p.A, p.M, p.K, p.lda) || !t5_make_map(&mapB, p.B, p.N, p.K, p.ldb)) CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-        Tc5P q;
+        if (!wg_make_map(&mapA, p.A, p.M, p.K, p.lda) || !wg_make_map(&mapB, p.B, p.N, p.K, p.ldb)) CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
+        WgP q;
         memset(&q, 0, sizeof(q));
         q.M = p.M; q.N = p.N; q.K = p.K; q.resid = p.resid; q.ldr = p.ldr; q.C = (bf16*)p.C; q.ldc = p.ldc;
         q.act = p.act == ACT_GELU_TANH ? 1 : (p.act == ACT_GELU_ERF ? 2 : 0); q.bias = p.bias; q.scale = p.scale;
-        return tc5_launch(st, mapA, mapB, q, (p.M + T5_BM - 1) / T5_BM);
+        return wg_launch(st, mapA, mapB, q, (p.M + WG_BM - 1) / WG_BM);
     }
     dim3 grid((p.N + DG_BN - 1) / DG_BN, (p.M + DG_BM - 1) / DG_BM, batch);
     CAR_LAUNCH(dense_gemm_kernel, grid, DG_THREADS, DG_SMEM, st, p);
@@ -56,7 +56,7 @@ static DenseP dp_plain(const bf16* A, int lda, const bf16* B, int ldb, int M, in
     p.A = A; p.B = B; p.M = M; p.N = N; p.K = K; p.lda = lda; p.ldb = ldb; p.C = C; p.ldc = ldc; p.alpha = 1.f;
     return p;
 }
-static inline int gsz(long long total, int block = 256) { return (int)std::min<long long>((total + block - 1) / block, 148 * 16); }
+static inline int gsz(long long total, int block = 256) { return (int)std::min<long long>((total + block - 1) / block, vis_sm_count() * 16); }
 
 struct Arena {   // grow-only device workspace, re-used across calls (no allocation in steady state)
     char* base = nullptr; size_t cap = 0, off = 0;
@@ -433,17 +433,17 @@ struct Act { bf16* p; int B, H, W, C; long long n() const { return (long long)B 
 static int conv_fwd(cudaStream_t st, const ConvW& c, const Act& x, int ups, int stride2, bf16* out, const bf16* resid, int Ho, int Wo,
                     float* out_nchw_f32 = nullptr) {
     if (x.C != c.cin_pad && !(c.k == 1 && x.C == c.cin_pad)) CAR_FAIL(CAR_ERR_STATE, "conv input channel mismatch");
-    if (c.k == 3 && !stride2 && !ups && !out_nchw_f32 && c.cin_pad % T5_BK == 0 && c.cout % 8 == 0 && Ho == x.H && Wo == x.W && x.H >= T5_TH && x.W >= T5_TW && tc5_on() &&
+    if (c.k == 3 && !stride2 && !ups && !out_nchw_f32 && c.cin_pad % WG_BK == 0 && c.cout % 8 == 0 && Ho == x.H && Wo == x.W && x.H >= WG_TH && x.W >= WG_TW && wg_on() &&
         ((uintptr_t)x.p % 16) == 0 && ((uintptr_t)out % 16) == 0 && (!resid || ((uintptr_t)resid % 16) == 0)) {
-        // 3x3 / pad 1 convolution on the tcgen05 kernel: one 4-D TMA box per (tap, 64-channel block), padding by TMA zero fill
+        // 3x3 / pad 1 convolution on the wgmma kernel: one 4-D TMA box per (tap, 64-channel block), padding by TMA zero fill
         alignas(64) CUtensorMap mapA, mapB;
-        if (!t5_make_map_nhwc(&mapA, x.p, x.B, x.H, x.W, c.cin_pad) || !t5_make_map(&mapB, c.w, c.cout, 9 * c.cin_pad, 9 * c.cin_pad))
+        if (!wg_make_map_nhwc(&mapA, x.p, x.B, x.H, x.W, c.cin_pad) || !wg_make_map(&mapB, c.w, c.cout, 9 * c.cin_pad, 9 * c.cin_pad))
             CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-        Tc5P q;
+        WgP q;
         memset(&q, 0, sizeof(q));
         q.M = x.B * x.H * x.W; q.N = c.cout; q.K = 9 * c.cin_pad; q.resid = resid; q.ldr = c.cout; q.C = out; q.ldc = c.cout; q.bias = c.b;
-        q.conv = 1; q.H = x.H; q.W = x.W; q.tiles_x = (x.W + T5_TW - 1) / T5_TW; q.tiles_y = (x.H + T5_TH - 1) / T5_TH; q.cblks = c.cin_pad / T5_BK;
-        return tc5_launch(st, mapA, mapB, q, x.B * q.tiles_x * q.tiles_y);
+        q.conv = 1; q.H = x.H; q.W = x.W; q.tiles_x = (x.W + WG_TW - 1) / WG_TW; q.tiles_y = (x.H + WG_TH - 1) / WG_TH; q.cblks = c.cin_pad / WG_BK;
+        return wg_launch(st, mapA, mapB, q, x.B * q.tiles_x * q.tiles_y);
     }
     DenseP p;
     memset(&p, 0, sizeof(p));
@@ -570,7 +570,7 @@ static int vq_decode_impl(CarVQ* m, const int32_t* codes, const float* quant, in
         }
         if (m->d_has_up[idx]) {   // Upsample (vq_model.py:368-379): nearest x2, then the 3x3 convolution
             bf16* o = flip(x.p);
-            if (tc5_on() && x.C % T5_BK == 0) {   // materialise the up-sampled tensor (bandwidth-trivial) so the convolution is a plain TMA box walk
+            if (wg_on() && x.C % WG_BK == 0) {   // materialise the up-sampled tensor (bandwidth-trivial) so the convolution is a plain TMA box walk
                 CAR_LAUNCH(upsample2x_nhwc_kernel, gsz((long long)B * x.H * 2 * x.W * 2 * (x.C / 8)), 256, 0, st, (const bf16*)x.p, s.t2, B, x.H, x.W, x.C);
                 Act u{s.t2, B, x.H * 2, x.W * 2, x.C};
                 CAR_TRY(conv_fwd(st, m->d_up[idx], u, 0, 0, o, nullptr, u.H, u.W));
@@ -743,8 +743,8 @@ extern "C" int car_resize_bilinear_aa(const float* in, int32_t B, int32_t Cc, in
     if (B <= 0 || Cc <= 0 || H <= 0 || W <= 0 || OH <= 0 || OW <= 0) CAR_FAIL(CAR_ERR_ARG, "bad shape");
     cudaStream_t st = (cudaStream_t)stream;
     const long long n1 = (long long)B * Cc * H * OW, n2 = (long long)B * Cc * OH * OW;
-    CAR_LAUNCH(resize_aa_axis_kernel, (int)std::min<long long>((n1 + 255) / 256, 148 * 16), 256, 0, st, in, tmp, (long long)B * Cc * H, W, OW, 1);
-    CAR_LAUNCH(resize_aa_axis_kernel, (int)std::min<long long>((n2 + 255) / 256, 148 * 16), 256, 0, st, (const float*)tmp, out, (long long)B * Cc, H, OH, OW);
+    CAR_LAUNCH(resize_aa_axis_kernel, (int)std::min<long long>((n1 + 255) / 256, vis_sm_count() * 16), 256, 0, st, in, tmp, (long long)B * Cc * H, W, OW, 1);
+    CAR_LAUNCH(resize_aa_axis_kernel, (int)std::min<long long>((n2 + 255) / 256, vis_sm_count() * 16), 256, 0, st, (const float*)tmp, out, (long long)B * Cc, H, OH, OW);
     return CAR_OK;
 }
 

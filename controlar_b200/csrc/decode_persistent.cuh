@@ -4,14 +4,14 @@
 //   Transformer.forward (decode branch)     autoregressive/models/gpt_t2i.py:444-470
 //   TransformerBlock / Attention / FeedForward / RMSNorm / KVCache.update   gpt_t2i.py:187-306
 //
-// Why it is built this way (measurements: profiles/r1_primitives.md):
+// Why it is built this way:
 //   * At B_eff = 16 a decode step is a chain of 5 all-to-all dependent phases per layer (qkv | attention | wo |
-//     w1w3 | w2); each per-kernel link of the launch chain costs 8-20 us, the data only 2-3 us.  Here the CTAs stay
-//     resident and the chain link is a tagged-packet exchange through L2 (1.1 us for 40 KB across 148 SMs) instead
+//     w1w3 | w2); each per-kernel link of the launch chain costs several times the time the data needs.  Here the CTAs stay
+//     resident and the chain link is a tagged-packet exchange through L2 instead
 //     of a kernel boundary (or a grid barrier + gather, 2.2 us).
 //   * Weights do not depend on activations: every CTA streams ITS weight slices, in consumption order, with
 //     cp.async.bulk into an 8 x 20 KB shared-memory ring that runs ahead of the compute — across phases, layers and
-//     tokens — so HBM stays busy while the dependent chain waits on L2 latency (7.1 TB/s measured for this pattern).
+//     tokens — so HBM stays busy while the dependent chain waits on L2 latency.
 //   * Activations cross CTAs as 8-byte packets {bf16 pair, tag}; the consumer polls the data itself
 //     (ld.relaxed.gpu — a weak .cg load can be served from a stale far-die copy) until the tag equals the expected
 //     epoch.  No fence, no counter, one L2 round trip.  Packets are laid out as the consumer's mma A fragments, so
@@ -131,8 +131,8 @@ __device__ __forceinline__ size_t pk_a_index(int r, int k) {
     return ((size_t)((s * 4 + p) * 32 + g * 4 + t)) * 2 + hi;
 }
 
-// Code-generation knobs (A/B-measured, profiles/r2_codegen_ab.md): the kernel is one 12 K-instruction function under a 128-register
-// cap, and ptxas' allocation for the layer loop shifts with unrelated code (a smaller sampler made the LAYERS 4 % slower).  Out-of-line
+// Code-generation knobs: the kernel is one large function under a 128-register cap, and ptxas' allocation for the layer loop
+// shifts with unrelated code (a smaller sampler can make the layers slower).  Out-of-line
 // phases get their own register allocation and keep the loop's code independent of the rest.
 #ifndef PK_ROPE_PRE           // qkv epilogue: RoPE table entry + column decomposition fetched before the packet wait (measured slower: off)
 #define PK_ROPE_PRE 0
@@ -244,7 +244,7 @@ __device__ __forceinline__ void pk_stream_issue(const PkParams& P, const PkSmem&
     pk_mbar_expect(&sm.full[slot], bytes);
     pk_bulk_g2s(sm.ring + (size_t)slot * PK_SLOT_BYTES, src, bytes, &sm.full[slot]);
     ++st.issued;
-    if (P.exp_flags & 16) pk_stream_prefetch(P, st);   // (experiment) HBM -> L2 run-ahead; measured slower (profiles/r1_decode_persistent.md)
+    if (P.exp_flags & 16) pk_stream_prefetch(P, st);   // (experiment) HBM -> L2 run-ahead; off by default
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -294,7 +294,7 @@ __device__ __forceinline__ void pk_poll_round(const unsigned char* __restrict__ 
 }
 
 // Cheap arrival hint before the full poll: warp 0 watches the first packet of 32 of the K/8 producer blocks (a different
-// subset per CTA) with back-off; the other warps wait at the CTA barrier.  148 x 32 eight-byte loads per round instead of
+// subset per CTA) with back-off; the other warps wait at the CTA barrier.  SM count x 32 eight-byte loads per round instead of
 // the whole tile from every waiting thread — waiting CTAs must not eat the L2 bandwidth of the ones still producing.
 __device__ __forceinline__ void pk_prepoll(const uint2* buf, int K, unsigned int tag, int mode, unsigned mode_sleep) {
     if (mode == 1) return;                             // (experiment) straight to the full poll

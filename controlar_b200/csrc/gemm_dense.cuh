@@ -11,8 +11,8 @@
 //   batched via blockIdx.z with element strides.
 //
 // Round-1 implementation note: mma.sync m16n8k16 + cp.async 3-stage pipeline + ldmatrix (the robust legacy tensor
-// path).  These stages are ~2 % of an image batch's wall time (BASELINE.md §3); the tcgen05/TMA rewrite of this
-// kernel is the next step for the dense path and keeps this interface.
+// path).  The plain GEMMs and 3x3 convolutions that fit
+// the TMA tile walk run on gemm_wgmma.cuh instead; this kernel takes the batched, strided and up-sampling cases.
 #pragma once
 #include "common.cuh"
 

@@ -1,6 +1,6 @@
 // t5.cuh — small kernels of the T5 text encoder forward (SURVEY.md §8 row f3): language/t5.py:58-79 calls HF
 // T5EncoderModel(input_ids, attention_mask).last_hidden_state in bf16 (transformers 5.5.0, models/t5/modeling_t5.py, un-pinned third
-// party).  The GEMMs run on the dense tcgen05 kernel (gemm_tc5.cuh); everything here mirrors the bf16 rounding points of the eager
+// party).  The GEMMs run on the dense wgmma kernel (gemm_wgmma.cuh); everything here mirrors the bf16 rounding points of the eager
 // HF modules: every elementwise PyTorch op on a bf16 tensor computes in fp32 and rounds its output to bf16.
 #pragma once
 #include "common.cuh"

@@ -3,7 +3,7 @@
 // autoregressive/train/train_t2i_canny.py:166-167).  Autocast numerics (oracle/train_oracle.py): the residual stream, the
 // embeddings and the RMSNorm stay fp32; every nn.Linear takes bf16 operands (cast of the fp32 tensor) and returns bf16;
 // fp32 + bf16 adds promote to fp32; GELU / SiLU / the SwiGLU product run on the bf16 tensors; cross-entropy is fp32.
-// First correct path: the GEMMs are the dense tensor-core kernels of the prefill (gemm_tc5.cuh / gemm_dense.cuh), everything
+// First correct path: the GEMMs are the dense tensor-core kernels of the prefill (gemm_wgmma.cuh / gemm_dense.cuh), everything
 // here is bandwidth-trivial glue plus a plain attention kernel; fusing them is the next step of this row.
 #pragma once
 #include "common.cuh"

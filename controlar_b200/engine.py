@@ -447,7 +447,7 @@ def op_linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = N
 
 
 def op_dense_linear(x: torch.Tensor, w: torch.Tensor, resid: Optional[torch.Tensor] = None, act: int = 0) -> torch.Tensor:
-    """y = act(x @ w.T) (+ resid) on the dense tcgen05 path (car_op_dense_linear); bf16."""
+    """y = act(x @ w.T) (+ resid) on the dense wgmma path (car_op_dense_linear); bf16."""
     lib = _lib.lib()
     M, K = x.shape
     N = w.shape[0]

@@ -2,7 +2,7 @@
 (oracle/inputs.py re-exports this module).
 
 Shapes follow SURVEY.md §8(d): T5 embeddings left-padded and zeroed like
-/root/reference/autoregressive/sample/sample_t2i.py:146-160; control maps in [-1, 1] with three identical
+autoregressive/sample/sample_t2i.py:146-160; control maps in [-1, 1] with three identical
 channels like sample_t2i.py:119-141 (`2*(x/255-0.5)`, `.repeat(1,3,1,1)`).
 """
 from __future__ import annotations
@@ -44,7 +44,7 @@ def xl_ctrl_in(B: int, N: int, dim: int, seed: int, dtype=torch.float32):
 
 
 def train_attn_mask(emb_masks: torch.Tensor, n_img: int) -> torch.Tensor:
-    """Per-sample training mask of the t2i datasets, /root/reference/dataset/t2i_control.py:134-139 followed by the slicing of
+    """Per-sample training mask of the t2i datasets, dataset/t2i_control.py:134-139 followed by the slicing of
     train_t2i_canny.py:165-167: causal [S,S] with S = T + n_img, padded text COLUMNS switched off, diagonal forced on,
     then [..., :-1, :-1].  Returns bool [B, 1, S-1, S-1]."""
     B, T = emb_masks.shape

@@ -1,5 +1,5 @@
 /*
- * controlar_b200.h — C ABI of the B200-native ControlAR conditional-decoding hot path.
+ * controlar_b200.h — C ABI of the H100-native (sm_90a) ControlAR conditional-decoding hot path.
  *
  * The reference (hustvl/ControlAR) has NO native/FFI layer: its boundary for this path is a pure-Python module
  * API (SURVEY.md §8b).  This header is therefore the boundary a maintainer binds *underneath* that Python API
@@ -16,7 +16,7 @@
  *   - handles are not thread-safe; distinct handles may be used from distinct threads.
  *   - dtype codes: CAR_BF16 = 0, CAR_F32 = 1 (storage type of weights, activations and KV cache).  There is no CAR_F16:
  *     the reference's `--precision fp16` (autoregressive/sample/sample_t2i.py:54,197; default bf16) is refused by the Python shells
- *     with an explicit error.  Reason: the tensor-core operand format (mma.sync / tcgen05 kind::f16 with bf16 inputs), the
+ *     with an explicit error.  Reason: the tensor-core operand format (mma.sync / wgmma with bf16 inputs), the
  *     fragment-packed weights and the 8-byte activation packets of the persistent decode kernel are all bf16, and the rounding
  *     points that parity is defined by (SURVEY.md section 8 a-notes) differ between bf16 and fp16; an fp16 twin of every kernel was
  *     not built.  fp16 checkpoints can be run by casting the module to bf16 (or fp32) first.

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — CPU restatement of ControlAR's conditional-decoding transformer path.
 
 This is the checker for the CUDA path (and the timed CPU baseline of bench.py); it is never shipped or called
-by the product.  Every function cites the reference lines it restates (paths relative to /root/reference).
+by the product.  Every function cites the reference lines it restates (paths relative to the reference checkout).
 It is pinned against the reference itself by tests/golden/make_golden.py -> tests/golden/*.pt
 (tests/test_oracle_golden.py); the reference has no golden vectors of its own (SURVEY.md §4).
 

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE — CPU restatement of the Canny control-map front-end (SURVEY.md §8 row f3):
-/root/reference/condition/canny.py:14 `cv2.Canny(img, low_threshold, high_threshold)` on an (H, W, 3) uint8 image -> (H, W) uint8 map
+condition/canny.py:14 `cv2.Canny(img, low_threshold, high_threshold)` on an (H, W, 3) uint8 image -> (H, W) uint8 map
 of {0, 255}, which the sampling / demo code turns into the control tensor `2 * (map / 255 - 0.5)` repeated over 3 channels.
 
 The arithmetic lives in a third-party dependency, OpenCV (`opencv-python`, unpinned in the reference's requirements.txt; installed

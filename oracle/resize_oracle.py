@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE — CPU restatement of the antialiased bilinear resize in front of the online VQ encode of the
 multi-resolution training scripts (SURVEY.md §8 row f2): `F.interpolate(x.float(), size, mode='bilinear', align_corners=False,
-antialias=True)`, /root/reference/autoregressive/train/train_t2i_depth_multiscale.py:44-56 (image and control map, then
+antialias=True)`, autoregressive/train/train_t2i_depth_multiscale.py:44-56 (image and control map, then
 `2*(image/255-0.5)` and `vq_model.encode`, :216-223; the encode itself is oracle/vision_oracle.py:vq_encode_oracle).
 
 The arithmetic lives in a third-party dependency, PyTorch (ATen `_upsample_bilinear2d_aa`, UpSampleKernel.cpp

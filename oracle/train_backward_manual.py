@@ -7,7 +7,7 @@ It restates autograd's result for `oracle/train_oracle.py::TrainOracle.forward` 
 produced, tests/test_train_oracle_golden.py); tests/test_train_backward_cpu.py checks the two against each other, which
 validates the formulas before they are transcribed to CUDA, and the GPU test compares the CUDA gradients with autograd's.
 
-Reference lines (relative to /root/reference): autoregressive/models/gpt_t2i.py:420-431,451-484 (forward), RMSNorm :193-198,
+Reference lines (relative to the reference checkout): autoregressive/models/gpt_t2i.py:420-431,451-484 (forward), RMSNorm :193-198,
 Attention :257-291, FeedForward :216-217, MLP :177-181, loss :474-481; the backward itself is autograd's in the reference
 (autoregressive/train/train_c2i_canny.py:200-211: `scaler.scale(loss).backward()` on bf16 no-op scaling)."""
 from __future__ import annotations

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — CPU restatement of ControlAR's teacher-forced *training* forward (SURVEY.md §8 row f1).
 
 Checker for the (round-2) CUDA training forward / backward; never shipped or called by the product.  Every function cites the
-reference lines it restates (paths relative to /root/reference).  Pinned against the reference itself (loss, logits, gradients)
+reference lines it restates (paths relative to the reference checkout).  Pinned against the reference itself (loss, logits, gradients)
 by tests/golden/make_golden.py::train_case -> tests/golden/train_*.pt, checked in tests/test_train_oracle_golden.py.
 
 Scope: `Transformer.forward` with both ``idx`` and ``cond_idx`` given, module in train mode

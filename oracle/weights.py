@@ -7,9 +7,9 @@ function in the golden-generation script (which loads them into the *reference* 
 fixed torch version, which the fixture header records.
 
 Key names / shapes follow the checkpoint contract in SURVEY.md §8(b):
-  gpt_t2i.Transformer  : /root/reference/autoregressive/models/gpt_t2i.py:310-389
+  gpt_t2i.Transformer  : autoregressive/models/gpt_t2i.py:310-389
   HF Dinov2Model       : transformers/models/dinov2/modeling_dinov2.py (installed 5.5.0)
-  VQModel              : /root/reference/tokenizer/tokenizer_image/vq_model.py:28-61
+  VQModel              : tokenizer/tokenizer_image/vq_model.py:28-61
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""dev: TFLOP/s of the dense tcgen05 GEMM on the prefill shapes (CUDA events, 20 iterations after 5 warm-ups)."""
+"""dev: TFLOP/s of the dense wgmma GEMM on the prefill shapes (CUDA events, 20 iterations after 5 warm-ups)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -8,8 +8,7 @@ autoregressive/train/train_c2i_canny.py:190-211 drives it:
 
 Prints one JSON line with CUDA-event times of the three stages (median of --steps after --warmup).  Synthetic inputs, random-init
 weights.  The training step is a SURVEY.md §8 "next" row and a first correct path (unfused backward, explicit transposes): this
-script exists so the number can be taken; it is not part of bench.py's contract.
-Round-2 measurement: profiles/r2_bench_train.md (39.0 / 135.6 / 3.15 ms on one B200)."""
+script exists so the number can be taken; it is not part of bench.py's contract."""
 import argparse
 import json
 import os

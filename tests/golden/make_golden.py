@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Generate the committed golden fixtures by running the REFERENCE ITSELF (read-only import from
-/root/reference) on CPU with procedural weights (oracle/weights.py).  Run from the repo root in the build
-container only:
+"""Generate the committed golden fixtures by running the REFERENCE ITSELF (read-only import from a checkout of the
+upstream ControlAR repository: $CONTROLAR_REFERENCE, default ../reference next to this repository) on CPU with procedural
+weights (oracle/weights.py).  Run from the repo root:
 
     python tests/golden/make_golden.py [case ...]
 
-The GPU box has no /root/reference; tests there only read tests/golden/*.pt.  Each fixture records the torch /
+The tests never import the reference; they only read tests/golden/*.  Each fixture records the torch /
 transformers versions it was made with.  Weights are NOT stored: tests rebuild them from (spec, seed).
 """
 from __future__ import annotations
@@ -17,7 +17,7 @@ import contextlib
 import io
 
 REPO = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-REF = "/root/reference"
+REF = os.environ.get("CONTROLAR_REFERENCE", os.path.join(os.path.dirname(REPO), "reference"))
 OUT = os.path.join(REPO, "tests", "golden")
 sys.path.insert(0, REPO)
 sys.path.insert(0, REF)       # reference first: `autoregressive.*`, `tokenizer.*`, `utils.*` resolve to it
@@ -454,6 +454,74 @@ def gptpy_case():
     print("gptpy greedy", tuple(greedy.shape), "raw", tuple(raw.shape), flush=True)
 
 
+def train_gptpy_case():
+    """The LEGACY class autoregressive/models/gpt.py (imported by train_c2i_canny.py) in train mode (fp32) with the only
+    configuration its scripts use (cls_token_num = 1, condition_token_num = 0): logits and loss, plus the CFG drop decision and
+    the adapter output it drew, so that the oracle can be run on the same draws (tests/test_train_oracle_golden.py)."""
+    from autoregressive.models.gpt import Transformer as RefLegacy, ModelArgs as RefArgs
+    from oracle.weights import vit_shapes, _fill
+    from oracle.inputs import code_inputs
+    seed, B, H, W = 0, 4, 64, 64
+    spec = GPTSpec(**SMALL, cls_token_num=1, block_size=(H // 16) * (W // 16), model_type="c2i")
+    with fake_vit_cwd(2), contextlib.redirect_stdout(io.StringIO()):
+        m = RefLegacy(RefArgs(dim=spec.dim, n_layer=spec.n_layer, n_head=spec.n_head, multiple_of=spec.multiple_of, vocab_size=spec.vocab_size,
+                              cls_token_num=1, block_size=spec.block_size, num_classes=spec.num_classes, model_type="c2i",
+                              condition_token_num=0, image_size=H, token_dropout_p=0.0, resid_dropout_p=0.0, ffn_dropout_p=0.0,
+                              class_dropout_prob=0.5))
+    full = dict(make_gpt_state_dict(spec, seed, with_adapter=False))
+    full.update(_fill(vit_shapes(384, layers=2, prefix="adapter.model."), seed, 0.02))
+    full["condition_norm.weight"] = torch.ones(spec.dim)
+    m.load_state_dict(full, strict=True)
+    m = m.float().train()
+    cond = class_inputs(spec.num_classes, B, seed + 1)
+    cmap = control_map(B, H, W, seed + 2, "canny", torch.float32)
+    z = code_inputs(spec.vocab_size, B, spec.block_size, seed + 4)
+    seen = {}
+    orig_drop = m.cls_embedding.token_drop
+
+    def spy_drop(*a, **k):
+        out = orig_drop(*a, **k)
+        seen["drop_ids"] = out[1].clone()
+        return out
+    m.cls_embedding.token_drop = spy_drop
+    hook = m.adapter.register_forward_hook(lambda mod, inp, out: seen.__setitem__("feat", out.detach().clone()))
+    torch.manual_seed(1)
+    with torch.no_grad(), math_sdpa():
+        logits, loss = m(cond_idx=cond, idx=z[:, :-1], targets=z, condition=cmap)
+    hook.remove()
+    out = {"header": header(), "spec": spec.__dict__, "seed": seed, "B": B, "H": H, "W": W,
+           "class": "autoregressive/models/gpt.py Transformer (legacy c2i class) in train mode, ViT layers = 2",
+           "drop_ids": seen["drop_ids"], "feat": seen["feat"], "logits": logits.float().clone(), "loss": loss.float().clone()}
+    torch.save(out, os.path.join(OUT, "train_gptpy_legacy.pt"))
+    print("train_gptpy_legacy", tuple(out["logits"].shape), float(out["loss"]), flush=True)
+
+
+def surface_case():
+    """The reference's public surface the drop-in modules must keep (tests/test_dropin_surface_cpu.py): ModelArgs fields with their
+    defaults, and the parameter lists of generate(), its sampling helpers and both Transformer.forward methods."""
+    import dataclasses
+    import inspect
+    import json
+    import autoregressive.models.gpt_t2i as t2i
+    import autoregressive.models.gpt as gpt
+    import autoregressive.models.generate as gen
+
+    def fields(cls):
+        return {f.name: (None if f.default is dataclasses.MISSING else f.default) for f in dataclasses.fields(cls)}
+
+    def params(fn):
+        return list(inspect.signature(fn).parameters)
+    out = {"generator": "tests/golden/make_golden.py surface",
+           "model_args": {"gpt_t2i": fields(t2i.ModelArgs), "gpt": fields(gpt.ModelArgs)},
+           "generate": params(gen.generate),
+           "helpers": {n: params(getattr(gen, n)) for n in ("sample", "top_k_top_p_filtering", "logits_to_probs")},
+           "forward": {"gpt_t2i": params(t2i.Transformer.forward), "gpt": params(gpt.Transformer.forward)}}
+    with open(os.path.join(OUT, "reference_surface.json"), "w") as fh:
+        json.dump(out, fh, indent=1)
+        fh.write("\n")
+    print("surface ok", flush=True)
+
+
 def train_case(name: str, spec: GPTSpec, B: int, H: int, W: int, autocast, use_mask: bool, valid, seed: int = 0,
                drop_prob: float = 0.5, rand_seed: int = 1):
     """SURVEY.md §8 row f1: the teacher-forced TRAINING forward (module in train mode, fp32 parameters, bf16 autocast like
@@ -628,6 +696,8 @@ CASES = {
     "hed": hed_case,
     "t5": t5_case,
     "c2i_gptpy_bf16": gptpy_case,
+    "train_gptpy_legacy": train_gptpy_case,
+    "surface": surface_case,
     "train_t2i_small_ac": lambda: train_case("train_t2i_small_ac", GPTSpec(**SMALL, cls_token_num=120, block_size=64, model_type="t2i"),
                                              B=3, H=128, W=128, autocast=torch.bfloat16, use_mask=True, valid=[1, 0, 1]),
     "train_t2i_small_fp32": lambda: train_case("train_t2i_small_fp32", GPTSpec(**SMALL, cls_token_num=120, block_size=64, model_type="t2i"),

@@ -10,6 +10,15 @@ from oracle.weights import GPTSpec, make_gpt_state_dict
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
+def log_measurement(filename: str, text: str, mode: str = "a") -> None:
+    """Record the values a test compares with its bars in $CAR_TEST_LOG_DIR/<filename>; nothing is written when it is unset."""
+    d = os.environ.get("CAR_TEST_LOG_DIR")
+    if d:
+        os.makedirs(d, exist_ok=True)
+        with open(os.path.join(d, filename), mode) as fh:
+            fh.write(text)
+
+
 def load_golden(name: str):
     return torch.load(os.path.join(GOLDEN, name + ".pt"), weights_only=False)
 

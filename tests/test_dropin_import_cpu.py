@@ -1,13 +1,17 @@
 """Row b (drop-in boundary): the PYTHONPATH configuration INTEGRATION.md documents must make the reference's own import lines
 (autoregressive/sample/sample_t2i.py:15-19, sample_c2i.py:19) resolve to this repository's modules — checked in a fresh interpreter,
-from a foreign working directory.  With /root/reference present (build container) the modules this repository does NOT replace
-must still resolve to the reference tree."""
+from a foreign working directory.  With the drop-in tree in front of a reference checkout (laid out here as a stand-in tree of
+empty modules) the modules this repository does NOT replace must still resolve to the reference tree."""
 import os
 import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+# module files of the reference checkout's layout (namespace packages, no __init__.py): the ones the drop-in tree replaces,
+# and two it does not (utils/drop_path.py, dataset/augmentation.py)
+REF_LAYOUT = ["autoregressive/models/gpt_t2i.py", "autoregressive/models/gpt.py", "autoregressive/models/generate.py",
+              "autoregressive/models/dinov2_adapter.py", "autoregressive/models/vit_adapter.py", "tokenizer/tokenizer_image/vq_model.py",
+              "utils/drop_path.py", "dataset/augmentation.py"]
 
 CODE = r"""
 import os, sys
@@ -44,7 +48,11 @@ def test_dropin_imports_resolve_to_this_repo(tmp_path):
 
 
 def test_dropin_in_front_of_the_reference_tree(tmp_path):
-    import pytest
-    if not os.path.isdir(REF):
-        pytest.skip("no /root/reference on this box")
-    _run([REF], [REF], tmp_path)
+    ref = tmp_path / "reference"
+    for rel in REF_LAYOUT:
+        p = ref / rel
+        p.parent.mkdir(parents=True, exist_ok=True)
+        p.write_text("# stand-in for the reference module of the same path\n")
+    cwd = tmp_path / "cwd"
+    cwd.mkdir()
+    _run([str(ref)], [str(ref)], cwd)

@@ -1,27 +1,25 @@
 """CPU: the drop-in surface (SURVEY.md §8b) — constructor fields, function signatures, registry keys and state-dict keys of
 the product shells against the reference.  The state-dict key sets come from oracle/weights.py, which
-tests/golden/make_golden.py asserts equal to the reference modules' own ``state_dict()``; where /root/reference is present
-(the build container) the dataclass fields and signatures are compared with the reference source directly."""
+tests/golden/make_golden.py asserts equal to the reference modules' own ``state_dict()``; the dataclass fields and signatures
+are compared with the reference's, recorded by tests/golden/make_golden.py::surface_case in tests/golden/reference_surface.json."""
 import dataclasses
 import inspect
+import json
 import os
-import sys
 
-import pytest
 import torch
 
 from oracle.weights import GPTSpec, gpt_shapes, vit_shapes, vq_shapes
 
-REF = "/root/reference"
+
+def _ref_surface():
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_surface.json")) as fh:
+        return json.load(fh)
 
 
-def _ref_module(name):
-    if not os.path.isdir(REF):
-        pytest.skip("reference tree not available on this machine")
-    if REF not in sys.path:
-        sys.path.append(REF)           # after the repo: `oracle`, `tests`, `controlar_b200` keep resolving to this repo
-    import importlib
-    return importlib.import_module(name)
+def _fields(cls):
+    """{name: default} of a dataclass, normalised like the stored surface (JSON values; no default -> None)."""
+    return json.loads(json.dumps({f.name: (None if f.default is dataclasses.MISSING else f.default) for f in dataclasses.fields(cls)}))
 
 
 def test_state_dict_keys_t2i_and_c2i():
@@ -64,29 +62,25 @@ def test_model_registries_and_public_attributes():
 
 
 def test_model_args_fields_match_reference():
-    ours_t2i = {f.name: f.default for f in dataclasses.fields(__import__(
-        "controlar_b200.autoregressive.models.gpt_t2i", fromlist=["ModelArgs"]).ModelArgs)}
-    ours_gpt = {f.name: f.default for f in dataclasses.fields(__import__(
-        "controlar_b200.autoregressive.models.gpt", fromlist=["ModelArgs"]).ModelArgs)}
-    ref_t2i = {f.name: f.default for f in dataclasses.fields(_ref_module("autoregressive.models.gpt_t2i").ModelArgs)}
-    ref_gpt = {f.name: f.default for f in dataclasses.fields(_ref_module("autoregressive.models.gpt").ModelArgs)}
-    assert ours_t2i == ref_t2i
-    assert ours_gpt == ref_gpt
+    from controlar_b200.autoregressive.models import gpt_t2i, gpt
+    ref = _ref_surface()["model_args"]
+    assert _fields(gpt_t2i.ModelArgs) == ref["gpt_t2i"]
+    assert _fields(gpt.ModelArgs) == ref["gpt"]
 
 
 def test_generate_and_forward_signatures_cover_the_reference():
     from controlar_b200.autoregressive.models import generate as og, gpt_t2i as ot, gpt as ol
-    rg = _ref_module("autoregressive.models.generate")
-    ref_params = list(inspect.signature(rg.generate).parameters)
+    ref = _ref_surface()
+    ref_params = ref["generate"]
     our_params = list(inspect.signature(og.generate).parameters)
     assert [p for p in our_params if p in ref_params] == ref_params                       # same names, same order
     assert set(our_params) - set(ref_params) <= {"noise", "seed"}                         # keyword-only extras
     for name in ("sample", "top_k_top_p_filtering", "logits_to_probs"):
-        rp, op = inspect.signature(getattr(rg, name)).parameters, inspect.signature(getattr(og, name)).parameters
+        rp, op = ref["helpers"][name], inspect.signature(getattr(og, name)).parameters
         assert list(rp)[:2] == list(op)[:2], name
-    rf = list(inspect.signature(_ref_module("autoregressive.models.gpt_t2i").Transformer.forward).parameters)
+    rf = ref["forward"]["gpt_t2i"]
     assert list(inspect.signature(ot.Transformer.forward).parameters) == rf
-    rl = list(inspect.signature(_ref_module("autoregressive.models.gpt").Transformer.forward).parameters)
+    rl = ref["forward"]["gpt"]
     assert list(inspect.signature(ol.Transformer.forward).parameters)[:len(rl)] == rl     # + control_strength (must stay 1)
 
 

@@ -91,7 +91,7 @@ def test_sampler_philox_is_seeded_and_distributional():
 @pytest.mark.parametrize("M,N,K,act,res", [(1920, 3584, 1280, 0, False), (1920, 1280, 3584, 0, True), (480, 768, 256, 1, False),
                                             (1000, 1288, 1096, 0, True), (130, 136, 72, 1, True), (16384, 1280, 1280, 1, False)])
 def test_dense_tcgen05_linear_vs_torch(M, N, K, act, res):
-    """gemm_tc5.cuh (TMA + tcgen05 + TMEM): y = act(x w^T) (+ resid) against an fp32 torch reference of the same rounding points
+    """gemm_wgmma.cuh (TMA + wgmma, accumulators in registers): y = act(x w^T) (+ resid) against an fp32 torch reference of the same rounding points
     (bf16 product rounding, GELU-tanh in bf16, residual add in bf16); includes M / N / K tails (K % 64 != 0, partial tiles)."""
     from controlar_b200 import engine
     g = torch.Generator(device="cuda").manual_seed(M + N + K)

@@ -17,8 +17,10 @@ def checker(tmp_path_factory):
 
 
 @pytest.mark.parametrize("grid,b_eff,H,n_lo,n_hi", [
-    (148, 16, 20, 1, 1144),      # config 2: GPT-XL, B = 8 + CFG, every context length of a 512 x 512 image
-    (148, 8, 20, 1, 1656),       # config 4: 768 x 512, B = 4 + CFG
+    (132, 16, 20, 1, 1144),      # config 2 on an H100 (132 SMs): GPT-XL, B = 8 + CFG, every context length of a 512 x 512 image
+    (132, 8, 20, 1, 1656),       # config 4 on an H100: 768 x 512, B = 4 + CFG
+    (148, 16, 20, 1, 1144),      # the same shapes at a larger grid
+    (148, 8, 20, 1, 1656),
     (148, 16, 12, 1, 400),       # GPT-B heads
     (148, 2, 20, 1, 300),        # fewer pairs than CTAs: a pair spans several CTAs
     (148, 4, 4, 1, 80),          # the small test models

@@ -2,7 +2,7 @@
 (dim 1280, 36 layers, V 16384; CFG 4, left-padded masks, control_strength 0.6) along a forced token grid; the CPU restatement
 (oracle/ar_oracle.py) replays prefill + 2 decode steps.  Two independent bf16 implementations of the same fp32-exact arithmetic
 differ by ~2.5e-2 worst-row rel-L2 at this depth (measured here: 2.48e-2 / 2.42e-2 / 2.43e-2 at steps 0 / 1 / 2, and the same
-level — 2.3e-2 ... 2.6e-2 — for the CUDA path, profiles/r2_parity.md): this is the noise floor the GPU tolerance is set against."""
+level — 2.2e-2 ... 2.7e-2 — for the CUDA path, tests/test_zz_xl_parity_gpu.py): this is the noise floor the GPU tolerance is set against."""
 import torch
 
 from oracle.weights import GPTSpec, make_gpt_state_dict
