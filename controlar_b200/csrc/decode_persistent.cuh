@@ -61,7 +61,7 @@ struct PkParams {
     const int* forced; int forced_ld;  // teacher forcing (parity tests): token fed to the next step = forced[b * forced_ld + step] instead of the sampled one
     long long* step_ts;                // optional [n_steps]: globaltimer (ns) when CTA 0 enters step s (bench: ms/step vs context length)
     float* trace;                      // optional [n_steps][b_eff][V] fp32: raw model logits of every step (trace[0] = prefill logits, copied by the host)
-    int exp_flags;                     // dev experiments (CAR_EXP)
+    int exp_flags;                     // dev experiments (CAR_EXP): bits 0-1 pre-poll variant, bits 8-11 pre-poll back-off
     long long* dbg; int dbg_step;      // dev instrumentation: [grid][64] globaltimer stamps (ns) of one step / layer 3
 };
 
@@ -97,9 +97,22 @@ __device__ __forceinline__ void pk_mbar_wait(uint64_t* b, uint32_t parity) {
         if (!ok && ++spins > (1u << 24)) __trap();       // never hang the box
     }
 }
+// L2 eviction priority (per-instruction cache hint).  Weight units pass through L2 once per token and K/V rows are read once
+// per layer and token, so neither is ever re-read from L2: both are marked evict-first and give way to the lines that are
+// (activation packets, attention partials, the K/V rows this token writes).  Measured: DESIGN §5.
+__device__ __forceinline__ uint64_t pk_pol_evict_first() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
 __device__ __forceinline__ void pk_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(pk_smem(dst)), "l"(src), "r"(bytes), "r"(pk_smem(bar)) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(pk_smem(dst)), "l"(src), "r"(bytes), "r"(pk_smem(bar)), "l"(pk_pol_evict_first()) : "memory");
+}
+__device__ __forceinline__ uint4 pk_ld_kv(const void* p, uint64_t pol) {
+    uint4 r;
+    asm volatile("ld.global.cg.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p), "l"(pol));
+    return r;
 }
 __device__ __forceinline__ void pk_grid_sync(unsigned int* bar, unsigned int& gen) {
     __syncthreads();
@@ -196,11 +209,9 @@ __device__ __forceinline__ PkSmem pk_smem_layout() {
 struct PkCursor { int step, l, phase, blk, sub; bool done; };
 struct PkStream {
     PkCursor c;                     // next unit to copy into the ring
-    PkCursor pf;                    // next unit to prefetch into L2 (PK_L2_AHEAD units further down the stream)
     unsigned int issued;
     int lo[5], hi[5];               // block ranges per phase (0 qkv, 1 wo, 2 w13, 3 w2, 4 head)
 };
-constexpr int PK_L2_AHEAD = 20;     // ~1.4 layers of this CTA's units: HBM -> L2 runs this far ahead of L2 -> shared memory
 
 __device__ __forceinline__ int pk_phase_ks(const PkParams& P, int phase) { return (phase == 3 ? P.F : P.dim) >> 5; }
 
@@ -231,12 +242,6 @@ __device__ __forceinline__ const uint4* pk_cursor_take(const PkParams& P, const 
     pk_cursor_skip_empty(P, st, c);
     return src;
 }
-__device__ __forceinline__ void pk_stream_prefetch(const PkParams& P, PkStream& st) {
-    if (st.pf.done) return;
-    uint32_t bytes;
-    const uint4* src = pk_cursor_take(P, st, st.pf, bytes);
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void pk_stream_issue(const PkParams& P, const PkSmem& sm, PkStream& st) {
     uint32_t bytes;
     const uint4* src = pk_cursor_take(P, st, st.c, bytes);
@@ -244,7 +249,6 @@ __device__ __forceinline__ void pk_stream_issue(const PkParams& P, const PkSmem&
     pk_mbar_expect(&sm.full[slot], bytes);
     pk_bulk_g2s(sm.ring + (size_t)slot * PK_SLOT_BYTES, src, bytes, &sm.full[slot]);
     ++st.issued;
-    if (P.exp_flags & 16) pk_stream_prefetch(P, st);   // (experiment) HBM -> L2 run-ahead; off by default
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -718,6 +722,7 @@ __device__ PK_ATTN_INLINE void pk_attn_phase(const PkParams& P, int layer, int p
     const bf16* kc = sm.kvp[2 * layer];
     const bf16* vc = sm.kvp[2 * layer + 1];
     float* sc = sm.red;                                    // [PK_WARPS][2][ENT]
+    const uint64_t kv_pol = pk_pol_evict_first();
 
     // q (and, for owner segments, this token's k and v) of every segment -> shared memory, polled in parallel:
     // warp sg, lanes 0-7 q, 8-15 k, 16-23 v (lane & 7 = 16-byte chunk = 4 packets)
@@ -768,7 +773,7 @@ __device__ PK_ATTN_INLINE void pk_attn_phase(const PkParams& P, int layer, int p
 #pragma unroll
             for (int u = 0; u < UNR; ++u) {
                 const int rr = min(rb + sub + 4 * u, k1 - 1);
-                kr[u] = ldg_cg128(kbase + (size_t)rr * 64); vr[u] = ldg_cg128(vbase + (size_t)rr * 64);
+                kr[u] = pk_ld_kv(kbase + (size_t)rr * 64, kv_pol); vr[u] = pk_ld_kv(vbase + (size_t)rr * 64, kv_pol);
                 mk[u] = (mrow != nullptr && rr < P.T) ? __ldg(mrow + rr) : 1;
             }
         };
@@ -920,19 +925,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) pk_decode_kernel(const __grid_c
         st.c.step = 0; st.c.l = 0; st.c.phase = 0; st.c.blk = 0; st.c.sub = 0; st.c.done = P.n_steps <= 1;
         st.issued = 0;
         pk_cursor_skip_empty(P, st, st.c);
-        st.pf = st.c;
-        const int ahead = ((P.exp_flags >> 12) & 15) ? 2 * ((P.exp_flags >> 12) & 15) : PK_L2_AHEAD;   // (experiment knob: CAR_EXP bits 12-15)
-        if (P.exp_flags & 16) for (int i = 0; i < PK_NSLOT + ahead; ++i) pk_stream_prefetch(P, st);     // (the ring's first units included)
-        st.pf = st.c;
-        { uint32_t b; for (int i = 0; i < PK_NSLOT + ahead && !st.pf.done; ++i) pk_cursor_take(P, st, st.pf, b); }
-        while (!st.c.done && st.issued < PK_NSLOT) { /* ring priming: no extra prefetch per unit yet */
-            uint32_t bytes;
-            const uint4* src = pk_cursor_take(P, st, st.c, bytes);
-            const int slot = st.issued % PK_NSLOT;
-            pk_mbar_expect(&sm.full[slot], bytes);
-            pk_bulk_g2s(sm.ring + (size_t)slot * PK_SLOT_BYTES, src, bytes, &sm.full[slot]);
-            ++st.issued;
-        }
+        while (!st.c.done && st.issued < PK_NSLOT) pk_stream_issue(P, sm, st);   // ring priming
     }
     __syncthreads();
     unsigned int cons = 0;
