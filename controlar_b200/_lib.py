@@ -77,6 +77,9 @@ PROTOTYPES = {
     "car_hed_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_hed_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "car_hed_destroy": (C.c_int, [C.c_void_p]),
+    "car_lineart_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "car_lineart_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "car_lineart_destroy": (C.c_int, [C.c_void_p]),
     "car_t5_create": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_t5_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_t5_destroy": (C.c_int, [C.c_void_p]),

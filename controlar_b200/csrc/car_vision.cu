@@ -8,6 +8,7 @@
 #include "gemm_wgmma.cuh"
 #include "vision.cuh"
 #include "frontend.cuh"
+#include "lineart.cuh"
 
 static int vis_sm_count() {
     int dev = 0, n = 132;
@@ -897,5 +898,160 @@ extern "C" int car_hed_forward(CarHED* m, const float* img, int32_t B, int32_t H
     }
     CAR_LAUNCH(hed_merge_kernel, gsz((long long)full), 256, 0, st, hm, B, H, W, edge_out);
     if (proj_out) CAR_CUDA(cudaMemcpyAsync(proj_out, maps, proj_elems * 4, cudaMemcpyDeviceToDevice, st));
+    return CAR_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// LineArt detector (row f3): condition/lineart.py:8-86 — 7x7 stem, two stride-2 downsampling convolutions, three residual blocks,
+// two transposed convolutions, 7x7 head + sigmoid, InstanceNorm2d (no parameters) after every convolution but the head.  fp32 in
+// the reference => fp32-grade here: fp32 activations, every convolution but the head on the split-bf16 window GEMM (lineart.cuh).
+// ---------------------------------------------------------------------------------------------------------
+struct LaConv { bf16* w3; float* b; int cin3, cout; };   // cin3 = 3 * Cin_pad (channels per pixel of the S3 source)
+struct CarLineArt {
+    std::vector<void*> owned;
+    LaConv stem, down[2], res[6], up[2];              // up[i].w3: the four parity classes back to back (lineart.cuh)
+    float *head_w, *head_b;                           // [64][7][7], [1]
+    Arena ws;
+};
+
+// tensors (fp32, device), state-dict order: model0.1, model1.0, model1.3, model2.{0,1,2}.conv_block.{1,5}, model3.0, model3.3,
+// model4.1 — each weight then bias
+extern "C" int car_lineart_create(const void* const* tensors, int32_t n_tensors, void* stream, CarLineArt** out) {
+    if (!tensors || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (n_tensors != 24) CAR_FAIL(CAR_ERR_ARG, "LineArt expects 24 tensors (12 x (weight, bias) in state-dict order)");
+    for (int i = 0; i < 24; ++i)
+        if (!tensors[i]) CAR_FAIL(CAR_ERR_ARG, "null tensor");
+    cudaStream_t st = (cudaStream_t)stream;
+    CarLineArt* m = new CarLineArt();
+    int rc = CAR_OK, ti = 0;
+    auto alloc = [&](void** p, size_t bytes) {
+        if (rc != CAR_OK) return;
+        if (cudaMalloc(p, bytes) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_lineart_create: cudaMalloc failed"; *p = nullptr; return; }
+        m->owned.push_back(*p);
+    };
+    auto keep = [&](const void* src, long long n, float** dst) {
+        alloc((void**)dst, (size_t)n * 4);
+        if (rc == CAR_OK && cudaMemcpyAsync(*dst, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_lineart_create: copy failed"; }
+    };
+    auto conv = [&](LaConv& c, int cin, int cin_pad, int cout, int k) {
+        c.cin3 = 3 * cin_pad; c.cout = cout;
+        const long long n3 = (long long)cout * k * k * cin_pad;
+        alloc((void**)&c.w3, (size_t)n3 * 3 * 2);
+        if (rc == CAR_OK) conv_weight_pack_x3_kernel<<<gsz(n3), 256, 0, st>>>((const float*)tensors[ti], c.w3, cout, cin, k, k, cin_pad);
+        keep(tensors[ti + 1], cout, &c.b);
+        ti += 2;
+    };
+    auto convT = [&](LaConv& c, int cin, int cout) {
+        c.cin3 = 3 * cin; c.cout = cout;
+        const long long n3 = 9LL * cout * cin;
+        alloc((void**)&c.w3, (size_t)n3 * 3 * 2);
+        if (rc == CAR_OK) convT_weight_pack_x3_kernel<<<gsz(n3), 256, 0, st>>>((const float*)tensors[ti], c.w3, cin, cout, cin);
+        keep(tensors[ti + 1], cout, &c.b);
+        ti += 2;
+    };
+    conv(m->stem, 3, 8, 64, 7);                       // 3 input channels padded to 8 (16-byte chunks), not 32
+    conv(m->down[0], 64, 64, 128, 3);
+    conv(m->down[1], 128, 128, 256, 3);
+    for (int i = 0; i < 6; ++i) conv(m->res[i], 256, 256, 256, 3);
+    convT(m->up[0], 256, 128);
+    convT(m->up[1], 128, 64);
+    keep(tensors[ti], 64 * 49, &m->head_w); keep(tensors[ti + 1], 1, &m->head_b);
+    if (rc == CAR_OK && cudaGetLastError() != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_lineart_create: weight packing failed"; }
+    if (rc != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return rc; }
+    *out = m;
+    return CAR_OK;
+}
+extern "C" int car_lineart_destroy(CarLineArt* m) {
+    if (!m) return CAR_OK;
+    for (void* p : m->owned) cudaFree(p);
+    m->ws.release();
+    delete m;
+    return CAR_OK;
+}
+
+// one window convolution (gemm_dense.cuh A_WIN): S3 source [B][Hs][Ws][cin3] -> fp32 [B][oH][oW][cout], row (b, oy, ox) of the
+// Ho x Wo grid stored at pixel (osy*oy + oay, osx*ox + oax)
+static int la_conv(cudaStream_t st, const bf16* a3, int B, int Hs, int Ws, int cin3, const bf16* w3, const float* bias, int cout, int kh, int kw,
+                   int stride, int Ho, int Wo, float* out, int oH, int oW, int osy = 1, int osx = 1, int oay = 0, int oax = 0) {
+    static DevOnce once;
+    if (once.first()) CAR_CUDA(cudaFuncSetAttribute(dense_win_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM));
+    DenseP p;
+    memset(&p, 0, sizeof(p));
+    p.A = a3; p.B = w3; p.M = B * Ho * Wo; p.N = cout; p.K = kh * kw * cin3; p.ldb = p.K; p.alpha = 1.f;
+    p.amode = A_WIN; p.Hs = Hs; p.Ws = Ws; p.Cin = cin3; p.Ho = Ho; p.Wo = Wo; p.kh = kh; p.kw = kw; p.ws = stride;
+    p.bias_f = bias; p.C = out; p.ldc = cout; p.out_mode = 1;
+    p.osy = osy; p.osx = osx; p.oay = oay; p.oax = oax; p.oH = oH; p.oW = oW;
+    dim3 grid((p.N + DG_BN - 1) / DG_BN, (p.M + DG_BM - 1) / DG_BM, 1);
+    CAR_LAUNCH(dense_win_gemm_kernel, grid, DG_THREADS, DG_SMEM, st, p);
+    return CAR_OK;
+}
+static int la_nch(int HW) { return std::max(1, std::min(64, (HW + 2047) / 2048)); }
+
+// image fp32 NCHW [B][3][H][W] (values 0..255) -> map fp32 [B][1][Ho][Wo] in [0, 1], Ho = 4 ceil(ceil(H/2)/2) (likewise Wo)
+extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, int32_t H, int32_t W, float* out, void* stream) {
+    if (!m || !img || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (B <= 0 || H <= 4 || W <= 4) CAR_FAIL(CAR_ERR_ARG, "image must be larger than 4 x 4 (the residual blocks' reflection padding needs a 2 x 2 map)");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int H1 = (H + 1) / 2, W1 = (W + 1) / 2, H2 = (H1 + 1) / 2, W2 = (W1 + 1) / 2, H3 = 2 * H2, W3 = 2 * W2, Ho = 2 * H3, Wo = 2 * W3;
+    const size_t Bz = (size_t)B;
+    const size_t f_bytes = Bz * 4 * std::max({(size_t)H * W * 64, (size_t)H1 * W1 * 128, (size_t)H2 * W2 * 256, (size_t)H3 * W3 * 128, (size_t)Ho * Wo * 64});
+    const size_t s_bytes = Bz * std::max({(size_t)(H + 6) * (W + 6) * 24 * 2, (size_t)(H + 2) * (W + 2) * 192 * 2, (size_t)(H1 + 2) * (W1 + 2) * 384 * 2,
+                                          (size_t)(H2 + 2) * (W2 + 2) * 768 * 2, (size_t)(H3 + 1) * (W3 + 1) * 384 * 2, (size_t)(Ho + 6) * (Wo + 6) * 64 * 4});
+    const size_t x_bytes = Bz * H2 * W2 * 256 * 4, p_bytes = Bz * 64 * 256 * 4, st_bytes = Bz * 256 * 2 * 4;
+    CAR_TRY(m->ws.reserve(f_bytes + s_bytes + 2 * x_bytes + 2 * p_bytes + st_bytes + 6 * 256));
+    m->ws.reset();
+    float* F = (float*)m->ws.take(f_bytes);
+    void* S = m->ws.take(s_bytes);
+    float* X[2] = {(float*)m->ws.take(x_bytes), (float*)m->ws.take(x_bytes)};
+    float* ps = (float*)m->ws.take(p_bytes);
+    float* pq = (float*)m->ws.take(p_bytes);
+    float* stats = (float*)m->ws.take(st_bytes);
+    bf16* S3 = (bf16*)S;
+    // InstanceNorm of F [B][h][w][C] (+ resid) (ReLU) -> padded S, optional carrier
+    auto inorm = [&](int h, int w, int C, const float* resid, float* carrier, InApply a) -> int {
+        const int nch = la_nch(h * w);
+        CAR_LAUNCH(instnorm_sum_kernel, dim3(C / 32, B, nch), IN_THREADS, 0, st, (const float*)F, ps, h * w, C);
+        CAR_LAUNCH(instnorm_sq_kernel, dim3(C / 32, B, nch), IN_THREADS, 0, st, (const float*)F, (const float*)ps, pq, h * w, C);
+        CAR_LAUNCH(instnorm_finish_kernel, (B * C + 255) / 256, 256, 0, st, (const float*)ps, (const float*)pq, stats, B, h * w, C, nch);
+        const long long n = (long long)B * (h + a.pt + a.pb) * (w + a.pl + a.pr) * C;
+        CAR_LAUNCH(instnorm_apply_pad_kernel, gsz(n), 256, 0, st, (const float*)F, (const float*)stats, resid, carrier, S, B, h, w, C, a);
+        return CAR_OK;
+    };
+    const InApply zero1{1, 1, 1, 1, 0, 1, 1}, refl1{1, 1, 1, 1, 1, 1, 1}, zero_br{0, 0, 1, 1, 0, 1, 1};
+    // model0: ReflectionPad2d(3), Conv 7x7 3 -> 64, IN, ReLU
+    CAR_LAUNCH(lineart_stem_split3_kernel, gsz(Bz * (H + 6) * (W + 6) * 8), 256, 0, st, img, S3, B, 3, H, W, 3, 8);
+    CAR_TRY(la_conv(st, S3, B, H + 6, W + 6, m->stem.cin3, m->stem.w3, m->stem.b, 64, 7, 7, 1, H, W, F, H, W));
+    CAR_TRY(inorm(H, W, 64, nullptr, nullptr, zero1));
+    // model1: 2 x [Conv 3x3 stride 2 pad 1 (zeros), IN, ReLU]
+    CAR_TRY(la_conv(st, S3, B, H + 2, W + 2, m->down[0].cin3, m->down[0].w3, m->down[0].b, 128, 3, 3, 2, H1, W1, F, H1, W1));
+    CAR_TRY(inorm(H1, W1, 128, nullptr, nullptr, zero1));
+    CAR_TRY(la_conv(st, S3, B, H1 + 2, W1 + 2, m->down[1].cin3, m->down[1].w3, m->down[1].b, 256, 3, 3, 2, H2, W2, F, H2, W2));
+    CAR_TRY(inorm(H2, W2, 256, nullptr, X[0], refl1));
+    // model2: 3 x ResidualBlock: x + [ReflPad 1, Conv, IN, ReLU, ReflPad 1, Conv, IN](x); the fp32 carrier x ping-pongs X[0] / X[1]
+    for (int r = 0; r < 3; ++r) {
+        const LaConv &c1 = m->res[2 * r], &c2 = m->res[2 * r + 1];
+        CAR_TRY(la_conv(st, S3, B, H2 + 2, W2 + 2, c1.cin3, c1.w3, c1.b, 256, 3, 3, 1, H2, W2, F, H2, W2));
+        CAR_TRY(inorm(H2, W2, 256, nullptr, nullptr, refl1));
+        CAR_TRY(la_conv(st, S3, B, H2 + 2, W2 + 2, c2.cin3, c2.w3, c2.b, 256, 3, 3, 1, H2, W2, F, H2, W2));
+        InApply a = r < 2 ? refl1 : zero_br;          // the last block feeds the transposed convolution
+        a.relu = 0;
+        CAR_TRY(inorm(H2, W2, 256, X[r & 1], r < 2 ? X[(r + 1) & 1] : nullptr, a));
+    }
+    // model3: 2 x [ConvTranspose2d 3x3 stride 2 pad 1 output_padding 1, IN, ReLU], four parity classes each
+    auto up = [&](const LaConv& c, int h, int w) -> int {
+        const bf16* wc = c.w3;
+        for (int cls = 0; cls < 4; ++cls) {
+            const int a = cls >> 1, b = cls & 1, kh = 1 + a, kw = 1 + b;
+            CAR_TRY(la_conv(st, S3, B, h + 1, w + 1, c.cin3, wc, c.b, c.cout, kh, kw, 1, h, w, F, 2 * h, 2 * w, 2, 2, a, b));
+            wc += (size_t)c.cout * kh * kw * c.cin3;
+        }
+        return CAR_OK;
+    };
+    CAR_TRY(up(m->up[0], H2, W2));
+    CAR_TRY(inorm(H3, W3, 128, nullptr, nullptr, zero_br));
+    CAR_TRY(up(m->up[1], H3, W3));
+    // model4: ReflectionPad2d(3), Conv 7x7 64 -> 1, Sigmoid (direct fp32 on the padded fp32 map)
+    CAR_TRY(inorm(Ho, Wo, 64, nullptr, nullptr, InApply{3, 3, 3, 3, 1, 0, 1}));
+    CAR_LAUNCH(lineart_head_kernel, gsz((long long)B * Ho * Wo * 32), 256, 0, st, (const float*)S, (const float*)m->head_w, (const float*)m->head_b, out, B, Ho, Wo);
     return CAR_OK;
 }

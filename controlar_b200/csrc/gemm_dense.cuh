@@ -7,6 +7,10 @@
 //                 nearest-2x up-sampled view of the source (Upsample, tokenizer/tokenizer_image/vq_model.py:368-379);
 //                 K index = tap*Cin + c, tap = ky*3+kx; row m = (b*Ho + y)*Wo + x
 //     A_CONV3x3S2: 3x3 / stride 2 on an input padded (0,1,0,1) (Downsample, vq_model.py:382-397)
+//     A_WIN      : kh x kw window, stride s, over an already padded NHWC source [B][Hs][Ws][Cin] (no bounds checks in the
+//                  window): row m = (b*Ho + oy)*Wo + ox reads pixels (s*oy + ky, s*ox + kx), K index = (ky*kw + kx)*Cin + c.
+//                  fp32 output through a pixel map: row (b, oy, ox) is stored at pixel (osy*oy + oay, osx*ox + oax) of an
+//                  [B][oH][oW][ldc] tensor.  Own instantiation (dense_win_gemm_kernel); dense_gemm_kernel does not take it.
 //   B operand: row-major [N, K] (nn.Linear / flattened conv weight [Cout, 9*Cin] in (ky,kx,c) order)
 //   batched via blockIdx.z with element strides.
 //
@@ -16,7 +20,7 @@
 #pragma once
 #include "common.cuh"
 
-enum { A_PLAIN = 0, A_CONV3x3 = 1, A_CONV3x3S2 = 2 };
+enum { A_PLAIN = 0, A_CONV3x3 = 1, A_CONV3x3S2 = 2, A_WIN = 3 };
 enum { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF = 2, ACT_RELU = 3 };
 
 struct DenseP {
@@ -35,6 +39,8 @@ struct DenseP {
     const bf16* resid; int ldr;        // residual added last: r(v + resid)
     void* C; int ldc;
     int out_mode;                      // 0: bf16 [M, ldc]; 1: fp32 [M, ldc]; 2: fp32 NCHW image: C[(b*N + n)*Ho*Wo + pix]
+    int kh, kw, ws;                    // A_WIN: window and stride
+    int osy, osx, oay, oax, oH, oW;    // A_WIN: output pixel map
 };
 
 constexpr int DG_BM = 128, DG_BN = 128, DG_BK = 32, DG_STAGES = 3, DG_THREADS = 256;
@@ -56,7 +62,8 @@ template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile(
 // ldmatrix (8 rows x 16 B) and the 16-B cp.async stores are bank-conflict free.
 __device__ __forceinline__ int dg_off(int row, int chunk) { return row * DG_BK + ((chunk ^ ((row >> 1) & 3)) << 3); }
 
-static __global__ void __launch_bounds__(DG_THREADS) dense_gemm_kernel(DenseP p) {   // (static: one copy per translation unit)
+template <bool WIN>
+__device__ __forceinline__ void dense_gemm_body(const DenseP& p) {
     extern __shared__ __align__(128) unsigned char dg_smem[];
     bf16* sA = reinterpret_cast<bf16*>(dg_smem);
     bf16* sB = sA + DG_STAGES * DG_BM * DG_BK;
@@ -98,6 +105,12 @@ static __global__ void __launch_bounds__(DG_THREADS) dense_gemm_kernel(DenseP p)
                 src = A + (size_t)(m0 + a_row[i]) * p.lda + k;
             } else {
                 const int tap = k / p.Cin, c = k - tap * p.Cin;
+                if constexpr (WIN) {
+                    const int ky = tap / p.kw, kx = tap - ky * p.kw;
+                    src = A + (((size_t)cb[i] * p.Hs + cy[i] * p.ws + ky) * p.Ws + cx[i] * p.ws + kx) * p.Cin + c;
+                    cp_async16_zfill(a_s + dg_off(a_row[i], a_kc[i]), ok ? src : A, ok);
+                    continue;
+                }
                 const int ky = tap / 3, kx = tap - ky * 3;
                 int yy, xx;
                 if (p.amode == A_CONV3x3) { yy = cy[i] + ky - 1; xx = cx[i] + kx - 1; }
@@ -176,6 +189,13 @@ static __global__ void __launch_bounds__(DG_THREADS) dense_gemm_kernel(DenseP p)
                 for (int e = 0; e < 2; ++e) {
                     const int n = n0 + wn * 32 + j * 8 + 2 * t + e;
                     if (n >= p.N) continue;
+                    if constexpr (WIN) {   // fp32 bias, pixel-mapped fp32 store
+                        const int hw = p.Ho * p.Wo;
+                        const int b = m / hw, r = m - b * hw, oy = r / p.Wo, ox = r - oy * p.Wo;
+                        const size_t pix = ((size_t)b * p.oH + p.osy * oy + p.oay) * p.oW + p.osx * ox + p.oax;
+                        ((float*)p.C)[pix * p.ldc + n] = acc[i][j][hh * 2 + e] + p.bias_f[n];
+                        continue;
+                    }
                     float v = acc[i][j][hh * 2 + e] * p.alpha;
                     if (p.bias) v += tof(p.bias[p.bias_along_m ? m : n]);
                     if (p.bias_f) v += p.bias_f[n];
@@ -198,3 +218,5 @@ static __global__ void __launch_bounds__(DG_THREADS) dense_gemm_kernel(DenseP p)
         }
     }
 }
+static __global__ void __launch_bounds__(DG_THREADS) dense_gemm_kernel(DenseP p) { dense_gemm_body<false>(p); }   // (static: one copy per translation unit)
+static __global__ void __launch_bounds__(DG_THREADS) dense_win_gemm_kernel(DenseP p) { dense_gemm_body<true>(p); }

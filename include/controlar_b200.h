@@ -287,6 +287,16 @@ int car_hed_create(const void* const* tensors, int32_t n_tensors, void* stream, 
 int car_hed_forward(CarHED* m, const float* img, int32_t B, int32_t H, int32_t W, float* edge_out, float* proj_out, void* stream);
 int car_hed_destroy(CarHED* m);
 
+/* LineArt detector: condition/lineart.py:8-86 (LineArt.forward), fp32 in the reference => fp32-grade split-bf16 convolutions here.
+ * car_lineart_create: 24 fp32 device tensors in state-dict order — model0.1, model1.0, model1.3, model2.{0,1,2}.conv_block.{1,5},
+ * model3.0 (ConvTranspose2d, [Cin][Cout][3][3]), model3.3, model4.1, each .weight then .bias — copied / packed (nothing borrowed).
+ * car_lineart_forward: image fp32 NCHW [B][3][H][W] in 0..255 (H, W > 4) -> map fp32 [B][1][Ho][Wo] in [0, 1] with
+ * Ho = 4 * ceil(ceil(H / 2) / 2), Wo likewise (70 x 90 in -> 72 x 92 out, as in the reference). */
+typedef struct CarLineArt CarLineArt;
+int car_lineart_create(const void* const* tensors, int32_t n_tensors, void* stream, CarLineArt** out);
+int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, int32_t H, int32_t W, float* out, void* stream);
+int car_lineart_destroy(CarLineArt* m);
+
 /* Fused multi-tensor AdamW step (row f1: autoregressive/train/train_c2i.py:28-50 builds torch.optim.AdamW(fused=True)).
  * tensors_dev: device array of { float* param; const float* grad; float* exp_avg; float* exp_avg_sq; int64 numel; float weight_decay;
  * int32 pad } (48 bytes each); chunks_dev: device array of int32 pairs { tensor index, chunk index } — chunk = 65536 elements;
