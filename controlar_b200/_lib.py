@@ -39,6 +39,12 @@ class CarSampling(C.Structure):
                 ("seed", C.c_uint64)]
 
 
+class CarDptDesc(C.Structure):
+    _fields_ = [("hidden", C.c_int32), ("n_layers", C.c_int32), ("n_heads", C.c_int32), ("mlp", C.c_int32),
+                ("out_indices", C.c_int32 * 4), ("neck", C.c_int32 * 4), ("fusion", C.c_int32), ("pos_grid", C.c_int32),
+                ("ln_eps", C.c_float)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/controlar_b200.h
 PROTOTYPES = {
     "car_last_error": (C.c_char_p, []),
@@ -80,6 +86,9 @@ PROTOTYPES = {
     "car_lineart_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_lineart_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_lineart_destroy": (C.c_int, [C.c_void_p]),
+    "car_dpt_create": (C.c_int, [C.POINTER(CarDptDesc), C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "car_dpt_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "car_dpt_destroy": (C.c_int, [C.c_void_p]),
     "car_t5_create": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_t5_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_t5_destroy": (C.c_int, [C.c_void_p]),

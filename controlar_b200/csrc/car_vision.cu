@@ -9,6 +9,7 @@
 #include "vision.cuh"
 #include "frontend.cuh"
 #include "lineart.cuh"
+#include "dpt.cuh"
 
 static int vis_sm_count() {
     int dev = 0, n = 132;
@@ -1053,5 +1054,285 @@ extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, i
     // model4: ReflectionPad2d(3), Conv 7x7 64 -> 1, Sigmoid (direct fp32 on the padded fp32 map)
     CAR_TRY(inorm(Ho, Wo, 64, nullptr, nullptr, InApply{3, 3, 3, 3, 1, 0, 1}));
     CAR_LAUNCH(lineart_head_kernel, gsz((long long)B * Ho * Wo * 32), 256, 0, st, (const float*)S, (const float*)m->head_w, (const float*)m->head_b, out, B, Ho, Wo);
+    return CAR_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// DPT depth detector (row f3): transformers DPTForDepthEstimation — ViT encoder, reassemble (readout "project", factors 4, 2, 1,
+// 0.5), neck 3x3 convolutions, four fusion stages, depth head.  fp32 in the reference => fp32-grade here: fp32 activations, every
+// GEMM and 3x3 stride-1 convolution on the fp32-output wgmma instantiation over split-bf16 operands, the stride-2 convolution on
+// the window GEMM (gemm_dense.cuh A_WIN), attention fused (dpt.cuh).  No eager or mma.sync fall-back for the wgmma stages.
+// ---------------------------------------------------------------------------------------------------------
+struct DptLin { bf16* w3; float* b; int n, k; };      // W3 [n][3k] (k = 9 cin for a 3x3 convolution), fp32 bias or null
+struct CarDpt {
+    CarDptDesc d;
+    std::vector<void*> owned;
+    DptLin patch;
+    float *cls, *pos;                                   // [C], [1 + g^2][C]
+    struct Layer { DptLin qkv, o, fc1, fc2; float *ln1w, *ln1b, *ln2w, *ln2b; };
+    std::vector<Layer> L;
+    DptLin proj[4], resize[4], readout[4], neck[4];     // resize: ConvTranspose2d GEMM (stages 0, 1), 3x3 stride-2 convolution (3)
+    DptLin fproj[4], rcu[4][2][2];                      // fusion layer j: projection, residual_layer{1,2}.convolution{1,2}
+    DptLin head0, head2;
+    float *head4w, *head4b;
+    Arena ws;
+};
+static const int DPT_FACTOR[4] = {4, 2, 1, 0};         // 0: the 0.5 stage (3x3 stride-2 convolution)
+
+extern "C" int car_dpt_create(const CarDptDesc* desc, const void* const* tensors, int32_t n_tensors, void* stream, CarDpt** out) {
+    if (!desc || !tensors || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    const CarDptDesc& d = *desc;
+    if (d.hidden <= 0 || d.hidden % 64 || d.n_heads * 64 != d.hidden) CAR_FAIL(CAR_ERR_UNSUPPORTED, "heads must be 64-dimensional (hidden == 64 * heads)");
+    if (d.n_layers <= 0 || d.mlp <= 0 || d.mlp % 8 || d.pos_grid <= 0 || !(d.ln_eps > 0.f)) CAR_FAIL(CAR_ERR_ARG, "bad layers / mlp / pos_grid / eps");
+    for (int i = 0; i < 4; ++i) {
+        if (d.neck[i] <= 0 || d.neck[i] % 64) CAR_FAIL(CAR_ERR_UNSUPPORTED, "neck sizes must be positive multiples of 64");
+        if (d.out_indices[i] < 0 || d.out_indices[i] >= d.n_layers || (i && d.out_indices[i] <= d.out_indices[i - 1]))
+            CAR_FAIL(CAR_ERR_ARG, "out indices must be ascending encoder layers");
+    }
+    if (d.fusion <= 0 || d.fusion % 128) CAR_FAIL(CAR_ERR_UNSUPPORTED, "fusion size must be a positive multiple of 128");
+    if (n_tensors != 4 + 16 * d.n_layers + 74) CAR_FAIL(CAR_ERR_ARG, "DPT expects 4 + 16 * n_layers + 74 tensors in state-dict order");
+    for (int i = 0; i < n_tensors; ++i)
+        if (!tensors[i]) CAR_FAIL(CAR_ERR_ARG, "null tensor");
+    cudaStream_t st = (cudaStream_t)stream;
+    CarDpt* m = new CarDpt();
+    m->d = d;
+    const int C = d.hidden, F = d.fusion;
+    int rc = CAR_OK, ti = 0;
+    auto alloc = [&](void** p, size_t bytes) {
+        if (rc != CAR_OK) return;
+        if (cudaMalloc(p, bytes) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_dpt_create: cudaMalloc failed"; *p = nullptr; return; }
+        m->owned.push_back(*p);
+    };
+    auto copy = [&](float* dst, const void* src, long long n) {
+        if (rc == CAR_OK && cudaMemcpyAsync(dst, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_dpt_create: copy failed"; }
+    };
+    auto keep = [&](long long n, float** dst) {
+        alloc((void**)dst, (size_t)n * 4);
+        copy(*dst, tensors[ti++], n);
+    };
+    // weight [n][cin][kh][kw] (kh = kw = 1: nn.Linear) -> W3 [n][kh][kw][3 cin]; then the bias when `bias`
+    auto lin = [&](DptLin& L, int n, int cin, int k, bool bias) {
+        L.n = n; L.k = k * k * cin; L.b = nullptr;
+        alloc((void**)&L.w3, (size_t)n * L.k * 3 * 2);
+        if (rc == CAR_OK) conv_weight_pack_x3_kernel<<<gsz((long long)n * L.k), 256, 0, st>>>((const float*)tensors[ti], L.w3, n, cin, k, k, cin);
+        ++ti;
+        if (bias) keep(n, &L.b);
+    };
+    // ConvTranspose2d(k = s = f): weight [cin][cin][f][f] -> W3 [f^2 cin][3 cin]; the bias repeated per (ky, kx)
+    auto convT = [&](DptLin& L, int cin, int f) {
+        L.n = f * f * cin; L.k = cin;
+        alloc((void**)&L.w3, (size_t)L.n * L.k * 3 * 2);
+        if (rc == CAR_OK) dpt_convT_pack_kernel<<<gsz((long long)L.n * L.k), 256, 0, st>>>((const float*)tensors[ti], L.w3, cin, cin, f);
+        ++ti;
+        alloc((void**)&L.b, (size_t)L.n * 4);
+        for (int t = 0; t < f * f; ++t) copy(L.b + (size_t)t * cin, tensors[ti], cin);
+        ++ti;
+    };
+    // dpt.embeddings
+    keep(C, &m->cls);
+    keep((long long)(1 + d.pos_grid * d.pos_grid) * C, &m->pos);
+    lin(m->patch, C, 3 * 256, 1, true);                 // [C][3][16][16] read as [C][768]
+    // dpt.encoder.layer.{i}: query, key, value (one [3C][3C] GEMM), output.dense, intermediate.dense, output.dense, LN before / after
+    m->L.resize(d.n_layers);
+    for (int l = 0; l < d.n_layers && rc == CAR_OK; ++l) {
+        CarDpt::Layer& Ly = m->L[l];
+        Ly.qkv.n = 3 * C; Ly.qkv.k = C;
+        alloc((void**)&Ly.qkv.w3, (size_t)3 * C * C * 3 * 2);
+        alloc((void**)&Ly.qkv.b, (size_t)3 * C * 4);
+        for (int j = 0; j < 3 && rc == CAR_OK; ++j) {
+            conv_weight_pack_x3_kernel<<<gsz((long long)C * C), 256, 0, st>>>((const float*)tensors[ti], Ly.qkv.w3 + (size_t)j * C * 3 * C, C, C, 1, 1, C);
+            copy(Ly.qkv.b + (size_t)j * C, tensors[ti + 1], C);
+            ti += 2;
+        }
+        lin(Ly.o, C, C, 1, true);
+        lin(Ly.fc1, d.mlp, C, 1, true);
+        lin(Ly.fc2, C, d.mlp, 1, true);
+        keep(C, &Ly.ln1w); keep(C, &Ly.ln1b); keep(C, &Ly.ln2w); keep(C, &Ly.ln2b);
+    }
+    ti += 2;                                            // dpt.layernorm: applied to last_hidden_state only, which depth does not use
+    // neck.reassemble_stage.layers.{i}: projection (1x1), resize
+    for (int i = 0; i < 4; ++i) {
+        lin(m->proj[i], d.neck[i], C, 1, true);
+        if (DPT_FACTOR[i] > 1) convT(m->resize[i], d.neck[i], DPT_FACTOR[i]);
+        else if (DPT_FACTOR[i] == 0) lin(m->resize[i], d.neck[i], d.neck[i], 3, true);
+    }
+    for (int i = 0; i < 4; ++i) lin(m->readout[i], C, 2 * C, 1, true);
+    for (int i = 0; i < 4; ++i) lin(m->neck[i], F, d.neck[i], 3, false);
+    for (int j = 0; j < 4; ++j) {
+        lin(m->fproj[j], F, F, 1, true);
+        for (int r = 0; r < 2; ++r)
+            for (int c = 0; c < 2; ++c) lin(m->rcu[j][r][c], F, F, 3, true);
+    }
+    lin(m->head0, F / 2, F, 3, true);
+    lin(m->head2, 32, F / 2, 3, true);
+    keep(32, &m->head4w); keep(1, &m->head4b);
+    if (rc == CAR_OK && ti != n_tensors) { rc = CAR_ERR_ARG; g_car_err = "car_dpt_create: tensor count mismatch"; }
+    if (rc == CAR_OK && cudaGetLastError() != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_dpt_create: weight packing failed"; }
+    if (rc != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return rc; }
+    *out = m;
+    return CAR_OK;
+}
+extern "C" int car_dpt_destroy(CarDpt* m) {
+    if (!m) return CAR_OK;
+    for (void* p : m->owned) cudaFree(p);
+    m->ws.release();
+    delete m;
+    return CAR_OK;
+}
+
+static int wg_launch_f32(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, const WgP& q, int tiles_m) {
+    static DevOnce once;
+    if (once.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_wgmma_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
+    const int ntiles = tiles_m * ((q.N + WG_BN - 1) / WG_BN);
+    CAR_LAUNCH(gemm_wgmma_f32_kernel, std::min(ntiles, vis_sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
+    return CAR_OK;
+}
+// out fp32 [M][ldc] = a3 (S3 rows [M][3 w.k]) · W3^T + bias (+ resid [M][ldc])
+static int dpt_gemm(cudaStream_t st, const DptLin& w, const bf16* a3, int M, float* out, int ldc, const float* resid = nullptr) {
+    alignas(64) CUtensorMap mapA, mapB;
+    if (!wg_make_map(&mapA, a3, M, 3 * w.k, 3 * w.k) || !wg_make_map(&mapB, w.w3, w.n, 3 * w.k, 3 * w.k)) CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
+    WgP q;
+    memset(&q, 0, sizeof(q));
+    q.M = M; q.N = w.n; q.K = 3 * w.k; q.bias_f = w.b; q.resid_f = resid; q.ldr = ldc; q.C32 = out; q.ldc = ldc;
+    return wg_launch_f32(st, mapA, mapB, q, (M + WG_BM - 1) / WG_BM);
+}
+// TMA convolution frame: a map smaller than one 16 x 8 pixel box is held in a zero-filled frame of at least that size
+static inline int dpt_fh(int H) { return std::max(H, WG_TH); }
+static inline int dpt_fw(int W) { return std::max(W, WG_TW); }
+// 3x3 / pad 1 / stride 1 convolution: S3 NHWC frame [B][dpt_fh(H)][dpt_fw(W)][3 cin] -> fp32 NHWC [B][H][W][w.n] (+ resid)
+static int dpt_conv3(cudaStream_t st, const DptLin& w, const bf16* s3, int B, int H, int W, float* out, const float* resid = nullptr) {
+    const int cin3 = 3 * (w.k / 9);
+    alignas(64) CUtensorMap mapA, mapB;
+    if (!wg_make_map_nhwc(&mapA, s3, B, dpt_fh(H), dpt_fw(W), cin3) || !wg_make_map(&mapB, w.w3, w.n, 3 * w.k, 3 * w.k))
+        CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
+    WgP q;
+    memset(&q, 0, sizeof(q));
+    q.M = B * H * W; q.N = w.n; q.K = 3 * w.k; q.bias_f = w.b; q.resid_f = resid; q.ldr = w.n; q.C32 = out; q.ldc = w.n;
+    q.conv = 1; q.H = H; q.W = W; q.tiles_x = (W + WG_TW - 1) / WG_TW; q.tiles_y = (H + WG_TH - 1) / WG_TH; q.cblks = cin3 / WG_BK;
+    return wg_launch_f32(st, mapA, mapB, q, B * q.tiles_x * q.tiles_y);
+}
+// S3 image producer (dpt.cuh dpt_image_split_kernel)
+static int dpt_img(cudaStream_t st, const float* a, const float* b, float* sum_out, bf16* y, DptImg q) {
+    CAR_LAUNCH(dpt_image_split_kernel, gsz((long long)q.B * q.Hp * q.Wp * q.C), 256, 0, st, a, b, sum_out, y, q);
+    return CAR_OK;
+}
+static DptImg dpt_frame(int B, int H, int W, int C) { return DptImg{B, H, W, C, dpt_fh(H), dpt_fw(W), 0, 0, 0, 0, 0}; }
+
+// pixel_values fp32 NCHW [B][3][H][W] -> predicted_depth fp32 [B][H][W]
+extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, int32_t H, int32_t W, float* depth, void* stream) {
+    if (!m || !pixel_values || !depth) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (B <= 0 || H != W || H % 32 || H < 64) CAR_FAIL(CAR_ERR_ARG, "pixel_values must be square with a side that is a multiple of 32 and at least 64");
+    if (!wg_encoder()) CAR_FAIL(CAR_ERR_UNSUPPORTED, "the DPT detector needs cuTensorMapEncodeTiled (TMA)");
+    cudaStream_t st = (cudaStream_t)stream;
+    const CarDptDesc& d = m->d;
+    const int C = d.hidden, F = d.fusion, h = H / 16, T = 1 + h * h, M = B * T, Mp = B * h * h;
+    const int side[4] = {4 * h, 2 * h, h, h / 2};
+    const size_t Bz = (size_t)B;
+    // workspace: encoder fp32 rows, fp32 temporaries, the four neck features, one S3 buffer (each operand is consumed before the next
+    // is written)
+    size_t ft = (size_t)M * std::max(3 * C, d.mlp);
+    size_t s3 = std::max({(size_t)M * 3 * std::max(C, d.mlp), (size_t)Mp * 3 * 768, (size_t)Mp * 6 * C});
+    for (int i = 0; i < 4; ++i) {
+        const int f = DPT_FACTOR[i];
+        ft = std::max({ft, (size_t)Mp * C, (size_t)Mp * (f > 1 ? f * f : 1) * d.neck[i]});
+        s3 = std::max({s3, (size_t)Mp * 3 * d.neck[i], Bz * (h + 2) * (h + 2) * 3 * d.neck[i],
+                       Bz * dpt_fh(side[i]) * dpt_fw(side[i]) * 3 * std::max(d.neck[i], F)});
+    }
+    ft = std::max({ft, Bz * 64 * h * h * F, Bz * 256 * h * h * 32});
+    s3 = std::max({s3, Bz * 64 * h * h * 3 * F, Bz * 256 * h * h * 3 * (F / 2)});
+    size_t feat = 0;
+    for (int i = 0; i < 4; ++i) feat += Bz * dpt_fh(side[i]) * dpt_fw(side[i]) * F * 4 + 256;
+    CAR_TRY(m->ws.reserve(6 * ((size_t)M * C * 4 + 256) + 3 * (ft * 4 + 256) + feat + s3 * 2 + 256));
+    m->ws.reset();
+    float* X = (float*)m->ws.take((size_t)M * C * 4);
+    float* X1 = (float*)m->ws.take((size_t)M * C * 4);
+    float* keep[4];
+    for (int i = 0; i < 4; ++i) keep[i] = (float*)m->ws.take((size_t)M * C * 4);
+    float* T0 = (float*)m->ws.take(ft * 4);
+    float* T1 = (float*)m->ws.take(ft * 4);
+    float* T2 = (float*)m->ws.take(ft * 4);
+    float* fe[4];
+    for (int i = 0; i < 4; ++i) fe[i] = (float*)m->ws.take(Bz * side[i] * side[i] * F * 4);
+    bf16* S = (bf16*)m->ws.take(s3 * 2);
+
+    // ---- embeddings: patch convolution as a GEMM, [CLS], resized position embeddings
+    CAR_LAUNCH(dpt_patchify_kernel, gsz((long long)Mp * 768), 256, 0, st, pixel_values, S, B, h);
+    CAR_TRY(dpt_gemm(st, m->patch, S, Mp, T0, C));
+    CAR_LAUNCH(dpt_assemble_kernel, gsz((long long)M * C), 256, 0, st, (const float*)T0, (const float*)m->cls, (const float*)m->pos, X, B, h, d.pos_grid, C);
+    // ---- encoder: pre-LN layers; the residual stream stays fp32, the out-index layers write their output into keep[]
+    float* x = X;
+    int kept = 0;
+    for (int l = 0; l < d.n_layers; ++l) {
+        const CarDpt::Layer& Ly = m->L[l];
+        CAR_LAUNCH(dpt_layernorm_split_kernel, M, DPT_LN_THREADS, 0, st, (const float*)x, (const float*)Ly.ln1w, (const float*)Ly.ln1b, S, C, d.ln_eps);
+        CAR_TRY(dpt_gemm(st, Ly.qkv, S, M, T0, 3 * C));
+        CAR_LAUNCH(dpt_attention_kernel, dim3((T + DPT_AT_B - 1) / DPT_AT_B, d.n_heads, B), 128, 0, st, (const float*)T0, S, T, C);
+        CAR_TRY(dpt_gemm(st, Ly.o, S, M, X1, C, x));
+        CAR_LAUNCH(dpt_layernorm_split_kernel, M, DPT_LN_THREADS, 0, st, (const float*)X1, (const float*)Ly.ln2w, (const float*)Ly.ln2b, S, C, d.ln_eps);
+        CAR_TRY(dpt_gemm(st, Ly.fc1, S, M, T0, d.mlp));
+        CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)M * d.mlp), 256, 0, st, (const float*)T0, S, (long long)M, d.mlp, 1);
+        float* dst = (kept < 4 && d.out_indices[kept] == l) ? keep[kept++] : X;
+        CAR_TRY(dpt_gemm(st, Ly.fc2, S, M, dst, C, X1));
+        x = dst;
+        if (kept == 4) break;                           // later layers feed nothing the depth map uses
+    }
+    // ---- reassemble: readout projection + GELU, 1x1 projection, resize; then the neck's 3x3 convolution -> fe[i] fp32 NHWC
+    for (int i = 0; i < 4; ++i) {
+        const int Cn = d.neck[i], f = DPT_FACTOR[i], s = side[i];
+        CAR_LAUNCH(dpt_readout_split_kernel, gsz((long long)Mp * 2 * C), 256, 0, st, (const float*)keep[i], S, B, h * h, C);
+        CAR_TRY(dpt_gemm(st, m->readout[i], S, Mp, T0, C));
+        CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)Mp * C), 256, 0, st, (const float*)T0, S, (long long)Mp, C, 1);
+        CAR_TRY(dpt_gemm(st, m->proj[i], S, Mp, T1, Cn));                           // [B][h][h][Cn]
+        DptImg q = dpt_frame(B, s, s, Cn);
+        if (f > 1) {
+            CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)Mp * Cn), 256, 0, st, (const float*)T1, S, (long long)Mp, Cn, 0);
+            CAR_TRY(dpt_gemm(st, m->resize[i], S, Mp, T0, f * f * Cn));          // [B][h][h][f][f][Cn]
+            q.shuf = f;
+            CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, q));
+        } else if (f == 0) {
+            CAR_TRY(dpt_img(st, T1, nullptr, nullptr, S, DptImg{B, h, h, Cn, h + 2, h + 2, 1, 1, 0, 0, 0}));
+            CAR_TRY(la_conv(st, S, B, h + 2, h + 2, 3 * Cn, m->resize[i].w3, m->resize[i].b, Cn, 3, 3, 2, s, s, T0, s, s));
+            CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, q));
+        } else {
+            CAR_TRY(dpt_img(st, T1, nullptr, nullptr, S, q));
+        }
+        CAR_TRY(dpt_conv3(st, m->neck[i], S, B, s, s, fe[i]));
+    }
+    // ---- fusion, from the coarsest feature: [prev + RCU1(feature)] -> RCU2 -> x2 bilinear (align_corners=True) -> 1x1 projection.
+    // RCU(r) = conv2(ReLU(conv1(ReLU(r)))) + r; the ReLUs, the add and the upsample are fused into the S3 producers.
+    float* prev = nullptr;                              // fp32 [B][s][s][F], in T1
+    for (int j = 0; j < 4; ++j) {
+        const int i = 3 - j, s = side[i];
+        DptImg rq = dpt_frame(B, s, s, F);
+        rq.relu = 1;
+        const float* xin = fe[i];                       // input of residual_layer2
+        if (prev) {
+            CAR_TRY(dpt_img(st, fe[i], nullptr, nullptr, S, rq));
+            CAR_TRY(dpt_conv3(st, m->rcu[j][0][0], S, B, s, s, T0));
+            CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, rq));
+            CAR_TRY(dpt_conv3(st, m->rcu[j][0][1], S, B, s, s, T0, fe[i]));
+            CAR_TRY(dpt_img(st, prev, T0, prev, S, rq));                             // prev += RCU1(feature), ReLU'd S3 of it
+            xin = prev;
+        } else {
+            CAR_TRY(dpt_img(st, fe[i], nullptr, nullptr, S, rq));
+        }
+        CAR_TRY(dpt_conv3(st, m->rcu[j][1][0], S, B, s, s, T0));
+        CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, rq));
+        CAR_TRY(dpt_conv3(st, m->rcu[j][1][1], S, B, s, s, T2, xin));
+        DptImg uq{B, 2 * s, 2 * s, F, 2 * s, 2 * s, 0, 0, 0, 1, 0};
+        CAR_TRY(dpt_img(st, T2, nullptr, nullptr, S, uq));
+        CAR_TRY(dpt_gemm(st, m->fproj[j], S, B * 4 * s * s, T1, F));
+        prev = T1;
+    }
+    // ---- head: conv 3x3 F -> F/2, x2 bilinear (align_corners=True), conv 3x3 F/2 -> 32, ReLU, conv 1x1 32 -> 1, ReLU
+    const int s8 = 8 * h;
+    CAR_TRY(dpt_img(st, prev, nullptr, nullptr, S, dpt_frame(B, s8, s8, F)));
+    CAR_TRY(dpt_conv3(st, m->head0, S, B, s8, s8, T0));
+    DptImg uq = dpt_frame(B, H, W, F / 2);
+    uq.up = 1;
+    CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, uq));
+    CAR_TRY(dpt_conv3(st, m->head2, S, B, H, W, T2));
+    CAR_LAUNCH(dpt_head_kernel, gsz((long long)B * H * W * 32), 256, 0, st, (const float*)T2, (const float*)m->head4w, (const float*)m->head4b, depth,
+               (long long)B * H * W);
     return CAR_OK;
 }

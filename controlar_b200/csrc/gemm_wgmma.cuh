@@ -14,6 +14,8 @@
 //                           left in flight; the stage of the previous k-block is released (empty, one arrive per warp) once
 //                           wgmma.wait_group 1 has retired it.  The epilogue applies bf16 round / GELU / LayerScale / residual (same
 //                           rounding points as gemm_dense.cuh) straight from the accumulator registers.
+// Two instantiations of one body: gemm_wgmma_kernel (the bf16 epilogue above) and gemm_wgmma_f32_kernel (acc + fp32 bias
+// (+ fp32 residual) stored as fp32, no rounding: the split-bf16 "x3" GEMMs and 3x3 convolutions of the DPT depth detector).
 // Shared-memory descriptors (sm_90 layout): start >> 4 | LBO (unused for swizzled K-major, 1) << 16 | SBO 1024 >> 4 << 32 |
 // layout 1 (128-byte swizzle) << 62; the k16 step inside a 128-byte swizzle atom advances the start address by 32 bytes.
 #pragma once
@@ -37,6 +39,10 @@ struct WgP {
     // (c0, 16 tx + kx - 1, 8 ty + ky - 1, n): out-of-bounds pixels (the padding) are zero-filled by TMA, and the box lands in shared
     // memory as 128 rows x 128 bytes — exactly the K-major SWIZZLE_128B operand tile of the plain GEMM.
     int conv, H, W, tiles_x, tiles_y, cblks;
+    // fp32-output instantiation (gemm_wgmma_f32_kernel, the split-bf16 "x3" path of vision.cuh): C32[row, n] = acc + bias_f[n]
+    // (+ resid_f[row, n]) stored as fp32 with no rounding; resid_f has row pitch ldr, C32 row pitch ldc.  The fields above that
+    // round to bf16 (resid, C, act, bias, scale) are not read there.
+    const float* bias_f; const float* resid_f; float* C32;
 };
 constexpr int WG_TW = 16, WG_TH = 8;                                            // output-pixel block of a conv tile (WG_TW * WG_TH = WG_BM)
 
@@ -104,8 +110,19 @@ __device__ __forceinline__ void wg_store_pair(const WgP& p, int row, int n, floa
     *reinterpret_cast<__nv_bfloat162*>(p.C + (size_t)row * p.ldc + n) = __floats2bfloat162_rn(f[0], f[1]);
 }
 
-static __global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                                                                          const WgP p) {
+// fp32 epilogue of one row and one pair of adjacent columns n, n + 1: the order of nn.Linear / Conv2d (bias) then `+ residual`
+__device__ __forceinline__ void wg_store_pair_f32(const WgP& p, int row, int n, float a0, float a1) {
+    float2 f = make_float2(a0, a1);
+    if (p.bias_f) { f.x += p.bias_f[n]; f.y += p.bias_f[n + 1]; }
+    if (p.resid_f) {
+        const float2 r = *reinterpret_cast<const float2*>(p.resid_f + (size_t)row * p.ldr + n);
+        f.x += r.x; f.y += r.y;
+    }
+    *reinterpret_cast<float2*>(p.C32 + (size_t)row * p.ldc + n) = f;
+}
+
+template <bool F32>
+__device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap& mapA, const CUtensorMap& mapB, const WgP& p) {
     extern __shared__ unsigned char wg_raw[];
     __shared__ __align__(8) uint64_t bar_full[WG_STAGES], bar_empty[WG_STAGES];
     const uint32_t smem0 = (wg_smem(wg_raw) + 1023u) & ~1023u;                 // stage s: A at smem0 + s * 32 KB, B 16 KB after
@@ -193,11 +210,21 @@ static __global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_kernel(const 
 #pragma unroll
             for (int j = 0; j < WG_BN / 8; ++j) {
                 const int n8 = tn * WG_BN + j * 8;
-                if (n8 < p.N)                                                   // N % 8 == 0 (host-checked): whole 8-column groups
-                    wg_store_pair(p, row, n8 + 2 * (lane & 3), acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                if (n8 < p.N) {                                                 // N % 8 == 0 (host-checked): whole 8-column groups
+                    if constexpr (F32) wg_store_pair_f32(p, row, n8 + 2 * (lane & 3), acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                    else wg_store_pair(p, row, n8 + 2 * (lane & 3), acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                }
             }
         }
     }
+}
+static __global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                                                                          const WgP p) {
+    gemm_wgmma_body<false>(mapA, mapB, p);
+}
+static __global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_f32_kernel(const __grid_constant__ CUtensorMap mapA,
+                                                                              const __grid_constant__ CUtensorMap mapB, const WgP p) {
+    gemm_wgmma_body<true>(mapA, mapB, p);
 }
 
 // ---- host: tensor maps (driver entry point fetched through the runtime: the library does not link libcuda) ----

@@ -297,6 +297,25 @@ int car_lineart_create(const void* const* tensors, int32_t n_tensors, void* stre
 int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, int32_t H, int32_t W, float* out, void* stream);
 int car_lineart_destroy(CarLineArt* m);
 
+/* DPT depth detector: transformers DPTForDepthEstimation (Intel/dpt-large, non-hybrid ViT backbone, readout "project",
+ * reassemble factors 4, 2, 1, 0.5, 64-dim heads, exact GELU, no fusion batch norm), fp32 in the reference => fp32-grade here: every
+ * GEMM and 3x3 convolution on split-bf16 operands with fp32 accumulation, attention fused.  car_dpt_create: n fp32 device tensors
+ * in state-dict order (4 + 16 * n_layers + 74 of them, dpt.layernorm included and unused) — copied / packed (nothing borrowed).
+ * Sizes: hidden % 64 == 0 (heads of 64), mlp % 8 == 0, neck sizes and fusion / 2 multiples of 64.
+ * car_dpt_forward: pixel_values fp32 NCHW [B][3][H][W] with H == W, H % 32 == 0, H >= 64 -> predicted_depth fp32 [B][H][W]. */
+typedef struct {
+    int32_t hidden, n_layers, n_heads, mlp;
+    int32_t out_indices[4];         /* encoder layers whose outputs feed the neck, ascending */
+    int32_t neck[4];                /* neck_hidden_sizes */
+    int32_t fusion;                 /* fusion_hidden_size */
+    int32_t pos_grid;               /* side of the stored position-embedding grid (image_size / 16) */
+    float ln_eps;
+} CarDptDesc;
+typedef struct CarDpt CarDpt;
+int car_dpt_create(const CarDptDesc* desc, const void* const* tensors, int32_t n_tensors, void* stream, CarDpt** out);
+int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, int32_t H, int32_t W, float* depth, void* stream);
+int car_dpt_destroy(CarDpt* m);
+
 /* Fused multi-tensor AdamW step (row f1: autoregressive/train/train_c2i.py:28-50 builds torch.optim.AdamW(fused=True)).
  * tensors_dev: device array of { float* param; const float* grad; float* exp_avg; float* exp_avg_sq; int64 numel; float weight_decay;
  * int32 pad } (48 bytes each); chunks_dev: device array of int32 pairs { tensor index, chunk index } — chunk = 65536 elements;
