@@ -89,6 +89,9 @@ PROTOTYPES = {
     "car_dpt_create": (C.c_int, [C.POINTER(CarDptDesc), C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_dpt_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_dpt_destroy": (C.c_int, [C.c_void_p]),
+    "car_midas_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "car_midas_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "car_midas_destroy": (C.c_int, [C.c_void_p]),
     "car_t5_create": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_t5_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_t5_destroy": (C.c_int, [C.c_void_p]),

@@ -10,6 +10,7 @@
 #include "frontend.cuh"
 #include "lineart.cuh"
 #include "dpt.cuh"
+#include "midas.cuh"
 
 static int vis_sm_count() {
     int dev = 0, n = 132;
@@ -1064,17 +1065,21 @@ extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, i
 // the window GEMM (gemm_dense.cuh A_WIN), attention fused (dpt.cuh).  No eager or mma.sync fall-back for the wgmma stages.
 // ---------------------------------------------------------------------------------------------------------
 struct DptLin { bf16* w3; float* b; int n, k; };      // W3 [n][3k] (k = 9 cin for a 3x3 convolution), fp32 bias or null
+struct DptLayer { DptLin qkv, o, fc1, fc2; float *ln1w, *ln1b, *ln2w, *ln2b; };
+struct DptDecoder {                                     // fusion stages and depth head (shared with MiDaS DPT-Hybrid)
+    DptLin fproj[4], rcu[4][2][2];                      // fusion layer j: projection, residual_layer{1,2}.convolution{1,2}
+    DptLin head0, head2;
+    float *head4w, *head4b;
+};
 struct CarDpt {
     CarDptDesc d;
     std::vector<void*> owned;
     DptLin patch;
     float *cls, *pos;                                   // [C], [1 + g^2][C]
-    struct Layer { DptLin qkv, o, fc1, fc2; float *ln1w, *ln1b, *ln2w, *ln2b; };
+    using Layer = DptLayer;
     std::vector<Layer> L;
     DptLin proj[4], resize[4], readout[4], neck[4];     // resize: ConvTranspose2d GEMM (stages 0, 1), 3x3 stride-2 convolution (3)
-    DptLin fproj[4], rcu[4][2][2];                      // fusion layer j: projection, residual_layer{1,2}.convolution{1,2}
-    DptLin head0, head2;
-    float *head4w, *head4b;
+    DptDecoder dec;
     Arena ws;
 };
 static const int DPT_FACTOR[4] = {4, 2, 1, 0};         // 0: the 0.5 stage (3x3 stride-2 convolution)
@@ -1159,13 +1164,13 @@ extern "C" int car_dpt_create(const CarDptDesc* desc, const void* const* tensors
     for (int i = 0; i < 4; ++i) lin(m->readout[i], C, 2 * C, 1, true);
     for (int i = 0; i < 4; ++i) lin(m->neck[i], F, d.neck[i], 3, false);
     for (int j = 0; j < 4; ++j) {
-        lin(m->fproj[j], F, F, 1, true);
+        lin(m->dec.fproj[j], F, F, 1, true);
         for (int r = 0; r < 2; ++r)
-            for (int c = 0; c < 2; ++c) lin(m->rcu[j][r][c], F, F, 3, true);
+            for (int c = 0; c < 2; ++c) lin(m->dec.rcu[j][r][c], F, F, 3, true);
     }
-    lin(m->head0, F / 2, F, 3, true);
-    lin(m->head2, 32, F / 2, 3, true);
-    keep(32, &m->head4w); keep(1, &m->head4b);
+    lin(m->dec.head0, F / 2, F, 3, true);
+    lin(m->dec.head2, 32, F / 2, 3, true);
+    keep(32, &m->dec.head4w); keep(1, &m->dec.head4b);
     if (rc == CAR_OK && ti != n_tensors) { rc = CAR_ERR_ARG; g_car_err = "car_dpt_create: tensor count mismatch"; }
     if (rc == CAR_OK && cudaGetLastError() != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_dpt_create: weight packing failed"; }
     if (rc != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return rc; }
@@ -1218,6 +1223,63 @@ static int dpt_img(cudaStream_t st, const float* a, const float* b, float* sum_o
 }
 static DptImg dpt_frame(int B, int H, int W, int C) { return DptImg{B, H, W, C, dpt_fh(H), dpt_fw(W), 0, 0, 0, 0, 0}; }
 
+// one pre-LN encoder layer over fp32 rows x [B][T][C] -> dst (x may equal dst); S, T0 and X1 are scratch
+static int dpt_layer(cudaStream_t st, const DptLayer& Ly, const float* x, float* dst, int B, int T, int C, int heads, int mlp, float eps, bf16* S,
+                     float* T0, float* X1) {
+    const int M = B * T;
+    CAR_LAUNCH(dpt_layernorm_split_kernel, M, DPT_LN_THREADS, 0, st, x, (const float*)Ly.ln1w, (const float*)Ly.ln1b, S, C, eps);
+    CAR_TRY(dpt_gemm(st, Ly.qkv, S, M, T0, 3 * C));
+    CAR_LAUNCH(dpt_attention_kernel, dim3((T + DPT_AT_B - 1) / DPT_AT_B, heads, B), 128, 0, st, (const float*)T0, S, T, C);
+    CAR_TRY(dpt_gemm(st, Ly.o, S, M, X1, C, x));
+    CAR_LAUNCH(dpt_layernorm_split_kernel, M, DPT_LN_THREADS, 0, st, (const float*)X1, (const float*)Ly.ln2w, (const float*)Ly.ln2b, S, C, eps);
+    CAR_TRY(dpt_gemm(st, Ly.fc1, S, M, T0, mlp));
+    CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)M * mlp), 256, 0, st, (const float*)T0, S, (long long)M, mlp, 1);
+    CAR_TRY(dpt_gemm(st, Ly.fc2, S, M, dst, C, X1));
+    return CAR_OK;
+}
+
+// fusion, from the coarsest feature: [prev + RCU1(feature)] -> RCU2 -> x2 bilinear (align_corners=True) -> 1x1 projection, then the
+// head: conv 3x3 F -> F/2, x2 bilinear (align_corners=True), conv 3x3 F/2 -> 32, ReLU, conv 1x1 32 -> 1, ReLU.
+// RCU(r) = conv2(ReLU(conv1(ReLU(r)))) + r; the ReLUs, the add and the upsample are fused into the S3 producers.
+// fe[i]: fp32 NHWC [B][sh[i]][sw[i]][F] (i = 0 finest, 2 sh[i] = sh[i-1]); the depth map is [B][H][W] with H = 4 sh[0]
+static int dpt_decode(cudaStream_t st, const DptDecoder& w, float* const fe[4], const int sh[4], const int sw[4], int B, int H, int W, int F,
+                      float* T0, float* T1, float* T2, bf16* S, float* depth) {
+    float* prev = nullptr;                              // fp32 [B][s][s][F], in T1
+    for (int j = 0; j < 4; ++j) {
+        const int i = 3 - j, s = sh[i], t = sw[i];
+        DptImg rq = dpt_frame(B, s, t, F);
+        rq.relu = 1;
+        const float* xin = fe[i];                       // input of residual_layer2
+        if (prev) {
+            CAR_TRY(dpt_img(st, fe[i], nullptr, nullptr, S, rq));
+            CAR_TRY(dpt_conv3(st, w.rcu[j][0][0], S, B, s, t, T0));
+            CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, rq));
+            CAR_TRY(dpt_conv3(st, w.rcu[j][0][1], S, B, s, t, T0, fe[i]));
+            CAR_TRY(dpt_img(st, prev, T0, prev, S, rq));                             // prev += RCU1(feature), ReLU'd S3 of it
+            xin = prev;
+        } else {
+            CAR_TRY(dpt_img(st, fe[i], nullptr, nullptr, S, rq));
+        }
+        CAR_TRY(dpt_conv3(st, w.rcu[j][1][0], S, B, s, t, T0));
+        CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, rq));
+        CAR_TRY(dpt_conv3(st, w.rcu[j][1][1], S, B, s, t, T2, xin));
+        DptImg uq{B, 2 * s, 2 * t, F, 2 * s, 2 * t, 0, 0, 0, 1, 0};
+        CAR_TRY(dpt_img(st, T2, nullptr, nullptr, S, uq));
+        CAR_TRY(dpt_gemm(st, w.fproj[j], S, B * 4 * s * t, T1, F));
+        prev = T1;
+    }
+    const int h2 = H / 2, w2 = W / 2;
+    CAR_TRY(dpt_img(st, prev, nullptr, nullptr, S, dpt_frame(B, h2, w2, F)));
+    CAR_TRY(dpt_conv3(st, w.head0, S, B, h2, w2, T0));
+    DptImg uq = dpt_frame(B, H, W, F / 2);
+    uq.up = 1;
+    CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, uq));
+    CAR_TRY(dpt_conv3(st, w.head2, S, B, H, W, T2));
+    CAR_LAUNCH(dpt_head_kernel, gsz((long long)B * H * W * 32), 256, 0, st, (const float*)T2, (const float*)w.head4w, (const float*)w.head4b, depth,
+               (long long)B * H * W);
+    return CAR_OK;
+}
+
 // pixel_values fp32 NCHW [B][3][H][W] -> predicted_depth fp32 [B][H][W]
 extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, int32_t H, int32_t W, float* depth, void* stream) {
     if (!m || !pixel_values || !depth) CAR_FAIL(CAR_ERR_ARG, "null argument");
@@ -1258,21 +1320,14 @@ extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, 
     // ---- embeddings: patch convolution as a GEMM, [CLS], resized position embeddings
     CAR_LAUNCH(dpt_patchify_kernel, gsz((long long)Mp * 768), 256, 0, st, pixel_values, S, B, h);
     CAR_TRY(dpt_gemm(st, m->patch, S, Mp, T0, C));
-    CAR_LAUNCH(dpt_assemble_kernel, gsz((long long)M * C), 256, 0, st, (const float*)T0, (const float*)m->cls, (const float*)m->pos, X, B, h, d.pos_grid, C);
+    CAR_LAUNCH(dpt_assemble_kernel, gsz((long long)M * C), 256, 0, st, (const float*)T0, (const float*)m->cls, (const float*)m->pos, X, B, h, h, d.pos_grid,
+               C);
     // ---- encoder: pre-LN layers; the residual stream stays fp32, the out-index layers write their output into keep[]
     float* x = X;
     int kept = 0;
     for (int l = 0; l < d.n_layers; ++l) {
-        const CarDpt::Layer& Ly = m->L[l];
-        CAR_LAUNCH(dpt_layernorm_split_kernel, M, DPT_LN_THREADS, 0, st, (const float*)x, (const float*)Ly.ln1w, (const float*)Ly.ln1b, S, C, d.ln_eps);
-        CAR_TRY(dpt_gemm(st, Ly.qkv, S, M, T0, 3 * C));
-        CAR_LAUNCH(dpt_attention_kernel, dim3((T + DPT_AT_B - 1) / DPT_AT_B, d.n_heads, B), 128, 0, st, (const float*)T0, S, T, C);
-        CAR_TRY(dpt_gemm(st, Ly.o, S, M, X1, C, x));
-        CAR_LAUNCH(dpt_layernorm_split_kernel, M, DPT_LN_THREADS, 0, st, (const float*)X1, (const float*)Ly.ln2w, (const float*)Ly.ln2b, S, C, d.ln_eps);
-        CAR_TRY(dpt_gemm(st, Ly.fc1, S, M, T0, d.mlp));
-        CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)M * d.mlp), 256, 0, st, (const float*)T0, S, (long long)M, d.mlp, 1);
         float* dst = (kept < 4 && d.out_indices[kept] == l) ? keep[kept++] : X;
-        CAR_TRY(dpt_gemm(st, Ly.fc2, S, M, dst, C, X1));
+        CAR_TRY(dpt_layer(st, m->L[l], x, dst, B, T, C, d.n_heads, d.mlp, d.ln_eps, S, T0, X1));
         x = dst;
         if (kept == 4) break;                           // later layers feed nothing the depth map uses
     }
@@ -1298,41 +1353,272 @@ extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, 
         }
         CAR_TRY(dpt_conv3(st, m->neck[i], S, B, s, s, fe[i]));
     }
-    // ---- fusion, from the coarsest feature: [prev + RCU1(feature)] -> RCU2 -> x2 bilinear (align_corners=True) -> 1x1 projection.
-    // RCU(r) = conv2(ReLU(conv1(ReLU(r)))) + r; the ReLUs, the add and the upsample are fused into the S3 producers.
-    float* prev = nullptr;                              // fp32 [B][s][s][F], in T1
-    for (int j = 0; j < 4; ++j) {
-        const int i = 3 - j, s = side[i];
-        DptImg rq = dpt_frame(B, s, s, F);
-        rq.relu = 1;
-        const float* xin = fe[i];                       // input of residual_layer2
-        if (prev) {
-            CAR_TRY(dpt_img(st, fe[i], nullptr, nullptr, S, rq));
-            CAR_TRY(dpt_conv3(st, m->rcu[j][0][0], S, B, s, s, T0));
-            CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, rq));
-            CAR_TRY(dpt_conv3(st, m->rcu[j][0][1], S, B, s, s, T0, fe[i]));
-            CAR_TRY(dpt_img(st, prev, T0, prev, S, rq));                             // prev += RCU1(feature), ReLU'd S3 of it
-            xin = prev;
-        } else {
-            CAR_TRY(dpt_img(st, fe[i], nullptr, nullptr, S, rq));
+    // ---- fusion and head
+    return dpt_decode(st, m->dec, fe, side, side, B, H, W, F, T0, T1, T2, S, depth);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// MiDaS DPT-Hybrid depth detector (row f3): condition/midas (DPTDepthModel, backbone vitb_rn50_384) — a ResNet-50 trunk (timm
+// ResNetV2: weight-standardised bias-free convolutions, GroupNorm(32), TF "SAME" padding, stages of 3, 4, 9 bottlenecks) whose
+// stage-2 map is the token grid of a ViT-B/16 (1x1 projection, [CLS], position embeddings resized to h x w), then reassemble
+// (stage outputs 0 and 1 as they are; readout "project" of blocks 8 and 11, 1x1 convolution, and a 3x3/2 convolution for the
+// last), the neck's 3x3 convolutions and the DPT fusion and head (dpt_decode).  fp32 in the reference => fp32-grade here: 1x1
+// convolutions and GEMMs on dpt_gemm, 3x3 stride-1 convolutions on dpt_conv3 (wgmma), the stem and the stride-2 convolutions on
+// the window GEMM (la_conv), GroupNorm in midas.cuh.  Token grids need not be square.
+// ---------------------------------------------------------------------------------------------------------
+struct MdNorm { float *w, *b; };
+struct MdBlock { DptLin dn, c1, c2, c3; MdNorm dnn, n1, n2, n3; int cin, mid, out, stride; };
+static const int MD_DEPTH[3] = {3, 4, 9}, MD_OUT[3] = {256, 512, 1024};
+constexpr int MD_BLOCKS = 16, MD_C = 768, MD_HEADS = 12, MD_MLP = 3072, MD_F = 256, MD_GRID = 24, MD_NT = 368;
+struct CarMidas {
+    std::vector<void*> owned;
+    float* zero;                                        // [1024] zeros: the bias of the bias-free window convolutions
+    DptLin stem;
+    MdNorm stem_n;
+    MdBlock blk[MD_BLOCKS];
+    DptLin patch;                                       // patch_embed.proj: 1x1 convolution 1024 -> 768 with bias
+    float *cls, *pos;                                   // [768], [1 + 24^2][768]
+    DptLayer L[12];
+    DptLin readout[2], proj[2], resize4, rn[4];         // act_postprocess{3,4}: readout, 1x1, (3x3/2); scratch.layer{1..4}_rn
+    DptDecoder dec;
+    Arena ws;
+};
+
+// tensors (fp32, device), state-dict order of controlar_b200.condition.midas.DPTDepthModel: pretrained.model.{cls_token, pos_embed,
+// patch_embed.backbone.{stem, stages.*.blocks.*}, patch_embed.proj, blocks.*, norm, head}, pretrained.act_postprocess{3,4},
+// scratch.layer{1..4}_rn, scratch.refinenet{1..4}, scratch.output_conv
+extern "C" int car_midas_create(const void* const* tensors, int32_t n_tensors, void* stream, CarMidas** out) {
+    if (!tensors || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (n_tensors != MD_NT) CAR_FAIL(CAR_ERR_ARG, "MiDaS DPT-Hybrid expects 368 tensors in state-dict order");
+    for (int i = 0; i < n_tensors; ++i)
+        if (!tensors[i]) CAR_FAIL(CAR_ERR_ARG, "null tensor");
+    cudaStream_t st = (cudaStream_t)stream;
+    CarMidas* m = new CarMidas();
+    int rc = CAR_OK, ti = 0;
+    auto alloc = [&](void** p, size_t bytes) {
+        if (rc != CAR_OK) return;
+        if (cudaMalloc(p, bytes) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_midas_create: cudaMalloc failed"; *p = nullptr; return; }
+        m->owned.push_back(*p);
+    };
+    auto keep = [&](long long n, float** dst) {
+        alloc((void**)dst, (size_t)n * 4);
+        if (rc == CAR_OK && cudaMemcpyAsync(*dst, tensors[ti], (size_t)n * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_midas_create: copy failed"; }
+        ++ti;
+    };
+    auto lin = [&](DptLin& L, int n, int cin, int k, bool bias) {
+        L.n = n; L.k = k * k * cin; L.b = nullptr;
+        alloc((void**)&L.w3, (size_t)n * L.k * 3 * 2);
+        if (rc == CAR_OK) conv_weight_pack_x3_kernel<<<gsz((long long)n * L.k), 256, 0, st>>>((const float*)tensors[ti], L.w3, n, cin, k, k, cin);
+        ++ti;
+        if (bias) keep(n, &L.b);
+    };
+    // weight-standardised convolution [n][cin][k][k] -> W3 [n][k][k][3 cin_pad]; the standardised fp32 weight goes through `wsd`,
+    // re-used in stream order (its largest user is a 3x3 256 -> 256 convolution)
+    float* wsd = nullptr;
+    alloc((void**)&wsd, (size_t)256 * 256 * 9 * 4);
+    auto sconv = [&](DptLin& L, int n, int cin, int k, int cin_pad) {
+        L.n = n; L.k = k * k * cin_pad; L.b = nullptr;
+        alloc((void**)&L.w3, (size_t)n * L.k * 3 * 2);
+        if (rc == CAR_OK) {
+            midas_ws_kernel<<<n, MD_THREADS, 0, st>>>((const float*)tensors[ti], wsd, cin * k * k, 1e-8);
+            conv_weight_pack_x3_kernel<<<gsz((long long)n * L.k), 256, 0, st>>>(wsd, L.w3, n, cin, k, k, cin_pad);
         }
-        CAR_TRY(dpt_conv3(st, m->rcu[j][1][0], S, B, s, s, T0));
-        CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, rq));
-        CAR_TRY(dpt_conv3(st, m->rcu[j][1][1], S, B, s, s, T2, xin));
-        DptImg uq{B, 2 * s, 2 * s, F, 2 * s, 2 * s, 0, 0, 0, 1, 0};
-        CAR_TRY(dpt_img(st, T2, nullptr, nullptr, S, uq));
-        CAR_TRY(dpt_gemm(st, m->fproj[j], S, B * 4 * s * s, T1, F));
-        prev = T1;
+        ++ti;
+    };
+    auto norm = [&](MdNorm& N, int c) { keep(c, &N.w); keep(c, &N.b); };
+    alloc((void**)&m->zero, 1024 * 4);
+    if (rc == CAR_OK && cudaMemsetAsync(m->zero, 0, 1024 * 4, st) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_midas_create: memset failed"; }
+    keep(MD_C, &m->cls);
+    keep((long long)(1 + MD_GRID * MD_GRID) * MD_C, &m->pos);
+    sconv(m->stem, 64, 3, 7, 8);                        // 3 input channels padded to 8 (16-byte chunks)
+    norm(m->stem_n, 64);
+    int cin = 64, bi = 0;
+    for (int s = 0; s < 3; ++s)
+        for (int b = 0; b < MD_DEPTH[s]; ++b, ++bi) {
+            MdBlock& k = m->blk[bi];
+            k.cin = cin; k.out = MD_OUT[s]; k.mid = k.out / 4; k.stride = (s > 0 && b == 0) ? 2 : 1;
+            if (b == 0) { sconv(k.dn, k.out, cin, 1, cin); norm(k.dnn, k.out); }
+            sconv(k.c1, k.mid, cin, 1, cin); norm(k.n1, k.mid);
+            sconv(k.c2, k.mid, k.mid, 3, k.mid); norm(k.n2, k.mid);
+            sconv(k.c3, k.out, k.mid, 1, k.mid); norm(k.n3, k.out);
+            cin = k.out;
+        }
+    lin(m->patch, MD_C, 1024, 1, true);
+    for (int l = 0; l < 12; ++l) {                      // blocks.{l}: norm1, attn.qkv (fused), attn.proj, norm2, mlp.fc1, mlp.fc2
+        DptLayer& Ly = m->L[l];
+        keep(MD_C, &Ly.ln1w); keep(MD_C, &Ly.ln1b);
+        lin(Ly.qkv, 3 * MD_C, MD_C, 1, true);
+        lin(Ly.o, MD_C, MD_C, 1, true);
+        keep(MD_C, &Ly.ln2w); keep(MD_C, &Ly.ln2b);
+        lin(Ly.fc1, MD_MLP, MD_C, 1, true);
+        lin(Ly.fc2, MD_C, MD_MLP, 1, true);
     }
-    // ---- head: conv 3x3 F -> F/2, x2 bilinear (align_corners=True), conv 3x3 F/2 -> 32, ReLU, conv 1x1 32 -> 1, ReLU
-    const int s8 = 8 * h;
-    CAR_TRY(dpt_img(st, prev, nullptr, nullptr, S, dpt_frame(B, s8, s8, F)));
-    CAR_TRY(dpt_conv3(st, m->head0, S, B, s8, s8, T0));
-    DptImg uq = dpt_frame(B, H, W, F / 2);
-    uq.up = 1;
-    CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, uq));
-    CAR_TRY(dpt_conv3(st, m->head2, S, B, H, W, T2));
-    CAR_LAUNCH(dpt_head_kernel, gsz((long long)B * H * W * 32), 256, 0, st, (const float*)T2, (const float*)m->head4w, (const float*)m->head4b, depth,
-               (long long)B * H * W);
+    ti += 4;                                            // norm, head: the ViT's final norm and classifier, unused by the depth map
+    for (int i = 0; i < 2; ++i) {
+        lin(m->readout[i], MD_C, 2 * MD_C, 1, true);
+        lin(m->proj[i], MD_C, MD_C, 1, true);
+    }
+    lin(m->resize4, MD_C, MD_C, 3, true);
+    const int rn_in[4] = {256, 512, MD_C, MD_C};
+    for (int i = 0; i < 4; ++i) lin(m->rn[i], MD_F, rn_in[i], 3, false);
+    for (int r = 1; r <= 4; ++r) {                      // refinenet{r} is fusion layer 4 - r (the coarsest runs first)
+        const int j = 4 - r;
+        lin(m->dec.fproj[j], MD_F, MD_F, 1, true);
+        for (int u = 0; u < 2; ++u)
+            for (int c = 0; c < 2; ++c) lin(m->dec.rcu[j][u][c], MD_F, MD_F, 3, true);
+    }
+    lin(m->dec.head0, MD_F / 2, MD_F, 3, true);
+    lin(m->dec.head2, 32, MD_F / 2, 3, true);
+    keep(32, &m->dec.head4w); keep(1, &m->dec.head4b);
+    if (rc == CAR_OK && ti != n_tensors) { rc = CAR_ERR_ARG; g_car_err = "car_midas_create: tensor count mismatch"; }
+    if (rc == CAR_OK && cudaGetLastError() != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_midas_create: weight packing failed"; }
+    if (rc != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return rc; }
+    *out = m;
     return CAR_OK;
+}
+extern "C" int car_midas_destroy(CarMidas* m) {
+    if (!m) return CAR_OK;
+    for (void* p : m->owned) cudaFree(p);
+    m->ws.release();
+    delete m;
+    return CAR_OK;
+}
+
+// x fp32 NCHW [B][3][H][W] -> depth fp32 [B][H][W]
+extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t H, int32_t W, float* depth, void* stream) {
+    if (!m || !x || !depth) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (B <= 0 || H % 32 || W % 32 || H < 64 || W < 64) CAR_FAIL(CAR_ERR_ARG, "x must be [B][3][H][W] with H and W multiples of 32 and at least 64");
+    if (!wg_encoder()) CAR_FAIL(CAR_ERR_UNSUPPORTED, "the MiDaS detector needs cuTensorMapEncodeTiled (TMA)");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int C = MD_C, F = MD_F, h = H / 16, w = W / 16, P = h * w, T = 1 + P, M = B * T, Mp = B * P;
+    const int sh[4] = {H / 4, H / 8, h, h / 2}, sw[4] = {W / 4, W / 8, w, w / 2};
+    const size_t Bz = (size_t)B, HW = (size_t)H * W;
+    // workspace: encoder rows, fp32 temporaries, trunk carriers, neck features, GroupNorm partials, one S3 buffer (each operand is
+    // consumed before the next is written)
+    const size_t ft = std::max({(size_t)M * MD_MLP, Bz * HW / 4 * F, Bz * HW * 32, Bz * HW / 4 * 64});
+    const size_t car = Bz * HW / 16 * 256;              // the widest trunk map: stage 0, 256 channels at H/4
+    size_t s3 = std::max({Bz * (H + 5) * (W + 5) * 24, (size_t)M * 3 * MD_MLP, (size_t)Mp * 6 * C, Bz * (h + 2) * (w + 2) * 3 * C,
+                          Bz * 4 * sh[0] * sw[0] * 3 * F, Bz * dpt_fh(H / 2) * dpt_fw(W / 2) * 3 * F, Bz * HW * 3 * (F / 2)});
+    {
+        int hh = H / 4, ww = W / 4, ci = 64;
+        for (int s = 0; s < 3; ++s) {
+            const int mid = MD_OUT[s] / 4, ho = s ? hh / 2 : hh, wo = s ? ww / 2 : ww;
+            s3 = std::max({s3, Bz * hh * ww * 3 * ci, Bz * (hh + 1) * (ww + 1) * 3 * mid, Bz * dpt_fh(hh) * dpt_fw(ww) * 3 * mid,
+                           Bz * ho * wo * 3 * MD_OUT[s]});
+            ci = MD_OUT[s]; hh = ho; ww = wo;
+        }
+        const int rn_in[4] = {256, 512, MD_C, MD_C};
+        for (int i = 0; i < 4; ++i) s3 = std::max(s3, Bz * dpt_fh(sh[i]) * dpt_fw(sw[i]) * 3 * std::max(rn_in[i], F));
+    }
+    size_t feat = 0;
+    for (int i = 0; i < 4; ++i) feat += Bz * sh[i] * sw[i] * F * 4 + 256;
+    const size_t part = Bz * 64 * MD_GROUPS * 4, stb = Bz * MD_GROUPS * 2 * 4;
+    CAR_TRY(m->ws.reserve(4 * ((size_t)M * C * 4 + 256) + 3 * (ft * 4 + 256) + 3 * (car * 4 + 256) + feat + 2 * (part + 256) + 2 * (stb + 256) +
+                          s3 * 2 + 256));
+    m->ws.reset();
+    float* X = (float*)m->ws.take((size_t)M * C * 4);
+    float* X1 = (float*)m->ws.take((size_t)M * C * 4);
+    float* K[2] = {(float*)m->ws.take((size_t)M * C * 4), (float*)m->ws.take((size_t)M * C * 4)};
+    float* T0 = (float*)m->ws.take(ft * 4);
+    float* T1 = (float*)m->ws.take(ft * 4);
+    float* T2 = (float*)m->ws.take(ft * 4);
+    float* Xa = (float*)m->ws.take(car * 4);
+    float* Xb = (float*)m->ws.take(car * 4);
+    float* Td = (float*)m->ws.take(car * 4);
+    float* fe[4];
+    for (int i = 0; i < 4; ++i) fe[i] = (float*)m->ws.take(Bz * sh[i] * sw[i] * F * 4);
+    float* ps = (float*)m->ws.take(part);
+    float* pq = (float*)m->ws.take(part);
+    float* stats = (float*)m->ws.take(stb);
+    float* rstats = (float*)m->ws.take(stb);
+    bf16* S = (bf16*)m->ws.take(s3 * 2);
+
+    // GroupNorm statistics of fp32 NHWC [B][hh][ww][Cc] -> stt [B][32][2]; chunks of about 4096 elements per (image, group)
+    auto gn_stats = [&](const float* src, int hh, int ww, int Cc, float* stt) -> int {
+        const int hw = hh * ww, nch = std::max(1, std::min(64, (hw * (Cc / MD_GROUPS) + 4095) / 4096));
+        CAR_LAUNCH(midas_gn_sum_kernel, dim3(MD_GROUPS, B, nch), MD_THREADS, 0, st, src, ps, hw, Cc);
+        CAR_LAUNCH(midas_gn_sq_kernel, dim3(MD_GROUPS, B, nch), MD_THREADS, 0, st, src, (const float*)ps, pq, hw, Cc);
+        CAR_LAUNCH(midas_gn_finish_kernel, (B * MD_GROUPS + 255) / 256, 256, 0, st, (const float*)ps, (const float*)pq, stt, B, hw, Cc, nch);
+        return CAR_OK;
+    };
+    // GN(src) (+ resid, normalised by rn when rn.stats) (ReLU) (max-pool) -> S3 frame in S, fp32 carrier when given
+    auto gn_apply = [&](const float* src, const MdNorm& N, const float* resid, GnAffine rn, float* carrier, int hh, int ww, int Cc, GnApply a) -> int {
+        CAR_LAUNCH(midas_gn_apply_kernel, gsz((long long)B * a.Hp * a.Wp * Cc), 256, 0, st, src, GnAffine{stats, N.w, N.b}, resid, rn, carrier, S, B, hh,
+                   ww, Cc, a);
+        return CAR_OK;
+    };
+    const GnAffine none{nullptr, nullptr, nullptr};
+
+    // ---- stem: conv 7x7/2 (SAME: 2 before, 3 after) -> GN + ReLU -> max-pool 3x3/2 (SAME: 0 before, 1 after) -> S3 rows
+    CAR_LAUNCH(midas_stem_split3_kernel, gsz((long long)Bz * (H + 5) * (W + 5) * 8), 256, 0, st, x, S, B, H, W);
+    CAR_TRY(la_conv(st, S, B, H + 5, W + 5, m->stem.k / 49 * 3, m->stem.w3, m->zero, 64, 7, 7, 2, H / 2, W / 2, T0, H / 2, W / 2));
+    CAR_TRY(gn_stats(T0, H / 2, W / 2, 64, stats));
+    int hh = H / 4, ww = W / 4;
+    CAR_TRY(gn_apply(T0, m->stem_n, nullptr, none, nullptr, H / 2, W / 2, 64, GnApply{0, 0, hh, ww, 1, 1}));
+    // ---- stages: bottlenecks conv1 1x1 -> GN+ReLU -> conv2 3x3 (stride) -> GN+ReLU -> conv3 1x1 -> GN -> + shortcut -> ReLU.  S holds
+    // the S3 rows of the block input; xin its fp32 carrier (the identity shortcut); the first block's shortcut is conv 1x1 (stride) + GN.
+    float* xin = nullptr;
+    int bi = 0;
+    for (int s = 0; s < 3; ++s) {
+        for (int b = 0; b < MD_DEPTH[s]; ++b, ++bi) {
+            const MdBlock& k = m->blk[bi];
+            const int ho = hh / k.stride, wo = ww / k.stride, Min = B * hh * ww, Mo = B * ho * wo;
+            GnAffine rn = none;
+            if (b == 0) {
+                if (k.stride == 1) CAR_TRY(dpt_gemm(st, k.dn, S, Min, Td, k.out));
+                else CAR_TRY(la_conv(st, S, B, hh, ww, 3 * k.cin, k.dn.w3, m->zero, k.out, 1, 1, 2, ho, wo, Td, ho, wo));
+                CAR_TRY(gn_stats(Td, ho, wo, k.out, rstats));
+                rn = GnAffine{rstats, k.dnn.w, k.dnn.b};
+            }
+            CAR_TRY(dpt_gemm(st, k.c1, S, Min, T0, k.mid));
+            CAR_TRY(gn_stats(T0, hh, ww, k.mid, stats));
+            if (k.stride == 1) {
+                CAR_TRY(gn_apply(T0, k.n1, nullptr, none, nullptr, hh, ww, k.mid, GnApply{0, 0, dpt_fh(hh), dpt_fw(ww), 1, 0}));
+                CAR_TRY(dpt_conv3(st, k.c2, S, B, hh, ww, T1));
+            } else {                                    // SAME for 3x3/2 on an even map: no padding before, one after
+                CAR_TRY(gn_apply(T0, k.n1, nullptr, none, nullptr, hh, ww, k.mid, GnApply{0, 0, hh + 1, ww + 1, 1, 0}));
+                CAR_TRY(la_conv(st, S, B, hh + 1, ww + 1, 3 * k.mid, k.c2.w3, m->zero, k.mid, 3, 3, 2, ho, wo, T1, ho, wo));
+            }
+            CAR_TRY(gn_stats(T1, ho, wo, k.mid, stats));
+            CAR_TRY(gn_apply(T1, k.n2, nullptr, none, nullptr, ho, wo, k.mid, GnApply{0, 0, ho, wo, 1, 0}));
+            CAR_TRY(dpt_gemm(st, k.c3, S, Mo, T2, k.out));
+            CAR_TRY(gn_stats(T2, ho, wo, k.out, stats));
+            float* xo = xin == Xa ? Xb : Xa;
+            CAR_TRY(gn_apply(T2, k.n3, b == 0 ? Td : xin, rn, xo, ho, wo, k.out, GnApply{0, 0, ho, wo, 1, 0}));
+            xin = xo; hh = ho; ww = wo;
+        }
+        if (s < 2) {                                    // stage outputs 0 and 1 are features 1 and 2: scratch.layer{1,2}_rn
+            CAR_TRY(dpt_img(st, xin, nullptr, nullptr, S, dpt_frame(B, hh, ww, MD_OUT[s])));
+            CAR_TRY(dpt_conv3(st, m->rn[s], S, B, hh, ww, fe[s]));
+            CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)B * hh * ww * MD_OUT[s]), 256, 0, st, (const float*)xin, S, (long long)B * hh * ww,
+                       MD_OUT[s], 0);
+        }
+    }
+    // ---- ViT-B/16: tokens = 1x1 projection of the stage-2 map, [CLS], position embeddings resized 24 x 24 -> h x w; blocks 8 and 11
+    // write their outputs into K[]
+    CAR_TRY(dpt_gemm(st, m->patch, S, Mp, T0, C));
+    CAR_LAUNCH(dpt_assemble_kernel, gsz((long long)M * C), 256, 0, st, (const float*)T0, (const float*)m->cls, (const float*)m->pos, X, B, h, w, MD_GRID, C);
+    float* xv = X;
+    for (int l = 0; l < 12; ++l) {
+        float* dst = l == 8 ? K[0] : l == 11 ? K[1] : X;
+        CAR_TRY(dpt_layer(st, m->L[l], xv, dst, B, T, C, MD_HEADS, MD_MLP, 1e-6f, S, T0, X1));
+        xv = dst;
+    }
+    // ---- reassemble 3 and 4: readout projection + GELU, 1x1 convolution, (3x3/2 convolution); then scratch.layer{3,4}_rn
+    for (int i = 0; i < 2; ++i) {
+        CAR_LAUNCH(dpt_readout_split_kernel, gsz((long long)Mp * 2 * C), 256, 0, st, (const float*)K[i], S, B, P, C);
+        CAR_TRY(dpt_gemm(st, m->readout[i], S, Mp, T0, C));
+        CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)Mp * C), 256, 0, st, (const float*)T0, S, (long long)Mp, C, 1);
+        CAR_TRY(dpt_gemm(st, m->proj[i], S, Mp, T1, C));                            // [B][h][w][C]
+        if (i == 0) {
+            CAR_TRY(dpt_img(st, T1, nullptr, nullptr, S, dpt_frame(B, h, w, C)));
+        } else {
+            CAR_TRY(dpt_img(st, T1, nullptr, nullptr, S, DptImg{B, h, w, C, h + 2, w + 2, 1, 1, 0, 0, 0}));
+            CAR_TRY(la_conv(st, S, B, h + 2, w + 2, 3 * C, m->resize4.w3, m->resize4.b, C, 3, 3, 2, sh[3], sw[3], T0, sh[3], sw[3]));
+            CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, dpt_frame(B, sh[3], sw[3], C)));
+        }
+        CAR_TRY(dpt_conv3(st, m->rn[2 + i], S, B, sh[2 + i], sw[2 + i], fe[2 + i]));
+    }
+    // ---- fusion (refinenet4 .. 1) and head (output_conv)
+    return dpt_decode(st, m->dec, fe, sh, sw, B, H, W, F, T0, T1, T2, S, depth);
 }

@@ -54,27 +54,27 @@ __global__ void dpt_patchify_kernel(const float* __restrict__ x, bf16* __restric
     }
 }
 
-// X [B][1 + h^2][C]: row 0 = cls + pos[0], row 1 + p = patch[b, p] + bilinear(pos grid g x g -> h x h, align_corners=False)[p]
+// X [B][1 + h w][C]: row 0 = cls + pos[0], row 1 + p = patch[b, p] + bilinear(pos grid g x g -> h x w, align_corners=False)[p]
 __global__ void dpt_assemble_kernel(const float* __restrict__ patch, const float* __restrict__ cls, const float* __restrict__ pos, float* __restrict__ X,
-                                    int B, int h, int g, int C) {
-    const int T = 1 + h * h;
+                                    int B, int h, int w, int g, int C) {
+    const int T = 1 + h * w;
     const long long total = (long long)B * T * C;
-    const float scale = (float)g / (float)h;
+    const float scale_y = (float)g / (float)h, scale_x = (float)g / (float)w;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int c = (int)(i % C);
         const long long r = i / C;
         const int t = (int)(r % T), b = (int)(r / T);
         if (t == 0) { X[i] = cls[c] + pos[c]; continue; }
-        const int p = t - 1, oy = p / h, ox = p - oy * h;
+        const int p = t - 1, oy = p / w, ox = p - oy * w;
         // torch upsample_bilinear2d, align_corners=False: src = max(scale * (dst + 0.5) - 0.5, 0)
-        const float sy = fmaxf(scale * (oy + 0.5f) - 0.5f, 0.f), sx = fmaxf(scale * (ox + 0.5f) - 0.5f, 0.f);
+        const float sy = fmaxf(scale_y * (oy + 0.5f) - 0.5f, 0.f), sx = fmaxf(scale_x * (ox + 0.5f) - 0.5f, 0.f);
         const int y0 = (int)sy, x0 = (int)sx, y1 = y0 + (y0 < g - 1), x1 = x0 + (x0 < g - 1);
         const float ly = sy - y0, lx = sx - x0;
         const float* P = pos + C + c;
         const float v00 = P[(size_t)(y0 * g + x0) * C], v01 = P[(size_t)(y0 * g + x1) * C];
         const float v10 = P[(size_t)(y1 * g + x0) * C], v11 = P[(size_t)(y1 * g + x1) * C];
         const float pe = (1.f - ly) * ((1.f - lx) * v00 + lx * v01) + ly * ((1.f - lx) * v10 + lx * v11);
-        X[i] = patch[((size_t)b * h * h + p) * C + c] + pe;
+        X[i] = patch[((size_t)b * h * w + p) * C + c] + pe;
     }
 }
 

@@ -316,6 +316,18 @@ int car_dpt_create(const CarDptDesc* desc, const void* const* tensors, int32_t n
 int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, int32_t H, int32_t W, float* depth, void* stream);
 int car_dpt_destroy(CarDpt* m);
 
+/* MiDaS DPT-Hybrid depth detector (reference condition/midas: DPTDepthModel, backbone vitb_rn50_384, features 256, readout
+ * "project", non_negative): a weight-standardised GroupNorm ResNet-50 trunk (stages 3, 4, 9, TF "SAME" padding) whose stage-2 map
+ * is the token grid of a ViT-B/16, then the DPT neck, fusion and head.  fp32 in the reference => fp32-grade here.  The network is
+ * fixed, so there is no descriptor.  car_midas_create: 368 fp32 device tensors in the state-dict order of
+ * controlar_b200.condition.midas.DPTDepthModel (the ViT's final norm and classifier included and unused) — copied / packed, the
+ * convolution weights standardised once (fp64 statistics).
+ * car_midas_forward: x fp32 NCHW [B][3][H][W], H % 32 == 0, W % 32 == 0, H, W >= 64 -> depth fp32 [B][H][W].  No host sync. */
+typedef struct CarMidas CarMidas;
+int car_midas_create(const void* const* tensors, int32_t n_tensors, void* stream, CarMidas** out);
+int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t H, int32_t W, float* depth, void* stream);
+int car_midas_destroy(CarMidas* m);
+
 /* Fused multi-tensor AdamW step (row f1: autoregressive/train/train_c2i.py:28-50 builds torch.optim.AdamW(fused=True)).
  * tensors_dev: device array of { float* param; const float* grad; float* exp_avg; float* exp_avg_sq; int64 numel; float weight_decay;
  * int32 pad } (48 bytes each); chunks_dev: device array of int32 pairs { tensor index, chunk index } — chunk = 65536 elements;
