@@ -60,7 +60,7 @@ PROTOTYPES = {
     "car_prefill": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int32, C.c_void_p]),
     "car_decode_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_sample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(CarSampling), C.c_int32, C.c_int32,
-                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "car_generate": (C.c_int, [C.c_void_p, C.POINTER(CarSampling), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "car_generate_forced": (C.c_int, [C.c_void_p, C.POINTER(CarSampling), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),

@@ -22,12 +22,15 @@ from ... import engine as _engine
 def top_k_top_p_filtering(logits, top_k: int = 0, top_p: float = 1.0, filter_value: float = -float("Inf"),
                           min_tokens_to_keep: int = 1):
     """Filters [B, V] logits IN PLACE and returns them, like the reference (generate.py:17-56: `logits[indices_to_remove] =
-    filter_value; return logits`); the kept set comes from the fused sampler kernel (the probabilities it returns)."""
+    filter_value; return logits`); the kept set comes from the fused sampler kernel.  It is the kernel's kept mask, not
+    `probs > 0`: a kept token far below the row maximum has a probability that underflows to 0 and still keeps its logit."""
     if min_tokens_to_keep != 1:
         raise NotImplementedError("min_tokens_to_keep != 1 is never used by ControlAR")
+    if top_k <= 0 and top_p >= 1.0:
+        return logits
     sp = _engine.make_sampling(temperature=1.0, top_k=top_k, top_p=top_p, sample_logits=False, cfg_scale=1.0)
-    _, probs = _engine.sample(logits, sp, return_probs=True)
-    logits.masked_fill_(~(probs > 0), filter_value)
+    _, kept = _engine.sample(logits, sp, return_kept=True)
+    logits.masked_fill_(~kept, filter_value)
     return logits
 
 

@@ -722,12 +722,12 @@ static int launch_sampler(const SampleArgs& a, cudaStream_t st) {
 }
 
 extern "C" int car_sample(const float* logits, int32_t b_eff, int32_t V, const CarSampling* sp, int32_t cfg_on, int32_t step,
-                          const float* noise, int32_t* idx_out, float* probs_out, void* stream) {
+                          const float* noise, int32_t* idx_out, float* probs_out, uint8_t* kept_out, void* stream) {
     if (!logits || !sp || !idx_out) CAR_FAIL(CAR_ERR_ARG, "null argument");
     SampleArgs a;
     CAR_TRY(fill_sample_args(a, sp, b_eff, V));
     a.logits = logits; a.cfg_on = cfg_on; a.cfg_interval = -1; a.step = step; a.noise = noise;
-    a.idx_out = idx_out; a.tokens_ld = 0; a.probs_out = probs_out;
+    a.idx_out = idx_out; a.tokens_ld = 0; a.probs_out = probs_out; a.kept_out = kept_out;
     return launch_sampler(a, (cudaStream_t)stream);
 }
 

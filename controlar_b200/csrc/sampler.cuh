@@ -13,8 +13,9 @@
 
 constexpr int SMP_THREADS = 1024;
 
-__device__ __forceinline__ uint32_t float_order_key(float f) {   // larger float -> larger key
-    const uint32_t u = __float_as_uint(f);
+__device__ __forceinline__ uint32_t float_order_key(float f) {   // larger float -> larger key; -0.0 and +0.0 share one key
+    uint32_t u = __float_as_uint(f);                               // (-0 == +0 in the reference's comparisons: a top-k threshold
+    u = u == 0x80000000u ? 0u : u;                                 //  of +0 keeps every -0 entry)
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
@@ -56,6 +57,7 @@ struct SampleArgs {
     int* idx_out;           // [B] (or tokens_out + step when tokens_ld > 0)
     int tokens_ld;
     float* probs_out;       // [B, V] or null
+    unsigned char* kept_out; // [B, V] or null: 1 where the token survives top-k and top-p (also when its probability underflows to 0)
     // fused next-step embedding (decode loop only; null => skip)
     void* h_out; const void* tok_emb; const void* ctrl0; int d; int n_img; int T; float cs; int dtype;
     int* tok_buf;           // [b_eff] int32 tokens consumed by teacher-free decode
@@ -372,11 +374,18 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
         m2 = smp_block_sum64<THREADS>(m2, red_q);
         sum = (float)m2 * (1.0f / SMP_FIX);                // soft-max over the surviving logits only
     }
-    if (a.probs_out) {
-        float* po = a.probs_out + (size_t)b * V;
-        for (int i4 = tid; i4 < V4; i4 += THREADS) reinterpret_cast<float4*>(po)[i4] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (a.probs_out || a.kept_out) {
+        float* po = a.probs_out ? a.probs_out + (size_t)b * V : nullptr;
+        unsigned char* ko = a.kept_out ? a.kept_out + (size_t)b * V : nullptr;
+        for (int i4 = tid; i4 < V4; i4 += THREADS) {
+            if (po) reinterpret_cast<float4*>(po)[i4] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (ko) reinterpret_cast<uchar4*>(ko)[i4] = make_uchar4(0, 0, 0, 0);
+        }
         __syncthreads();
-        for_kept([&](int i, float z) { const float e = expf(z - mx); if (float_order_key(e / sum_pre) >= p_key) po[i] = e / sum; });
+        for_kept([&](int i, float z) {
+            const float e = expf(z - mx);
+            if (float_order_key(e / sum_pre) >= p_key) { if (po) po[i] = e / sum; if (ko) ko[i] = 1; }
+        });
     }
     SMP_STAMP(3);
     // ---- draw: arg-max of p (greedy) or of p / q (exponential race); lowest index wins ties

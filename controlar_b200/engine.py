@@ -5,6 +5,7 @@ PyTorch is plumbing here (device memory, streams); all arithmetic happens in lib
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import List, Optional
 
 import torch
@@ -411,26 +412,36 @@ class ARStateHandle(_lib.NativeHandle):
 
 def make_sampling(temperature=1.0, top_k=0, top_p=1.0, sample_logits=True, cfg_scale=1.0, cfg_interval=-1,
                   seed=0) -> CarSampling:
+    # generate.py:121 turns CFG off at decode step i when `cfg_interval > -1 and i > cfg_interval`, and the sample scripts parse
+    # --cfg-interval as a float.  For cfg_interval > -1, int(floor(cfg_interval)) gives the same decisions on integer steps, except
+    # in (-1, 0), where the reference turns CFG off from decode step 0 and no integer can say so.
+    if -1 < cfg_interval < 0:
+        raise ValueError(f"cfg_interval={cfg_interval}: values in (-1, 0) are not supported (CFG off from the first decode "
+                         "step cannot be expressed); use -1 to keep CFG on, or an integer >= 0")
+    cfg_interval = math.floor(cfg_interval) if cfg_interval > -1 else -1
     return CarSampling(temperature=float(temperature), top_k=int(top_k or 0), top_p=float(top_p),
                        sample_logits=1 if sample_logits else 0, cfg_scale=float(cfg_scale),
                        cfg_interval=int(cfg_interval), seed=int(seed) & 0xFFFFFFFFFFFFFFFF)
 
 
 def sample(logits: torch.Tensor, sp: CarSampling, cfg_on: bool = True, step: int = 0,
-           noise: Optional[torch.Tensor] = None, return_probs: bool = False):
-    """generate.sample() + CFG combine on [b_eff, V] fp32 logits (car_sample)."""
+           noise: Optional[torch.Tensor] = None, return_probs: bool = False, return_kept: bool = False):
+    """generate.sample() + CFG combine on [b_eff, V] fp32 logits (car_sample).  Returns idx, then probs [B, V] if return_probs,
+    then the kept set (bool [B, V]: survives top-k and top-p, also where its probability underflows to 0) if return_kept."""
     lib = _lib.lib()
     logits = logits.to(torch.float32).contiguous()
     b_eff, V = logits.shape
     B = b_eff // 2 if sp.cfg_scale > 1.0 else b_eff
     idx = torch.empty((B,), dtype=torch.int32, device=logits.device)
     probs = torch.empty((B, V), dtype=torch.float32, device=logits.device) if return_probs else None
+    kept = torch.empty((B, V), dtype=torch.uint8, device=logits.device) if return_kept else None
     if noise is not None:
         noise = noise.to(torch.float32).contiguous()
     with torch.cuda.device(logits.device):
         check(lib.car_sample(_ptr(logits), b_eff, V, C.byref(sp), 1 if cfg_on else 0, int(step), _ptr(noise), _ptr(idx),
-                             _ptr(probs), cur_stream()), "car_sample")
-    return (idx, probs) if return_probs else idx
+                             _ptr(probs), _ptr(kept), cur_stream()), "car_sample")
+    out = (idx,) + ((probs,) if return_probs else ()) + ((kept.bool(),) if return_kept else ())
+    return out if len(out) > 1 else idx
 
 
 def op_linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, act: int = 0) -> torch.Tensor:

@@ -124,10 +124,11 @@ int car_prefill(CarState* s, const void* cond, const void* condition, float cont
 int car_decode_step(CarState* s, const int32_t* tok, int32_t pos, float* logits_out, void* stream);
 
 /* ---- sampling: generate.sample() + CFG combine (generate.py:59-74,89-90,103-107) on fp32 logits
- * [b_eff, V] -> idx int32 [B] (B = b_eff/2 when cfg_scale > 1).  probs_out (fp32 [B, V]) and noise
+ * [b_eff, V] -> idx int32 [B] (B = b_eff/2 when cfg_scale > 1).  probs_out (fp32 [B, V]), kept_out (uint8 [B, V]:
+ * 1 where the token survives top-k and top-p, also when its probability underflows to 0) and noise
  * (fp32 [B, V] Exp(1) draws; NULL = in-kernel Philox) are optional.  step is the Philox sub-stream index. */
 int car_sample(const float* logits, int32_t b_eff, int32_t V, const CarSampling* sp, int32_t cfg_on, int32_t step,
-               const float* noise, int32_t* idx_out, float* probs_out, void* stream);
+               const float* noise, int32_t* idx_out, float* probs_out, uint8_t* kept_out, void* stream);
 
 /* ---- device-side generation loop: generate()'s prefill-sample + decode_n_tokens (generate.py:113-131,
  * 195-204).  Must follow car_prefill(...) on the same state.  Runs n_tokens sampling steps (the first one on

@@ -154,6 +154,36 @@ def sampler_case():
     print("sampler ok", flush=True)
 
 
+def sampler_edges_case():
+    """The reference's sample() / top_k_top_p_filtering() on the seeded row catalogue of oracle/sampler_oracle.py (random, bf16 and
+    CFG-combined bf16 rows, a far outlier, all-equal rows, -inf rows, a 3000-way tie across the top-k rank, +-0 ties, the
+    divide/reciprocal pair, V in {4, 12, 1000, 4100}) at temperatures 1, 0.5 and 2 (z / T == z * (1 / T) exactly there).
+    Stored per row set and configuration: the kept mask (bit-packed), the probabilities at oracle.sampler_oracle.probe_cols and
+    the greedy index.  The kept mask is read with a finite filter value so that kept -inf entries stay distinguishable."""
+    import numpy as np
+    import autoregressive.models.generate as G
+    from oracle.sampler_oracle import fixture_rows, fixture_configs, resolve_k, probe_cols
+    SENT = -3.0e38
+    res = {"torch_version": np.array(str(torch.__version__))}
+    cfgs = fixture_configs()
+    for name, rows in fixture_rows().items():
+        R, V = rows.shape
+        cols = torch.stack([probe_cols(rows[r]) for r in range(R)])
+        kept, probs, idx = [], [], []
+        for (T, k, p) in cfgs:
+            kk = resolve_k(k, V)
+            filt = G.top_k_top_p_filtering(rows.clone() / T, top_k=kk, top_p=p, filter_value=SENT)
+            kept.append(np.packbits((filt != SENT).numpy(), axis=-1))
+            i, pr = G.sample(rows.clone()[:, None, :], temperature=T, top_k=kk, top_p=p, sample_logits=False)
+            probs.append(torch.gather(pr, 1, cols).numpy())
+            idx.append(i[:, 0].numpy())
+        res[f"{name}_kept"] = np.stack(kept)
+        res[f"{name}_probs"] = np.stack(probs).astype(np.float32)
+        res[f"{name}_idx"] = np.stack(idx).astype(np.int64)
+    np.savez_compressed(os.path.join(OUT, "sampler_edges.npz"), **res)
+    print("sampler_edges ok", len(cfgs), "configurations", flush=True)
+
+
 def vq_case():
     from tokenizer.tokenizer_image.vq_model import VQ_models
     vq = VQ_models["VQ-16"](codebook_size=16384, codebook_embed_dim=8)
@@ -688,6 +718,7 @@ CASES = {
                                                   B=2, H=128, W=128, cfg_scale=4.0, cs=0.6, dtype=torch.bfloat16,
                                                   sampled=False, save_all_logits=False, force_math=False),
     "sampler": sampler_case,
+    "sampler_edges": sampler_edges_case,
     "vq16": vq_case,
     "dinov2": dino_case,
     "vit": vit_case,
