@@ -6,7 +6,7 @@ import ctypes as C
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("CAR_LIB") or os.path.join(HERE, "lib", "libcontrolar_b200.so")   # CAR_LIB: dev A/B runs of another build
+LIB_PATH = os.path.join(HERE, "lib", "libcontrolar_b200.so")
 
 CAR_BF16, CAR_F32 = 0, 1
 
@@ -113,8 +113,6 @@ def lib():
                 "(controlar_b200 has no CPU / eager-PyTorch fallback)")
         l = C.CDLL(LIB_PATH)
         for name, (res, args) in PROTOTYPES.items():
-            if os.environ.get("CAR_LIB") and not hasattr(l, name):
-                continue                                  # an older dev build may lack the newest entry points
             fn = getattr(l, name)
             fn.restype = res
             fn.argtypes = args

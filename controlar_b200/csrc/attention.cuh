@@ -35,7 +35,7 @@ template <typename T>
 __global__ void __launch_bounds__(AD_THREADS, 6)
 attn_decode_kernel(const T* __restrict__ q, const T* __restrict__ kc, const T* __restrict__ vc,
                    const int* __restrict__ emb_mask, int mask_ld, const int* __restrict__ pos_ptr, int H, int S,
-                   int Tpre, int nsplit, int flags, float* __restrict__ part, int* __restrict__ tickets, T* __restrict__ out) {
+                   int Tpre, int nsplit, float* __restrict__ part, int* __restrict__ tickets, T* __restrict__ out) {
     constexpr int LPR = RowLanes<T>::LPR, EPL = RowLanes<T>::EPL, RPW = 32 / LPR;
     constexpr int UNR = 4;
     __shared__ float sm_m[AD_WARPS * RPW], sm_l[AD_WARPS * RPW];
@@ -54,7 +54,7 @@ attn_decode_kernel(const T* __restrict__ q, const T* __restrict__ kc, const T* _
     chunk = (chunk + 7) & ~7;
     const int k0 = split * chunk, k1 = min(n, k0 + chunk);
     // pull this CTA's slice of the cache towards L2 while the QKV GEMM is still running (rows < pos are final)
-    if (flags & 1) {
+    {
         const char* kb = reinterpret_cast<const char*>(kc + ((size_t)bh * S + k0) * 64);
         const char* vb = reinterpret_cast<const char*>(vc + ((size_t)bh * S + k0) * 64);
         const int lines = max(0, min(k1, pos) - k0) * 64 * (int)sizeof(T) / 128;

@@ -21,25 +21,6 @@
 thread_local std::string g_car_err;
 std::atomic<long long> g_car_launches{0};
 
-// development knobs (environment, read once): CAR_MEGA (0 = per-kernel graph chain instead of the persistent decode kernel),
-// CAR_DBG (trace step; needs a -DPK_TRACE build), CAR_EXP (experiment bits of decode_persistent.cuh), CAR_TC5 (0 = mma.sync dense
-// GEMM in the prefill), CAR_PDL, CAR_L2PF, CAR_NSPLIT, CAR_NB_QKV/WO/W13/W2/HEAD (per-kernel chain)
-struct Tune { int pdl, l2pf, nsplit, nb[5], skip, empty, dbg, mega, mega_pf; };
-static long long* g_dbg = nullptr;   // [5 kernels][8] clock stamps (CAR_DBG=1)
-__global__ void empty_kernel(int) {}
-static const Tune& tune() {
-    static Tune t = [] {
-        Tune x;
-        auto gi = [](const char* n, int d) { const char* v = getenv(n); return v ? atoi(v) : d; };
-        x.mega = gi("CAR_MEGA", 1); x.mega_pf = gi("CAR_MEGA_PF", 1); x.dbg = gi("CAR_DBG", 0); x.skip = gi("CAR_SKIP", 0); x.empty = gi("CAR_EMPTY", 0);
-        x.pdl = gi("CAR_PDL", 1); x.l2pf = gi("CAR_L2PF", 1); x.nsplit = gi("CAR_NSPLIT", 0);
-        x.nb[EPI_STORE] = 0; x.nb[EPI_QKV] = gi("CAR_NB_QKV", 0); x.nb[EPI_RESID] = gi("CAR_NB_RESID", 0);
-        x.nb[EPI_SWIGLU] = gi("CAR_NB_W13", 0); x.nb[EPI_LOGITS] = gi("CAR_NB_HEAD", 0);
-        return x;
-    }();
-    return t;
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // structures
 // ---------------------------------------------------------------------------------------------------------
@@ -166,10 +147,7 @@ static int launch_skinny_bf16_inst(cudaStream_t st, const bf16* A, int lda, cons
         const unsigned cap = (unsigned)sm_count() * (unsigned)std::max(1, std::min(occ, 2));
         if (grid.x > cap) grid.x = cap;
     }
-    const int flags = tune().l2pf ? 1 : 0;
-    if (tune().empty) { CAR_LAUNCH(empty_kernel, grid, SK_THREADS, smem, st, 0); return CAR_OK; }
-    if (tune().pdl) CAR_LAUNCH_PDL((skinny_gemm_bf16<NB, U, NORM>), grid, dim3(SK_THREADS), smem, st, A, lda, (const uint4*)Wp, nw, eps, K, nblk, flags, ep);
-    else CAR_LAUNCH((skinny_gemm_bf16<NB, U, NORM>), grid, SK_THREADS, smem, st, A, lda, (const uint4*)Wp, nw, eps, K, nblk, flags, ep);
+    CAR_LAUNCH_PDL((skinny_gemm_bf16<NB, U, NORM>), grid, dim3(SK_THREADS), smem, st, A, lda, (const uint4*)Wp, nw, eps, K, nblk, ep);
     return CAR_OK;
 }
 
@@ -208,7 +186,6 @@ static int launch_skinny(cudaStream_t st, int dtype, const void* A, int lda, con
         const int want = (nblk + sm_count() - 1) / sm_count();
         NB = want > 4 ? 8 : (want > 2 ? 4 : (want > 1 ? 2 : 1));
     }
-    if (mtiles == 1 && tune().nb[ep.kind] > 0) NB = tune().nb[ep.kind];
     if (ep.kind == EPI_SWIGLU && NB == 1) NB = 2;
     if (NB == 8) U = 2; else if (NB * U > 16) U = 4;   // register budget
     const bf16* Ab = (const bf16*)A; const bf16* nwb = (const bf16*)nw;
@@ -402,7 +379,6 @@ extern "C" int car_state_create(CarModel* m, int32_t b_eff, int32_t S, int32_t N
     const size_t dd = d.dim, F = d.ffn_dim, V = d.vocab_size;
     const size_t MP = (size_t)b_eff * T, MC = (size_t)b_eff * N;
     s->nsplit = std::max(1, std::min(16, (4 * sm_count() + b_eff * d.n_head - 1) / (b_eff * d.n_head)));
-    if (tune().nsplit > 0) s->nsplit = std::min(32, tune().nsplit);
     int r = CAR_OK;
     auto A = [&](void** p, size_t bytes) { if (r == CAR_OK) r = alloc_dev(s->owned, p, bytes); };
     A(&s->h, b_eff * dd * es); A(&s->q, b_eff * dd * es); A(&s->attn, b_eff * dd * es); A(&s->act, b_eff * F * es);
@@ -466,14 +442,8 @@ template <typename T>
 static int launch_attn_decode(CarState* s, int l, cudaStream_t st) {
     const CarModelDesc& d = s->m->d;
     dim3 grid(s->b_eff * d.n_head, s->nsplit);
-    const int flags = tune().l2pf ? 1 : 0;
-    if (tune().pdl)
-        CAR_LAUNCH_PDL((attn_decode_kernel<T>), grid, dim3(AD_THREADS), 0, st, (const T*)s->q, (const T*)s->kc[l], (const T*)s->vc[l],
-                       (const int*)s->emb_mask, s->T, (const int*)s->pos, d.n_head, s->S, s->T, s->nsplit, flags, s->attn_part,
-                       s->tickets, (T*)s->attn);
-    else
-        CAR_LAUNCH((attn_decode_kernel<T>), grid, AD_THREADS, 0, st, (const T*)s->q, (const T*)s->kc[l], (const T*)s->vc[l],
-                   (const int*)s->emb_mask, s->T, (const int*)s->pos, d.n_head, s->S, s->T, s->nsplit, flags, s->attn_part,
+    CAR_LAUNCH_PDL((attn_decode_kernel<T>), grid, dim3(AD_THREADS), 0, st, (const T*)s->q, (const T*)s->kc[l], (const T*)s->vc[l],
+                   (const int*)s->emb_mask, s->T, (const int*)s->pos, d.n_head, s->S, s->T, s->nsplit, s->attn_part,
                    s->tickets, (T*)s->attn);
     return CAR_OK;
 }
@@ -505,8 +475,7 @@ static int dense_linear(cudaStream_t st, const void* A, int lda, const void* W, 
         CAR_CUDA(cudaFuncSetAttribute(dense_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM));
     }
     if (M <= 0 || N <= 0) return CAR_OK;
-    static const bool use_tc5 = [] { const char* e = getenv("CAR_TC5"); return e ? atoi(e) != 0 : true; }();
-    if (use_tc5 && K % 8 == 0 && N % 8 == 0 && lda % 8 == 0 && ldo % 8 == 0 && (resid == nullptr || ldr % 8 == 0) &&
+    if (K % 8 == 0 && N % 8 == 0 && lda % 8 == 0 && ldo % 8 == 0 && (resid == nullptr || ldr % 8 == 0) &&
         ((uintptr_t)A % 16) == 0 && ((uintptr_t)W % 16) == 0 && wg_encoder() != nullptr) {
         // wgmma path (gemm_wgmma.cuh): TMA tensor-map loads, accumulators in registers, persistent warp-specialised CTAs
         static DevOnce once5;
@@ -540,13 +509,9 @@ static int enqueue_block_dense(CarState* s, int l, cudaStream_t st) {
     CAR_TRY(dense_linear(st, s->t1, dim, m->wqkv[l], rows, 3 * dim, dim, ACT_NONE, nullptr, 0, s->qkvP, 3 * dim));
     CAR_LAUNCH(rope_kv_write_kernel, sm_count() * 8, 256, 0, st, (const bf16*)s->qkvP, s->rope, (bf16*)s->qP, (bf16*)s->kc[l], (bf16*)s->vc[l], rows, s->T, dim,
                d.n_head, s->S);
-    static const bool fa = [] { const char* e = getenv("CAR_PREFILL_FA"); return e ? atoi(e) != 0 : true; }();
-    if (fa) {   // prefix attention on the tensor cores (attention.cuh): 64 query rows per CTA
-        CAR_LAUNCH(attn_prefill_mma_kernel, dim3((s->T + 63) / 64, d.n_head, s->b_eff), 128, 0, st, (const bf16*)s->qP, (const bf16*)s->kc[l],
-                   (const bf16*)s->vc[l], (const int*)s->emb_mask, s->T, d.n_head, s->S, s->T, s->T, (bf16*)s->attnP);
-    } else {
-        CAR_TRY(launch_attn_prefill<bf16>(s, l, st));
-    }
+    // prefix attention on the tensor cores (attention.cuh): 64 query rows per CTA
+    CAR_LAUNCH(attn_prefill_mma_kernel, dim3((s->T + 63) / 64, d.n_head, s->b_eff), 128, 0, st, (const bf16*)s->qP, (const bf16*)s->kc[l],
+               (const bf16*)s->vc[l], (const int*)s->emb_mask, s->T, d.n_head, s->S, s->T, s->T, (bf16*)s->attnP);
     CAR_TRY(dense_linear(st, s->attnP, dim, m->wo[l], rows, dim, dim, ACT_NONE, s->hP, dim, s->hP, dim));
     CAR_LAUNCH((rmsnorm_rows_kernel<bf16>), rows, 256, 0, st, (const bf16*)s->hP, (const bf16*)m->ffn_norm[l], (bf16*)s->t1, dim, d.norm_eps);
     CAR_TRY(dense_linear(st, s->t1, dim, m->w1[l], rows, F, dim, ACT_NONE, nullptr, 0, s->gP, F));
@@ -572,25 +537,18 @@ static int enqueue_block(CarState* s, int l, bool decode, cudaStream_t st) {
     EpiParams e1 = epi_base(EPI_QKV);
     e1.rpb = rpb; e1.pos_ptr = posp; e1.rope = s->rope; e1.kc = s->kc[l]; e1.vc = s->vc[l]; e1.q = q; e1.S = s->S;
     e1.H = d.n_head; e1.d = dim;
-    const int skip = decode ? tune().skip : 0;
-    if (tune().dbg && decode && l == 3) {
-        if (!g_dbg) { cudaMalloc(&g_dbg, 5 * 8 * 8); cudaMemset(g_dbg, 0, 5 * 8 * 8); }
-        e1.dbg = g_dbg;
-    }
-    if (!(skip & 1)) CAR_TRY(launch_skinny(st, dt, h, dim, m->g_wqkv[l], m->attention_norm[l], d.norm_eps, rows, 3 * dim, dim, e1, true));
+    CAR_TRY(launch_skinny(st, dt, h, dim, m->g_wqkv[l], m->attention_norm[l], d.norm_eps, rows, 3 * dim, dim, e1, true));
 
-    if (decode) { if (!(skip & 2)) { if (dt == CAR_BF16) CAR_TRY(launch_attn_decode<bf16>(s, l, st)); else CAR_TRY(launch_attn_decode<float>(s, l, st)); } }
+    if (decode) { if (dt == CAR_BF16) CAR_TRY(launch_attn_decode<bf16>(s, l, st)); else CAR_TRY(launch_attn_decode<float>(s, l, st)); }
     else { if (dt == CAR_BF16) CAR_TRY(launch_attn_prefill<bf16>(s, l, st)); else CAR_TRY(launch_attn_prefill<float>(s, l, st)); }
 
     EpiParams e2 = epi_base(EPI_RESID);
     e2.rpb = rpb; e2.pos_ptr = posp; e2.h = h; e2.ldh = dim;
-    if (tune().dbg && decode && l == 3) e2.dbg = g_dbg + 8;
-    if (!(skip & 4)) CAR_TRY(launch_skinny(st, dt, attn, dim, m->g_wo[l], nullptr, 0.f, rows, dim, dim, e2, false));
+    CAR_TRY(launch_skinny(st, dt, attn, dim, m->g_wo[l], nullptr, 0.f, rows, dim, dim, e2, false));
 
     EpiParams e3 = epi_base(EPI_SWIGLU);
     e3.rpb = rpb; e3.out = act; e3.ldo = F;
-    if (tune().dbg && decode && l == 3) e3.dbg = g_dbg + 16;
-    if (!(skip & 8)) CAR_TRY(launch_skinny(st, dt, h, dim, m->g_w13[l], m->ffn_norm[l], d.norm_eps, rows, 2 * F, dim, e3, true));
+    CAR_TRY(launch_skinny(st, dt, h, dim, m->g_w13[l], m->ffn_norm[l], d.norm_eps, rows, 2 * F, dim, e3, true));
 
     EpiParams e4 = epi_base(EPI_RESID);
     e4.rpb = rpb; e4.pos_ptr = posp; e4.h = h; e4.ldh = dim;
@@ -599,9 +557,7 @@ static int enqueue_block(CarState* s, int l, bool decode, cudaStream_t st) {
         // control add of the NEXT layer group fused here (gpt_t2i.py:466)
         e4.ctrl = s->ctrl[(l + 1) / step3]; e4.n_img = s->N; e4.T = s->T; e4.cs = s->cs;
     }
-    if (tune().dbg && decode && l == 3) e4.dbg = g_dbg + 24;
-    if (!(skip & 16)) CAR_TRY(launch_skinny(st, dt, act, F, m->g_w2[l], nullptr, 0.f, rows, dim, F, e4, false));
-    return CAR_OK;
+    return launch_skinny(st, dt, act, F, m->g_w2[l], nullptr, 0.f, rows, dim, F, e4, false);
 }
 
 static int enqueue_head(CarState* s, const void* hrows, int rows, float* logits, cudaStream_t st) {
@@ -782,7 +738,6 @@ static int launch_pk(CarState* s, const SampleArgs& a, int n_tokens, cudaStream_
     P.smp = a; P.n_steps = n_tokens;
     P.forced = forced; P.forced_ld = n_tokens; P.trace = trace; P.step_ts = s->pk_step_ts;
     if (trace) CAR_CUDA(cudaMemcpyAsync(trace, s->logits, (size_t)s->b_eff * d.vocab_size * 4, cudaMemcpyDeviceToDevice, st));
-    { const char* e = getenv("CAR_EXP"); P.exp_flags = e ? atoi(e) : 0; }
     static DevOnce once;
     if (once.first()) {
         CAR_CUDA(cudaFuncSetAttribute(pk_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PK_SMEM_TOTAL));
@@ -790,18 +745,23 @@ static int launch_pk(CarState* s, const SampleArgs& a, int n_tokens, cudaStream_
     int occ = 0;
     CAR_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pk_decode_kernel, PK_THREADS, PK_SMEM_TOTAL));
     if (occ < 1) CAR_FAIL(CAR_ERR_UNSUPPORTED, "persistent decode kernel does not fit on an SM");
+#ifdef PK_TRACE
+    // phase timings of one decode step (CAR_DBG=<step>), printed to stderr after the launch
+    static const int trace_step = [] { const char* e = getenv("CAR_DBG"); return e ? atoi(e) : 0; }();
     static long long* mdbg = nullptr;
     const size_t dbg_n = (size_t)s->pk_grid * 64 + 5 * 256;
-    if (tune().dbg) {
+    if (trace_step) {
         if (!mdbg) { cudaMalloc(&mdbg, dbg_n * 8); }
         cudaMemsetAsync(mdbg, 0, dbg_n * 8, st);
-        P.dbg = mdbg; P.dbg_step = std::max(0, std::min(n_tokens - 2, tune().dbg));
+        P.dbg = mdbg; P.dbg_step = std::max(0, std::min(n_tokens - 2, trace_step));
     }
+#endif
     void* args[] = {&P};
     CAR_CUDA(cudaLaunchCooperativeKernel((const void*)pk_decode_kernel, dim3(s->pk_grid), dim3(PK_THREADS), args, PK_SMEM_TOTAL, st));
     s->pk_bar_count += (unsigned int)(n_tokens - 1) * (unsigned int)s->pk_grid;        // one grid barrier per decoded token
     g_car_launches.fetch_add(1, std::memory_order_relaxed);
-    if (tune().dbg) {
+#ifdef PK_TRACE
+    if (trace_step) {
         cudaStreamSynchronize(st);
         std::vector<long long> t(dbg_n);
         cudaMemcpy(t.data(), mdbg, dbg_n * 8, cudaMemcpyDeviceToHost);
@@ -818,7 +778,6 @@ static int launch_pk(CarState* s, const SampleArgs& a, int n_tokens, cudaStream_
             fprintf(stderr, "[pk] %-22s n=%3zu  min %8.2f  med %8.2f  max %8.2f us (CTA %d)\n", name, v.size(), v.front() * 1e-3, v[v.size() / 2] * 1e-3,
                     v.back() * 1e-3, amax);
         };
-        if (!t[0] && !t[64]) fprintf(stderr, "[pk] no stamps: rebuild with CAR_PK_TRACE=1 (python -m controlar_b200.build --force)\n");
         fprintf(stderr, "[pk] step %d, times relative to the first CTA entering the sampler; layer 3 phases\n", P.dbg_step);
         stat(0, "step start"); stat(1, "sampler done");
         if (t[48]) fprintf(stderr, "[pk] sampler top-k of CTA 0: histogram built %.2f | boundary bin found %.2f | candidates gathered %.2f\n",
@@ -855,6 +814,7 @@ static int launch_pk(CarState* s, const SampleArgs& a, int n_tokens, cudaStream_
             }
         }
     }
+#endif
     return CAR_OK;
 }
 
@@ -866,7 +826,7 @@ extern "C" int car_generate(CarState* s, const CarSampling* sp, int32_t n_tokens
     cudaStream_t st = (cudaStream_t)stream;
     SampleArgs a;
     CAR_TRY(loop_sample_args(s, sp, noise, a));
-    if (s->m->d.dtype == CAR_BF16 && tune().mega && s->pk_ok) {
+    if (s->m->d.dtype == CAR_BF16 && s->pk_ok) {
         CAR_TRY(launch_pk(s, a, n_tokens, st));
         CAR_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)n_tokens * 4, s->tokens, (size_t)s->N * 4, (size_t)n_tokens * 4, a.B,
                                    cudaMemcpyDeviceToDevice, st));
@@ -901,17 +861,6 @@ extern "C" int car_generate(CarState* s, const CarSampling* sp, int32_t n_tokens
     CAR_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)n_tokens * 4, s->tokens, (size_t)s->N * 4, (size_t)n_tokens * 4, B,
                                cudaMemcpyDeviceToDevice, st));
     s->prefilled = false;
-    if (tune().dbg && g_dbg) {
-        cudaStreamSynchronize(st);
-        long long hbuf[40];
-        cudaMemcpy(hbuf, g_dbg, sizeof(hbuf), cudaMemcpyDeviceToHost);
-        const char* names[4] = {"qkv", "wo", "w13", "w2"};
-        for (int k = 0; k < 4; ++k) {
-            long long* t = hbuf + 8 * k;
-            fprintf(stderr, "[dbg] %-4s wait %6lld | stage %6lld | main %6lld | reduce %6lld | epi %6lld | total %6lld cycles\n", names[k],
-                    t[1] - t[0], t[2] - t[1], t[3] - t[2], t[4] - t[3], t[5] - t[4], t[5] - t[0]);
-        }
-    }
     return CAR_OK;
 }
 
@@ -967,7 +916,8 @@ extern "C" int car_op_linear(int32_t dtype, const void* x, const void* w, const 
 }
 
 // the dense (M >= 64 rows) tensor-core linear of the prefill / MLP path, exposed for unit tests and micro-benchmarks:
-// y[M,N] = act(x[M,K] · w[N,K]^T) (+ resid), bf16, fp32 accumulate (gemm_wgmma.cuh; CAR_TC5=0 selects the mma.sync kernel)
+// y[M,N] = act(x[M,K] · w[N,K]^T) (+ resid), bf16, fp32 accumulate (gemm_wgmma.cuh; the mma.sync kernel of gemm_dense.cuh when the
+// operands are not 16-byte aligned or the TMA tensor-map encoder is unavailable)
 extern "C" int car_op_dense_linear(const void* x, const void* w, const void* resid, void* y, int32_t M, int32_t N, int32_t K, int32_t act,
                                    void* stream) {
     if (!x || !w || !y) CAR_FAIL(CAR_ERR_ARG, "null argument");

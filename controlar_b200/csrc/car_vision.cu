@@ -19,11 +19,7 @@ static int vis_sm_count() {
     return n;
 }
 // wgmma path of the vision stages (gemm_wgmma.cuh): TMA tensor-map loads, accumulators in registers, persistent warp-specialised CTAs.
-// CAR_TC5=0 sends everything back to the mma.sync kernel (dev A/B).
-static bool wg_on() {
-    static const bool on = [] { const char* e = getenv("CAR_TC5"); return e ? atoi(e) != 0 : true; }();
-    return on && wg_encoder() != nullptr;
-}
+// Used only where the driver provides the TMA tensor-map encoder (wg_encoder() != nullptr).
 static int wg_launch(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, const WgP& q, int tiles_m) {
     static DevOnce once5;
     if (once5.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
@@ -38,7 +34,7 @@ static int dense(cudaStream_t st, DenseP p, int batch = 1) {
     if (p.M <= 0 || p.N <= 0) return CAR_OK;
     if (p.alpha == 0.f) p.alpha = 1.f;
     // plain bf16 -> bf16 GEMMs (DINOv2 linears, 1x1 convolutions) go to the wgmma kernel; same epilogue order as below
-    if (batch == 1 && p.amode == A_PLAIN && p.out_mode == 0 && !p.bias_along_m && p.alpha == 1.f && !p.bias_f && !p.resid_f && wg_on() &&
+    if (batch == 1 && p.amode == A_PLAIN && p.out_mode == 0 && !p.bias_along_m && p.alpha == 1.f && !p.bias_f && !p.resid_f && wg_encoder() != nullptr &&
         p.K % 8 == 0 && p.N % 8 == 0 && p.lda % 8 == 0 && p.ldb % 8 == 0 && p.ldc % 8 == 0 && (!p.resid || p.ldr % 8 == 0) &&
         ((uintptr_t)p.A % 16) == 0 && ((uintptr_t)p.B % 16) == 0 && ((uintptr_t)p.C % 16) == 0 && (!p.resid || ((uintptr_t)p.resid % 16) == 0)) {
         alignas(64) CUtensorMap mapA, mapB;
@@ -177,7 +173,7 @@ template <typename TI>
 static int dino_forward_t(CarDino* m, const TI* image, int B, int H, int W, void* out, int apply_mlp, cudaStream_t st) {
     const CarDinoDesc& d = m->d;
     const int C = d.hidden, h = H / 16, w = W / 16, hw = h * w, Tn = hw + 1, heads = d.heads;
-    const int Tp = (Tn + 31) & ~31;                      // key axis padded for the P·V GEMM
+    const int Tp = (Tn + 31) & ~31;                      // key axis of V^T, zero padded (vit_attention_kernel reads it in 8-key chunks)
     const long long rows = (long long)B * Tn;
     // workspace
     size_t need = 0;
@@ -185,7 +181,7 @@ static int dino_forward_t(CarDino* m, const TI* image, int B, int H, int W, void
     const int KP = m->kpad;
     sz((size_t)B * hw * KP * 2); sz((size_t)B * hw * C * 2); sz((size_t)hw * C * 2);
     sz(rows * C * 2); sz(rows * C * 2); sz(rows * 2 * C * 2); sz((size_t)B * C * Tp * 2);
-    sz((size_t)B * heads * Tn * Tp * 4); sz((size_t)B * heads * Tn * Tp * 2); sz(rows * C * 2); sz(rows * 4 * C * 2);
+    sz(rows * C * 2); sz(rows * 4 * C * 2);
     sz((size_t)B * hw * C * 2); sz((size_t)B * hw * std::max(m->ad_dim, 1) * 2);
     CAR_TRY(m->ws.reserve(need));
     m->ws.reset();
@@ -196,8 +192,6 @@ static int dino_forward_t(CarDino* m, const TI* image, int B, int H, int W, void
     bf16* xn = (bf16*)m->ws.take(rows * C * 2);
     bf16* qk = (bf16*)m->ws.take(rows * 2 * C * 2);
     bf16* vT = (bf16*)m->ws.take((size_t)B * C * Tp * 2);
-    float* S = (float*)m->ws.take((size_t)B * heads * Tn * Tp * 4);
-    bf16* P = (bf16*)m->ws.take((size_t)B * heads * Tn * Tp * 2);
     bf16* ctx = (bf16*)m->ws.take(rows * C * 2);
     bf16* hid = (bf16*)m->ws.take(rows * 4 * C * 2);
     bf16* feat = (bf16*)m->ws.take((size_t)B * hw * C * 2);
@@ -229,24 +223,9 @@ static int dino_forward_t(CarDino* m, const TI* image, int B, int H, int W, void
             p.sB = (long long)Tn * C; p.sC = (long long)C * Tp; p.bias = (const bf16*)Ly.b_v; p.bias_along_m = 1;
             CAR_TRY(dense(st, p, B));
         }
-        static const bool fused_attn = [] { const char* e = getenv("CAR_VIT_FA"); return e ? atoi(e) != 0 : true; }();
-        if (fused_attn && C % 64 == 0 && ((uintptr_t)qk % 16) == 0 && ((uintptr_t)vT % 16) == 0) {
-            // fused attention (vision.cuh): scores / probabilities never leave the SM
-            CAR_LAUNCH(vit_attention_kernel, dim3((Tn + 63) / 64, heads, B), 128, 0, st, (const bf16*)qk, (const bf16*)vT, ctx, Tn, Tp, C, scale);
-        } else {
-        // scores S[b,hd] = q k^T * 1/8  (fp32), soft-max -> P (bf16, zero padded), ctx = P V
-        for (int hd = 0; hd < heads; ++hd) {
-            DenseP p = dp_plain(qk + hd * 64, 2 * C, qk + C + hd * 64, 2 * C, Tn, Tn, 64, S + (size_t)hd * Tn * Tp, Tp);
-            p.sA = (long long)Tn * 2 * C; p.sB = (long long)Tn * 2 * C; p.sC = (long long)heads * Tn * Tp; p.alpha = scale; p.out_mode = 1;
-            CAR_TRY(dense(st, p, B));
-        }
-        CAR_LAUNCH(softmax_rows_kernel, (unsigned)((long long)B * heads * Tn), 128, 0, st, S, P, Tn, Tp, Tp);
-        for (int hd = 0; hd < heads; ++hd) {
-            DenseP p = dp_plain(P + (size_t)hd * Tn * Tp, Tp, vT + (size_t)hd * 64 * Tp, Tp, Tn, 64, Tp, ctx + hd * 64, C);
-            p.sA = (long long)heads * Tn * Tp; p.sB = (long long)C * Tp; p.sC = (long long)Tn * C;
-            CAR_TRY(dense(st, p, B));
-        }
-        }
+        // fused attention (vision.cuh): scores / probabilities never leave the SM.  hidden % 64 == 0 (car_dino_create) and the
+        // 256-byte aligned workspace give the kernel its 16-byte aligned rows.
+        CAR_LAUNCH(vit_attention_kernel, dim3((Tn + 63) / 64, heads, B), 128, 0, st, (const bf16*)qk, (const bf16*)vT, ctx, Tn, Tp, C, scale);
         {   // x = x + ls1 * (dense(ctx) + b)
             DenseP p = dp_plain(ctx, C, (const bf16*)Ly.w_o, C, (int)rows, C, C, x, C);
             p.bias = (const bf16*)Ly.b_o; p.scale = (const bf16*)Ly.ls1; p.resid = x; p.ldr = C;
@@ -436,7 +415,7 @@ struct Act { bf16* p; int B, H, W, C; long long n() const { return (long long)B 
 static int conv_fwd(cudaStream_t st, const ConvW& c, const Act& x, int ups, int stride2, bf16* out, const bf16* resid, int Ho, int Wo,
                     float* out_nchw_f32 = nullptr) {
     if (x.C != c.cin_pad && !(c.k == 1 && x.C == c.cin_pad)) CAR_FAIL(CAR_ERR_STATE, "conv input channel mismatch");
-    if (c.k == 3 && !stride2 && !ups && !out_nchw_f32 && c.cin_pad % WG_BK == 0 && c.cout % 8 == 0 && Ho == x.H && Wo == x.W && x.H >= WG_TH && x.W >= WG_TW && wg_on() &&
+    if (c.k == 3 && !stride2 && !ups && !out_nchw_f32 && c.cin_pad % WG_BK == 0 && c.cout % 8 == 0 && Ho == x.H && Wo == x.W && x.H >= WG_TH && x.W >= WG_TW && wg_encoder() != nullptr &&
         ((uintptr_t)x.p % 16) == 0 && ((uintptr_t)out % 16) == 0 && (!resid || ((uintptr_t)resid % 16) == 0)) {
         // 3x3 / pad 1 convolution on the wgmma kernel: one 4-D TMA box per (tap, 64-channel block), padding by TMA zero fill
         alignas(64) CUtensorMap mapA, mapB;
@@ -573,7 +552,7 @@ static int vq_decode_impl(CarVQ* m, const int32_t* codes, const float* quant, in
         }
         if (m->d_has_up[idx]) {   // Upsample (vq_model.py:368-379): nearest x2, then the 3x3 convolution
             bf16* o = flip(x.p);
-            if (wg_on() && x.C % WG_BK == 0) {   // materialise the up-sampled tensor (bandwidth-trivial) so the convolution is a plain TMA box walk
+            if (wg_encoder() != nullptr && x.C % WG_BK == 0) {   // materialise the up-sampled tensor (bandwidth-trivial) so the convolution is a plain TMA box walk
                 CAR_LAUNCH(upsample2x_nhwc_kernel, gsz((long long)B * x.H * 2 * x.W * 2 * (x.C / 8)), 256, 0, st, (const bf16*)x.p, s.t2, B, x.H, x.W, x.C);
                 Act u{s.t2, B, x.H * 2, x.W * 2, x.C};
                 CAR_TRY(conv_fwd(st, m->d_up[idx], u, 0, 0, o, nullptr, u.H, u.W));

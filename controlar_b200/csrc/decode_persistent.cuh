@@ -61,8 +61,7 @@ struct PkParams {
     const int* forced; int forced_ld;  // teacher forcing (parity tests): token fed to the next step = forced[b * forced_ld + step] instead of the sampled one
     long long* step_ts;                // optional [n_steps]: globaltimer (ns) when CTA 0 enters step s (bench: ms/step vs context length)
     float* trace;                      // optional [n_steps][b_eff][V] fp32: raw model logits of every step (trace[0] = prefill logits, copied by the host)
-    int exp_flags;                     // dev experiments (CAR_EXP): bits 0-1 pre-poll variant, bits 8-11 pre-poll back-off
-    long long* dbg; int dbg_step;      // dev instrumentation: [grid][64] globaltimer stamps (ns) of one step / layer 3
+    long long* dbg; int dbg_step;      // PK_TRACE builds: [grid][64] globaltimer stamps (ns) of one step / layer 3
 };
 
 // ---------------------------------------------------------------------------------------------------------
@@ -143,31 +142,6 @@ __device__ __forceinline__ size_t pk_a_index(int r, int k) {
     const int s = k >> 5, t = (k >> 3) & 3, p = (k >> 1) & 3, g = r & 7, hi = r >> 3;
     return ((size_t)((s * 4 + p) * 32 + g * 4 + t)) * 2 + hi;
 }
-
-// Code-generation knobs: the kernel is one large function under a 128-register cap, and ptxas' allocation for the layer loop
-// shifts with unrelated code (a smaller sampler can make the layers slower).  Out-of-line
-// phases get their own register allocation and keep the loop's code independent of the rest.
-#ifndef PK_ROPE_PRE           // qkv epilogue: RoPE table entry + column decomposition fetched before the packet wait (measured slower: off)
-#define PK_ROPE_PRE 0
-#endif
-#ifndef PK_OUTLINE            // bit 0: sampler, bit 1: attention phase, bit 2: GEMM phase (1 = the A/B winner)
-#define PK_OUTLINE 1
-#endif
-#if PK_OUTLINE & 1
-#define PK_SMP_INLINE __noinline__
-#else
-#define PK_SMP_INLINE __forceinline__
-#endif
-#if PK_OUTLINE & 2
-#define PK_ATTN_INLINE __noinline__
-#else
-#define PK_ATTN_INLINE __forceinline__
-#endif
-#if PK_OUTLINE & 4
-#define PK_GEMM_INLINE __noinline__
-#else
-#define PK_GEMM_INLINE __forceinline__
-#endif
 
 extern __shared__ __align__(128) unsigned char pk_smem_raw[];
 
@@ -300,23 +274,12 @@ __device__ __forceinline__ void pk_poll_round(const unsigned char* __restrict__ 
 // Cheap arrival hint before the full poll: warp 0 watches the first packet of 32 of the K/8 producer blocks (a different
 // subset per CTA) with back-off; the other warps wait at the CTA barrier.  SM count x 32 eight-byte loads per round instead of
 // the whole tile from every waiting thread — waiting CTAs must not eat the L2 bandwidth of the ones still producing.
-__device__ __forceinline__ void pk_prepoll(const uint2* buf, int K, unsigned int tag, int mode, unsigned mode_sleep) {
-    if (mode == 1) return;                             // (experiment) straight to the full poll
+__device__ __forceinline__ void pk_prepoll(const uint2* buf, int K, unsigned int tag) {
     const int nblk = K >> 3;
-    if (mode == 2) {                                   // (experiment) every warp watches one packet of its own first k-step
-        if ((threadIdx.x & 31) == 0 && (int)(threadIdx.x >> 5) * 4 < nblk) {
-            const uint2* pkt = buf + pk_a_index(0, (int)(threadIdx.x >> 5) * 32 + (blockIdx.x & 3) * 8);
-            unsigned int spins = 0;
-            while (pk_ld64(pkt).y != tag) { __nanosleep(100); pk_spin_check(spins); }
-        }
-        __syncwarp();
-        return;
-    }
     if (threadIdx.x < 32) {
         const uint2* pkt = buf + pk_a_index(0, (int)((blockIdx.x * 7u + threadIdx.x * (unsigned)max(1, nblk >> 5)) % (unsigned)nblk) * 8);
         unsigned int spins = 0;
-        const unsigned ns = mode_sleep;
-        while (!__all_sync(0xffffffffu, pk_ld64(pkt).y == tag)) { __nanosleep(ns); pk_spin_check(spins); }
+        while (!__all_sync(0xffffffffu, pk_ld64(pkt).y == tag)) { __nanosleep(120); pk_spin_check(spins); }
     }
     __syncthreads();
 }
@@ -339,9 +302,9 @@ __device__ __forceinline__ const bf16* pk_ctrl_next(const PkParams& P, int l) {
     return (P.has_ctrl && (l + 1) < P.L && (l + 1) % step3 == 0) ? P.ctrl[(l + 1) / step3] : nullptr;
 }
 
-__device__ PK_GEMM_INLINE unsigned int pk_gemm_phase(const PkParams& P, const int kind, const int l, const int pos,
-                                                      const unsigned int tag, int blk_lo, int blk_hi, unsigned int cons, long long* dbg, long long* wdbg_base,
-                                                      float* trace_rows = nullptr) {
+__device__ __forceinline__ unsigned int pk_gemm_phase(const PkParams& P, const int kind, const int l, const int pos,
+                                                       const unsigned int tag, int blk_lo, int blk_hi, unsigned int cons, long long* dbg, long long* wdbg_base,
+                                                       float* trace_rows = nullptr) {
     const PkSmem sm = pk_smem_layout();
     const int par = l & 1;
     const bool NORM = (kind == 0 || kind == 2 || kind == 4);
@@ -388,17 +351,6 @@ __device__ PK_GEMM_INLINE unsigned int pk_gemm_phase(const PkParams& P, const in
         }
     }
 
-    // qkv epilogue: section / head / element of this thread's column pair and its RoPE (cos, sin) — the 64-bit-free division and the
-    // table load (an L2 round trip) are taken off the path between the reduction and the packet stores
-    int q_col = 0;                                         // sec << 16 | head << 6 | el (one register across the poll and the MMA)
-    float2 q_cs = make_float2(1.f, 0.f);
-    if (PK_ROPE_PRE && kind == 0 && er == 0 && blk_lo + ej < blk_hi) {
-        const int n = (blk_lo + ej) * 8 + 2 * ecp;
-        const int sec = n / P.dim, w = n - sec * P.dim;
-        q_col = (sec << 16) | w;
-        if (sec < 2) q_cs = __ldg(reinterpret_cast<const float2*>(P.rope + ((size_t)pos * 32 + ((w & 63) >> 1)) * 2));
-    }
-
     if (NORM) {   // this phase's RMSNorm weights -> shared memory, asynchronously, while we wait for the A packets
         const bf16* nwg = kind == 0 ? sm.nwp[2 * l] : kind == 2 ? sm.nwp[2 * l + 1] : P.norm_w;
         if (tid < (K >> 3))
@@ -412,7 +364,7 @@ __device__ PK_GEMM_INLINE unsigned int pk_gemm_phase(const PkParams& P, const in
         const unsigned char* base = reinterpret_cast<const unsigned char*>(pk_a_buf(P, kind, par));
         const bool need_lo = g < M, need_hi = g + 8 < M;
         if (kind != 3) {
-            pk_prepoll(pk_a_buf(P, kind, par), K, tag, P.exp_flags & 3, ((P.exp_flags >> 8) & 15) == 0 ? 120u : 20u * ((P.exp_flags >> 8) & 15));
+            pk_prepoll(pk_a_buf(P, kind, par), K, tag);
             PK_W(1);
             if (M == 16) pk_poll_round<0, PK_MAXA_NORM, true>(base, nst, warp, lane, tag, true, true, alo, ahi);
             else pk_poll_round<0, PK_MAXA_NORM, false>(base, nst, warp, lane, tag, need_lo, need_hi, alo, ahi);
@@ -421,7 +373,7 @@ __device__ PK_GEMM_INLINE unsigned int pk_gemm_phase(const PkParams& P, const in
 #pragma unroll
                 for (int p = 0; p < 4; ++p) { alo[i][p] = 0u; ahi[i][p] = 0u; }
         } else {
-            pk_prepoll(pk_a_buf(P, kind, par), K, tag, P.exp_flags & 3, ((P.exp_flags >> 8) & 15) == 0 ? 120u : 20u * ((P.exp_flags >> 8) & 15));
+            pk_prepoll(pk_a_buf(P, kind, par), K, tag);
             PK_W(1);
             if (M == 16) {
                 pk_poll_round<0, 4, true>(base, nst, warp, lane, tag, true, true, alo, ahi);
@@ -585,15 +537,11 @@ __device__ PK_GEMM_INLINE unsigned int pk_gemm_phase(const PkParams& P, const in
             if (active && er == 0) {
                 const int r_lo = eg, r_hi = eg + 8;
                 if (kind == 0) {
-                    int sec = q_col >> 16, head = (q_col & 0xffff) >> 6, el = q_col & 63;
-                    float2 cs2 = q_cs;
-                    if (!PK_ROPE_PRE || bb != blk_lo) {   // later batches (only models with more than 4 qkv blocks per CTA): recompute
-                        const int n = (bb + ej) * 8 + 2 * ecp;
-                        sec = n / P.dim;
-                        const int w = n - sec * P.dim;
-                        head = w >> 6; el = w & 63;
-                        if (sec < 2) cs2 = __ldg(reinterpret_cast<const float2*>(P.rope + ((size_t)pos * 32 + (el >> 1)) * 2));
-                    }
+                    const int n = (bb + ej) * 8 + 2 * ecp;
+                    const int sec = n / P.dim, w = n - sec * P.dim;
+                    const int head = w >> 6, el = w & 63;
+                    float2 cs2 = make_float2(1.f, 0.f);
+                    if (sec < 2) cs2 = __ldg(reinterpret_cast<const float2*>(P.rope + ((size_t)pos * 32 + (el >> 1)) * 2));
                     float a0 = rnd<bf16>(v00), a1 = rnd<bf16>(v01), c0 = rnd<bf16>(v10), c1 = rnd<bf16>(v11);
                     if (sec < 2) {   // apply_rotary_emb gpt_t2i.py:522-532 (interleaved pairs, fp32, then cast)
                         const float x0 = a0 * cs2.x - a1 * cs2.y, x1 = a1 * cs2.x + a0 * cs2.y;
@@ -704,7 +652,7 @@ __device__ __forceinline__ void pk_attn_finalize(const PkParams& P, float Mx, fl
 // ("parts").  Within a part the four 8-lane row slots of the warp take rows k0 + sub + 4 i, the loads of two blocks of 4 rows
 // per slot in flight at once; the slots are merged with shuffles and the warp leaves one partial per part in shared memory:
 // entry (warp, part) = {-, m, l, -, acc[64]}.
-__device__ PK_ATTN_INLINE void pk_attn_phase(const PkParams& P, int layer, int pos, unsigned int tag, int par, long long* dbg) {
+__device__ __forceinline__ void pk_attn_phase(const PkParams& P, int layer, int pos, unsigned int tag, int par, long long* dbg) {
     const PkSmem sm = pk_smem_layout();
     constexpr int EPL = 8, UNR = 4, ENT = 68;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, sub = lane >> 3, cl = lane & 7;
@@ -893,7 +841,10 @@ __device__ __forceinline__ void pk_write_embedding(const PkParams& P, uint2* h2,
     }
 }
 
-__device__ PK_SMP_INLINE void pk_sample(const SampleArgs& a, int b) {
+// Out of line: the kernel is one large function under a 128-register cap, and ptxas' allocation for the layer loop shifts with
+// unrelated code (a smaller sampler can make the layers slower).  The outlined sampler gets its own register allocation and keeps
+// the loop's code independent of it; the GEMM and attention phases stay inlined (measured faster than outlined).
+__device__ __noinline__ void pk_sample(const SampleArgs& a, int b) {
     static_assert(SMP_SCRATCH <= PK_SMEM_RED, "the sampler's scratch aliases the reduction buffer");
     sample_body<PK_THREADS>(a, b, pk_smem_raw + PK_SMEM_RING);
 }

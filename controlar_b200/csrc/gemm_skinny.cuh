@@ -33,7 +33,6 @@ struct EpiParams {
     const float* rope; void* kc; void* vc; void* q; int S; int H; int d;
     // EPI_LOGITS
     float* logits; long long ldl;
-    long long* dbg;       // dev instrumentation: per-phase clock64 stamps of CTA 0 (null in production)
 };
 
 // tile: [16][ldt] fp32 accumulators for columns [nb0*8, nb0*8 + ncols) of rows [m0, m0+16)
@@ -125,7 +124,7 @@ static inline size_t skinny_smem_bytes(int K, int NB) {
 template <int NB, int U, bool NORM>
 __global__ void __launch_bounds__(SK_THREADS)
 skinny_gemm_bf16(const bf16* __restrict__ A, int lda, const uint4* __restrict__ Wp, const bf16* __restrict__ nw,
-                 float eps, int K, int nblk, int flags, EpiParams ep) {
+                 float eps, int K, int nblk, EpiParams ep) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int KS = K + 32;                                  // bf16 elements per smem row (+64 B: conflict-free)
     bf16* As = reinterpret_cast<bf16*>(smem_raw);
@@ -138,8 +137,6 @@ skinny_gemm_bf16(const bf16* __restrict__ A, int lda, const uint4* __restrict__ 
     const int ksteps = K >> 5;
     const int nsteps = (ksteps - warp + SK_WARPS - 1) / SK_WARPS;   // k32-steps owned by this warp: warp, warp+8, ..
 
-    const bool dbg_on = ep.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && tid == 0;
-    if (dbg_on) ep.dbg[0] = clock64();
     // ---- 1. first batch of weight fragments in flight before anything that depends on the previous kernel
     uint4 wf[U][NB];
     auto load_batch = [&](int i0) {
@@ -157,8 +154,10 @@ skinny_gemm_bf16(const bf16* __restrict__ A, int lda, const uint4* __restrict__ 
     };
     pdl_launch_dependents();
     load_batch(0);
-    // the rest of this warp's weight stream goes to L2 now, so the post-dependency loop never waits on HBM
-    for (int i = U; (flags & 1) && i < nsteps; ++i) {
+    // the rest of this warp's weight stream goes to L2 now, so the post-dependency loop never waits on HBM (fire-and-forget
+    // prefetches: unrolling the loop only adds code in front of pdl_wait())
+#pragma unroll 1
+    for (int i = U; i < nsteps; ++i) {
         const int s = warp + i * SK_WARPS;
 #pragma unroll
         for (int j = 0; j < NB; ++j)
@@ -166,7 +165,6 @@ skinny_gemm_bf16(const bf16* __restrict__ A, int lda, const uint4* __restrict__ 
                 prefetch_l2(Wp + ((size_t)(nb0 + j) * ksteps + s) * 32 + lane);
     }
     pdl_wait();   // ---- everything below may read what the previous kernel wrote
-    if (dbg_on) ep.dbg[1] = clock64();
 
     // ---- 2. stage the 16-row activation tile (RMSNorm fused when NORM): one pass over global memory
     const int chunks = K >> 3;   // 16-byte chunks per row
@@ -234,7 +232,6 @@ skinny_gemm_bf16(const bf16* __restrict__ A, int lda, const uint4* __restrict__ 
     }
     __syncthreads();
 
-    if (dbg_on) ep.dbg[2] = clock64();
     // ---- 3. main loop: this warp's k-steps, all NB column blocks; the CTA then strides to its next column group
     // (grid.x is capped at one wave, the staged activation tile is reused)
     float* tile = reinterpret_cast<float*>(smem_raw + (size_t)16 * KS * 2 + (size_t)SK_WARPS * NB * 128 * 4);   // [16][NB*8]
@@ -262,7 +259,6 @@ skinny_gemm_bf16(const bf16* __restrict__ A, int lda, const uint4* __restrict__ 
         }
     }
 
-    if (dbg_on && first) ep.dbg[3] = clock64();
     // ---- 4. cross-warp K reduction in fixed order, then the fused epilogue
 #pragma unroll
     for (int j = 0; j < NB; ++j) {
@@ -281,10 +277,8 @@ skinny_gemm_bf16(const bf16* __restrict__ A, int lda, const uint4* __restrict__ 
         tile[(e >> 3) * (NB * 8) + j * 8 + (e & 7)] = s;
     }
     __syncthreads();
-    if (dbg_on && first) ep.dbg[4] = clock64();
     const int ncols = min(NB, nblk - nb0) * 8;
     run_epilogue<bf16>(ep, tile, NB * 8, m0, nb0, ncols, tid, SK_THREADS);
-    if (dbg_on && first) ep.dbg[5] = clock64();
   }
 }
 

@@ -5,7 +5,6 @@ the 512^2 level-0 convolutions) and VQ `encode` indices (vq_model.py:41-46,216-2
 margins.  Every measured value is logged to vision512.jsonl (tests/helpers.py: log_measurement)."""
 import json
 import math
-import os
 
 import pytest
 import torch
@@ -90,7 +89,6 @@ def test_vq_encode_512_indices_vs_reference_golden():
     # best code — the reference's own median best-vs-second margin is 2.2e-2.)  Measured on an H100 80GB HBM3 with the fp32-grade
     # path: 1024 of 1024 indices identical.  Bar: >= 99.9 % identical and every mismatch a near-tie of the reference's own distances (gap < 1e-4;
     # 0.1 % of the positions have a reference margin below that).
-    tie = float(os.environ.get("CAR_VQ_TIE", "1e-4"))
-    assert worst_gap < tie, f"a mismatching index is {worst_gap:.3e} worse than the reference's best in the reference's own distances"
-    assert agree >= float(os.environ.get("CAR_VQ_AGREE", "0.999")), agree
+    assert worst_gap < 1e-4, f"a mismatching index is {worst_gap:.3e} worse than the reference's best in the reference's own distances"
+    assert agree >= 0.999, agree
     assert quant.shape == (1, 8, 32, 32)
