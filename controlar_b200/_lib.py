@@ -98,6 +98,10 @@ PROTOTYPES = {
     "car_adamw_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32, C.c_void_p]),
     "car_op_rmsnorm": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float,
                                  C.c_void_p]),
+    "car_op_attn_decode": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
+                                     C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "car_op_attn_prefill": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

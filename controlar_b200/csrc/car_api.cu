@@ -362,6 +362,9 @@ static int pk_state_setup(CarState* s) {
     return CAR_OK;
 }
 
+// key splits of the decode attention: about four CTAs per SM over all (b, h) rows, at most 16 per row
+static int attn_decode_nsplit(int bh) { return std::max(1, std::min(16, (4 * sm_count() + bh - 1) / bh)); }
+
 extern "C" int car_state_create(CarModel* m, int32_t b_eff, int32_t S, int32_t N, void* const* k_cache, void* const* v_cache,
                                 const float* rope_table, CarState** out) {
     if (!m || !k_cache || !v_cache || !rope_table || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
@@ -378,7 +381,7 @@ extern "C" int car_state_create(CarModel* m, int32_t b_eff, int32_t S, int32_t N
     const size_t es = m->esize();
     const size_t dd = d.dim, F = d.ffn_dim, V = d.vocab_size;
     const size_t MP = (size_t)b_eff * T, MC = (size_t)b_eff * N;
-    s->nsplit = std::max(1, std::min(16, (4 * sm_count() + b_eff * d.n_head - 1) / (b_eff * d.n_head)));
+    s->nsplit = attn_decode_nsplit(b_eff * d.n_head);
     int r = CAR_OK;
     auto A = [&](void** p, size_t bytes) { if (r == CAR_OK) r = alloc_dev(s->owned, p, bytes); };
     A(&s->h, b_eff * dd * es); A(&s->q, b_eff * dd * es); A(&s->attn, b_eff * dd * es); A(&s->act, b_eff * F * es);
@@ -438,22 +441,36 @@ extern "C" int car_state_destroy(CarState* s) {
 // ---------------------------------------------------------------------------------------------------------
 // kernel chains
 // ---------------------------------------------------------------------------------------------------------
-template <typename T>
-static int launch_attn_decode(CarState* s, int l, cudaStream_t st) {
-    const CarModelDesc& d = s->m->d;
-    dim3 grid(s->b_eff * d.n_head, s->nsplit);
-    CAR_LAUNCH_PDL((attn_decode_kernel<T>), grid, dim3(AD_THREADS), 0, st, (const T*)s->q, (const T*)s->kc[l], (const T*)s->vc[l],
-                   (const int*)s->emb_mask, s->T, (const int*)s->pos, d.n_head, s->S, s->T, s->nsplit, s->attn_part,
-                   s->tickets, (T*)s->attn);
+// The three attention launches (attention.cuh), shared by the model chains and by car_op_attn_decode / car_op_attn_prefill so that
+// the unit tests exercise exactly the launch the product makes.  Caches [B, H, S, 64]; emb_mask [B][mask_ld] gates key columns < Tpre.
+static int launch_attn_decode(int dtype, cudaStream_t st, const void* q, const void* kc, const void* vc, const int* emb_mask, int mask_ld,
+                              const int* pos, int B, int H, int S, int Tpre, int nsplit, float* part, int* tickets, void* out) {
+    const dim3 grid(B * H, nsplit);
+    if (dtype == CAR_BF16)
+        CAR_LAUNCH_PDL((attn_decode_kernel<bf16>), grid, dim3(AD_THREADS), 0, st, (const bf16*)q, (const bf16*)kc, (const bf16*)vc,
+                       emb_mask, mask_ld, pos, H, S, Tpre, nsplit, part, tickets, (bf16*)out);
+    else
+        CAR_LAUNCH_PDL((attn_decode_kernel<float>), grid, dim3(AD_THREADS), 0, st, (const float*)q, (const float*)kc, (const float*)vc,
+                       emb_mask, mask_ld, pos, H, S, Tpre, nsplit, part, tickets, (float*)out);
     return CAR_OK;
 }
 
-template <typename T>
-static int launch_attn_prefill(CarState* s, int l, cudaStream_t st) {
-    const CarModelDesc& d = s->m->d;
-    const long long items = (long long)s->b_eff * d.n_head * s->T;
-    CAR_LAUNCH((attn_prefill_kernel<T>), (unsigned)((items + 3) / 4), 128, 0, st, (const T*)s->qP, (const T*)s->kc[l],
-               (const T*)s->vc[l], (const int*)s->emb_mask, s->T, s->b_eff, d.n_head, s->S, s->T, s->T, (T*)s->attnP);
+static int launch_attn_prefill(int dtype, cudaStream_t st, const void* q, const void* kc, const void* vc, const int* emb_mask,
+                               int mask_ld, int B, int H, int S, int Tq, int Tpre, void* out) {
+    const unsigned blocks = (unsigned)(((long long)B * H * Tq + 3) / 4);
+    if (dtype == CAR_BF16)
+        CAR_LAUNCH((attn_prefill_kernel<bf16>), blocks, 128, 0, st, (const bf16*)q, (const bf16*)kc, (const bf16*)vc, emb_mask, mask_ld,
+                   B, H, S, Tq, Tpre, (bf16*)out);
+    else
+        CAR_LAUNCH((attn_prefill_kernel<float>), blocks, 128, 0, st, (const float*)q, (const float*)kc, (const float*)vc, emb_mask, mask_ld,
+                   B, H, S, Tq, Tpre, (float*)out);
+    return CAR_OK;
+}
+
+static int launch_attn_prefill_mma(cudaStream_t st, const void* q, const void* kc, const void* vc, const int* emb_mask, int mask_ld,
+                                   int B, int H, int S, int Tq, int Tpre, void* out) {
+    CAR_LAUNCH(attn_prefill_mma_kernel, dim3((Tq + 63) / 64, H, B), 128, 0, st, (const bf16*)q, (const bf16*)kc, (const bf16*)vc,
+               emb_mask, mask_ld, H, S, Tq, Tpre, (bf16*)out);
     return CAR_OK;
 }
 
@@ -510,8 +527,7 @@ static int enqueue_block_dense(CarState* s, int l, cudaStream_t st) {
     CAR_LAUNCH(rope_kv_write_kernel, sm_count() * 8, 256, 0, st, (const bf16*)s->qkvP, s->rope, (bf16*)s->qP, (bf16*)s->kc[l], (bf16*)s->vc[l], rows, s->T, dim,
                d.n_head, s->S);
     // prefix attention on the tensor cores (attention.cuh): 64 query rows per CTA
-    CAR_LAUNCH(attn_prefill_mma_kernel, dim3((s->T + 63) / 64, d.n_head, s->b_eff), 128, 0, st, (const bf16*)s->qP, (const bf16*)s->kc[l],
-               (const bf16*)s->vc[l], (const int*)s->emb_mask, s->T, d.n_head, s->S, s->T, s->T, (bf16*)s->attnP);
+    CAR_TRY(launch_attn_prefill_mma(st, s->qP, s->kc[l], s->vc[l], s->emb_mask, s->T, s->b_eff, d.n_head, s->S, s->T, s->T, s->attnP));
     CAR_TRY(dense_linear(st, s->attnP, dim, m->wo[l], rows, dim, dim, ACT_NONE, s->hP, dim, s->hP, dim));
     CAR_LAUNCH((rmsnorm_rows_kernel<bf16>), rows, 256, 0, st, (const bf16*)s->hP, (const bf16*)m->ffn_norm[l], (bf16*)s->t1, dim, d.norm_eps);
     CAR_TRY(dense_linear(st, s->t1, dim, m->w1[l], rows, F, dim, ACT_NONE, nullptr, 0, s->gP, F));
@@ -539,8 +555,11 @@ static int enqueue_block(CarState* s, int l, bool decode, cudaStream_t st) {
     e1.H = d.n_head; e1.d = dim;
     CAR_TRY(launch_skinny(st, dt, h, dim, m->g_wqkv[l], m->attention_norm[l], d.norm_eps, rows, 3 * dim, dim, e1, true));
 
-    if (decode) { if (dt == CAR_BF16) CAR_TRY(launch_attn_decode<bf16>(s, l, st)); else CAR_TRY(launch_attn_decode<float>(s, l, st)); }
-    else { if (dt == CAR_BF16) CAR_TRY(launch_attn_prefill<bf16>(s, l, st)); else CAR_TRY(launch_attn_prefill<float>(s, l, st)); }
+    if (decode)
+        CAR_TRY(launch_attn_decode(dt, st, s->q, s->kc[l], s->vc[l], s->emb_mask, s->T, s->pos, s->b_eff, d.n_head, s->S, s->T, s->nsplit,
+                                   s->attn_part, s->tickets, s->attn));
+    else
+        CAR_TRY(launch_attn_prefill(dt, st, s->qP, s->kc[l], s->vc[l], s->emb_mask, s->T, s->b_eff, d.n_head, s->S, s->T, s->T, s->attnP));
 
     EpiParams e2 = epi_base(EPI_RESID);
     e2.rpb = rpb; e2.pos_ptr = posp; e2.h = h; e2.ldh = dim;
@@ -930,6 +949,49 @@ extern "C" int car_op_rmsnorm(int32_t dtype, const void* x, const void* w, void*
     if (dtype == CAR_BF16) CAR_LAUNCH((rmsnorm_rows_kernel<bf16>), M, 256, 0, st, (const bf16*)x, (const bf16*)w, (bf16*)y, K, eps);
     else CAR_LAUNCH((rmsnorm_rows_kernel<float>), M, 256, 0, st, (const float*)x, (const float*)w, (float*)y, K, eps);
     return CAR_OK;
+}
+
+// shape and mask checks common to the two attention ops
+static int attn_op_check(int dtype, const void* q, const void* kc, const void* vc, const int32_t* emb_mask, int mask_ld, int B, int H,
+                         int S, int Tpre, const void* out) {
+    if (!q || !kc || !vc || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (dtype != CAR_BF16 && dtype != CAR_F32) CAR_FAIL(CAR_ERR_ARG, "dtype must be CAR_BF16 or CAR_F32");
+    if (B <= 0 || H <= 0 || S <= 0 || B > 65535 || H > 65535 || (long long)B * H > (1 << 30)) CAR_FAIL(CAR_ERR_ARG, "need 0 < B, H <= 65535 and S > 0");
+    if (Tpre < 0) CAR_FAIL(CAR_ERR_ARG, "Tpre must be >= 0");
+    if (emb_mask && mask_ld < Tpre) CAR_FAIL(CAR_ERR_ARG, "mask_ld must be >= Tpre");
+    if (((uintptr_t)kc | (uintptr_t)vc) % 16) CAR_FAIL(CAR_ERR_ARG, "k_cache and v_cache must be 16-byte aligned");
+    return CAR_OK;
+}
+
+extern "C" int car_op_attn_decode(int32_t dtype, const void* q, const void* k_cache, const void* v_cache, const int32_t* emb_mask,
+                                  int32_t mask_ld, const int32_t* pos_dev, int32_t B, int32_t H, int32_t S, int32_t Tpre, int32_t nsplit,
+                                  float* part, int32_t* tickets, void* out, void* stream) {
+    CAR_TRY(attn_op_check(dtype, q, k_cache, v_cache, emb_mask, mask_ld, B, H, S, Tpre, out));
+    if (!pos_dev || !part || !tickets) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (nsplit < 0 || nsplit > 16) CAR_FAIL(CAR_ERR_ARG, "nsplit must be in [0, 16]");
+    cudaStream_t st = (cudaStream_t)stream;
+    // the kernel reads pos on the device; read it back to check the invariant car_decode_step guarantees by pos >= T: the key at
+    // pos is an image key, so every row has at least one unmasked key (the decode kernel does not force the diagonal)
+    int32_t pos = -1;
+    CAR_CUDA(cudaMemcpyAsync(&pos, pos_dev, sizeof(pos), cudaMemcpyDeviceToHost, st));
+    CAR_CUDA(cudaStreamSynchronize(st));
+    if (pos < Tpre || pos >= S) CAR_FAIL(CAR_ERR_ARG, "need Tpre <= *pos_dev < S");
+    return launch_attn_decode(dtype, st, q, k_cache, v_cache, emb_mask, mask_ld, pos_dev, B, H, S, Tpre,
+                              nsplit ? nsplit : attn_decode_nsplit(B * H), part, tickets, out);
+}
+
+extern "C" int car_op_attn_prefill(int32_t dtype, const void* q, const void* k_cache, const void* v_cache, const int32_t* emb_mask,
+                                   int32_t mask_ld, int32_t B, int32_t H, int32_t S, int32_t Tq, int32_t Tpre, int32_t impl, void* out,
+                                   void* stream) {
+    CAR_TRY(attn_op_check(dtype, q, k_cache, v_cache, emb_mask, mask_ld, B, H, S, Tpre, out));
+    if (Tq < 1 || Tq > 256) CAR_FAIL(CAR_ERR_ARG, "Tq must be in [1, 256]");
+    if (Tq > S || Tpre > Tq) CAR_FAIL(CAR_ERR_ARG, "need Tpre <= Tq <= S");
+    if (impl != 0 && impl != 1) CAR_FAIL(CAR_ERR_ARG, "impl must be 0 (scalar) or 1 (tensor cores)");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (impl == 0) return launch_attn_prefill(dtype, st, q, k_cache, v_cache, emb_mask, mask_ld, B, H, S, Tq, Tpre, out);
+    if (dtype != CAR_BF16) CAR_FAIL(CAR_ERR_UNSUPPORTED, "the tensor-core prefill attention is bf16 only");
+    if (((uintptr_t)q | (uintptr_t)out) % 4) CAR_FAIL(CAR_ERR_ARG, "q and out must be 4-byte aligned");
+    return launch_attn_prefill_mma(st, q, k_cache, v_cache, emb_mask, mask_ld, B, H, S, Tq, Tpre, out);
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -477,3 +477,47 @@ def op_rmsnorm(x: torch.Tensor, w: torch.Tensor, eps: float) -> torch.Tensor:
     check(lib.car_op_rmsnorm(dtype_code(x.dtype), _ptr(x2), _ptr(w.detach().contiguous()), _ptr(y), x2.shape[0], K,
                              float(eps), cur_stream()), "car_op_rmsnorm")
     return y.reshape(x.shape)
+
+
+def _attn_mask(emb_mask: Optional[torch.Tensor]):
+    """int32 [B, mask_ld] on the device, or (None, 0)."""
+    if emb_mask is None:
+        return None, 0
+    m = emb_mask.to(torch.int32).contiguous()
+    return m, m.shape[-1]
+
+
+def op_attn_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, pos, Tpre: int,
+                   emb_mask: Optional[torch.Tensor] = None, nsplit: int = 0, part: Optional[torch.Tensor] = None,
+                   tickets: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The decode step's KV-cache attention (car_op_attn_decode): q [B, H*64] at position `pos` (int, or a device int32 scalar) against
+    caches [B, H, S, 64] -> [B, H*64].  nsplit 0 = the product's choice.  part (fp32, >= B*H*16*68) and tickets (int32 [B*H], zero)
+    are allocated when not given; pass them to reuse the split bookkeeping across calls.  out: optional [B, H*64] destination."""
+    lib = _lib.lib()
+    B, H, S, _ = k_cache.shape
+    dev = q.device
+    if not torch.is_tensor(pos):
+        pos = torch.tensor([int(pos)], dtype=torch.int32, device=dev)
+    part = torch.empty(B * H * 16 * 68, dtype=torch.float32, device=dev) if part is None else part
+    tickets = torch.zeros(B * H, dtype=torch.int32, device=dev) if tickets is None else tickets
+    out = torch.empty((B, H * 64), dtype=q.dtype, device=dev) if out is None else out
+    m, ld = _attn_mask(emb_mask)
+    with torch.cuda.device(dev):
+        check(lib.car_op_attn_decode(dtype_code(q.dtype), _ptr(q.contiguous()), _ptr(k_cache), _ptr(v_cache), _ptr(m), ld, _ptr(pos),
+                                     B, H, S, int(Tpre), int(nsplit), _ptr(part), _ptr(tickets), _ptr(out), cur_stream()),
+              "car_op_attn_decode")
+    return out
+
+
+def op_attn_prefill(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, Tq: int, Tpre: int,
+                    emb_mask: Optional[torch.Tensor] = None, impl: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The prefix rows' KV-cache attention (car_op_attn_prefill): q [B*Tq, H*64] at positions 0..Tq-1 against caches [B, H, S, 64]
+    -> [B*Tq, H*64].  impl 0 = the scalar kernel (bf16 / fp32), 1 = the bf16 tensor-core kernel.  out: optional destination."""
+    lib = _lib.lib()
+    B, H, S, _ = k_cache.shape
+    out = torch.empty((B * Tq, H * 64), dtype=q.dtype, device=q.device) if out is None else out
+    m, ld = _attn_mask(emb_mask)
+    with torch.cuda.device(q.device):
+        check(lib.car_op_attn_prefill(dtype_code(q.dtype), _ptr(q.contiguous()), _ptr(k_cache), _ptr(v_cache), _ptr(m), ld, B, H, S,
+                                      int(Tq), int(Tpre), int(impl), _ptr(out), cur_stream()), "car_op_attn_prefill")
+    return out

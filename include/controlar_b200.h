@@ -169,6 +169,23 @@ int car_op_dense_linear(const void* x, const void* w, const void* resid, void* y
 int car_op_rmsnorm(int32_t dtype, const void* x, const void* w, void* y, int32_t M, int32_t K, float eps,
                    void* stream);
 
+/* KV-cache attention (csrc/attention.cuh), launched exactly as the model chains launch it.  k_cache, v_cache: [B, H, S, 64] in dtype,
+ * 16-byte aligned.  Mask (generate.py:184-193): key s is visible to query position i iff s <= i and (s >= Tpre or emb_mask[b][s] != 0
+ * or s == i); emb_mask int32 [B][mask_ld], mask_ld >= Tpre, or NULL (all ones).  Scale 1/8, fp32 arithmetic, output rounded to dtype.
+ * car_op_attn_decode: the decode step's attn_decode_kernel.  q [B, H*64] -> out [B, H*64], the query at position pos = *pos_dev
+ * (device int32; Tpre <= pos < S, read back to check it, which synchronises the stream) against keys [0, pos].  nsplit in [0, 16]
+ * CTAs per (b, h), 0 = the choice car_state_create makes.  part: fp32 scratch of B * H * nsplit * 68 floats (B * H * 16 * 68 always
+ * suffices); tickets: int32 [B * H], zero before the call and left zero by it.
+ * car_op_attn_prefill: the prefix rows.  q [B * Tq, H*64] (rows b * Tq + i) -> out [B * Tq, H*64], queries at positions i < Tq
+ * (1 <= Tq <= 256, Tpre <= Tq <= S) against keys [0, i].  impl 0: attn_prefill_kernel (one warp per query row; bf16 or fp32);
+ * impl 1: attn_prefill_mma_kernel (bf16 tensor cores, probabilities rounded to bf16 before the value product). */
+int car_op_attn_decode(int32_t dtype, const void* q, const void* k_cache, const void* v_cache, const int32_t* emb_mask, int32_t mask_ld,
+                       const int32_t* pos_dev, int32_t B, int32_t H, int32_t S, int32_t Tpre, int32_t nsplit, float* part,
+                       int32_t* tickets, void* out, void* stream);
+int car_op_attn_prefill(int32_t dtype, const void* q, const void* k_cache, const void* v_cache, const int32_t* emb_mask,
+                        int32_t mask_ld, int32_t B, int32_t H, int32_t S, int32_t Tq, int32_t Tpre, int32_t impl, void* out,
+                        void* stream);
+
 /* =====================================================================================================
  * Control encoder: Dinov2_Adapter.forward (autoregressive/models/dinov2_adapter.py:16-29) = resize to multiples
  * of 14 -> HF Dinov2Model (third-party: transformers, unpinned in requirements.txt:19; 5.5.0 restated) -> drop CLS,

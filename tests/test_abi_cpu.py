@@ -34,6 +34,33 @@ def test_ctypes_prototypes_cover_header():
     assert b"null" in l.car_last_error()
 
 
+def test_attention_ops_reject_bad_arguments_before_any_launch():
+    """Each call differs from a valid one in one argument, which the op must refuse before it touches the device (the pointers are
+    never dereferenced)."""
+    from controlar_b200 import _lib
+    l = _lib.lib()
+    P = 1 << 20                                        # a 16-byte-aligned stand-in pointer
+    dec = dict(dtype=0, q=P, k=P, v=P, m=P, ld=120, pos=P, B=2, H=3, S=200, Tpre=120, nsplit=0, part=P, tickets=P, out=P)
+    bad_dec = [dict(dtype=2), dict(q=None), dict(k=None), dict(pos=None), dict(part=None), dict(tickets=None), dict(out=None),
+               dict(B=0), dict(H=-1), dict(S=0), dict(Tpre=-1), dict(ld=119), dict(nsplit=-1), dict(nsplit=17), dict(k=P + 8)]
+    for change in bad_dec:
+        a = {**dec, **change}
+        rc = l.car_op_attn_decode(a["dtype"], a["q"], a["k"], a["v"], a["m"], a["ld"], a["pos"], a["B"], a["H"], a["S"], a["Tpre"],
+                                  a["nsplit"], a["part"], a["tickets"], a["out"], None)
+        assert rc < 0, change
+        assert l.car_last_error(), change
+    pre = dict(dtype=0, q=P, k=P, v=P, m=P, ld=120, B=2, H=3, S=200, Tq=150, Tpre=120, impl=1, out=P)
+    bad_pre = [dict(dtype=5), dict(q=None), dict(v=None), dict(out=None), dict(Tq=0), dict(Tq=257, S=300), dict(Tq=201),
+               dict(Tpre=151), dict(ld=100), dict(impl=2), dict(impl=-1), dict(dtype=1), dict(q=P + 2), dict(out=P + 2),
+               dict(v=P + 4), dict(B=70000)]
+    for change in bad_pre:
+        a = {**pre, **change}
+        rc = l.car_op_attn_prefill(a["dtype"], a["q"], a["k"], a["v"], a["m"], a["ld"], a["B"], a["H"], a["S"], a["Tq"], a["Tpre"],
+                                   a["impl"], a["out"], None)
+        assert rc < 0, change
+        assert l.car_last_error(), change
+
+
 def test_product_fails_loudly_without_gpu():
     import torch
     if torch.cuda.is_available():
