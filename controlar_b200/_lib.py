@@ -169,6 +169,47 @@ class NativeHandle:
         return (_no_handle, ())
 
 
+def param_signature(params) -> tuple:
+    """What a handle built from `params` depends on: replacing, updating in place, casting or moving a parameter changes it."""
+    return tuple((p.data_ptr(), p._version, p.dtype, str(p.device)) for p in params)
+
+
+class ModuleHandle(NativeHandle):
+    """A library handle built from a module's parameters and released by the entry point named `destroy` (e.g. "car_hed_destroy").
+    `get(params, create)` returns it, built first by `create(out)` — which fills the c_void_p `out` — with the parameters' device
+    current, and built again whenever `param_signature(params)` changed.  The old handle is cleared and destroyed before a rebuild,
+    so a failed create leaves no stale pointer, and every handle is destroyed exactly once."""
+
+    def __init__(self, destroy: str):
+        self.destroy = destroy
+        self.handle = C.c_void_p()
+        self.sig = None
+
+    def get(self, params, create):
+        import torch
+        sig = param_signature(params)
+        if not self.handle or sig != self.sig:
+            if params[0].device.type != "cuda":
+                raise RuntimeError("controlar_b200: the module's parameters must be on a CUDA device (there is no CPU path)")
+            self.close()
+            with torch.cuda.device(params[0].device):
+                create(self.handle)
+                torch.cuda.current_stream().synchronize()      # the library has copied / packed what it read
+            self.sig = sig
+        return self.handle
+
+    def close(self):
+        h, self.handle, self.sig = self.handle, C.c_void_p(), None
+        if h:
+            getattr(lib(), self.destroy)(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def _ptr(t):
     """Device pointer of a contiguous CUDA tensor (None passes through)."""
     if t is None:

@@ -151,8 +151,7 @@ class DPTForDepthEstimation(nn.Module):
         self.head = _Module()
         self.head.head = nn.Sequential(_conv(F, F // 2, 3, padding=1), nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True),
                                        _conv(F // 2, 32, 3, padding=1), nn.ReLU(), _conv(32, 1, 1), nn.ReLU())
-        self._h = None
-        self._sig = None
+        self._car_dpt = None
 
     # ---- constructors
     @classmethod
@@ -191,29 +190,21 @@ class DPTForDepthEstimation(nn.Module):
         d.fusion, d.pos_grid, d.ln_eps = c.fusion_hidden_size, c.image_size // 16, c.layer_norm_eps
         return d
 
+    def _create(self, out):
+        ts = [p.detach().contiguous() for p in self.parameters()]     # state-dict order
+        arr = _ptr_array(ts)
+        desc = self._desc()
+        check(_lib.lib().car_dpt_create(C.byref(desc), C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(out)),
+              "car_dpt_create")
+
     def _handle(self):
-        ps = list(self.parameters())                      # state-dict order
-        if ps[0].device.type != "cuda":
-            raise RuntimeError("controlar_b200 DPTForDepthEstimation needs the module on a CUDA device (no CPU path)")
+        ps = list(self.parameters())
         bad = {p.dtype for p in ps} - {torch.float32}
         if bad:
             raise RuntimeError(f"controlar_b200 DPTForDepthEstimation runs in fp32, as the reference does; parameters are {sorted(map(str, bad))}")
-        sig = tuple((p.data_ptr(), p._version) for p in ps)
-        if self._h is None or sig != self._sig:
-            lib = _lib.lib()
-            if self._h is not None:
-                lib.car_dpt_destroy(self._h)
-                self._h = None
-            ts = [p.detach().contiguous() for p in ps]
-            h = C.c_void_p()
-            arr = _ptr_array(ts)
-            desc = self._desc()
-            with torch.cuda.device(ts[0].device):
-                check(lib.car_dpt_create(C.byref(desc), C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(h)),
-                      "car_dpt_create")
-                torch.cuda.current_stream().synchronize()  # the library copied / packed everything: `ts` may go
-            self._h, self._sig = h, sig
-        return self._h
+        if self._car_dpt is None:
+            object.__setattr__(self, "_car_dpt", _lib.ModuleHandle("car_dpt_destroy"))
+        return self._car_dpt.get(ps, self._create)
 
     def forward(self, pixel_values, labels=None, **unused):
         """pixel_values (B, 3, H, W), H == W, H % 32 == 0, H >= 64 -> DepthEstimatorOutput(predicted_depth=(B, H, W) fp32)."""
@@ -231,10 +222,3 @@ class DPTForDepthEstimation(nn.Module):
         with torch.cuda.device(x.device):
             check(_lib.lib().car_dpt_forward(self._handle(), _ptr(x), B, H, W, _ptr(out), cur_stream()), "car_dpt_forward")
         return DepthEstimatorOutput(predicted_depth=out)
-
-    def __del__(self):
-        try:
-            if self._h is not None:
-                _lib.lib().car_dpt_destroy(self._h)
-        except Exception:
-            pass

@@ -36,8 +36,7 @@ class ControlNetHED_Apache2(nn.Module):
         self.norm = nn.Parameter(torch.zeros(size=(1, 3, 1, 1)))
         for b, (cin, cout, n) in enumerate(BLOCKS, start=1):
             setattr(self, f"block{b}", DoubleConvBlock(cin, cout, n))
-        self._h = None
-        self._sig = None
+        self._car_hed = None
 
     def _tensors(self):
         ts = [self.norm.detach().reshape(3)]
@@ -48,22 +47,15 @@ class ControlNetHED_Apache2(nn.Module):
             ts += [blk.projection.weight.detach().reshape(-1), blk.projection.bias.detach()]
         return [t.to(torch.float32).contiguous() for t in ts]
 
-    def _handle(self):
+    def _create(self, out):
         ts = self._tensors()
-        if ts[0].device.type != "cuda":
-            raise RuntimeError("controlar_b200 HED needs the module on a CUDA device (no CPU path)")
-        sig = tuple((t.data_ptr(), t._version) for t in ts) + tuple(p._version for p in self.parameters())
-        if self._h is None or sig != self._sig:
-            lib = _lib.lib()
-            if self._h is not None:
-                lib.car_hed_destroy(self._h)
-            h = C.c_void_p()
-            arr = _ptr_array(ts)
-            with torch.cuda.device(ts[0].device):
-                check(lib.car_hed_create(C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(h)), "car_hed_create")
-                torch.cuda.current_stream().synchronize()          # the library copied / packed everything: `ts` may go
-            self._h, self._sig = h, sig
-        return self._h
+        arr = _ptr_array(ts)
+        check(_lib.lib().car_hed_create(C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(out)), "car_hed_create")
+
+    def _handle(self):
+        if self._car_hed is None:
+            object.__setattr__(self, "_car_hed", _lib.ModuleHandle("car_hed_destroy"))
+        return self._car_hed.get(list(self.parameters()), self._create)
 
     def run(self, x: torch.Tensor, want_projections: bool = False):
         if x.device.type != "cuda":
@@ -88,13 +80,6 @@ class ControlNetHED_Apache2(nn.Module):
 
     def __call__(self, x):
         return self.run(x, want_projections=True)[1]
-
-    def __del__(self):
-        try:
-            if self._h is not None:
-                _lib.lib().car_hed_destroy(self._h)
-        except Exception:
-            pass
 
 
 class HEDdetector(nn.Module):

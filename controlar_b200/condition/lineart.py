@@ -48,29 +48,17 @@ class LineArt(nn.Module):
             cin //= 2
         self.model3 = nn.Sequential(*model3)
         self.model4 = nn.Sequential(nn.ReflectionPad2d(3), nn.Conv2d(64, output_nc, 7), nn.Sigmoid())
-        self._h = None
-        self._sig = None
+        self._car_lineart = None
 
-    def _tensors(self):
-        return [p.detach().to(torch.float32).contiguous() for p in self.parameters()]   # state-dict order, 24 tensors
+    def _create(self, out):
+        ts = [p.detach().to(torch.float32).contiguous() for p in self.parameters()]   # state-dict order, 24 tensors
+        arr = _ptr_array(ts)
+        check(_lib.lib().car_lineart_create(C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(out)), "car_lineart_create")
 
     def _handle(self):
-        ts = self._tensors()
-        if ts[0].device.type != "cuda":
-            raise RuntimeError("controlar_b200 LineArt needs the module on a CUDA device (no CPU path)")
-        sig = tuple((t.data_ptr(), t._version) for t in ts) + tuple(p._version for p in self.parameters())
-        if self._h is None or sig != self._sig:
-            lib = _lib.lib()
-            if self._h is not None:
-                lib.car_lineart_destroy(self._h)
-                self._h = None
-            h = C.c_void_p()
-            arr = _ptr_array(ts)
-            with torch.cuda.device(ts[0].device):
-                check(lib.car_lineart_create(C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(h)), "car_lineart_create")
-                torch.cuda.current_stream().synchronize()          # the library copied / packed everything: `ts` may go
-            self._h, self._sig = h, sig
-        return self._h
+        if self._car_lineart is None:
+            object.__setattr__(self, "_car_lineart", _lib.ModuleHandle("car_lineart_destroy"))
+        return self._car_lineart.get(list(self.parameters()), self._create)
 
     @staticmethod
     def output_size(H: int, W: int):
@@ -89,10 +77,3 @@ class LineArt(nn.Module):
         with torch.cuda.device(x.device):
             check(_lib.lib().car_lineart_forward(self._handle(), _ptr(x), B, H, W, _ptr(out), cur_stream()), "car_lineart_forward")
         return out
-
-    def __del__(self):
-        try:
-            if self._h is not None:
-                _lib.lib().car_lineart_destroy(self._h)
-        except Exception:
-            pass

@@ -109,30 +109,21 @@ class DPTDepthModel(nn.Module):
             setattr(sc, f"refinenet{i}", r)
         sc.output_conv = nn.Sequential(nn.Conv2d(F, F // 2, 3, padding=1), nn.Identity(), nn.Conv2d(F // 2, 32, 3, padding=1), nn.ReLU(True),
                                        nn.Conv2d(32, 1, 1), nn.ReLU(True), nn.Identity())
-        self._h = None
-        self._sig = None
+        self._car_midas = None
+
+    def _create(self, out):
+        ts = [p.detach().contiguous() for p in self.parameters()]     # state-dict order
+        arr = _ptr_array(ts)
+        check(_lib.lib().car_midas_create(C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(out)), "car_midas_create")
 
     def _handle(self):
-        ps = list(self.parameters())                      # state-dict order
-        if ps[0].device.type != "cuda":
-            raise RuntimeError("controlar_b200 DPTDepthModel needs the module on a CUDA device (no CPU path)")
+        ps = list(self.parameters())
         bad = {p.dtype for p in ps} - {torch.float32}
         if bad:
             raise RuntimeError(f"controlar_b200 DPTDepthModel runs in fp32, as the reference does; parameters are {sorted(map(str, bad))}")
-        sig = tuple((p.data_ptr(), p._version) for p in ps)
-        if self._h is None or sig != self._sig:
-            lib = _lib.lib()
-            if self._h is not None:
-                lib.car_midas_destroy(self._h)
-                self._h = None
-            ts = [p.detach().contiguous() for p in ps]
-            h = C.c_void_p()
-            arr = _ptr_array(ts)
-            with torch.cuda.device(ts[0].device):
-                check(lib.car_midas_create(C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(h)), "car_midas_create")
-                torch.cuda.current_stream().synchronize()  # the library copied / packed everything: `ts` may go
-            self._h, self._sig = h, sig
-        return self._h
+        if self._car_midas is None:
+            object.__setattr__(self, "_car_midas", _lib.ModuleHandle("car_midas_destroy"))
+        return self._car_midas.get(ps, self._create)
 
     def forward(self, x):
         """x (B, 3, H, W), H and W multiples of 32 and at least 64 -> depth (B, H, W) fp32."""
@@ -148,13 +139,6 @@ class DPTDepthModel(nn.Module):
         with torch.cuda.device(x.device):
             check(_lib.lib().car_midas_forward(self._handle(), _ptr(x), B, H, W, _ptr(out), cur_stream()), "car_midas_forward")
         return out
-
-    def __del__(self):
-        try:
-            if self._h is not None:
-                _lib.lib().car_midas_destroy(self._h)
-        except Exception:
-            pass
 
 
 def load_state_dict_file(path):

@@ -72,12 +72,103 @@ struct Arena {   // grow-only device workspace, re-used across calls (no allocat
     void release() { if (base) cudaFree(base); base = nullptr; cap = 0; }
 };
 
+// Base of every handle: the device memory its create call allocated and its forward workspace, both freed by `delete`.
+struct CarOwned {
+    std::vector<void*> owned;
+    Arena ws;
+    ~CarOwned() {
+        for (void* p : owned) cudaFree(p);
+        ws.release();
+    }
+};
+
+template <typename... KArgs, typename... Args>
+static int launch_on(cudaStream_t st, void (*kernel)(KArgs...), unsigned grid, unsigned block, Args... args) {
+    CAR_LAUNCH(kernel, grid, block, 0, st, args...);
+    return CAR_OK;
+}
+
+// Reader of the flat tensor list a create call takes (device pointers in state-dict order, fp32), copying and packing each tensor
+// into memory the handle owns.  The list comes from the caller: the constructor refuses a null entry before any CUDA call, and every
+// read is bounds-checked.  The first error sticks — later calls allocate, copy and launch nothing, and return null — and finish()
+// returns it; messages name the entry point `fn`.
+struct TensorReader {
+    const char* fn;
+    const void* const* t;
+    int n, i = 0, rc = CAR_OK;
+    cudaStream_t st;
+    CarOwned* m;
+
+    TensorReader(const char* fn, const void* const* t, int n, void* stream, CarOwned* m)
+        : fn(fn), t(t), n(n), st((cudaStream_t)stream), m(m) {
+        for (int k = 0; k < n && rc == CAR_OK; ++k)
+            if (!t[k]) fail(CAR_ERR_ARG, "null tensor");
+    }
+    bool ok() const { return rc == CAR_OK; }
+    void fail(int code, const std::string& msg) {
+        if (rc != CAR_OK) return;
+        rc = code;
+        g_car_err = std::string(fn) + ": " + msg;
+    }
+    void cuda(cudaError_t e, const char* what) {
+        if (e != cudaSuccess) fail(CAR_ERR_CUDA, std::string(what) + " -> " + cudaGetErrorString(e));
+    }
+    const float* next() {
+        if (ok() && i >= n) fail(CAR_ERR_ARG, "tensor list too short");
+        return ok() ? (const float*)t[i++] : nullptr;
+    }
+    void skip(int k) {
+        for (int j = 0; j < k; ++j) next();
+    }
+    void* alloc(size_t bytes) {
+        void* p = nullptr;
+        if (!ok()) return nullptr;
+        cuda(cudaMalloc(&p, bytes), "cudaMalloc");
+        if (!ok()) return nullptr;
+        m->owned.push_back(p);
+        return p;
+    }
+    void copy(float* dst, const float* src, long long count) {
+        if (ok()) cuda(cudaMemcpyAsync(dst, src, (size_t)count * 4, cudaMemcpyDeviceToDevice, st), "copy");
+    }
+    template <typename... KArgs, typename... Args> void launch(void (*kernel)(KArgs...), unsigned grid, unsigned block, Args... args) {
+        if (ok() && launch_on(st, kernel, grid, block, args...) != CAR_OK) fail(CAR_ERR_CUDA, g_car_err);
+    }
+    // one launch of a grid-stride packing kernel over `total` elements
+    template <typename... KArgs, typename... Args> void pack(void (*kernel)(KArgs...), long long total, Args... args) {
+        if (ok()) launch(kernel, gsz(total), 256, args...);
+    }
+    float* f32(const float* src, long long count) {
+        float* p = (float*)alloc((size_t)count * 4);
+        copy(p, src, count);
+        return p;
+    }
+    float* f32(long long count) { return f32(next(), count); }
+    float* zeros(long long count) {
+        float* p = (float*)alloc((size_t)count * 4);
+        if (ok()) cuda(cudaMemsetAsync(p, 0, (size_t)count * 4, st), "memset");
+        return p;
+    }
+    // split-bf16 weight of the x3 GEMMs: [cout][cin][k][k] -> [cout][k][k][3 cin_pad] = [ w_hi | w_hi | w_lo ] per tap
+    bf16* x3(const float* src, int cout, int cin, int k, int cin_pad) {
+        const long long n3 = (long long)cout * k * k * cin_pad;
+        bf16* w3 = (bf16*)alloc((size_t)n3 * 3 * 2);
+        pack(conv_weight_pack_x3_kernel, n3, src, w3, cout, cin, k, k, cin_pad);
+        return w3;
+    }
+    bf16* x3(int cout, int cin, int k, int cin_pad) { return x3(next(), cout, cin, k, cin_pad); }
+    // the create's last step: the whole list was read and nothing failed
+    int finish() {
+        if (ok() && i != n) fail(CAR_ERR_ARG, "tensor list length does not match the architecture");
+        return rc;
+    }
+};
+
 // =========================================================================================================
 // DINOv2 control encoder
 // =========================================================================================================
-struct CarDino {
+struct CarDino : CarOwned {
     CarDinoDesc d;
-    std::vector<void*> owned;
     // bf16 GEMM-ready weights
     bf16* w_patch;                      // [C][kpad]  (k = 3 * patch^2 = 588 -> 608 for DINOv2, 768 for ViT-S/16)
     int kpatch, kpad;
@@ -86,7 +177,6 @@ struct CarDino {
     std::vector<Layer> L;
     bf16 *ad_fc1, *ad_fc2;              // adapter_mlp (bias-free)
     int ad_dim;
-    Arena ws;
 };
 
 template <typename TI>
@@ -156,15 +246,12 @@ extern "C" int car_dino_create(const CarDinoDesc* desc, const CarDinoWeights* w,
         m->ad_fc1 = (bf16*)cv(w->adapter_fc1, (long long)d.adapter_out_dim * C);
         m->ad_fc2 = (bf16*)cv(w->adapter_fc2, (long long)d.adapter_out_dim * d.adapter_out_dim);
     }
-    if (r != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return r; }
+    if (r != CAR_OK) { delete m; return r; }
     *out = m;
     return CAR_OK;
 }
 
 extern "C" int car_dino_destroy(CarDino* m) {
-    if (!m) return CAR_OK;
-    for (void* p : m->owned) cudaFree(p);
-    m->ws.release();
     delete m;
     return CAR_OK;
 }
@@ -276,9 +363,8 @@ struct NormW { bf16 *w, *b; int c; float *wf, *bff; };                          
 struct ResW { NormW n1, n2; ConvW c1, c2, nin; bool has_nin; };
 struct AttnW { NormW n; ConvW q, k, v, o; };
 
-struct CarVQ {
+struct CarVQ : CarOwned {
     CarVQDesc d;
-    std::vector<void*> owned;
     float* codebook_n;                 // l2-normalised fp32 [n_codes][e_dim]
     // decoder
     ConvW post_quant, d_conv_in, d_conv_out; NormW d_norm_out;
@@ -288,107 +374,45 @@ struct CarVQ {
     ConvW quant_conv, e_conv_in, e_conv_out; NormW e_norm_out;
     ResW e_mid0, e_mid2; AttnW e_mid1;
     std::vector<std::vector<ResW>> e_res; std::vector<std::vector<AttnW>> e_attn; std::vector<ConvW> e_down; std::vector<bool> e_has_down;
-    Arena ws;
 };
 
-struct TensorCursor { const void* const* t; int n; int i; };
-
-static int keep_f32(CarVQ* m, cudaStream_t st, const void* src, long long n, float** dst) {
-    CAR_CUDA(cudaMalloc((void**)dst, (size_t)n * 4));
-    m->owned.push_back(*dst);
-    CAR_CUDA(cudaMemcpyAsync(*dst, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
-    return CAR_OK;
+static bf16* take_bf16(TensorReader& tc, const float* src, long long n) {
+    bf16* p = (bf16*)tc.alloc((size_t)n * 2);
+    tc.pack(cast_to_bf16_kernel<float>, n, src, p, n);
+    return p;
 }
-static int take_conv(CarVQ* m, cudaStream_t st, TensorCursor& tc, int cout, int cin, int k, ConvW* c, bool x3 = false) {
-    if (tc.i + 2 > tc.n) CAR_FAIL(CAR_ERR_ARG, "tensor list too short");
+static void take_conv(TensorReader& tc, int cout, int cin, int k, ConvW* c, bool x3 = false) {
     c->cin = cin; c->cout = cout; c->k = k; c->cin_pad = (cin + 31) & ~31; c->w3 = nullptr; c->bf = nullptr;
+    const float* w = tc.next();
+    const float* b = tc.next();
     if (x3) {   // fp32-grade encoder path (vision.cuh "x3"): [w_hi | w_hi | w_lo] per tap + the fp32 bias
-        const long long n3 = (long long)cout * k * k * c->cin_pad;
-        CAR_CUDA(cudaMalloc((void**)&c->w3, (size_t)n3 * 3 * 2));
-        m->owned.push_back(c->w3);
-        CAR_LAUNCH(conv_weight_pack_x3_kernel, gsz(n3), 256, 0, st, (const float*)tc.t[tc.i], c->w3, cout, cin, k, k, c->cin_pad);
-        CAR_TRY(keep_f32(m, st, tc.t[tc.i + 1], cout, &c->bf));
+        c->w3 = tc.x3(w, cout, cin, k, c->cin_pad);
+        c->bf = tc.f32(b, cout);
     }
     const long long n = (long long)cout * k * k * c->cin_pad;
-    CAR_CUDA(cudaMalloc((void**)&c->w, (size_t)n * 2));
-    m->owned.push_back(c->w);
-    CAR_LAUNCH((conv_weight_pack_kernel<float>), gsz(n), 256, 0, st, (const float*)tc.t[tc.i], c->w, cout, cin, k, k, c->cin_pad);
-    CAR_TRY(to_bf16<float>(st, m->owned, tc.t[tc.i + 1], cout, &c->b));
-    tc.i += 2;
-    return CAR_OK;
+    c->w = (bf16*)tc.alloc((size_t)n * 2);
+    tc.pack(conv_weight_pack_kernel<float>, n, w, c->w, cout, cin, k, k, c->cin_pad);
+    c->b = take_bf16(tc, b, cout);
 }
-static int take_norm(CarVQ* m, cudaStream_t st, TensorCursor& tc, int c, NormW* nw, bool x3 = false) {
-    if (tc.i + 2 > tc.n) CAR_FAIL(CAR_ERR_ARG, "tensor list too short");
+static void take_norm(TensorReader& tc, int c, NormW* nw, bool x3 = false) {
     nw->c = c; nw->wf = nullptr; nw->bff = nullptr;
-    if (x3) { CAR_TRY(keep_f32(m, st, tc.t[tc.i], c, &nw->wf)); CAR_TRY(keep_f32(m, st, tc.t[tc.i + 1], c, &nw->bff)); }
-    CAR_TRY(to_bf16<float>(st, m->owned, tc.t[tc.i], c, &nw->w));
-    CAR_TRY(to_bf16<float>(st, m->owned, tc.t[tc.i + 1], c, &nw->b));
-    tc.i += 2;
-    return CAR_OK;
+    const float* w = tc.next();
+    const float* b = tc.next();
+    if (x3) { nw->wf = tc.f32(w, c); nw->bff = tc.f32(b, c); }
+    nw->w = take_bf16(tc, w, c);
+    nw->b = take_bf16(tc, b, c);
 }
 // canonical order inside a ResnetBlock: norm1.{w,b} conv1.{w,b} norm2.{w,b} conv2.{w,b} [nin_shortcut.{w,b}]
-static int take_res(CarVQ* m, cudaStream_t st, TensorCursor& tc, int cin, int cout, ResW* r, bool x3 = false) {
-    CAR_TRY(take_norm(m, st, tc, cin, &r->n1, x3)); CAR_TRY(take_conv(m, st, tc, cout, cin, 3, &r->c1, x3));
-    CAR_TRY(take_norm(m, st, tc, cout, &r->n2, x3)); CAR_TRY(take_conv(m, st, tc, cout, cout, 3, &r->c2, x3));
+static void take_res(TensorReader& tc, int cin, int cout, ResW* r, bool x3 = false) {
+    take_norm(tc, cin, &r->n1, x3); take_conv(tc, cout, cin, 3, &r->c1, x3);
+    take_norm(tc, cout, &r->n2, x3); take_conv(tc, cout, cout, 3, &r->c2, x3);
     r->has_nin = cin != cout;
-    if (r->has_nin) CAR_TRY(take_conv(m, st, tc, cout, cin, 1, &r->nin, x3));
-    return CAR_OK;
+    if (r->has_nin) take_conv(tc, cout, cin, 1, &r->nin, x3);
 }
 // AttnBlock: norm.{w,b} q.{w,b} k.{w,b} v.{w,b} proj_out.{w,b}
-static int take_attn(CarVQ* m, cudaStream_t st, TensorCursor& tc, int c, AttnW* a, bool x3 = false) {
-    CAR_TRY(take_norm(m, st, tc, c, &a->n, x3)); CAR_TRY(take_conv(m, st, tc, c, c, 1, &a->q, x3)); CAR_TRY(take_conv(m, st, tc, c, c, 1, &a->k, x3));
-    CAR_TRY(take_conv(m, st, tc, c, c, 1, &a->v, x3)); CAR_TRY(take_conv(m, st, tc, c, c, 1, &a->o, x3));
-    return CAR_OK;
-}
-
-static int vq_build(CarVQ* m, const void* const* tensors, int n, cudaStream_t st) {
-    const CarVQDesc& d = m->d;
-    TensorCursor tc{tensors, n, 0};
-    const int ch = d.ch, nres = d.n_levels, nrb = d.num_res_blocks;
-    // ---- encoder (vq_model.py:65-125)
-    CAR_TRY(take_conv(m, st, tc, ch, 3, 3, &m->e_conv_in, true));
-    m->e_res.resize(nres); m->e_attn.resize(nres); m->e_down.resize(nres); m->e_has_down.assign(nres, false);
-    int block_in = ch;
-    for (int lvl = 0; lvl < nres; ++lvl) {
-        block_in = ch * (lvl == 0 ? 1 : d.ch_mult[lvl - 1]);
-        const int block_out = ch * d.ch_mult[lvl];
-        for (int b = 0; b < nrb; ++b) {
-            ResW r; CAR_TRY(take_res(m, st, tc, block_in, block_out, &r, true)); m->e_res[lvl].push_back(r);
-            block_in = block_out;
-            if (lvl == nres - 1) { AttnW a; CAR_TRY(take_attn(m, st, tc, block_in, &a, true)); m->e_attn[lvl].push_back(a); }
-        }
-        if (lvl != nres - 1) { CAR_TRY(take_conv(m, st, tc, block_in, block_in, 3, &m->e_down[lvl], true)); m->e_has_down[lvl] = true; }
-    }
-    CAR_TRY(take_res(m, st, tc, block_in, block_in, &m->e_mid0, true)); CAR_TRY(take_attn(m, st, tc, block_in, &m->e_mid1, true));
-    CAR_TRY(take_res(m, st, tc, block_in, block_in, &m->e_mid2, true));
-    CAR_TRY(take_norm(m, st, tc, block_in, &m->e_norm_out, true)); CAR_TRY(take_conv(m, st, tc, d.z_channels, block_in, 3, &m->e_conv_out, true));
-    // ---- decoder (vq_model.py:129-195)
-    block_in = ch * d.ch_mult[nres - 1];
-    CAR_TRY(take_conv(m, st, tc, block_in, d.z_channels, 3, &m->d_conv_in));
-    CAR_TRY(take_res(m, st, tc, block_in, block_in, &m->d_mid0)); CAR_TRY(take_attn(m, st, tc, block_in, &m->d_mid1));
-    CAR_TRY(take_res(m, st, tc, block_in, block_in, &m->d_mid2));
-    m->d_res.resize(nres); m->d_attn.resize(nres); m->d_up.resize(nres); m->d_has_up.assign(nres, false);
-    for (int idx = 0; idx < nres; ++idx) {
-        const int lvl = nres - 1 - idx;
-        const int block_out = ch * d.ch_mult[lvl];
-        for (int b = 0; b < nrb + 1; ++b) {
-            ResW r; CAR_TRY(take_res(m, st, tc, block_in, block_out, &r)); m->d_res[idx].push_back(r);
-            block_in = block_out;
-            if (lvl == nres - 1) { AttnW a; CAR_TRY(take_attn(m, st, tc, block_in, &a)); m->d_attn[idx].push_back(a); }
-        }
-        if (lvl != 0) { CAR_TRY(take_conv(m, st, tc, block_in, block_in, 3, &m->d_up[idx])); m->d_has_up[idx] = true; }
-    }
-    CAR_TRY(take_norm(m, st, tc, block_in, &m->d_norm_out)); CAR_TRY(take_conv(m, st, tc, 3, block_in, 3, &m->d_conv_out));
-    // ---- quantiser + 1x1 convs
-    if (tc.i + 1 > tc.n) CAR_FAIL(CAR_ERR_ARG, "tensor list too short");
-    CAR_CUDA(cudaMalloc((void**)&m->codebook_n, (size_t)d.codebook_size * d.embed_dim * 4));
-    m->owned.push_back(m->codebook_n);
-    CAR_LAUNCH(codebook_normalize_kernel, (d.codebook_size + 255) / 256, 256, 0, st, (const float*)tc.t[tc.i], m->codebook_n, d.codebook_size, d.embed_dim);
-    tc.i += 1;
-    CAR_TRY(take_conv(m, st, tc, d.embed_dim, d.z_channels, 1, &m->quant_conv, true));
-    CAR_TRY(take_conv(m, st, tc, d.z_channels, d.embed_dim, 1, &m->post_quant));
-    if (tc.i != tc.n) CAR_FAIL(CAR_ERR_ARG, "tensor list length does not match the VQ architecture");
-    return CAR_OK;
+static void take_attn(TensorReader& tc, int c, AttnW* a, bool x3 = false) {
+    take_norm(tc, c, &a->n, x3); take_conv(tc, c, c, 1, &a->q, x3); take_conv(tc, c, c, 1, &a->k, x3);
+    take_conv(tc, c, c, 1, &a->v, x3); take_conv(tc, c, c, 1, &a->o, x3);
 }
 
 extern "C" int car_vq_create(const CarVQDesc* desc, const void* const* tensors, int32_t n_tensors, void* stream, CarVQ** out) {
@@ -396,15 +420,55 @@ extern "C" int car_vq_create(const CarVQDesc* desc, const void* const* tensors, 
     if (desc->embed_dim > 8 || desc->n_levels > 8 || desc->ch % 32) CAR_FAIL(CAR_ERR_UNSUPPORTED, "unsupported VQ shape");
     CarVQ* m = new CarVQ();
     m->d = *desc;
-    int r = vq_build(m, tensors, n_tensors, (cudaStream_t)stream);
-    if (r != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return r; }
+    const CarVQDesc& d = m->d;
+    TensorReader tc(__func__, tensors, n_tensors, stream, m);
+    const int ch = d.ch, nres = d.n_levels, nrb = d.num_res_blocks;
+    // ---- encoder (vq_model.py:65-125)
+    take_conv(tc, ch, 3, 3, &m->e_conv_in, true);
+    m->e_res.resize(nres); m->e_attn.resize(nres); m->e_down.resize(nres); m->e_has_down.assign(nres, false);
+    int block_in = ch;
+    for (int lvl = 0; lvl < nres; ++lvl) {
+        block_in = ch * (lvl == 0 ? 1 : d.ch_mult[lvl - 1]);
+        const int block_out = ch * d.ch_mult[lvl];
+        for (int b = 0; b < nrb; ++b) {
+            ResW r; take_res(tc, block_in, block_out, &r, true); m->e_res[lvl].push_back(r);
+            block_in = block_out;
+            if (lvl == nres - 1) { AttnW a; take_attn(tc, block_in, &a, true); m->e_attn[lvl].push_back(a); }
+        }
+        if (lvl != nres - 1) { take_conv(tc, block_in, block_in, 3, &m->e_down[lvl], true); m->e_has_down[lvl] = true; }
+    }
+    take_res(tc, block_in, block_in, &m->e_mid0, true); take_attn(tc, block_in, &m->e_mid1, true);
+    take_res(tc, block_in, block_in, &m->e_mid2, true);
+    take_norm(tc, block_in, &m->e_norm_out, true); take_conv(tc, d.z_channels, block_in, 3, &m->e_conv_out, true);
+    // ---- decoder (vq_model.py:129-195)
+    block_in = ch * d.ch_mult[nres - 1];
+    take_conv(tc, block_in, d.z_channels, 3, &m->d_conv_in);
+    take_res(tc, block_in, block_in, &m->d_mid0); take_attn(tc, block_in, &m->d_mid1);
+    take_res(tc, block_in, block_in, &m->d_mid2);
+    m->d_res.resize(nres); m->d_attn.resize(nres); m->d_up.resize(nres); m->d_has_up.assign(nres, false);
+    for (int idx = 0; idx < nres; ++idx) {
+        const int lvl = nres - 1 - idx;
+        const int block_out = ch * d.ch_mult[lvl];
+        for (int b = 0; b < nrb + 1; ++b) {
+            ResW r; take_res(tc, block_in, block_out, &r); m->d_res[idx].push_back(r);
+            block_in = block_out;
+            if (lvl == nres - 1) { AttnW a; take_attn(tc, block_in, &a); m->d_attn[idx].push_back(a); }
+        }
+        if (lvl != 0) { take_conv(tc, block_in, block_in, 3, &m->d_up[idx]); m->d_has_up[idx] = true; }
+    }
+    take_norm(tc, block_in, &m->d_norm_out); take_conv(tc, 3, block_in, 3, &m->d_conv_out);
+    // ---- quantiser + 1x1 convs
+    const float* codebook = tc.next();
+    m->codebook_n = (float*)tc.alloc((size_t)d.codebook_size * d.embed_dim * 4);
+    tc.launch(codebook_normalize_kernel, (d.codebook_size + 255) / 256, 256, codebook, m->codebook_n, d.codebook_size, d.embed_dim);
+    take_conv(tc, d.embed_dim, d.z_channels, 1, &m->quant_conv, true);
+    take_conv(tc, d.z_channels, d.embed_dim, 1, &m->post_quant);
+    const int rc = tc.finish();
+    if (rc != CAR_OK) { delete m; return rc; }
     *out = m;
     return CAR_OK;
 }
 extern "C" int car_vq_destroy(CarVQ* m) {
-    if (!m) return CAR_OK;
-    for (void* p : m->owned) cudaFree(p);
-    m->ws.release();
     delete m;
     return CAR_OK;
 }
@@ -781,12 +845,10 @@ extern "C" int car_left_pad_captions(const void* embs, const int64_t* masks, int
 // HED soft-edge detector (row f3): condition/hed.py:17-84 — 13 ReLU 3x3 convolutions in five blocks with 2x2 max-pooling between
 // them, a 1x1 projection per block, bilinear resize of the five maps, mean, sigmoid.  fp32 in the reference => fp32-grade here.
 // ---------------------------------------------------------------------------------------------------------
-struct CarHED {
-    std::vector<void*> owned;
+struct CarHED : CarOwned {
     std::vector<ConvW> conv;           // 13, in forward order
     float* norm;                       // [3]
     float* pw[5]; float* pb[5];        // projection weights [C] / bias [1]
-    Arena ws;
 };
 static const int HED_BLK[5][3] = {{3, 64, 2}, {64, 128, 2}, {128, 256, 3}, {256, 512, 3}, {512, 512, 3}};
 
@@ -794,44 +856,29 @@ static const int HED_BLK[5][3] = {{3, 64, 2}, {64, 128, 2}, {128, 256, 3}, {256,
 extern "C" int car_hed_create(const void* const* tensors, int32_t n_tensors, void* stream, CarHED** out) {
     if (!tensors || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
     if (n_tensors != 1 + 2 * 13 + 2 * 5) CAR_FAIL(CAR_ERR_ARG, "HED expects 37 tensors (norm, 13 x (weight, bias), 5 x (projection weight, bias))");
-    cudaStream_t st = (cudaStream_t)stream;
     CarHED* m = new CarHED();
-    int rc = CAR_OK, ti = 0;
-    auto keep = [&](const void* src, long long n, float** dst) {
-        if (rc != CAR_OK) return;
-        if (cudaMalloc((void**)dst, (size_t)n * 4) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_hed_create: cudaMalloc failed"; return; }
-        m->owned.push_back(*dst);
-        if (cudaMemcpyAsync(*dst, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_hed_create: copy failed"; }
-    };
-    keep(tensors[ti++], 3, &m->norm);
-    for (int b = 0; b < 5 && rc == CAR_OK; ++b) {
+    TensorReader tc(__func__, tensors, n_tensors, stream, m);
+    m->norm = tc.f32(3);
+    for (int b = 0; b < 5; ++b) {
         int cin = HED_BLK[b][0];
         const int cout = HED_BLK[b][1];
-        for (int i = 0; i < HED_BLK[b][2] && rc == CAR_OK; ++i) {
+        for (int i = 0; i < HED_BLK[b][2]; ++i) {
             ConvW c;
             memset(&c, 0, sizeof(c));
             c.cin = cin; c.cout = cout; c.k = 3; c.cin_pad = (cin + 31) & ~31;
-            const long long n3 = (long long)cout * 9 * c.cin_pad;
-            if (cudaMalloc((void**)&c.w3, (size_t)n3 * 3 * 2) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_hed_create: cudaMalloc failed"; break; }
-            m->owned.push_back(c.w3);
-            conv_weight_pack_x3_kernel<<<gsz(n3), 256, 0, st>>>((const float*)tensors[ti], c.w3, cout, cin, 3, 3, c.cin_pad);
-            keep(tensors[ti + 1], cout, &c.bf);
-            ti += 2;
+            c.w3 = tc.x3(cout, cin, 3, c.cin_pad);
+            c.bf = tc.f32(cout);
             m->conv.push_back(c);
             cin = cout;
         }
-        keep(tensors[ti], cout, &m->pw[b]); keep(tensors[ti + 1], 1, &m->pb[b]);
-        ti += 2;
+        m->pw[b] = tc.f32(cout); m->pb[b] = tc.f32(1);
     }
-    if (rc == CAR_OK && cudaGetLastError() != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_hed_create: weight packing failed"; }
-    if (rc != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return rc; }
+    const int rc = tc.finish();
+    if (rc != CAR_OK) { delete m; return rc; }
     *out = m;
     return CAR_OK;
 }
 extern "C" int car_hed_destroy(CarHED* m) {
-    if (!m) return CAR_OK;
-    for (void* p : m->owned) cudaFree(p);
-    m->ws.release();
     delete m;
     return CAR_OK;
 }
@@ -888,11 +935,9 @@ extern "C" int car_hed_forward(CarHED* m, const float* img, int32_t B, int32_t H
 // the reference => fp32-grade here: fp32 activations, every convolution but the head on the split-bf16 window GEMM (lineart.cuh).
 // ---------------------------------------------------------------------------------------------------------
 struct LaConv { bf16* w3; float* b; int cin3, cout; };   // cin3 = 3 * Cin_pad (channels per pixel of the S3 source)
-struct CarLineArt {
-    std::vector<void*> owned;
+struct CarLineArt : CarOwned {
     LaConv stem, down[2], res[6], up[2];              // up[i].w3: the four parity classes back to back (lineart.cuh)
     float *head_w, *head_b;                           // [64][7][7], [1]
-    Arena ws;
 };
 
 // tensors (fp32, device), state-dict order: model0.1, model1.0, model1.3, model2.{0,1,2}.conv_block.{1,5}, model3.0, model3.3,
@@ -900,35 +945,20 @@ struct CarLineArt {
 extern "C" int car_lineart_create(const void* const* tensors, int32_t n_tensors, void* stream, CarLineArt** out) {
     if (!tensors || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
     if (n_tensors != 24) CAR_FAIL(CAR_ERR_ARG, "LineArt expects 24 tensors (12 x (weight, bias) in state-dict order)");
-    for (int i = 0; i < 24; ++i)
-        if (!tensors[i]) CAR_FAIL(CAR_ERR_ARG, "null tensor");
-    cudaStream_t st = (cudaStream_t)stream;
     CarLineArt* m = new CarLineArt();
-    int rc = CAR_OK, ti = 0;
-    auto alloc = [&](void** p, size_t bytes) {
-        if (rc != CAR_OK) return;
-        if (cudaMalloc(p, bytes) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_lineart_create: cudaMalloc failed"; *p = nullptr; return; }
-        m->owned.push_back(*p);
-    };
-    auto keep = [&](const void* src, long long n, float** dst) {
-        alloc((void**)dst, (size_t)n * 4);
-        if (rc == CAR_OK && cudaMemcpyAsync(*dst, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_lineart_create: copy failed"; }
-    };
+    TensorReader tc(__func__, tensors, n_tensors, stream, m);
     auto conv = [&](LaConv& c, int cin, int cin_pad, int cout, int k) {
         c.cin3 = 3 * cin_pad; c.cout = cout;
-        const long long n3 = (long long)cout * k * k * cin_pad;
-        alloc((void**)&c.w3, (size_t)n3 * 3 * 2);
-        if (rc == CAR_OK) conv_weight_pack_x3_kernel<<<gsz(n3), 256, 0, st>>>((const float*)tensors[ti], c.w3, cout, cin, k, k, cin_pad);
-        keep(tensors[ti + 1], cout, &c.b);
-        ti += 2;
+        c.w3 = tc.x3(cout, cin, k, cin_pad);
+        c.b = tc.f32(cout);
     };
     auto convT = [&](LaConv& c, int cin, int cout) {
         c.cin3 = 3 * cin; c.cout = cout;
         const long long n3 = 9LL * cout * cin;
-        alloc((void**)&c.w3, (size_t)n3 * 3 * 2);
-        if (rc == CAR_OK) convT_weight_pack_x3_kernel<<<gsz(n3), 256, 0, st>>>((const float*)tensors[ti], c.w3, cin, cout, cin);
-        keep(tensors[ti + 1], cout, &c.b);
-        ti += 2;
+        const float* w = tc.next();
+        c.w3 = (bf16*)tc.alloc((size_t)n3 * 3 * 2);
+        tc.pack(convT_weight_pack_x3_kernel, n3, w, c.w3, cin, cout, cin);
+        c.b = tc.f32(cout);
     };
     conv(m->stem, 3, 8, 64, 7);                       // 3 input channels padded to 8 (16-byte chunks), not 32
     conv(m->down[0], 64, 64, 128, 3);
@@ -936,16 +966,13 @@ extern "C" int car_lineart_create(const void* const* tensors, int32_t n_tensors,
     for (int i = 0; i < 6; ++i) conv(m->res[i], 256, 256, 256, 3);
     convT(m->up[0], 256, 128);
     convT(m->up[1], 128, 64);
-    keep(tensors[ti], 64 * 49, &m->head_w); keep(tensors[ti + 1], 1, &m->head_b);
-    if (rc == CAR_OK && cudaGetLastError() != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_lineart_create: weight packing failed"; }
-    if (rc != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return rc; }
+    m->head_w = tc.f32(64 * 49); m->head_b = tc.f32(1);
+    const int rc = tc.finish();
+    if (rc != CAR_OK) { delete m; return rc; }
     *out = m;
     return CAR_OK;
 }
 extern "C" int car_lineart_destroy(CarLineArt* m) {
-    if (!m) return CAR_OK;
-    for (void* p : m->owned) cudaFree(p);
-    m->ws.release();
     delete m;
     return CAR_OK;
 }
@@ -1050,16 +1077,14 @@ struct DptDecoder {                                     // fusion stages and dep
     DptLin head0, head2;
     float *head4w, *head4b;
 };
-struct CarDpt {
+struct CarDpt : CarOwned {
     CarDptDesc d;
-    std::vector<void*> owned;
     DptLin patch;
     float *cls, *pos;                                   // [C], [1 + g^2][C]
     using Layer = DptLayer;
     std::vector<Layer> L;
     DptLin proj[4], resize[4], readout[4], neck[4];     // resize: ConvTranspose2d GEMM (stages 0, 1), 3x3 stride-2 convolution (3)
     DptDecoder dec;
-    Arena ws;
 };
 static const int DPT_FACTOR[4] = {4, 2, 1, 0};         // 0: the 0.5 stage (3x3 stride-2 convolution)
 
@@ -1075,65 +1100,48 @@ extern "C" int car_dpt_create(const CarDptDesc* desc, const void* const* tensors
     }
     if (d.fusion <= 0 || d.fusion % 128) CAR_FAIL(CAR_ERR_UNSUPPORTED, "fusion size must be a positive multiple of 128");
     if (n_tensors != 4 + 16 * d.n_layers + 74) CAR_FAIL(CAR_ERR_ARG, "DPT expects 4 + 16 * n_layers + 74 tensors in state-dict order");
-    for (int i = 0; i < n_tensors; ++i)
-        if (!tensors[i]) CAR_FAIL(CAR_ERR_ARG, "null tensor");
-    cudaStream_t st = (cudaStream_t)stream;
     CarDpt* m = new CarDpt();
     m->d = d;
     const int C = d.hidden, F = d.fusion;
-    int rc = CAR_OK, ti = 0;
-    auto alloc = [&](void** p, size_t bytes) {
-        if (rc != CAR_OK) return;
-        if (cudaMalloc(p, bytes) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_dpt_create: cudaMalloc failed"; *p = nullptr; return; }
-        m->owned.push_back(*p);
-    };
-    auto copy = [&](float* dst, const void* src, long long n) {
-        if (rc == CAR_OK && cudaMemcpyAsync(dst, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_dpt_create: copy failed"; }
-    };
-    auto keep = [&](long long n, float** dst) {
-        alloc((void**)dst, (size_t)n * 4);
-        copy(*dst, tensors[ti++], n);
-    };
+    TensorReader tc(__func__, tensors, n_tensors, stream, m);
     // weight [n][cin][kh][kw] (kh = kw = 1: nn.Linear) -> W3 [n][kh][kw][3 cin]; then the bias when `bias`
     auto lin = [&](DptLin& L, int n, int cin, int k, bool bias) {
-        L.n = n; L.k = k * k * cin; L.b = nullptr;
-        alloc((void**)&L.w3, (size_t)n * L.k * 3 * 2);
-        if (rc == CAR_OK) conv_weight_pack_x3_kernel<<<gsz((long long)n * L.k), 256, 0, st>>>((const float*)tensors[ti], L.w3, n, cin, k, k, cin);
-        ++ti;
-        if (bias) keep(n, &L.b);
+        L.n = n; L.k = k * k * cin;
+        L.w3 = tc.x3(n, cin, k, cin);
+        L.b = bias ? tc.f32(n) : nullptr;
     };
     // ConvTranspose2d(k = s = f): weight [cin][cin][f][f] -> W3 [f^2 cin][3 cin]; the bias repeated per (ky, kx)
     auto convT = [&](DptLin& L, int cin, int f) {
         L.n = f * f * cin; L.k = cin;
-        alloc((void**)&L.w3, (size_t)L.n * L.k * 3 * 2);
-        if (rc == CAR_OK) dpt_convT_pack_kernel<<<gsz((long long)L.n * L.k), 256, 0, st>>>((const float*)tensors[ti], L.w3, cin, cin, f);
-        ++ti;
-        alloc((void**)&L.b, (size_t)L.n * 4);
-        for (int t = 0; t < f * f; ++t) copy(L.b + (size_t)t * cin, tensors[ti], cin);
-        ++ti;
+        const float* w = tc.next();
+        L.w3 = (bf16*)tc.alloc((size_t)L.n * L.k * 3 * 2);
+        tc.pack(dpt_convT_pack_kernel, (long long)L.n * L.k, w, L.w3, cin, cin, f);
+        const float* b = tc.next();
+        L.b = (float*)tc.alloc((size_t)L.n * 4);
+        for (int t = 0; t < f * f; ++t) tc.copy(L.b + (size_t)t * cin, b, cin);
     };
     // dpt.embeddings
-    keep(C, &m->cls);
-    keep((long long)(1 + d.pos_grid * d.pos_grid) * C, &m->pos);
+    m->cls = tc.f32(C);
+    m->pos = tc.f32((long long)(1 + d.pos_grid * d.pos_grid) * C);
     lin(m->patch, C, 3 * 256, 1, true);                 // [C][3][16][16] read as [C][768]
     // dpt.encoder.layer.{i}: query, key, value (one [3C][3C] GEMM), output.dense, intermediate.dense, output.dense, LN before / after
     m->L.resize(d.n_layers);
-    for (int l = 0; l < d.n_layers && rc == CAR_OK; ++l) {
+    for (int l = 0; l < d.n_layers; ++l) {
         CarDpt::Layer& Ly = m->L[l];
         Ly.qkv.n = 3 * C; Ly.qkv.k = C;
-        alloc((void**)&Ly.qkv.w3, (size_t)3 * C * C * 3 * 2);
-        alloc((void**)&Ly.qkv.b, (size_t)3 * C * 4);
-        for (int j = 0; j < 3 && rc == CAR_OK; ++j) {
-            conv_weight_pack_x3_kernel<<<gsz((long long)C * C), 256, 0, st>>>((const float*)tensors[ti], Ly.qkv.w3 + (size_t)j * C * 3 * C, C, C, 1, 1, C);
-            copy(Ly.qkv.b + (size_t)j * C, tensors[ti + 1], C);
-            ti += 2;
+        Ly.qkv.w3 = (bf16*)tc.alloc((size_t)3 * C * C * 3 * 2);
+        Ly.qkv.b = (float*)tc.alloc((size_t)3 * C * 4);
+        for (int j = 0; j < 3 && tc.ok(); ++j) {
+            const float* w = tc.next();
+            tc.pack(conv_weight_pack_x3_kernel, (long long)C * C, w, Ly.qkv.w3 + (size_t)j * C * 3 * C, C, C, 1, 1, C);
+            tc.copy(Ly.qkv.b + (size_t)j * C, tc.next(), C);
         }
         lin(Ly.o, C, C, 1, true);
         lin(Ly.fc1, d.mlp, C, 1, true);
         lin(Ly.fc2, C, d.mlp, 1, true);
-        keep(C, &Ly.ln1w); keep(C, &Ly.ln1b); keep(C, &Ly.ln2w); keep(C, &Ly.ln2b);
+        Ly.ln1w = tc.f32(C); Ly.ln1b = tc.f32(C); Ly.ln2w = tc.f32(C); Ly.ln2b = tc.f32(C);
     }
-    ti += 2;                                            // dpt.layernorm: applied to last_hidden_state only, which depth does not use
+    tc.skip(2);                                         // dpt.layernorm: applied to last_hidden_state only, which depth does not use
     // neck.reassemble_stage.layers.{i}: projection (1x1), resize
     for (int i = 0; i < 4; ++i) {
         lin(m->proj[i], d.neck[i], C, 1, true);
@@ -1149,17 +1157,13 @@ extern "C" int car_dpt_create(const CarDptDesc* desc, const void* const* tensors
     }
     lin(m->dec.head0, F / 2, F, 3, true);
     lin(m->dec.head2, 32, F / 2, 3, true);
-    keep(32, &m->dec.head4w); keep(1, &m->dec.head4b);
-    if (rc == CAR_OK && ti != n_tensors) { rc = CAR_ERR_ARG; g_car_err = "car_dpt_create: tensor count mismatch"; }
-    if (rc == CAR_OK && cudaGetLastError() != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_dpt_create: weight packing failed"; }
-    if (rc != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return rc; }
+    m->dec.head4w = tc.f32(32); m->dec.head4b = tc.f32(1);
+    const int rc = tc.finish();
+    if (rc != CAR_OK) { delete m; return rc; }
     *out = m;
     return CAR_OK;
 }
 extern "C" int car_dpt_destroy(CarDpt* m) {
-    if (!m) return CAR_OK;
-    for (void* p : m->owned) cudaFree(p);
-    m->ws.release();
     delete m;
     return CAR_OK;
 }
@@ -1349,8 +1353,7 @@ struct MdNorm { float *w, *b; };
 struct MdBlock { DptLin dn, c1, c2, c3; MdNorm dnn, n1, n2, n3; int cin, mid, out, stride; };
 static const int MD_DEPTH[3] = {3, 4, 9}, MD_OUT[3] = {256, 512, 1024};
 constexpr int MD_BLOCKS = 16, MD_C = 768, MD_HEADS = 12, MD_MLP = 3072, MD_F = 256, MD_GRID = 24, MD_NT = 368;
-struct CarMidas {
-    std::vector<void*> owned;
+struct CarMidas : CarOwned {
     float* zero;                                        // [1024] zeros: the bias of the bias-free window convolutions
     DptLin stem;
     MdNorm stem_n;
@@ -1360,7 +1363,6 @@ struct CarMidas {
     DptLayer L[12];
     DptLin readout[2], proj[2], resize4, rn[4];         // act_postprocess{3,4}: readout, 1x1, (3x3/2); scratch.layer{1..4}_rn
     DptDecoder dec;
-    Arena ws;
 };
 
 // tensors (fp32, device), state-dict order of controlar_b200.condition.midas.DPTDepthModel: pretrained.model.{cls_token, pos_embed,
@@ -1369,46 +1371,25 @@ struct CarMidas {
 extern "C" int car_midas_create(const void* const* tensors, int32_t n_tensors, void* stream, CarMidas** out) {
     if (!tensors || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
     if (n_tensors != MD_NT) CAR_FAIL(CAR_ERR_ARG, "MiDaS DPT-Hybrid expects 368 tensors in state-dict order");
-    for (int i = 0; i < n_tensors; ++i)
-        if (!tensors[i]) CAR_FAIL(CAR_ERR_ARG, "null tensor");
-    cudaStream_t st = (cudaStream_t)stream;
     CarMidas* m = new CarMidas();
-    int rc = CAR_OK, ti = 0;
-    auto alloc = [&](void** p, size_t bytes) {
-        if (rc != CAR_OK) return;
-        if (cudaMalloc(p, bytes) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_midas_create: cudaMalloc failed"; *p = nullptr; return; }
-        m->owned.push_back(*p);
-    };
-    auto keep = [&](long long n, float** dst) {
-        alloc((void**)dst, (size_t)n * 4);
-        if (rc == CAR_OK && cudaMemcpyAsync(*dst, tensors[ti], (size_t)n * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_midas_create: copy failed"; }
-        ++ti;
-    };
+    TensorReader tc(__func__, tensors, n_tensors, stream, m);
     auto lin = [&](DptLin& L, int n, int cin, int k, bool bias) {
-        L.n = n; L.k = k * k * cin; L.b = nullptr;
-        alloc((void**)&L.w3, (size_t)n * L.k * 3 * 2);
-        if (rc == CAR_OK) conv_weight_pack_x3_kernel<<<gsz((long long)n * L.k), 256, 0, st>>>((const float*)tensors[ti], L.w3, n, cin, k, k, cin);
-        ++ti;
-        if (bias) keep(n, &L.b);
+        L.n = n; L.k = k * k * cin;
+        L.w3 = tc.x3(n, cin, k, cin);
+        L.b = bias ? tc.f32(n) : nullptr;
     };
     // weight-standardised convolution [n][cin][k][k] -> W3 [n][k][k][3 cin_pad]; the standardised fp32 weight goes through `wsd`,
     // re-used in stream order (its largest user is a 3x3 256 -> 256 convolution)
-    float* wsd = nullptr;
-    alloc((void**)&wsd, (size_t)256 * 256 * 9 * 4);
+    float* wsd = (float*)tc.alloc((size_t)256 * 256 * 9 * 4);
     auto sconv = [&](DptLin& L, int n, int cin, int k, int cin_pad) {
         L.n = n; L.k = k * k * cin_pad; L.b = nullptr;
-        alloc((void**)&L.w3, (size_t)n * L.k * 3 * 2);
-        if (rc == CAR_OK) {
-            midas_ws_kernel<<<n, MD_THREADS, 0, st>>>((const float*)tensors[ti], wsd, cin * k * k, 1e-8);
-            conv_weight_pack_x3_kernel<<<gsz((long long)n * L.k), 256, 0, st>>>(wsd, L.w3, n, cin, k, k, cin_pad);
-        }
-        ++ti;
+        tc.launch(midas_ws_kernel, n, MD_THREADS, tc.next(), wsd, cin * k * k, 1e-8);
+        L.w3 = tc.x3(wsd, n, cin, k, cin_pad);
     };
-    auto norm = [&](MdNorm& N, int c) { keep(c, &N.w); keep(c, &N.b); };
-    alloc((void**)&m->zero, 1024 * 4);
-    if (rc == CAR_OK && cudaMemsetAsync(m->zero, 0, 1024 * 4, st) != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_midas_create: memset failed"; }
-    keep(MD_C, &m->cls);
-    keep((long long)(1 + MD_GRID * MD_GRID) * MD_C, &m->pos);
+    auto norm = [&](MdNorm& N, int c) { N.w = tc.f32(c); N.b = tc.f32(c); };
+    m->zero = tc.zeros(1024);
+    m->cls = tc.f32(MD_C);
+    m->pos = tc.f32((long long)(1 + MD_GRID * MD_GRID) * MD_C);
     sconv(m->stem, 64, 3, 7, 8);                        // 3 input channels padded to 8 (16-byte chunks)
     norm(m->stem_n, 64);
     int cin = 64, bi = 0;
@@ -1425,14 +1406,14 @@ extern "C" int car_midas_create(const void* const* tensors, int32_t n_tensors, v
     lin(m->patch, MD_C, 1024, 1, true);
     for (int l = 0; l < 12; ++l) {                      // blocks.{l}: norm1, attn.qkv (fused), attn.proj, norm2, mlp.fc1, mlp.fc2
         DptLayer& Ly = m->L[l];
-        keep(MD_C, &Ly.ln1w); keep(MD_C, &Ly.ln1b);
+        Ly.ln1w = tc.f32(MD_C); Ly.ln1b = tc.f32(MD_C);
         lin(Ly.qkv, 3 * MD_C, MD_C, 1, true);
         lin(Ly.o, MD_C, MD_C, 1, true);
-        keep(MD_C, &Ly.ln2w); keep(MD_C, &Ly.ln2b);
+        Ly.ln2w = tc.f32(MD_C); Ly.ln2b = tc.f32(MD_C);
         lin(Ly.fc1, MD_MLP, MD_C, 1, true);
         lin(Ly.fc2, MD_C, MD_MLP, 1, true);
     }
-    ti += 4;                                            // norm, head: the ViT's final norm and classifier, unused by the depth map
+    tc.skip(4);                                         // norm, head: the ViT's final norm and classifier, unused by the depth map
     for (int i = 0; i < 2; ++i) {
         lin(m->readout[i], MD_C, 2 * MD_C, 1, true);
         lin(m->proj[i], MD_C, MD_C, 1, true);
@@ -1448,17 +1429,13 @@ extern "C" int car_midas_create(const void* const* tensors, int32_t n_tensors, v
     }
     lin(m->dec.head0, MD_F / 2, MD_F, 3, true);
     lin(m->dec.head2, 32, MD_F / 2, 3, true);
-    keep(32, &m->dec.head4w); keep(1, &m->dec.head4b);
-    if (rc == CAR_OK && ti != n_tensors) { rc = CAR_ERR_ARG; g_car_err = "car_midas_create: tensor count mismatch"; }
-    if (rc == CAR_OK && cudaGetLastError() != cudaSuccess) { rc = CAR_ERR_CUDA; g_car_err = "car_midas_create: weight packing failed"; }
-    if (rc != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return rc; }
+    m->dec.head4w = tc.f32(32); m->dec.head4b = tc.f32(1);
+    const int rc = tc.finish();
+    if (rc != CAR_OK) { delete m; return rc; }
     *out = m;
     return CAR_OK;
 }
 extern "C" int car_midas_destroy(CarMidas* m) {
-    if (!m) return CAR_OK;
-    for (void* p : m->owned) cudaFree(p);
-    m->ws.release();
     delete m;
     return CAR_OK;
 }

@@ -7,7 +7,7 @@ from typing import List
 import torch
 
 from . import _lib
-from ._lib import check, cur_stream, dtype_code, _ptr, _ptr_array
+from ._lib import check, cur_stream, dtype_code, param_signature, _ptr, _ptr_array
 
 
 class CarDinoDesc(C.Structure):
@@ -46,10 +46,6 @@ _PROTOS = {
 _lib.PROTOTYPES.update(_PROTOS)
 
 
-def _sig(params) -> tuple:
-    return tuple((p.data_ptr(), p._version, p.dtype, str(p.device)) for p in params)
-
-
 # ---------------------------------------------------------------------------------------------------------------
 # DINOv2
 # ---------------------------------------------------------------------------------------------------------------
@@ -74,12 +70,11 @@ def _on_module_device(attr):
     return deco
 
 
-class DinoHandle(_lib.NativeHandle):
+class DinoHandle(_lib.ModuleHandle):
     def __init__(self, adapter, adapter_mlp=None):
+        super().__init__("car_dino_destroy")
         self.lib = _lib.lib()
         self.adapter, self.adapter_mlp = adapter, adapter_mlp
-        self.handle = C.c_void_p()
-        self.sig = None
         self._build()
 
     def _params(self):
@@ -143,17 +138,15 @@ class DinoHandle(_lib.NativeHandle):
         mode = 0 if (is_vit or self.adapter.condition_type in ("canny", "seg")) else 1
         d = CarDinoDesc(dtype=dtype_code(dt), hidden=m.hidden, heads=m.heads, layers=m.n_layers, patch=m.patch,
                         pos_grid=m.pos_grid, resize_mode=mode, adapter_out_dim=out_dim, eps=m.eps)
-        if self.handle:
-            self.lib.car_dino_destroy(self.handle)
-            self.handle = C.c_void_p()
+        self.close()
         check(self.lib.car_dino_create(C.byref(d), C.byref(w), cur_stream(), C.byref(self.handle)), "car_dino_create")
         torch.cuda.current_stream().synchronize()     # conversions read `keep` tensors; safe to drop afterwards
         self.dtype, self.hidden, self.out_dim = dt, m.hidden, out_dim
-        self.sig = _sig(self._params())
+        self.sig = param_signature(self._params())
 
     @_on_module_device("adapter")
     def forward(self, x: torch.Tensor, apply_mlp: bool) -> torch.Tensor:
-        if _sig(self._params()) != self.sig:
+        if param_signature(self._params()) != self.sig:
             self._build()
         B, _, H, W = x.shape
         x = x.to(self.dtype).contiguous()
@@ -163,13 +156,6 @@ class DinoHandle(_lib.NativeHandle):
               "car_dino_forward")
         self._keep = x
         return out.to(self.dtype)
-
-    def __del__(self):
-        try:
-            if self.handle:
-                self.lib.car_dino_destroy(self.handle)
-        except Exception:
-            pass
 
 
 def dinov2_forward(adapter, x: torch.Tensor) -> torch.Tensor:
@@ -185,7 +171,7 @@ def dinov2_forward(adapter, x: torch.Tensor) -> torch.Tensor:
 # VQGAN
 # ---------------------------------------------------------------------------------------------------------------
 def vq_tensor_order(vq) -> List[torch.Tensor]:
-    """Canonical order consumed by car_vq_create (csrc/car_vision.cu: vq_build)."""
+    """Canonical order consumed by car_vq_create (csrc/car_vision.cu: car_vq_create)."""
     out: List[torch.Tensor] = []
 
     def conv(c): out.extend([c.weight, c.bias])
@@ -224,12 +210,11 @@ def vq_tensor_order(vq) -> List[torch.Tensor]:
     return out
 
 
-class VQHandle(_lib.NativeHandle):
+class VQHandle(_lib.ModuleHandle):
     def __init__(self, vq):
+        super().__init__("car_vq_destroy")
         self.lib = _lib.lib()
         self.vq = vq
-        self.handle = C.c_void_p()
-        self.sig = None
         self._build()
 
     @_on_module_device("vq")
@@ -243,18 +228,16 @@ class VQHandle(_lib.NativeHandle):
         assert list(cfg.encoder_ch_mult) == list(cfg.decoder_ch_mult)
         for i, v in enumerate(cfg.decoder_ch_mult):
             d.ch_mult[i] = int(v)
-        if self.handle:
-            self.lib.car_vq_destroy(self.handle)
-            self.handle = C.c_void_p()
+        self.close()
         check(self.lib.car_vq_create(C.byref(d), C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(self.handle)),
               "car_vq_create")
         torch.cuda.current_stream().synchronize()
-        self.sig = _sig(vq_tensor_order(vq))
+        self.sig = param_signature(vq_tensor_order(vq))
         self.down = 2 ** (len(cfg.decoder_ch_mult) - 1)
         self.e_dim = cfg.codebook_embed_dim
 
     def _fresh(self):
-        if _sig(vq_tensor_order(self.vq)) != self.sig:
+        if param_signature(vq_tensor_order(self.vq)) != self.sig:
             self._build()
 
     @_on_module_device("vq")
@@ -287,13 +270,6 @@ class VQHandle(_lib.NativeHandle):
         check(self.lib.car_vq_encode(self.handle, _ptr(img), B, H, W, _ptr(idx), _ptr(quant), cur_stream()), "car_vq_encode")
         self._keep = img
         return quant, idx
-
-    def __del__(self):
-        try:
-            if self.handle:
-                self.lib.car_vq_destroy(self.handle)
-        except Exception:
-            pass
 
 
 def resize_bilinear_aa(x: torch.Tensor, size) -> torch.Tensor:

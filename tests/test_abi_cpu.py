@@ -61,6 +61,43 @@ def test_attention_ops_reject_bad_arguments_before_any_launch():
         assert l.car_last_error(), change
 
 
+def test_tensor_list_creates_reject_bad_lists_before_any_cuda_call():
+    """The detector and tokenizer creates take a flat list of device pointers from the caller.  A null list, a null `out`, a wrong
+    length, and the right length of null entries must each be refused with a message that names the entry point, before any
+    allocation or launch (no entry is ever a valid pointer, so nothing is dereferenced)."""
+    import ctypes as C
+    import torch
+    from controlar_b200 import _lib, vision
+    from controlar_b200.tokenizer.tokenizer_image.vq_model import VQ_models
+    l = _lib.lib()
+    dpt = _lib.CarDptDesc(hidden=64, n_layers=4, n_heads=1, mlp=64, fusion=128, pos_grid=2, ln_eps=1e-12)
+    for i in range(4):
+        dpt.out_indices[i], dpt.neck[i] = i, 64
+    with torch.device("meta"):
+        vq_model = VQ_models["VQ-16"](codebook_size=16384, codebook_embed_dim=8)
+    cfg = vq_model.config
+    vq = vision.CarVQDesc(codebook_size=cfg.codebook_size, embed_dim=cfg.codebook_embed_dim, ch=128, z_channels=cfg.z_channels,
+                          n_levels=len(cfg.decoder_ch_mult), num_res_blocks=2)
+    for i, v in enumerate(cfg.decoder_ch_mult):
+        vq.ch_mult[i] = v
+    creates = {
+        "car_hed_create": (37, lambda ts, n, out: l.car_hed_create(ts, n, None, out)),
+        "car_lineart_create": (24, lambda ts, n, out: l.car_lineart_create(ts, n, None, out)),
+        "car_dpt_create": (4 + 16 * 4 + 74, lambda ts, n, out: l.car_dpt_create(C.byref(dpt), ts, n, None, out)),
+        "car_midas_create": (368, lambda ts, n, out: l.car_midas_create(ts, n, None, out)),
+        "car_vq_create": (len(vision.vq_tensor_order(vq_model)), lambda ts, n, out: l.car_vq_create(C.byref(vq), ts, n, None, out)),
+    }
+
+    def nulls(n):
+        return C.cast((C.c_void_p * n)(), C.POINTER(C.c_void_p))
+    for name, (n, create) in creates.items():
+        h = C.c_void_p()
+        for ts, count, out in [(None, n, C.byref(h)), (nulls(n), n, None), (nulls(n - 1), n - 1, C.byref(h)), (nulls(n), n, C.byref(h))]:
+            assert create(ts, count, out) < 0, (name, count)
+            assert name.encode() in l.car_last_error(), (name, count)
+        assert not h, name
+
+
 def test_product_fails_loudly_without_gpu():
     import torch
     if torch.cuda.is_available():

@@ -90,8 +90,13 @@ def test_modules_with_live_library_handles_can_be_deep_copied():
     import copy
     import ctypes as C
     import pickle
-    from controlar_b200 import engine, vision
+    from controlar_b200 import _lib, engine, vision
     from controlar_b200.autoregressive.models.gpt_t2i import Transformer, ModelArgs
+    from controlar_b200.condition.depth import DPTForDepthEstimation
+    from controlar_b200.condition.hed import ControlNetHED_Apache2
+    from controlar_b200.condition.lineart import LineArt
+    from controlar_b200.condition.midas import DPTDepthModel
+    from tests.dpt_oracle import DPT_SMALL
 
     def fake(cls):
         class F(cls):
@@ -108,3 +113,11 @@ def test_modules_with_live_library_handles_can_be_deep_copied():
         assert clone._car_model is None and clone._car_state is None and clone._car_train is None and clone.adapter._car_dino is None
         assert all(torch.equal(a, b) for a, b in zip(m.state_dict().values(), clone.state_dict().values()))
     assert m._car_model is not None                    # the original keeps its handles
+    detectors = [(ControlNetHED_Apache2(), "_car_hed"), (LineArt(), "_car_lineart"), (DPTForDepthEstimation(DPT_SMALL), "_car_dpt"),
+                 (DPTDepthModel(), "_car_midas")]
+    for det, attr in detectors:
+        object.__setattr__(det, attr, fake(_lib.ModuleHandle))
+        for clone in (copy.deepcopy(det), pickle.loads(pickle.dumps(det))):
+            assert getattr(clone, attr) is None, attr
+            assert all(torch.equal(a, b) for a, b in zip(det.state_dict().values(), clone.state_dict().values())), attr
+        assert isinstance(getattr(det, attr), _lib.ModuleHandle), attr

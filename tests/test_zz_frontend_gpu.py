@@ -85,6 +85,70 @@ def test_hed_detector_vs_reference_golden():
         assert perr < 1e-3, (name, perr)
 
 
+def _hed(seed):
+    from controlar_b200.condition.hed import ControlNetHED_Apache2
+    from oracle.weights import make_hed_state_dict
+    m = ControlNetHED_Apache2()
+    m.load_state_dict(make_hed_state_dict(seed=seed), strict=True)
+    return m.cuda()
+
+
+def test_hed_weight_update_rebuilds_handle():
+    from oracle.weights import make_hed_state_dict
+    from tests.golden.make_golden import hed_inputs
+    x = next(iter(hed_inputs().values())).cuda()
+    m = _hed(0)
+    with torch.no_grad():
+        y0 = m.run(x)[0]
+        m.load_state_dict(make_hed_state_dict(seed=5))
+        y5 = m.run(x)[0]
+    assert torch.equal(y5, _hed(5).run(x)[0]) and not torch.equal(y0, y5)
+
+
+def test_hed_failed_recreate_leaves_no_stale_handle(monkeypatch):
+    """A weight update whose re-create fails leaves no handle behind: the next call builds a new one, and every handle the library
+    created is destroyed exactly once.  The library's own create and destroy run; only the refusal of one create is injected."""
+    import ctypes as C
+    import gc
+    from controlar_b200 import _lib
+    from tests.golden.make_golden import hed_inputs
+    real = _lib.lib()
+    created, destroyed, live, refuse = [], [], set(), [False]
+
+    class Lib:                                             # the library, with car_hed_create / car_hed_destroy observed
+        def __getattr__(self, name):
+            return getattr(real, name)
+
+        def car_hed_create(self, ts, n, stream, out):
+            if refuse[0]:
+                return -1
+            rc = real.car_hed_create(ts, n, stream, out)
+            created.append(out._obj.value)
+            live.add(out._obj.value)
+            return rc
+
+        def car_hed_destroy(self, h):
+            destroyed.append(h.value)
+            if h.value not in live:                        # recorded, but a freed handle never reaches the library
+                return 0
+            live.discard(h.value)
+            return real.car_hed_destroy(h)
+    monkeypatch.setattr(_lib, "_lib", Lib())
+    x = next(iter(hed_inputs().values())).cuda()
+    m = _hed(0)
+    with torch.no_grad():
+        m.run(x)
+        m.norm.add_(1.0)                                   # an in-place update: the next call rebuilds
+        refuse[0] = True
+        with pytest.raises(RuntimeError, match="car_hed_create"):
+            m.run(x)
+        refuse[0] = False
+        m.run(x)
+    del m
+    gc.collect()
+    assert len(created) == 2 and sorted(destroyed) == sorted(created), (created, destroyed)
+
+
 def test_t5_encoder_vs_hf_golden():
     """T5 encoder forward (reference language/t5.py:69-75 -> HF T5EncoderModel, bf16) against the fixture HF itself produced on
     procedural weights (tests/golden/make_golden.py:t5_case): right-padded prompts, a one-token prompt, distances beyond the
