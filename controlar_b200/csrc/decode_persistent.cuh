@@ -652,7 +652,7 @@ __device__ __forceinline__ void pk_attn_finalize(const PkParams& P, float Mx, fl
 // ("parts").  Within a part the four 8-lane row slots of the warp take rows k0 + sub + 4 i, the loads of two blocks of 4 rows
 // per slot in flight at once; the slots are merged with shuffles and the warp leaves one partial per part in shared memory:
 // entry (warp, part) = {-, m, l, -, acc[64]}.
-__device__ __forceinline__ void pk_attn_phase(const PkParams& P, int layer, int pos, unsigned int tag, int par, long long* dbg) {
+__device__ __forceinline__ void pk_attn_phase(const PkParams& P, int layer, int pos, unsigned int tag, int par, const int* klo, long long* dbg) {
     const PkSmem sm = pk_smem_layout();
     constexpr int EPL = 8, UNR = 4, ENT = 68;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, sub = lane >> 3, cl = lane & 7;
@@ -766,8 +766,12 @@ __device__ __forceinline__ void pk_attn_phase(const PkParams& P, int layer, int 
                 m_run = m_new;
             }
         };
-        load_block(kA, vA, mA, k0);
-        for (int rb = k0; rb < k1; rb += 8 * UNR) {        // warp-uniform trip count
+        // Captions are left-padded: the blocks of 4 x UNR keys that lie wholly inside the sequence's leading masked keys come
+        // before any key with weight, so they leave (m, l, acc) at its initial state and are not read.  The remaining blocks
+        // keep their offsets from k0, so the arithmetic is exactly that of the whole range.
+        const int kfirst = k0 + ((max(min(klo[b], k1), k0) - k0) / (4 * UNR)) * (4 * UNR);
+        load_block(kA, vA, mA, kfirst);
+        for (int rb = kfirst; rb < k1; rb += 8 * UNR) {    // warp-uniform trip count
             load_block(kB, vB, mB, rb + 4 * UNR);
             use_block(kA, vA, mA, rb);
             load_block(kA, vA, mA, rb + 8 * UNR);
@@ -852,12 +856,19 @@ __device__ __noinline__ void pk_sample(const SampleArgs& a, int b) {
 __global__ void __launch_bounds__(PK_THREADS, 1) pk_decode_kernel(const __grid_constant__ PkParams P) {
     __shared__ int s_tok;
     __shared__ int s_lo[5], s_hi[5];                       // this CTA's block ranges per GEMM kind
+    __shared__ int s_klo[16];                              // leading masked caption keys per sequence (pk_attn_phase)
     const PkSmem sm = pk_smem_layout();
     const int tid = threadIdx.x;
     const int G = gridDim.x;
     if (tid == 0) {
         for (int s = 0; s < PK_NSLOT; ++s) pk_mbar_init(&sm.full[s], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    if (tid < P.b_eff) {                                   // (host-checked: b_eff <= 16)
+        int k = 0;
+        if (P.emb_mask != nullptr)
+            while (k < P.T && __ldg(P.emb_mask + (size_t)tid * P.T + k) == 0) ++k;
+        s_klo[tid] = k;
     }
     __syncthreads();
     if (tid < P.L) {   // (host-checked: L <= PK_MAXL)
@@ -926,7 +937,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) pk_decode_kernel(const __grid_c
             const int nph = l < P.L ? 5 : 1;
             for (int ph = 0; ph < nph; ++ph) {
                 long long* dbg = (dbg_step && l == 3) ? dbg_cta + 8 + 8 * ph : (dbg_step && l == P.L) ? dbg_cta + 56 : nullptr;   // (head: slots 56 .. 60)
-                if (l < P.L && ph == 1) { pk_attn_phase(P, l, p, tag, par, dbg); continue; }
+                if (l < P.L && ph == 1) { pk_attn_phase(P, l, p, tag, par, s_klo, dbg); continue; }
                 const int kind = l == P.L ? 4 : (ph == 0 ? 0 : ph - 1);
                 cons = pk_gemm_phase(P, kind, l, p, tag, s_lo[kind], s_hi[kind], cons, dbg,
                               (dbg != nullptr && (int)blockIdx.x == 77 % (int)gridDim.x) ? P.dbg + (size_t)gridDim.x * 64 + (size_t)ph * 256 : nullptr,
