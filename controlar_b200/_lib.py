@@ -145,12 +145,21 @@ def cur_stream(device=None) -> int:
     return torch.cuda.current_stream(device).cuda_stream
 
 
-def on_device(t):
-    """Context manager that makes the device of tensor `t` current for the duration of a library call: the library launches on
-    the current device and takes the stream from it (the reference wraps its calls in `with torch.device(device)`,
-    generate.py:179-182)."""
-    import torch
-    return torch.cuda.device(t.device)
+def on_own_device(fn):
+    """Run a handle method with `self.device` current: the library launches on the current device and `cur_stream()` is that
+    device's current stream, so a model on cuda:1 works without torch.cuda.set_device(1) (the reference wraps its calls in
+    `with torch.device(device)`, generate.py:179-182)."""
+    import functools
+
+    @functools.wraps(fn)
+    def wrapped(self, *a, **k):
+        import torch
+        dev = self.device
+        if dev.type != "cuda":
+            return fn(self, *a, **k)
+        with torch.cuda.device(dev):
+            return fn(self, *a, **k)
+    return wrapped
 
 
 def _no_handle():
@@ -158,9 +167,26 @@ def _no_handle():
 
 
 class NativeHandle:
-    """Base of the objects that own a library handle.  Handles are never copied: `copy.deepcopy` / pickling of the owning module
-    (e.g. `ema = deepcopy(model)` of the train scripts, train_c2i_canny.py:117, after the model has been used) yields None in the
-    copy, which rebuilds its own handle lazily on first use — instead of ctypes' "objects containing pointers cannot be pickled"."""
+    """Owner of one library pointer, released by the entry point named `destroy` (e.g. "car_hed_destroy").  `close()` clears the
+    pointer before it destroys it, so a failed re-create leaves no stale pointer and every pointer is destroyed exactly once.
+    Handles are never copied: `copy.deepcopy` / pickling of the owning module (e.g. `ema = deepcopy(model)` of the train scripts,
+    train_c2i_canny.py:117, after the model has been used) yields None in the copy, which rebuilds its own handle lazily on first
+    use — instead of ctypes' "objects containing pointers cannot be pickled"."""
+
+    def __init__(self, destroy: str):
+        self.destroy = destroy
+        self.handle = C.c_void_p()
+
+    def close(self):
+        h, self.handle = self.handle, C.c_void_p()
+        if h:
+            getattr(lib(), self.destroy)(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
     def __deepcopy__(self, memo):
         return None
@@ -175,14 +201,11 @@ def param_signature(params) -> tuple:
 
 
 class ModuleHandle(NativeHandle):
-    """A library handle built from a module's parameters and released by the entry point named `destroy` (e.g. "car_hed_destroy").
-    `get(params, create)` returns it, built first by `create(out)` — which fills the c_void_p `out` — with the parameters' device
-    current, and built again whenever `param_signature(params)` changed.  The old handle is cleared and destroyed before a rebuild,
-    so a failed create leaves no stale pointer, and every handle is destroyed exactly once."""
+    """A library handle built from a module's parameters.  `get(params, create)` returns it, built first by `create(out)` — which
+    fills the c_void_p `out` — with the parameters' device current, and built again whenever `param_signature(params)` changed."""
 
     def __init__(self, destroy: str):
-        self.destroy = destroy
-        self.handle = C.c_void_p()
+        super().__init__(destroy)
         self.sig = None
 
     def get(self, params, create):
@@ -197,17 +220,6 @@ class ModuleHandle(NativeHandle):
                 torch.cuda.current_stream().synchronize()      # the library has copied / packed what it read
             self.sig = sig
         return self.handle
-
-    def close(self):
-        h, self.handle, self.sig = self.handle, C.c_void_p(), None
-        if h:
-            getattr(lib(), self.destroy)(h)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def _ptr(t):

@@ -24,7 +24,7 @@ std::atomic<long long> g_car_launches{0};
 // ---------------------------------------------------------------------------------------------------------
 // structures
 // ---------------------------------------------------------------------------------------------------------
-struct CarModel {
+struct CarModel : CarOwned {
     CarModelDesc d;
     // borrowed originals
     const void *tok_emb, *norm, *output, *cap_fc1, *cap_fc2, *label_table, *cond_fc1, *cond_fc2, *ctl_fc1[3], *ctl_fc2[3];
@@ -33,16 +33,15 @@ struct CarModel {
     std::vector<void*> g_wqkv, g_wo, g_w13, g_w2;
     void *g_output, *g_cap_fc1, *g_cap_fc2, *g_cond_fc1, *g_cond_fc2, *g_ctl_fc1[3], *g_ctl_fc2[3];
     unsigned int pack_gen = 0;       // bumped by every (re)pack: states refresh their device pointer tables when it moves
-    std::vector<void*> owned;
     size_t esize() const { return d.dtype == CAR_BF16 ? 2 : 4; }
 };
 
-struct CarState {
+struct CarState : CarOwned {
     CarModel* m;
     int b_eff, S, N, T;
     std::vector<void*> kc, vc;
     const float* rope;
-    int* emb_mask;       // [b_eff][T] or null (= all ones)
+    int* emb_mask = nullptr;       // [b_eff][T] or null (= all ones)
     int* emb_mask_store;
     // decode scratch (b_eff rows)
     void *h, *q, *attn, *act;
@@ -52,34 +51,34 @@ struct CarState {
     int nsplit;
     // control tokens [3][b_eff][N][d]
     void* ctrl[3];
-    bool has_ctrl;
-    float cs;
+    bool has_ctrl = false;
+    float cs = 1.f;
     // prefill scratch
     void *hP, *qP, *attnP, *actP, *t1, *t2;
-    void *qkvP, *gP, *uP;     // dense prefill path (bf16): qkv [rows][3d], w1 / w3 outputs [rows][F]
-    bool prefilled;
+    void *qkvP = nullptr, *gP = nullptr, *uP = nullptr;     // dense prefill path (bf16): qkv [rows][3d], w1 / w3 outputs [rows][F]
+    bool prefilled = false;
     // decode graph
-    cudaGraphExec_t gexec;
-    cudaStream_t cap_stream;   // capture happens on a private stream (the legacy default stream cannot capture)
-    bool graph_ok; unsigned int graph_pack_gen;
-    CarSampling gsp;
-    const float* gnoise;
+    cudaGraphExec_t gexec = nullptr;
+    cudaStream_t cap_stream = nullptr;   // capture happens on a private stream (the legacy default stream cannot capture)
+    bool graph_ok = false; unsigned int graph_pack_gen = 0;
+    CarSampling gsp{};
+    const float* gnoise = nullptr;
     // persistent decode kernel (decode_persistent.cuh)
-    void** pk_ptrs;          // device arrays of per-layer pointers [8][L]
-    int* pk_part;            // [4][grid + 1] block offsets per CTA
+    void** pk_ptrs = nullptr;          // device arrays of per-layer pointers [8][L]
+    int* pk_part = nullptr;            // [4][grid + 1] block offsets per CTA
     uint2 *pk_h2[2], *pk_h1[2], *pk_att[2], *pk_act[2], *pk_qkv[2], *pk_partial[2];
-    int pk_part_slots, pk_grid; bool pk_ok; unsigned int pk_ptrs_gen;
-    unsigned int* pk_bar; unsigned int pk_bar_count, pk_tag_gen;
-    size_t pk_pkt_bytes; void* pk_pkt_base;
-    long long* pk_step_ts;   // caller-provided device buffer [N] for per-step timestamps (car_state_set_step_timer) or null
-    std::vector<void*> owned;
-};
+    int pk_part_slots = 0, pk_grid = 0; bool pk_ok = false; unsigned int pk_ptrs_gen = 0;
+    unsigned int* pk_bar = nullptr; unsigned int pk_bar_count = 0, pk_tag_gen = 0;
+    size_t pk_pkt_bytes = 0; void* pk_pkt_base = nullptr;
+    long long* pk_step_ts = nullptr;   // caller-provided device buffer [N] for per-step timestamps (car_state_set_step_timer) or null
 
-static int alloc_dev(std::vector<void*>& owned, void** p, size_t bytes) {
-    CAR_CUDA(cudaMalloc(p, bytes ? bytes : 16));
-    owned.push_back(*p);
-    return CAR_OK;
-}
+    // Releases the graph and the capture stream; the device memory goes with CarOwned.  It must not read `m`: a layout change
+    // destroys the old CarModel (gpt_t2i.setup_caches) before the state built on it is closed.
+    ~CarState() {
+        if (gexec) cudaGraphExecDestroy(gexec);
+        if (cap_stream) cudaStreamDestroy(cap_stream);
+    }
+};
 
 // Device buffers that other SMs POLL (packet tags, barrier counters) are initialised with SM stores, not cudaMemset: a
 // recycled allocation that was zeroed by cudaMemset has been observed to still return the previous owner's packets to strong
@@ -115,16 +114,6 @@ extern "C" int64_t car_launch_count(int32_t reset) {
     long long v = g_car_launches.load();
     if (reset) g_car_launches.store(0);
     return v;
-}
-
-// SM count of the CURRENT device (the Python handles make the tensors' device current around every call)
-static int sm_count() {
-    static int cached[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) dev = 0;
-    if (cached[dev] == 0) { int n = 0; cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); cached[dev] = n > 0 ? n : 132; }
-    return cached[dev];
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -207,14 +196,14 @@ static int pack_one(CarModel* m, cudaStream_t st, const void* w, const void* w3,
                     bool allocate) {
     // N = rows of the logical (possibly interleaved) matrix
     if (m->d.dtype == CAR_BF16) {
-        if (allocate) CAR_TRY(alloc_dev(m->owned, dst, (size_t)N * K * 2));
+        if (allocate) CAR_TRY(m->alloc(dst, (size_t)N * K * 2));
         const int nblk = N / 8;
         const long long total = (long long)nblk * (K / 32) * 32;
         const int blocks = (int)std::min<long long>((total + 255) / 256, 4096);
         CAR_LAUNCH(pack_weight_bf16_kernel, blocks, 256, 0, st, (const bf16*)w, (const bf16*)w3, (uint4*)*dst, nblk, K, interleave ? 1 : 0);
     } else {
         if (!interleave) { *dst = const_cast<void*>(w); return CAR_OK; }
-        if (allocate) CAR_TRY(alloc_dev(m->owned, dst, (size_t)N * K * 4));
+        if (allocate) CAR_TRY(m->alloc(dst, (size_t)N * K * 4));
         CAR_LAUNCH(interleave_rows_f32_kernel, 2048, 256, 0, st, (const float*)w, (const float*)w3, (float*)*dst, N / 2, K);
     }
     return CAR_OK;
@@ -266,7 +255,7 @@ extern "C" int car_model_create(const CarModelDesc* desc, const CarWeights* w, v
     CarModel* m = new CarModel();
     m->d = d;
     int r = model_pack_all(m, w, (cudaStream_t)stream, true);
-    if (r != CAR_OK) { for (void* p : m->owned) cudaFree(p); delete m; return r; }
+    if (r != CAR_OK) { delete m; return r; }
     *out = m;
     return CAR_OK;
 }
@@ -277,8 +266,6 @@ extern "C" int car_model_repack(CarModel* m, const CarWeights* w, void* stream) 
 }
 
 extern "C" int car_model_destroy(CarModel* m) {
-    if (!m) return CAR_OK;
-    for (void* p : m->owned) cudaFree(p);
     delete m;
     return CAR_OK;
 }
@@ -324,10 +311,7 @@ static std::vector<const void*> pk_pointer_table(const CarState* s) {
 
 static int pk_state_setup(CarState* s) {
     const CarModelDesc& d = s->m->d;
-    int dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int G = sms, L = d.n_layer;
+    const int G = sm_count(), L = d.n_layer;
     s->pk_grid = G;
     const int nbh = s->b_eff * d.n_head;
     // shapes the kernel is instantiated for (else car_generate falls back to the per-kernel graph chain)
@@ -343,10 +327,10 @@ static int pk_state_setup(CarState* s) {
     const size_t a_d = (size_t)(d.dim / 32) * 2048, a_f = (size_t)(d.ffn_dim / 32) * 2048;
     const size_t qkv_b = (size_t)3 * 16 * d.n_head * 8 * 4 * 8, part_b = (size_t)nbh * s->pk_part_slots * 66 * 8;
     const size_t total = 2 * (3 * a_d + a_f + qkv_b + part_b);
-    CAR_TRY(alloc_dev(s->owned, (void**)&s->pk_ptrs, hp.size() * sizeof(void*)));
-    CAR_TRY(alloc_dev(s->owned, (void**)&s->pk_part, table.size() * sizeof(int)));
-    CAR_TRY(alloc_dev(s->owned, (void**)&s->pk_bar, 64));
-    CAR_TRY(alloc_dev(s->owned, &s->pk_pkt_base, total));
+    CAR_TRY(s->alloc(&s->pk_ptrs, hp.size() * sizeof(void*)));
+    CAR_TRY(s->alloc(&s->pk_part, table.size() * sizeof(int)));
+    CAR_TRY(s->alloc(&s->pk_bar, 64));
+    CAR_TRY(s->alloc(&s->pk_pkt_base, total));
     s->pk_pkt_bytes = total;
     unsigned char* q = (unsigned char*)s->pk_pkt_base;
     for (int par = 0; par < 2; ++par) {
@@ -365,51 +349,48 @@ static int pk_state_setup(CarState* s) {
 // key splits of the decode attention: about four CTAs per SM over all (b, h) rows, at most 16 per row
 static int attn_decode_nsplit(int bh) { return std::max(1, std::min(16, (4 * sm_count() + bh - 1) / bh)); }
 
+// everything car_state_create allocates and initialises; on failure the caller deletes the half-built state
+static int state_init(CarState* s, void* const* k_cache, void* const* v_cache) {
+    const CarModelDesc& d = s->m->d;
+    const int b_eff = s->b_eff;
+    s->kc.assign(k_cache, k_cache + d.n_layer); s->vc.assign(v_cache, v_cache + d.n_layer);
+    CAR_CUDA(cudaStreamCreateWithFlags(&s->cap_stream, cudaStreamNonBlocking));
+    const size_t es = s->m->esize();
+    const size_t dd = d.dim, F = d.ffn_dim, V = d.vocab_size;
+    const size_t MP = (size_t)b_eff * s->T, MC = (size_t)b_eff * s->N;
+    s->nsplit = attn_decode_nsplit(b_eff * d.n_head);
+    CAR_TRY(s->alloc(&s->h, b_eff * dd * es)); CAR_TRY(s->alloc(&s->q, b_eff * dd * es));
+    CAR_TRY(s->alloc(&s->attn, b_eff * dd * es)); CAR_TRY(s->alloc(&s->act, b_eff * F * es));
+    CAR_TRY(s->alloc(&s->logits, b_eff * V * 4)); CAR_TRY(s->alloc(&s->tok, b_eff * 4)); CAR_TRY(s->alloc(&s->pos, 4 * 4));
+    CAR_TRY(s->alloc(&s->tickets, (size_t)b_eff * d.n_head * 4));
+    CAR_TRY(s->alloc(&s->tokens, (size_t)b_eff * s->N * 4));
+    CAR_TRY(s->alloc(&s->attn_part, (size_t)b_eff * d.n_head * s->nsplit * AD_PART * 4));
+    for (int j = 0; j < 3; ++j) CAR_TRY(s->alloc(&s->ctrl[j], MC * dd * es));
+    CAR_TRY(s->alloc(&s->hP, MP * dd * es)); CAR_TRY(s->alloc(&s->qP, MP * dd * es));
+    CAR_TRY(s->alloc(&s->attnP, MP * dd * es)); CAR_TRY(s->alloc(&s->actP, MP * F * es));
+    CAR_TRY(s->alloc(&s->t1, std::max(MC, MP) * dd * es)); CAR_TRY(s->alloc(&s->t2, std::max(MC, MP) * dd * es));
+    if (d.dtype == CAR_BF16) {
+        CAR_TRY(s->alloc(&s->qkvP, MP * 3 * dd * es)); CAR_TRY(s->alloc(&s->gP, MP * F * es)); CAR_TRY(s->alloc(&s->uP, MP * F * es));
+    }
+    CAR_TRY(s->alloc(&s->emb_mask_store, MP * 4));
+    CAR_CUDA(cudaMemset(s->tickets, 0, (size_t)b_eff * d.n_head * 4));
+    CAR_CUDA(cudaMemset(s->pos, 0, 16));
+    s->done_ctr = s->pos + 1;
+    s->pk_tag_gen = g_pk_tag_gen.load();
+    return d.dtype == CAR_BF16 ? pk_state_setup(s) : CAR_OK;     // persistent decode kernel resources (bf16 only)
+}
+
 extern "C" int car_state_create(CarModel* m, int32_t b_eff, int32_t S, int32_t N, void* const* k_cache, void* const* v_cache,
                                 const float* rope_table, CarState** out) {
     if (!m || !k_cache || !v_cache || !rope_table || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (b_eff <= 0 || N <= 0) CAR_FAIL(CAR_ERR_ARG, "need b_eff > 0, N > 0");
     const CarModelDesc& d = m->d;
-    const int T = d.cls_token_num;
-    if (b_eff <= 0 || N <= 0 || S < T + N) CAR_FAIL(CAR_ERR_ARG, "need b_eff > 0, N > 0, S >= T + N");
+    if (S < d.cls_token_num + N) CAR_FAIL(CAR_ERR_ARG, "need S >= T + N");
     if (N > d.block_size) CAR_FAIL(CAR_ERR_ARG, "N exceeds block_size (RoPE table rows)");
     CarState* s = new CarState();
-    s->m = m; s->b_eff = b_eff; s->S = S; s->N = N; s->T = T;
-    s->kc.assign(k_cache, k_cache + d.n_layer); s->vc.assign(v_cache, v_cache + d.n_layer);
-    s->rope = rope_table; s->emb_mask = nullptr; s->has_ctrl = false; s->cs = 1.f; s->prefilled = false;
-    s->gexec = nullptr; s->graph_ok = false; s->gnoise = nullptr; s->cap_stream = nullptr;
-    if (cudaStreamCreateWithFlags(&s->cap_stream, cudaStreamNonBlocking) != cudaSuccess) { delete s; CAR_FAIL(CAR_ERR_CUDA, "cudaStreamCreateWithFlags failed"); }
-    const size_t es = m->esize();
-    const size_t dd = d.dim, F = d.ffn_dim, V = d.vocab_size;
-    const size_t MP = (size_t)b_eff * T, MC = (size_t)b_eff * N;
-    s->nsplit = attn_decode_nsplit(b_eff * d.n_head);
-    int r = CAR_OK;
-    auto A = [&](void** p, size_t bytes) { if (r == CAR_OK) r = alloc_dev(s->owned, p, bytes); };
-    A(&s->h, b_eff * dd * es); A(&s->q, b_eff * dd * es); A(&s->attn, b_eff * dd * es); A(&s->act, b_eff * F * es);
-    A((void**)&s->logits, b_eff * V * 4); A((void**)&s->tok, b_eff * 4); A((void**)&s->pos, 4 * 4);
-    A((void**)&s->tickets, (size_t)b_eff * d.n_head * 4);
-    A((void**)&s->tokens, (size_t)b_eff * N * 4);
-    A((void**)&s->attn_part, (size_t)b_eff * d.n_head * s->nsplit * AD_PART * 4);
-    for (int j = 0; j < 3; ++j) A(&s->ctrl[j], MC * dd * es);
-    A(&s->hP, MP * dd * es); A(&s->qP, MP * dd * es); A(&s->attnP, MP * dd * es); A(&s->actP, MP * F * es);
-    A(&s->t1, std::max(MC, MP) * dd * es); A(&s->t2, std::max(MC, MP) * dd * es);
-    s->qkvP = s->gP = s->uP = nullptr;
-    if (d.dtype == CAR_BF16) { A(&s->qkvP, MP * 3 * dd * es); A(&s->gP, MP * F * es); A(&s->uP, MP * F * es); }
-    A((void**)&s->emb_mask, MP * 4);
-    if (r == CAR_OK && cudaMemset(s->tickets, 0, (size_t)b_eff * d.n_head * 4) != cudaSuccess) r = CAR_ERR_CUDA;
-    if (r == CAR_OK && cudaMemset(s->pos, 0, 16) != cudaSuccess) r = CAR_ERR_CUDA;
-    if (r != CAR_OK) { for (void* p : s->owned) cudaFree(p); delete s; return r; }
-    s->done_ctr = s->pos + 1;
-    // persistent decode kernel resources (bf16 only)
-    s->pk_ptrs = nullptr; s->pk_part = nullptr; s->pk_bar = nullptr; s->pk_grid = 0; s->pk_ok = false;
-    s->pk_step_ts = nullptr;
-    s->pk_bar_count = 0; s->pk_tag_gen = g_pk_tag_gen.load(); s->pk_pkt_base = nullptr; s->pk_pkt_bytes = 0;
-    if (d.dtype == CAR_BF16) {
-        int r2 = pk_state_setup(s);
-        if (r2 != CAR_OK) { for (void* p : s->owned) cudaFree(p); delete s; return r2; }
-    }
-    s->emb_mask_store = s->emb_mask;
-    s->emb_mask = nullptr;                           // all-ones until car_state_set_emb_mask
-    s->gsp = CarSampling{};
+    s->m = m; s->b_eff = b_eff; s->S = S; s->N = N; s->T = d.cls_token_num; s->rope = rope_table;
+    const int rc = state_init(s, k_cache, v_cache);
+    if (rc != CAR_OK) { delete s; return rc; }
     *out = s;
     return CAR_OK;
 }
@@ -430,10 +411,6 @@ extern "C" int car_state_set_step_timer(CarState* s, int64_t* step_ns_dev) {
 }
 
 extern "C" int car_state_destroy(CarState* s) {
-    if (!s) return CAR_OK;
-    if (s->gexec) cudaGraphExecDestroy(s->gexec);
-    if (s->cap_stream) cudaStreamDestroy(s->cap_stream);
-    for (void* p : s->owned) if (p) cudaFree(p);
     delete s;
     return CAR_OK;
 }
@@ -998,7 +975,7 @@ extern "C" int car_op_attn_prefill(int32_t dtype, const void* q, const void* k_c
 // training forward (SURVEY.md §8 row f1): Transformer.forward(idx, cond_idx, targets, mask, valid, condition) in train mode,
 // fp32 parameters under bf16 autocast — gpt_t2i.py:420-431,451-484.  First correct path: prefill GEMM kernels + train.cuh glue.
 // ---------------------------------------------------------------------------------------------------------
-struct CarTrain {
+struct CarTrain : CarOwned {
     CarModelDesc d;
     CarTrainWeights w;
     std::vector<const void*> attention_norm, wqkv, wo, ffn_norm, w1, w3, w2;   // borrowed fp32
@@ -1020,18 +997,67 @@ struct CarTrain {
     const uint8_t *f_drop = nullptr, *f_mask = nullptr;
     const float* f_valid = nullptr;
     bool fwd_ok = false;
-    std::vector<void*> owned;
 };
 
 static int tr_cast(cudaStream_t st, const void* src, bf16* dst, long long n) {
-    CAR_LAUNCH(tr_cast_bf16_kernel, (int)std::min<long long>((n + 255) / 256, sm_count() * 16), 256, 0, st, (const float*)src, dst, n);
+    CAR_LAUNCH(tr_cast_bf16_kernel, gsz(n), 256, 0, st, (const float*)src, dst, n);
     return CAR_OK;
 }
-static int tr_grid(long long n) { return (int)std::min<long long>((n + 255) / 256, sm_count() * 16); }
 // MLP.forward gpt_t2i.py:177-181 on bf16 operands: out = fc2(gelu_tanh(fc1 x))
 static int tr_mlp(cudaStream_t st, const bf16* x, int rows, int K, const bf16* fc1, const bf16* fc2, int d, bf16* tmp, bf16* out) {
     CAR_TRY(dense_linear(st, x, K, fc1, rows, d, K, ACT_GELU_TANH, nullptr, 0, tmp, d));
     return dense_linear(st, tmp, d, fc2, rows, d, d, ACT_NONE, nullptr, 0, out, d);
+}
+
+// everything car_train_create allocates; on failure the caller deletes the half-built handle
+static int train_init(CarTrain* t) {
+    const CarModelDesc& d = t->d;
+    const int L = d.n_layer, dim = d.dim, F = d.ffn_dim, V = d.vocab_size;
+    auto copyp = [&](std::vector<const void*>& v, const void* const* src) { v.assign(src, src + L); };
+    const CarWeights& w = t->w.w;
+    copyp(t->attention_norm, w.attention_norm); copyp(t->wqkv, w.wqkv); copyp(t->wo, w.wo); copyp(t->ffn_norm, w.ffn_norm);
+    copyp(t->w1, w.w1); copyp(t->w3, w.w3); copyp(t->w2, w.w2);
+    t->b_wqkv.resize(L); t->b_wo.resize(L); t->b_w1.resize(L); t->b_w3.resize(L); t->b_w2.resize(L);
+    for (int l = 0; l < L; ++l) {
+        CAR_TRY(t->alloc(&t->b_wqkv[l], (size_t)3 * dim * dim * 2)); CAR_TRY(t->alloc(&t->b_wo[l], (size_t)dim * dim * 2));
+        CAR_TRY(t->alloc(&t->b_w1[l], (size_t)F * dim * 2)); CAR_TRY(t->alloc(&t->b_w3[l], (size_t)F * dim * 2));
+        CAR_TRY(t->alloc(&t->b_w2[l], (size_t)dim * F * 2));
+    }
+    CAR_TRY(t->alloc(&t->b_out, (size_t)V * dim * 2));
+    if (d.model_type == 1) { CAR_TRY(t->alloc(&t->b_cap1, (size_t)dim * d.caption_dim * 2)); CAR_TRY(t->alloc(&t->b_cap2, (size_t)dim * dim * 2)); }
+    CAR_TRY(t->alloc(&t->b_cond1, (size_t)dim * dim * 2)); CAR_TRY(t->alloc(&t->b_cond2, (size_t)dim * dim * 2));
+    for (int j = 0; j < 3; ++j) { CAR_TRY(t->alloc(&t->b_ctl1[j], (size_t)dim * dim * 2)); CAR_TRY(t->alloc(&t->b_ctl2[j], (size_t)dim * dim * 2)); }
+    CAR_TRY(t->alloc(&t->b_ad1, (size_t)dim * t->w.adapter_dim * 2)); CAR_TRY(t->alloc(&t->b_ad2, (size_t)dim * dim * 2));
+    const size_t R = (size_t)t->maxB * t->maxS, RC = (size_t)t->maxB * t->maxN;
+    CAR_TRY(t->alloc(&t->h, R * dim * 4));
+    CAR_TRY(t->alloc(&t->nll, RC * 4));
+    CAR_TRY(t->alloc(&t->x, std::max(R * dim, (size_t)t->maxB * d.cls_token_num * std::max(d.caption_dim, dim)) * 2));
+    CAR_TRY(t->alloc(&t->qkv, R * 3 * dim * 2)); CAR_TRY(t->alloc(&t->q, R * dim * 2)); CAR_TRY(t->alloc(&t->kc, R * dim * 2));
+    CAR_TRY(t->alloc(&t->vc, R * dim * 2)); CAR_TRY(t->alloc(&t->att, R * dim * 2));
+    CAR_TRY(t->alloc(&t->g, R * F * 2)); CAR_TRY(t->alloc(&t->u, R * F * 2)); CAR_TRY(t->alloc(&t->act, R * F * 2)); CAR_TRY(t->alloc(&t->o, R * dim * 2));
+    CAR_TRY(t->alloc(&t->cin, RC * dim * 2)); CAR_TRY(t->alloc(&t->ctmp, std::max(RC, (size_t)t->maxB * d.cls_token_num) * dim * 2));
+    CAR_TRY(t->alloc(&t->ctok, RC * dim * 2)); CAR_TRY(t->alloc(&t->cadd, RC * dim * 2));
+    CAR_TRY(t->alloc(&t->lg, RC * V * 2));
+    // backward workspaces
+    const size_t cap = (size_t)(d.model_type == 1 ? d.caption_dim : 8), ad = (size_t)t->w.adapter_dim;
+    const size_t rows_mlp = std::max(RC, (size_t)t->maxB * d.cls_token_num);
+    const size_t Rp = (std::max(R, rows_mlp) + 63) / 64 * 64;
+    const size_t maxN = std::max({(size_t)3 * dim, (size_t)F, (size_t)V}), maxK = std::max({(size_t)F, (size_t)dim, cap, ad});
+    const size_t maxW = std::max({(size_t)3 * dim * dim, (size_t)F * dim, (size_t)V * dim, (size_t)dim * cap, (size_t)dim * ad});
+    t->Rp_max = Rp;
+    CAR_TRY(t->alloc(&t->hs, (size_t)L * R * dim * 4)); CAR_TRY(t->alloc(&t->dh, R * dim * 4)); CAR_TRY(t->alloc(&t->h0, R * dim * 4));
+    CAR_TRY(t->alloc(&t->scr, R * dim * 4)); CAR_TRY(t->alloc(&t->part, (size_t)TR_COLSUM_CHUNKS * dim * 4));
+    CAR_TRY(t->alloc(&t->lse, (size_t)t->maxB * d.n_head * t->maxS * 4)); CAR_TRY(t->alloc(&t->dsum, (size_t)t->maxB * d.n_head * t->maxS * 4));
+    CAR_TRY(t->alloc(&t->capx, (size_t)t->maxB * d.cls_token_num * cap * 2));
+    CAR_TRY(t->alloc(&t->x2, R * dim * 2)); CAR_TRY(t->alloc(&t->db, R * dim * 2)); CAR_TRY(t->alloc(&t->dact, R * F * 2));
+    CAR_TRY(t->alloc(&t->dg, R * F * 2)); CAR_TRY(t->alloc(&t->du, R * F * 2)); CAR_TRY(t->alloc(&t->dx, R * dim * 2));
+    CAR_TRY(t->alloc(&t->datt, R * dim * 2)); CAR_TRY(t->alloc(&t->dq, R * dim * 2)); CAR_TRY(t->alloc(&t->dk, R * dim * 2));
+    CAR_TRY(t->alloc(&t->dv, R * dim * 2)); CAR_TRY(t->alloc(&t->dqkv, R * 3 * dim * 2)); CAR_TRY(t->alloc(&t->dlg, RC * V * 2));
+    CAR_TRY(t->alloc(&t->wT, maxW * 2)); CAR_TRY(t->alloc(&t->dWb, maxW * 2)); CAR_TRY(t->alloc(&t->yT, maxN * Rp * 2)); CAR_TRY(t->alloc(&t->xT, maxK * Rp * 2));
+    CAR_TRY(t->alloc(&t->m_t, rows_mlp * dim * 2)); CAR_TRY(t->alloc(&t->m_a, rows_mlp * dim * 2));
+    CAR_TRY(t->alloc(&t->m_da, rows_mlp * dim * 2)); CAR_TRY(t->alloc(&t->m_dt, rows_mlp * dim * 2));
+    CAR_TRY(t->alloc(&t->dctok, RC * dim * 2)); CAR_TRY(t->alloc(&t->dcin, RC * dim * 2)); CAR_TRY(t->alloc(&t->dadd, rows_mlp * dim * 2));
+    return CAR_OK;
 }
 
 extern "C" int car_train_create(const CarModelDesc* desc, const CarTrainWeights* w, int32_t max_batch, int32_t max_img_tokens,
@@ -1039,7 +1065,7 @@ extern "C" int car_train_create(const CarModelDesc* desc, const CarTrainWeights*
     if (!desc || !w || !out || !rope_table) CAR_FAIL(CAR_ERR_ARG, "null argument");
     const CarModelDesc& d = *desc;
     if (d.dtype != CAR_F32) CAR_FAIL(CAR_ERR_UNSUPPORTED, "training forward takes the fp32 master weights (bf16 autocast is applied inside)");
-    if (d.dim % 64 != 0 || d.dim / d.n_head != 64 || d.n_layer % 3 != 0 || d.ffn_dim % 8 != 0 || d.vocab_size % 8 != 0 || w->adapter_dim % 8 != 0 ||
+    if (d.n_head <= 0 || d.dim != d.n_head * 64 || d.n_layer % 3 != 0 || d.ffn_dim % 8 != 0 || d.vocab_size % 8 != 0 || w->adapter_dim % 8 != 0 ||
         (d.model_type == 1 && d.caption_dim % 8 != 0))
         CAR_FAIL(CAR_ERR_UNSUPPORTED, "shape not supported (head_dim 64, dims multiple of 8, n_layer multiple of 3)");
     if (max_batch <= 0 || max_img_tokens <= 0) CAR_FAIL(CAR_ERR_ARG, "bad capacity");
@@ -1047,57 +1073,13 @@ extern "C" int car_train_create(const CarModelDesc* desc, const CarTrainWeights*
     CarTrain* t = new CarTrain();
     t->d = d; t->w = *w; t->rope = rope_table;
     t->maxB = max_batch; t->maxN = max_img_tokens; t->maxS = d.cls_token_num + max_img_tokens - 1;
-    const int L = d.n_layer, dim = d.dim, F = d.ffn_dim, V = d.vocab_size;
-    auto copyp = [&](std::vector<const void*>& v, const void* const* src) { v.assign(src, src + L); };
-    copyp(t->attention_norm, w->w.attention_norm); copyp(t->wqkv, w->w.wqkv); copyp(t->wo, w->w.wo); copyp(t->ffn_norm, w->w.ffn_norm);
-    copyp(t->w1, w->w.w1); copyp(t->w3, w->w.w3); copyp(t->w2, w->w.w2);
-    int rc = CAR_OK;
-    auto A = [&](bf16** p, size_t elems) { if (rc == CAR_OK) rc = alloc_dev(t->owned, (void**)p, elems * 2); };
-    t->b_wqkv.resize(L); t->b_wo.resize(L); t->b_w1.resize(L); t->b_w3.resize(L); t->b_w2.resize(L);
-    for (int l = 0; l < L; ++l) {
-        A(&t->b_wqkv[l], (size_t)3 * dim * dim); A(&t->b_wo[l], (size_t)dim * dim);
-        A(&t->b_w1[l], (size_t)F * dim); A(&t->b_w3[l], (size_t)F * dim); A(&t->b_w2[l], (size_t)dim * F);
-    }
-    A(&t->b_out, (size_t)V * dim);
-    t->b_cap1 = t->b_cap2 = nullptr;
-    if (d.model_type == 1) { A(&t->b_cap1, (size_t)dim * d.caption_dim); A(&t->b_cap2, (size_t)dim * dim); }
-    A(&t->b_cond1, (size_t)dim * dim); A(&t->b_cond2, (size_t)dim * dim);
-    for (int j = 0; j < 3; ++j) { A(&t->b_ctl1[j], (size_t)dim * dim); A(&t->b_ctl2[j], (size_t)dim * dim); }
-    A(&t->b_ad1, (size_t)dim * w->adapter_dim); A(&t->b_ad2, (size_t)dim * dim);
-    const size_t R = (size_t)t->maxB * t->maxS, RC = (size_t)t->maxB * t->maxN;
-    if (rc == CAR_OK) rc = alloc_dev(t->owned, (void**)&t->h, R * dim * 4);
-    if (rc == CAR_OK) rc = alloc_dev(t->owned, (void**)&t->nll, RC * 4);
-    A(&t->x, std::max(R * dim, (size_t)t->maxB * d.cls_token_num * std::max(d.caption_dim, dim)));
-    A(&t->qkv, R * 3 * dim); A(&t->q, R * dim); A(&t->kc, R * dim); A(&t->vc, R * dim); A(&t->att, R * dim);
-    A(&t->g, R * F); A(&t->u, R * F); A(&t->act, R * F); A(&t->o, R * dim);
-    A(&t->cin, RC * dim); A(&t->ctmp, std::max(RC, (size_t)t->maxB * d.cls_token_num) * dim); A(&t->ctok, RC * dim); A(&t->cadd, RC * dim);
-    A(&t->lg, RC * V);
-    // backward workspaces
-    {
-        auto AF = [&](float** p, size_t elems) { if (rc == CAR_OK) rc = alloc_dev(t->owned, (void**)p, elems * 4); };
-        const size_t cap = (size_t)(d.model_type == 1 ? d.caption_dim : 8), ad = (size_t)w->adapter_dim;
-        const size_t rows_mlp = std::max(RC, (size_t)t->maxB * d.cls_token_num);
-        const size_t Rp = (std::max(R, rows_mlp) + 63) / 64 * 64;
-        const size_t maxN = std::max({(size_t)3 * dim, (size_t)F, (size_t)V}), maxK = std::max({(size_t)F, (size_t)dim, cap, ad});
-        const size_t maxW = std::max({(size_t)3 * dim * dim, (size_t)F * dim, (size_t)V * dim, (size_t)dim * cap, (size_t)dim * ad});
-        t->Rp_max = Rp;
-        AF(&t->hs, (size_t)L * R * dim); AF(&t->dh, R * dim); AF(&t->h0, R * dim); AF(&t->scr, R * dim);
-        AF(&t->part, (size_t)TR_COLSUM_CHUNKS * dim); AF(&t->lse, (size_t)t->maxB * d.n_head * t->maxS); AF(&t->dsum, (size_t)t->maxB * d.n_head * t->maxS);
-        A(&t->capx, (size_t)t->maxB * d.cls_token_num * cap);
-        A(&t->x2, R * dim); A(&t->db, R * dim); A(&t->dact, R * F); A(&t->dg, R * F); A(&t->du, R * F); A(&t->dx, R * dim);
-        A(&t->datt, R * dim); A(&t->dq, R * dim); A(&t->dk, R * dim); A(&t->dv, R * dim); A(&t->dqkv, R * 3 * dim); A(&t->dlg, RC * V);
-        A(&t->wT, maxW); A(&t->dWb, maxW); A(&t->yT, maxN * Rp); A(&t->xT, maxK * Rp);
-        A(&t->m_t, rows_mlp * dim); A(&t->m_a, rows_mlp * dim); A(&t->m_da, rows_mlp * dim); A(&t->m_dt, rows_mlp * dim);
-        A(&t->dctok, RC * dim); A(&t->dcin, RC * dim); A(&t->dadd, rows_mlp * dim);
-    }
-    if (rc != CAR_OK) { for (void* p : t->owned) cudaFree(p); delete t; return rc; }
+    const int rc = train_init(t);
+    if (rc != CAR_OK) { delete t; return rc; }
     *out = t;
     return CAR_OK;
 }
 
 extern "C" int car_train_destroy(CarTrain* t) {
-    if (!t) return CAR_OK;
-    for (void* p : t->owned) cudaFree(p);
     delete t;
     return CAR_OK;
 }
@@ -1121,7 +1103,7 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     const int n = n_img - 1, S = T + n, R = B * S, RC = B * n_img, step3 = L / 3;
     if (has_feat && l % step3 == 0) {
         CAR_TRY(tr_mlp(st, t->ctok, RC, dim, t->b_ctl1[l / step3], t->b_ctl2[l / step3], dim, t->ctmp, t->cadd));
-        CAR_LAUNCH(tr_add_rows_kernel, tr_grid((long long)RC * dim), 256, 0, st, t->h, (const bf16*)t->cadd, B, n_img, S, T - 1, dim);
+        CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)RC * dim), 256, 0, st, t->h, (const bf16*)t->cadd, B, n_img, S, T - 1, dim);
     }
     if (for_bwd) CAR_CUDA(cudaMemcpyAsync(t->h0, t->h, (size_t)R * dim * 4, cudaMemcpyDeviceToDevice, st));
     size_t att_smem = 0;
@@ -1132,7 +1114,7 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     CAR_LAUNCH(tr_attention_kernel, (unsigned)(((long long)B * H * S + TRA_WARPS - 1) / TRA_WARPS), TRA_WARPS * 32, att_smem, st, (const bf16*)t->q,
                (const bf16*)t->kc, (const bf16*)t->vc, mask, B, H, S, t->att);
     CAR_TRY(dense_linear(st, t->att, dim, t->b_wo[l], R, dim, dim, ACT_NONE, nullptr, 0, t->o, dim));
-    CAR_LAUNCH(tr_add_rows_kernel, tr_grid((long long)R * dim), 256, 0, st, t->h, (const bf16*)t->o, B, S, S, 0, dim);
+    CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)R * dim), 256, 0, st, t->h, (const bf16*)t->o, B, S, S, 0, dim);
     bf16* xn = for_bwd ? t->x2 : t->x;
     CAR_LAUNCH(tr_rmsnorm_kernel, R, 256, 0, st, (const float*)t->h, (const float*)t->ffn_norm[l], xn, dim, d.norm_eps, S, S, 0);
     CAR_TRY(dense_linear(st, xn, dim, t->b_w1[l], R, F, dim, ACT_NONE, nullptr, 0, t->g, F));
@@ -1140,7 +1122,7 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     CAR_LAUNCH(swiglu_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, t->act, (long long)R * F);
     if (for_bwd) return CAR_OK;
     CAR_TRY(dense_linear(st, t->act, F, t->b_w2[l], R, dim, F, ACT_NONE, nullptr, 0, t->o, dim));
-    CAR_LAUNCH(tr_add_rows_kernel, tr_grid((long long)R * dim), 256, 0, st, t->h, (const bf16*)t->o, B, S, S, 0, dim);
+    CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)R * dim), 256, 0, st, t->h, (const bf16*)t->o, B, S, S, 0, dim);
     return CAR_OK;
 }
 
@@ -1171,10 +1153,10 @@ extern "C" int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const in
     }
     // 1. prefix rows: CaptionEmbedder (token_drop, cap_proj) gpt_t2i.py:145-162 or LabelEmbedder :78-97; image-token rows :423
     if (d.model_type == 1) {
-        CAR_LAUNCH(tr_caption_select_kernel, tr_grid((long long)B * T * d.caption_dim), 256, 0, st, (const float*)cond, (const float*)t->w.cap_uncond,
+        CAR_LAUNCH(tr_caption_select_kernel, gsz((long long)B * T * d.caption_dim), 256, 0, st, (const float*)cond, (const float*)t->w.cap_uncond,
                    drop_ids, t->capx, B, T, d.caption_dim);
         CAR_TRY(tr_mlp(st, t->capx, B * T, d.caption_dim, t->b_cap1, t->b_cap2, dim, t->ctmp, t->o));
-        CAR_LAUNCH(tr_put_rows_bf16_kernel, tr_grid((long long)B * T * dim), 256, 0, st, (const bf16*)t->o, t->h, B, T, S, 0, dim);
+        CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const bf16*)t->o, t->h, B, T, S, 0, dim);
     } else {
         CAR_LAUNCH(tr_embed_rows_kernel, B, 256, 0, st, (const float*)t->w.w.label_table, (const int*)cond, 1, drop_ids, t->w.num_classes, t->h, B, 1, S, 0, dim);
     }
@@ -1182,7 +1164,7 @@ extern "C" int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const in
     // 2. control tokens: adapter_mlp -> token_drop -> condition_mlp  gpt_t2i.py:424-427 (feat = the control encoder's output tokens)
     if (feat) {
         CAR_TRY(tr_mlp(st, (const bf16*)feat, RC, t->w.adapter_dim, t->b_ad1, t->b_ad2, dim, t->ctmp, t->cin));
-        CAR_LAUNCH(tr_select_uncond_kernel, tr_grid((long long)RC * dim), 256, 0, st, t->cin, (const float*)t->w.cond_uncond, drop_ids, B, (long long)n_img * dim);
+        CAR_LAUNCH(tr_select_uncond_kernel, gsz((long long)RC * dim), 256, 0, st, t->cin, (const float*)t->w.cond_uncond, drop_ids, B, (long long)n_img * dim);
         CAR_TRY(tr_mlp(st, t->cin, RC, dim, t->b_cond1, t->b_cond2, dim, t->ctmp, t->ctok));
     }
     // 3. blocks  gpt_t2i.py:456-468; the stream at every block input is kept for the backward's recompute
@@ -1197,7 +1179,7 @@ extern "C" int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const in
         CAR_LAUNCH(tr_ce_rows_kernel, RC, 256, 0, st, (const bf16*)t->lg, (const int*)targets, logits_out, t->nll, V);
         CAR_LAUNCH(tr_ce_reduce_kernel, 1, 1024, 0, st, (const float*)t->nll, valid, B, n_img, loss_out);
     } else if (logits_out) {
-        CAR_LAUNCH(tr_put_rows_bf16_kernel, tr_grid((long long)RC * V), 256, 0, st, (const bf16*)t->lg, logits_out, 1, RC, RC, 0, V);
+        CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)RC * V), 256, 0, st, (const bf16*)t->lg, logits_out, 1, RC, RC, 0, V);
     }
     t->fB = B; t->fN = n_img; t->f_idx = idx; t->f_cond = cond; t->f_feat = feat; t->f_drop = drop_ids; t->f_mask = mask; t->f_targets = targets;
     t->f_valid = valid;
@@ -1219,7 +1201,7 @@ static int tr_wgrad(CarTrain* t, cudaStream_t st, const bf16* dY, const bf16* X,
     CAR_LAUNCH(tr_transpose_pad_kernel, dim3(Rp / 32, (N + 31) / 32), dim3(32, 8), 0, st, dY, t->yT, rows, N, Rp);
     CAR_LAUNCH(tr_transpose_pad_kernel, dim3(Rp / 32, (K + 31) / 32), dim3(32, 8), 0, st, X, t->xT, rows, K, Rp);
     CAR_TRY(dense_linear(st, t->yT, Rp, t->xT, N, K, Rp, ACT_NONE, nullptr, 0, t->dWb, K));
-    CAR_LAUNCH(tr_bf16_to_f32_kernel, tr_grid((long long)N * K), 256, 0, st, (const bf16*)t->dWb, grad, (long long)N * K);
+    CAR_LAUNCH(tr_bf16_to_f32_kernel, gsz((long long)N * K), 256, 0, st, (const bf16*)t->dWb, grad, (long long)N * K);
     return CAR_OK;
 }
 // RMSNorm backward on `rows` output rows (row map like tr_rmsnorm_kernel) + the weight gradient
@@ -1237,10 +1219,10 @@ static int tr_mlp_bwd(CarTrain* t, cudaStream_t st, const bf16* x, int rows, int
                       const bf16* resid, bf16* dX, float* g1, float* g2) {
     const int dim = t->d.dim;
     CAR_TRY(dense_linear(st, x, K, fc1, rows, dim, K, ACT_NONE, nullptr, 0, t->m_t, dim));
-    CAR_LAUNCH(tr_gelu_kernel, tr_grid((long long)rows * dim), 256, 0, st, (const bf16*)t->m_t, t->m_a, (long long)rows * dim);
+    CAR_LAUNCH(tr_gelu_kernel, gsz((long long)rows * dim), 256, 0, st, (const bf16*)t->m_t, t->m_a, (long long)rows * dim);
     CAR_TRY(tr_wgrad(t, st, dY, t->m_a, rows, dim, dim, g2));
     CAR_TRY(tr_dgrad(t, st, dY, fc2, rows, dim, dim, nullptr, t->m_da));
-    CAR_LAUNCH(tr_gelu_bwd_kernel, tr_grid((long long)rows * dim), 256, 0, st, (const bf16*)t->m_t, (const bf16*)t->m_da, t->m_dt, (long long)rows * dim);
+    CAR_LAUNCH(tr_gelu_bwd_kernel, gsz((long long)rows * dim), 256, 0, st, (const bf16*)t->m_t, (const bf16*)t->m_da, t->m_dt, (long long)rows * dim);
     CAR_TRY(tr_wgrad(t, st, t->m_dt, x, rows, dim, K, g1));
     if (dX) CAR_TRY(tr_dgrad(t, st, t->m_dt, fc1, rows, dim, K, resid, dX));
     return CAR_OK;
@@ -1277,7 +1259,7 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         CAR_CUDA(cudaMemcpyAsync(t->h, t->hs + (size_t)l * R * dim, (size_t)R * dim * 4, cudaMemcpyDeviceToDevice, st));
         CAR_TRY(tr_block_fwd(t, st, l, B, n_img, mask, has_feat, true));
         // feed-forward: h_out = h_mid + w2(silu(w1 x2) * w3 x2)
-        CAR_LAUNCH(tr_take_rows_bf16_kernel, tr_grid((long long)R * dim), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim);
+        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)R * dim), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim);
         CAR_TRY(tr_wgrad(t, st, t->db, t->act, R, dim, F, g->w.w2 ? (float*)g->w.w2[l] : nullptr));
         CAR_TRY(tr_dgrad(t, st, t->db, t->b_w2[l], R, dim, F, nullptr, t->dact));
         CAR_LAUNCH(tr_swiglu_bwd_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, (const bf16*)t->dact, t->dg, t->du, (long long)R * F);
@@ -1287,7 +1269,7 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         CAR_TRY(tr_dgrad(t, st, t->du, t->b_w3[l], R, F, dim, t->dx, t->dx));
         CAR_TRY(tr_norm_bwd(t, st, t->h, t->ffn_norm[l], t->dx, R, S, S, 0, g->w.ffn_norm ? (float*)g->w.ffn_norm[l] : nullptr));
         // attention: h_mid = h0 + wo(sdpa(rope(wqkv x1)))
-        CAR_LAUNCH(tr_take_rows_bf16_kernel, tr_grid((long long)R * dim), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim);
+        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)R * dim), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim);
         CAR_TRY(tr_wgrad(t, st, t->db, t->att, R, dim, dim, g->w.wo ? (float*)g->w.wo[l] : nullptr));
         CAR_TRY(tr_dgrad(t, st, t->db, t->b_wo[l], R, dim, dim, nullptr, t->datt));
         CAR_LAUNCH(tr_attn_bwd_q_kernel, att_grid, TRA_WARPS * 32, smem_q, st, (const bf16*)t->q, (const bf16*)t->kc, (const bf16*)t->vc, mask,
@@ -1301,7 +1283,7 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         // control add h[:, T-1:] += condition_layers[j](condition_token)
         if (has_feat && l % step3 == 0) {
             const int j = l / step3;
-            CAR_LAUNCH(tr_take_rows_bf16_kernel, tr_grid((long long)RC * dim), 256, 0, st, (const float*)t->dh, t->dadd, B, n_img, S, T - 1, dim);
+            CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)RC * dim), 256, 0, st, (const float*)t->dh, t->dadd, B, n_img, S, T - 1, dim);
             CAR_TRY(tr_mlp_bwd(t, st, t->ctok, RC, dim, t->b_ctl1[j], t->b_ctl2[j], t->dadd, first_ctl ? nullptr : t->dctok, t->dctok,
                                (float*)g->w.ctl_fc1[j], (float*)g->w.ctl_fc2[j]));
             first_ctl = false;
@@ -1314,7 +1296,7 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
                    (float*)g->w.tok_embeddings, B, n, S, T, dim);
     }
     if (d.model_type == 1) {
-        CAR_LAUNCH(tr_take_rows_bf16_kernel, tr_grid((long long)B * T * dim), 256, 0, st, (const float*)t->dh, t->dadd, B, T, S, 0, dim);
+        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const float*)t->dh, t->dadd, B, T, S, 0, dim);
         CAR_TRY(tr_mlp_bwd(t, st, t->capx, B * T, d.caption_dim, t->b_cap1, t->b_cap2, t->dadd, nullptr, nullptr, (float*)g->w.cap_fc1, (float*)g->w.cap_fc2));
     } else if (g->w.label_table) {
         CAR_CUDA(cudaMemsetAsync((void*)g->w.label_table, 0, (size_t)(t->w.num_classes + 1) * dim * 4, st));
@@ -1323,7 +1305,7 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
     }
     if (has_feat) {
         CAR_TRY(tr_mlp_bwd(t, st, t->cin, RC, dim, t->b_cond1, t->b_cond2, t->dctok, nullptr, t->dcin, (float*)g->w.cond_fc1, (float*)g->w.cond_fc2));
-        CAR_LAUNCH(tr_zero_dropped_kernel, tr_grid((long long)RC * dim), 256, 0, st, t->dcin, t->f_drop, B, (long long)n_img * dim);
+        CAR_LAUNCH(tr_zero_dropped_kernel, gsz((long long)RC * dim), 256, 0, st, t->dcin, t->f_drop, B, (long long)n_img * dim);
         CAR_TRY(tr_mlp_bwd(t, st, (const bf16*)t->f_feat, RC, t->w.adapter_dim, t->b_ad1, t->b_ad2, t->dcin, nullptr, (bf16*)d_feat,
                            (float*)g->adapter_fc1, (float*)g->adapter_fc2));
     }
@@ -1346,14 +1328,23 @@ extern "C" int car_adamw_step(const void* tensors_dev, const void* chunks_dev, i
 // v1.1 / flan architecture: gated gelu_new feed-forward, no biases, RMS layer norm (eps 1e-6), relative position bias of block 0
 // shared by every block, no 1/sqrt(d) scaling.  GEMMs: dense_linear (wgmma); glue: t5.cuh.
 // ---------------------------------------------------------------------------------------------------------
-struct CarT5 {
+struct CarT5 : CarOwned {
     CarT5Desc d;
     const void *embed, *rel_bias, *final_norm;
     std::vector<const void*> ln1, wq, wk, wv, wo, ln2, wi0, wi1, wo2;
     int max_rows;
     bf16 *h, *x, *q, *k, *v, *att, *g, *u, *act;
-    std::vector<void*> owned;
 };
+
+static int t5_init(CarT5* t) {
+    const CarT5Desc& d = t->d;
+    const size_t R = (size_t)t->max_rows, inner = (size_t)d.n_heads * 64;
+    CAR_TRY(t->alloc(&t->h, R * d.d_model * 2)); CAR_TRY(t->alloc(&t->x, R * d.d_model * 2));
+    CAR_TRY(t->alloc(&t->q, R * inner * 2)); CAR_TRY(t->alloc(&t->k, R * inner * 2)); CAR_TRY(t->alloc(&t->v, R * inner * 2));
+    CAR_TRY(t->alloc(&t->att, R * inner * 2));
+    CAR_TRY(t->alloc(&t->g, R * d.d_ff * 2)); CAR_TRY(t->alloc(&t->u, R * d.d_ff * 2)); CAR_TRY(t->alloc(&t->act, R * d.d_ff * 2));
+    return CAR_OK;
+}
 
 extern "C" int car_t5_create(const CarT5Desc* desc, const CarT5Weights* w, int32_t max_rows, void* stream, CarT5** out) {
     if (!desc || !w || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
@@ -1368,18 +1359,12 @@ extern "C" int car_t5_create(const CarT5Desc* desc, const CarT5Weights* w, int32
     auto cp = [&](std::vector<const void*>& v, const void* const* src) { v.assign(src, src + L); };
     cp(t->ln1, w->ln1); cp(t->wq, w->q); cp(t->wk, w->k); cp(t->wv, w->v); cp(t->wo, w->o); cp(t->ln2, w->ln2);
     cp(t->wi0, w->wi_0); cp(t->wi1, w->wi_1); cp(t->wo2, w->wo);
-    const size_t R = (size_t)max_rows, inner = (size_t)d.n_heads * 64;
-    int rc = CAR_OK;
-    auto A = [&](bf16** p, size_t elems) { if (rc == CAR_OK) rc = alloc_dev(t->owned, (void**)p, elems * 2); };
-    A(&t->h, R * d.d_model); A(&t->x, R * d.d_model); A(&t->q, R * inner); A(&t->k, R * inner); A(&t->v, R * inner); A(&t->att, R * inner);
-    A(&t->g, R * d.d_ff); A(&t->u, R * d.d_ff); A(&t->act, R * d.d_ff);
-    if (rc != CAR_OK) { for (void* p : t->owned) cudaFree(p); delete t; return rc; }
+    const int rc = t5_init(t);
+    if (rc != CAR_OK) { delete t; return rc; }
     *out = t;
     return CAR_OK;
 }
 extern "C" int car_t5_destroy(CarT5* t) {
-    if (!t) return CAR_OK;
-    for (void* p : t->owned) cudaFree(p);
     delete t;
     return CAR_OK;
 }
@@ -1407,7 +1392,7 @@ extern "C" int car_t5_forward(CarT5* t, const int32_t* ids, const int32_t* mask,
         CAR_LAUNCH((rmsnorm_rows_kernel<bf16>), R, 256, 0, st, (const bf16*)t->h, (const bf16*)t->ln2[l], t->x, dm, d.eps);
         CAR_TRY(dense_linear(st, t->x, dm, t->wi0[l], R, F, dm, ACT_NONE, nullptr, 0, t->g, F));
         CAR_TRY(dense_linear(st, t->x, dm, t->wi1[l], R, F, dm, ACT_NONE, nullptr, 0, t->u, F));
-        CAR_LAUNCH(t5_geglu_kernel, (int)std::min<long long>(((long long)R * F + 255) / 256, sm_count() * 16), 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, t->act,
+        CAR_LAUNCH(t5_geglu_kernel, gsz((long long)R * F), 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, t->act,
                    (long long)R * F);
         CAR_TRY(dense_linear(st, t->act, F, t->wo2[l], R, dm, F, ACT_NONE, t->h, dm, t->h, dm));
     }

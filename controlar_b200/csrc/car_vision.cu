@@ -12,19 +12,13 @@
 #include "dpt.cuh"
 #include "midas.cuh"
 
-static int vis_sm_count() {
-    int dev = 0, n = 132;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-    return n;
-}
 // wgmma path of the vision stages (gemm_wgmma.cuh): TMA tensor-map loads, accumulators in registers, persistent warp-specialised CTAs.
 // Used only where the driver provides the TMA tensor-map encoder (wg_encoder() != nullptr).
 static int wg_launch(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, const WgP& q, int tiles_m) {
     static DevOnce once5;
     if (once5.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
     const int ntiles = tiles_m * ((q.N + WG_BN - 1) / WG_BN);
-    CAR_LAUNCH(gemm_wgmma_kernel, std::min(ntiles, vis_sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
+    CAR_LAUNCH(gemm_wgmma_kernel, std::min(ntiles, sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
     return CAR_OK;
 }
 
@@ -55,33 +49,6 @@ static DenseP dp_plain(const bf16* A, int lda, const bf16* B, int ldb, int M, in
     p.A = A; p.B = B; p.M = M; p.N = N; p.K = K; p.lda = lda; p.ldb = ldb; p.C = C; p.ldc = ldc; p.alpha = 1.f;
     return p;
 }
-static inline int gsz(long long total, int block = 256) { return (int)std::min<long long>((total + block - 1) / block, vis_sm_count() * 16); }
-
-struct Arena {   // grow-only device workspace, re-used across calls (no allocation in steady state)
-    char* base = nullptr; size_t cap = 0, off = 0;
-    int reserve(size_t bytes) {
-        if (bytes <= cap) return CAR_OK;
-        if (base) cudaFree(base);
-        base = nullptr; cap = 0;
-        CAR_CUDA(cudaMalloc(&base, bytes));
-        cap = bytes;
-        return CAR_OK;
-    }
-    void reset() { off = 0; }
-    void* take(size_t bytes) { void* p = base + off; off += (bytes + 255) & ~(size_t)255; return p; }
-    void release() { if (base) cudaFree(base); base = nullptr; cap = 0; }
-};
-
-// Base of every handle: the device memory its create call allocated and its forward workspace, both freed by `delete`.
-struct CarOwned {
-    std::vector<void*> owned;
-    Arena ws;
-    ~CarOwned() {
-        for (void* p : owned) cudaFree(p);
-        ws.release();
-    }
-};
-
 template <typename... KArgs, typename... Args>
 static int launch_on(cudaStream_t st, void (*kernel)(KArgs...), unsigned grid, unsigned block, Args... args) {
     CAR_LAUNCH(kernel, grid, block, 0, st, args...);
@@ -122,11 +89,8 @@ struct TensorReader {
     }
     void* alloc(size_t bytes) {
         void* p = nullptr;
-        if (!ok()) return nullptr;
-        cuda(cudaMalloc(&p, bytes), "cudaMalloc");
-        if (!ok()) return nullptr;
-        m->owned.push_back(p);
-        return p;
+        if (ok() && m->alloc(&p, bytes) != CAR_OK) fail(CAR_ERR_CUDA, g_car_err);
+        return ok() ? p : nullptr;
     }
     void copy(float* dst, const float* src, long long count) {
         if (ok()) cuda(cudaMemcpyAsync(dst, src, (size_t)count * 4, cudaMemcpyDeviceToDevice, st), "copy");
@@ -180,14 +144,13 @@ struct CarDino : CarOwned {
 };
 
 template <typename TI>
-static int to_bf16(cudaStream_t st, std::vector<void*>& owned, const void* src, long long n, bf16** dst) {
-    CAR_CUDA(cudaMalloc((void**)dst, (size_t)n * 2));
-    owned.push_back(*dst);
+static int to_bf16(cudaStream_t st, CarOwned* m, const void* src, long long n, bf16** dst) {
+    CAR_TRY(m->alloc(dst, (size_t)n * 2));
     CAR_LAUNCH((cast_to_bf16_kernel<TI>), gsz(n), 256, 0, st, (const TI*)src, *dst, n);
     return CAR_OK;
 }
-static int to_bf16_any(cudaStream_t st, int dtype, std::vector<void*>& owned, const void* src, long long n, bf16** dst) {
-    return dtype == CAR_BF16 ? to_bf16<bf16>(st, owned, src, n, dst) : to_bf16<float>(st, owned, src, n, dst);
+static int to_bf16_any(cudaStream_t st, int dtype, CarOwned* m, const void* src, long long n, bf16** dst) {
+    return dtype == CAR_BF16 ? to_bf16<bf16>(st, m, src, n, dst) : to_bf16<float>(st, m, src, n, dst);
 }
 
 extern "C" int car_dino_create(const CarDinoDesc* desc, const CarDinoWeights* w, void* stream, CarDino** out) {
@@ -206,17 +169,16 @@ extern "C" int car_dino_create(const CarDinoDesc* desc, const CarDinoWeights* w,
     m->kpad = (m->kpatch + 31) & ~31;
     {
         bf16* tmp = nullptr;
-        T(to_bf16_any(st, dt, m->owned, w->patch_w, (long long)C * m->kpatch, &tmp));
-        if (r == CAR_OK && cudaMalloc((void**)&m->w_patch, (size_t)C * m->kpad * 2) != cudaSuccess) r = CAR_ERR_CUDA;
+        T(to_bf16_any(st, dt, m, w->patch_w, (long long)C * m->kpatch, &tmp));
+        if (r == CAR_OK) r = m->alloc(&m->w_patch, (size_t)C * m->kpad * 2);
         if (r == CAR_OK) {
-            m->owned.push_back(m->w_patch);
             cudaMemsetAsync(m->w_patch, 0, (size_t)C * m->kpad * 2, st);
             cudaMemcpy2DAsync(m->w_patch, (size_t)m->kpad * 2, tmp, (size_t)m->kpatch * 2, (size_t)m->kpatch * 2, C, cudaMemcpyDeviceToDevice, st);
         }
     }
     auto cv = [&](const void* src, long long n) -> const void* {   // bf16 view of a (possibly fp32) vector / matrix
         bf16* p = nullptr;
-        T(to_bf16_any(st, dt, m->owned, src, n, &p));
+        T(to_bf16_any(st, dt, m, src, n, &p));
         return p;
     };
     m->b_patch = cv(w->patch_b, C); m->cls = w->cls_token; m->pos = w->pos_emb;
@@ -225,8 +187,9 @@ extern "C" int car_dino_create(const CarDinoDesc* desc, const CarDinoWeights* w,
     for (int l = 0; l < d.layers && r == CAR_OK; ++l) {
         CarDino::Layer& Ly = m->L[l];
         // q and k fused into one [2C][C] weight (+bias); v kept separate (computed transposed)
-        if (cudaMalloc((void**)&Ly.w_qk, (size_t)2 * C * C * 2) != cudaSuccess || cudaMalloc((void**)&Ly.b_qk, (size_t)2 * C * 2) != cudaSuccess) { r = CAR_ERR_CUDA; break; }
-        m->owned.push_back(Ly.w_qk); m->owned.push_back(Ly.b_qk);
+        r = m->alloc(&Ly.w_qk, (size_t)2 * C * C * 2);
+        if (r == CAR_OK) r = m->alloc(&Ly.b_qk, (size_t)2 * C * 2);
+        if (r != CAR_OK) break;
         const bf16 *wq = (const bf16*)cv(w->q_w[l], (long long)C * C), *wk = (const bf16*)cv(w->k_w[l], (long long)C * C);
         const bf16 *bq = (const bf16*)cv(w->q_b[l], C), *bk = (const bf16*)cv(w->k_b[l], C);
         if (r != CAR_OK) break;
@@ -789,8 +752,8 @@ extern "C" int car_resize_bilinear_aa(const float* in, int32_t B, int32_t Cc, in
     if (B <= 0 || Cc <= 0 || H <= 0 || W <= 0 || OH <= 0 || OW <= 0) CAR_FAIL(CAR_ERR_ARG, "bad shape");
     cudaStream_t st = (cudaStream_t)stream;
     const long long n1 = (long long)B * Cc * H * OW, n2 = (long long)B * Cc * OH * OW;
-    CAR_LAUNCH(resize_aa_axis_kernel, (int)std::min<long long>((n1 + 255) / 256, vis_sm_count() * 16), 256, 0, st, in, tmp, (long long)B * Cc * H, W, OW, 1);
-    CAR_LAUNCH(resize_aa_axis_kernel, (int)std::min<long long>((n2 + 255) / 256, vis_sm_count() * 16), 256, 0, st, (const float*)tmp, out, (long long)B * Cc, H, OH, OW);
+    CAR_LAUNCH(resize_aa_axis_kernel, gsz(n1), 256, 0, st, in, tmp, (long long)B * Cc * H, W, OW, 1);
+    CAR_LAUNCH(resize_aa_axis_kernel, gsz(n2), 256, 0, st, (const float*)tmp, out, (long long)B * Cc, H, OH, OW);
     return CAR_OK;
 }
 
@@ -1172,7 +1135,7 @@ static int wg_launch_f32(cudaStream_t st, const CUtensorMap& mapA, const CUtenso
     static DevOnce once;
     if (once.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_wgmma_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
     const int ntiles = tiles_m * ((q.N + WG_BN - 1) / WG_BN);
-    CAR_LAUNCH(gemm_wgmma_f32_kernel, std::min(ntiles, vis_sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
+    CAR_LAUNCH(gemm_wgmma_f32_kernel, std::min(ntiles, sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
     return CAR_OK;
 }
 // out fp32 [M][ldc] = a3 (S3 rows [M][3 w.k]) · W3^T + bias (+ resid [M][ldc])

@@ -3,9 +3,11 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include <algorithm>
 #include <atomic>
 #include <string>
 #include <cstring>
+#include <vector>
 
 #include "../../include/controlar_b200.h"
 
@@ -43,6 +45,50 @@ extern std::atomic<long long> g_car_launches;
 struct DevOnce {
     bool done[64] = {false};
     bool first() { int dev = 0; cudaGetDevice(&dev); if (dev < 0 || dev >= 64) return true; const bool f = !done[dev]; done[dev] = true; return f; }
+};
+
+// SM count of the CURRENT device (the Python handles make the tensors' device current around every call)
+inline int sm_count() {
+    static int cached[64] = {0};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64) dev = 0;
+    if (cached[dev] == 0) { int n = 0; cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); cached[dev] = n > 0 ? n : 132; }
+    return cached[dev];
+}
+
+// grid of a grid-stride loop over `total` elements in blocks of 256 threads: at most 16 CTAs per SM
+inline int gsz(long long total) { return (int)std::min<long long>((total + 255) / 256, sm_count() * 16); }
+
+struct Arena {   // grow-only device workspace, re-used across calls (no allocation in steady state)
+    char* base = nullptr; size_t cap = 0, off = 0;
+    int reserve(size_t bytes) {
+        if (bytes <= cap) return CAR_OK;
+        if (base) cudaFree(base);
+        base = nullptr; cap = 0;
+        CAR_CUDA(cudaMalloc(&base, bytes));
+        cap = bytes;
+        return CAR_OK;
+    }
+    void reset() { off = 0; }
+    void* take(size_t bytes) { void* p = base + off; off += (bytes + 255) & ~(size_t)255; return p; }
+    void release() { if (base) cudaFree(base); base = nullptr; cap = 0; }
+};
+
+// Base of every handle: the device memory its create call allocated and its forward workspace, both freed by `delete`.
+struct CarOwned {
+    std::vector<void*> owned;
+    Arena ws;
+    // device memory that lives as long as the handle (a zero-byte request still gets its own allocation)
+    template <typename T> int alloc(T** p, size_t bytes) {
+        CAR_CUDA(cudaMalloc((void**)p, bytes ? bytes : 16));
+        owned.push_back((void*)*p);
+        return CAR_OK;
+    }
+    ~CarOwned() {
+        for (void* p : owned) cudaFree(p);
+        ws.release();
+    }
 };
 
 // every kernel launch goes through this so that car_launch_count() is an honest count

@@ -11,141 +11,102 @@ from typing import List, Optional
 import torch
 
 from . import _lib
-import functools
+from ._lib import (CarModelDesc, CarSampling, CarTrainWeights, CarWeights, check, cur_stream, dtype_code, on_own_device,
+                   param_signature, _ptr, _ptr_array)
 
-from ._lib import CarModelDesc, CarSampling, CarWeights, check, cur_stream, dtype_code, _ptr, _ptr_array
+
+def _desc(m) -> CarModelDesc:
+    cfg = m.config
+    t2i = m.model_type == "t2i"
+    return CarModelDesc(dtype=dtype_code(m.tok_embeddings.weight.dtype), dim=cfg.dim, n_layer=cfg.n_layer, n_head=cfg.n_head,
+                        ffn_dim=m.layers[0].feed_forward.w1.weight.shape[0], vocab_size=cfg.vocab_size,
+                        cls_token_num=cfg.cls_token_num, block_size=cfg.block_size, caption_dim=cfg.caption_dim if t2i else 0,
+                        model_type=1 if t2i else 0, norm_eps=cfg.norm_eps, rope_base=cfg.rope_base)
 
 
-def _on_own_device(fn):
-    """Run a handle method with the handle's device current: the library launches on the current device and `cur_stream()` is that
-    device's current stream — a model on cuda:1 works without torch.cuda.set_device(1) (ADVICE r1; the reference wraps its calls
-    in `with torch.device(device)`, generate.py:179-182)."""
-    @functools.wraps(fn)
-    def wrapped(self, *a, **k):
-        dev = getattr(self, "device", None)
-        if dev is None or dev.type != "cuda":
-            return fn(self, *a, **k)
-        with torch.cuda.device(dev):
-            return fn(self, *a, **k)
-    return wrapped
+def _weights(m):
+    """CarWeights over the transformer's weights, and the tensors whose storage the library borrows through it (the per-layer
+    pointer arrays are kept alive by the CarWeights itself)."""
+    w = CarWeights()
+    ts = []
+
+    def P(t):
+        t = t.detach()
+        ts.append(t)
+        return _ptr(t)
+    w.tok_embeddings, w.norm, w.output = P(m.tok_embeddings.weight), P(m.norm.weight), P(m.output.weight)
+    for name, get in [("attention_norm", lambda b: b.attention_norm.weight), ("wqkv", lambda b: b.attention.wqkv.weight),
+                      ("wo", lambda b: b.attention.wo.weight), ("ffn_norm", lambda b: b.ffn_norm.weight),
+                      ("w1", lambda b: b.feed_forward.w1.weight), ("w3", lambda b: b.feed_forward.w3.weight),
+                      ("w2", lambda b: b.feed_forward.w2.weight)]:
+        arr = (C.c_void_p * len(m.layers))(*[P(get(b)) for b in m.layers])
+        setattr(w, name, C.cast(arr, C.POINTER(C.c_void_p)))
+    if m.model_type == "t2i":
+        w.cap_fc1, w.cap_fc2 = P(m.cls_embedding.cap_proj.fc1.weight), P(m.cls_embedding.cap_proj.fc2.weight)
+    else:
+        w.label_table = P(m.cls_embedding.embedding_table.weight)
+    w.cond_fc1, w.cond_fc2 = P(m.condition_mlp.cap_proj.fc1.weight), P(m.condition_mlp.cap_proj.fc2.weight)
+    for j in range(3):
+        w.ctl_fc1[j], w.ctl_fc2[j] = P(m.condition_layers[j].fc1.weight), P(m.condition_layers[j].fc2.weight)
+    return w, ts
+
+
+def _layout(m):
+    """What the packed buffers were sized for: a change here needs a new CarModel, anything else a repack in place."""
+    w = m.tok_embeddings.weight
+    return (w.dtype, str(w.device), tuple(w.shape), len(m.layers), tuple(m.layers[0].feed_forward.w1.weight.shape))
 
 
 class ARModelHandle(_lib.NativeHandle):
     """CarModel: GEMM-ready copies of the transformer weights (re-packed when the module's weights change)."""
 
     def __init__(self, module):
+        super().__init__("car_model_destroy")
         self.lib = _lib.lib()
         self.module = module
-        self.handle = C.c_void_p()
-        self.version = None
-        self._keep = None
         self._dirty = 0
-        self.device = module.tok_embeddings.weight.device
         self.generation = 0          # bumped whenever the CarModel handle is re-created: states compare THIS, not the raw pointer
         self._build()
 
-    # the tensors whose storage the library borrows
-    def _weights(self):
-        m = self.module
-        layers = list(m.layers)
-        w = CarWeights()
-        keep = []
+    @property
+    def device(self):
+        return self.module.tok_embeddings.weight.device
 
-        def P(t):
-            keep.append(t)
-            return _ptr(t.detach())
-        w.tok_embeddings = P(m.tok_embeddings.weight)
-        w.norm = P(m.norm.weight)
-        w.output = P(m.output.weight)
-        arrs = {}
-        for name, get in [("attention_norm", lambda b: b.attention_norm.weight), ("wqkv", lambda b: b.attention.wqkv.weight),
-                          ("wo", lambda b: b.attention.wo.weight), ("ffn_norm", lambda b: b.ffn_norm.weight),
-                          ("w1", lambda b: b.feed_forward.w1.weight), ("w3", lambda b: b.feed_forward.w3.weight),
-                          ("w2", lambda b: b.feed_forward.w2.weight)]:
-            ts = [get(b).detach() for b in layers]
-            keep.extend(ts)
-            arrs[name] = _ptr_array(ts)
-            setattr(w, name, C.cast(arrs[name], C.POINTER(C.c_void_p)))
-        if m.model_type == "t2i":
-            w.cap_fc1 = P(m.cls_embedding.cap_proj.fc1.weight)
-            w.cap_fc2 = P(m.cls_embedding.cap_proj.fc2.weight)
-        else:
-            w.label_table = P(m.cls_embedding.embedding_table.weight)
-        w.cond_fc1 = P(m.condition_mlp.cap_proj.fc1.weight)
-        w.cond_fc2 = P(m.condition_mlp.cap_proj.fc2.weight)
-        for j in range(3):
-            w.ctl_fc1[j] = P(m.condition_layers[j].fc1.weight)
-            w.ctl_fc2[j] = P(m.condition_layers[j].fc2.weight)
-        keep.append(arrs)
-        return w, keep
-
-    def _signature(self):
-        """Changes when parameters are replaced (data_ptr / dtype / device) or updated through autograd-visible in-place ops
-        (`_version`).  Writes through `p.data` do NOT bump `_version`: call `invalidate()` after such updates."""
-        m = self.module
-        ps = [m.tok_embeddings.weight, m.output.weight, m.layers[0].attention.wqkv.weight]
-        return tuple((p.data_ptr(), p._version, p.dtype, str(p.device)) for p in ps) + \
-            (sum(p._version for p in m.parameters()), self._dirty)
-
-    def _layout(self):
-        """What the packed buffers were sized for: a change here needs a new CarModel, anything else a repack in place."""
-        m = self.module
-        w = m.tok_embeddings.weight
-        return (w.dtype, str(w.device), tuple(w.shape), len(m.layers), tuple(m.layers[0].feed_forward.w1.weight.shape))
+    def _signature(self, ts):
+        """Changes when a borrowed tensor is replaced (data_ptr / dtype / device; also through `p.data = t`) or updated through
+        autograd-visible in-place ops (`_version`).  Writes into `p.data` in place do NOT bump `_version`: call `invalidate()`."""
+        return param_signature(ts), self._dirty
 
     def invalidate(self):
-        """Force a repack at the next use (after `param.data` writes, which PyTorch's version counters do not see)."""
+        """Force a repack at the next use (after in-place writes into `param.data`, which PyTorch's version counters do not see)."""
         self._dirty += 1
 
-    @_on_own_device
+    @on_own_device
     def _build(self):
         m = self.module
-        self.device = m.tok_embeddings.weight.device
-        cfg = m.config
-        dt = m.tok_embeddings.weight.dtype
-        d = CarModelDesc(dtype=dtype_code(dt), dim=cfg.dim, n_layer=cfg.n_layer, n_head=cfg.n_head,
-                         ffn_dim=m.layers[0].feed_forward.w1.weight.shape[0], vocab_size=cfg.vocab_size,
-                         cls_token_num=cfg.cls_token_num, block_size=cfg.block_size,
-                         caption_dim=cfg.caption_dim if m.model_type == "t2i" else 0,
-                         model_type=1 if m.model_type == "t2i" else 0, norm_eps=cfg.norm_eps, rope_base=cfg.rope_base)
-        w, keep = self._weights()
-        if self.handle:
-            check(self.lib.car_model_destroy(self.handle), "car_model_destroy")
-            self.handle = C.c_void_p()
+        w, ts = _weights(m)
+        d = _desc(m)
+        self.close()
         check(self.lib.car_model_create(C.byref(d), C.byref(w), cur_stream(), C.byref(self.handle)), "car_model_create")
-        self._keep = keep
-        self.version = self._signature()
-        self.layout = self._layout()
-        self.dtype = dt
-        self.desc = d
+        self._keep, self.sig = ts, self._signature(ts)
+        self.layout, self.dtype, self.desc = _layout(m), m.tok_embeddings.weight.dtype, d
         self.generation += 1
 
-    @_on_own_device
+    @on_own_device
     def refresh(self):
-        """Bring the packed copies up to date if parameters were replaced / updated since the last pack.  Same layout:
+        """Bring the packed copies up to date if a borrowed tensor was replaced / updated since the last pack.  Same layout:
         `car_model_repack` rewrites the library-owned buffers IN PLACE (the CarModel and every device pointer a live CarState holds
-        stay valid — ADVICE r1: re-creating the model under a live state was a use-after-free).  Different dtype / device / shapes:
-        a new CarModel (generation bumps; `setup_caches` then rebuilds the state)."""
-        if self._signature() == self.version:
-            return
-        if self._layout() != self.layout:
+        stay valid — ADVICE r1: re-creating the model under a live state was a use-after-free).  Different dtype / device / shapes,
+        or no CarModel after a failed create: a new CarModel (generation bumps; `setup_caches` then rebuilds the state)."""
+        if not self.handle or _layout(self.module) != self.layout:
             self._build()
             return
-        w, keep = self._weights()
+        w, ts = _weights(self.module)
+        sig = self._signature(ts)
+        if sig == self.sig:
+            return
         check(self.lib.car_model_repack(self.handle, C.byref(w), cur_stream()), "car_model_repack")
-        self._keep = keep
-        self.version = self._signature()
-
-    def close(self):
-        if self.handle:
-            self.lib.car_model_destroy(self.handle)
-            self.handle = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._keep, self.sig = ts, sig
 
 
 class ARTrainHandle(_lib.NativeHandle):
@@ -153,18 +114,27 @@ class ARTrainHandle(_lib.NativeHandle):
     under bf16-autocast numerics.  Weights are borrowed (re-cast to bf16 inside every forward, like autocast does)."""
 
     def __init__(self, module, max_batch: int, max_img_tokens: int):
-        from ._lib import CarTrainWeights
+        super().__init__("car_train_destroy")
         self.lib = _lib.lib()
         m = module
         cfg = m.config
         if m.tok_embeddings.weight.dtype != torch.float32:
             raise NotImplementedError("controlar_b200 training forward: fp32 parameters (bf16 autocast is applied inside), as the train scripts keep them")
-        w, keep = ARModelHandle._weights(self_like(m))
+        self.device = m.tok_embeddings.weight.device
+        self.max_batch, self.max_img_tokens = max_batch, max_img_tokens
+        self.V, self.T = cfg.vocab_size, cfg.cls_token_num
+        self.key = tuple(p.data_ptr() for p in m.parameters())
+        self.generation = 0          # a backward belongs to the forward that produced its loss
+        self._create(m)
+
+    @on_own_device
+    def _create(self, m):
+        w, keep = _weights(m)
         tw = CarTrainWeights()
         tw.w = w
         tw.adapter_fc1 = _ptr(m.adapter_mlp.fc1.weight.detach()); tw.adapter_fc2 = _ptr(m.adapter_mlp.fc2.weight.detach())
         tw.adapter_dim = m.adapter_mlp.fc1.weight.shape[1]
-        tw.num_classes = cfg.num_classes
+        tw.num_classes = m.config.num_classes
         if m.model_type == "t2i":
             unc = m.cls_embedding.uncond_embedding.detach().to(torch.float32).contiguous()
             keep.append(unc)
@@ -174,21 +144,12 @@ class ARTrainHandle(_lib.NativeHandle):
             keep.append(cunc)
             tw.cond_uncond = _ptr(cunc)
         # else: the legacy gpt.py class gives dropped samples literal zeros (gpt.py:118-119): NULL = zeros in the library
-        d = CarModelDesc(dtype=_lib.CAR_F32, dim=cfg.dim, n_layer=cfg.n_layer, n_head=cfg.n_head,
-                         ffn_dim=m.layers[0].feed_forward.w1.weight.shape[0], vocab_size=cfg.vocab_size,
-                         cls_token_num=cfg.cls_token_num, block_size=cfg.block_size,
-                         caption_dim=cfg.caption_dim if m.model_type == "t2i" else 0,
-                         model_type=1 if m.model_type == "t2i" else 0, norm_eps=cfg.norm_eps, rope_base=cfg.rope_base)
-        dev = m.tok_embeddings.weight.device
-        self.rope = m.freqs_cis.to(device=dev, dtype=torch.float32).contiguous()
-        self.handle = C.c_void_p()
-        check(self.lib.car_train_create(C.byref(d), C.byref(tw), max_batch, max_img_tokens, _ptr(self.rope), cur_stream(), C.byref(self.handle)),
-              "car_train_create")
+        self.rope = m.freqs_cis.to(device=self.device, dtype=torch.float32).contiguous()
+        check(self.lib.car_train_create(C.byref(_desc(m)), C.byref(tw), self.max_batch, self.max_img_tokens, _ptr(self.rope), cur_stream(),
+                                        C.byref(self.handle)), "car_train_create")
         self._keep = (keep, tw)
-        self.max_batch, self.max_img_tokens = max_batch, max_img_tokens
-        self.V, self.T = cfg.vocab_size, cfg.cls_token_num
-        self.key = tuple(p.data_ptr() for p in m.parameters())
 
+    @on_own_device
     def forward(self, idx, cond, feat, drop_ids, mask, targets, valid):
         B, n = idx.shape
         n_img = n + 1
@@ -210,7 +171,7 @@ class ARTrainHandle(_lib.NativeHandle):
                                          None if vf is None else _ptr(vf), _ptr(logits), None if loss is None else _ptr(loss), cur_stream()),
               "car_train_forward")
         self._last = (idx, cond, feat, drop, m8, tg, vf)      # car_train_backward reads them again
-        self.generation = getattr(self, "generation", 0) + 1  # a backward belongs to the forward that produced its loss
+        self.generation += 1
         return logits, (None if loss is None else loss[0])
 
     # ---- backward ---------------------------------------------------------------------------------------------------
@@ -237,10 +198,10 @@ class ARTrainHandle(_lib.NativeHandle):
         out += [("adapter_mlp.fc1.weight", m.adapter_mlp.fc1.weight), ("adapter_mlp.fc2.weight", m.adapter_mlp.fc2.weight)]
         return out
 
+    @on_own_device
     def backward(self, module, loss_grad=None, want_feat_grad=True):
         """Gradients of the last forward(targets=...) on this handle -> ({name: fp32 grad}, d_feat bf16 or None).
         loss_grad: 0-dim / [1] fp32 CUDA tensor (d / d loss) or None = 1."""
-        from ._lib import CarTrainWeights
         if getattr(self, "_last", None) is None:
             raise RuntimeError("controlar_b200: backward() needs a preceding training forward with targets")
         idx, cond, feat, drop, m8, tg, vf = self._last
@@ -281,39 +242,18 @@ class ARTrainHandle(_lib.NativeHandle):
         self._last = None
         return G, dfeat
 
-    def close(self):
-        if self.handle:
-            self.lib.car_train_destroy(self.handle)
-            self.handle = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class _ModuleView:
-    def __init__(self, module):
-        self.module = module
-
-
-def self_like(module):
-    """ARModelHandle._weights only reads ``self.module``."""
-    return _ModuleView(module)
-
 
 class ARStateHandle(_lib.NativeHandle):
     """CarState: KV caches (PyTorch-owned, reference layout), control tokens, scratch, the persistent decode kernel's packet
     buffers (and the CUDA graph of the per-kernel fallback chain)."""
 
     def __init__(self, model: ARModelHandle, b_eff: int, S: int, N: int, k_caches, v_caches, rope: torch.Tensor):
+        super().__init__("car_state_destroy")
         self.lib = model.lib
         self.model = model
         self.device = rope.device
         self.b_eff, self.S, self.N = b_eff, S, N
         self._keep = (list(k_caches), list(v_caches), rope)
-        self.handle = C.c_void_p()
         ka, va = _ptr_array(self._keep[0]), _ptr_array(self._keep[1])
         with torch.cuda.device(self.device):
             check(self.lib.car_state_create(model.handle, b_eff, S, N, C.cast(ka, C.POINTER(C.c_void_p)),
@@ -322,7 +262,7 @@ class ARStateHandle(_lib.NativeHandle):
         self.V = model.desc.vocab_size
         self.T = model.desc.cls_token_num
 
-    @_on_own_device
+    @on_own_device
     def set_emb_mask(self, emb_mask: Optional[torch.Tensor]):
         if emb_mask is None:
             check(self.lib.car_state_set_emb_mask(self.handle, None, cur_stream()), "car_state_set_emb_mask")
@@ -332,7 +272,7 @@ class ARStateHandle(_lib.NativeHandle):
         check(self.lib.car_state_set_emb_mask(self.handle, _ptr(em), cur_stream()), "car_state_set_emb_mask")
         self._mask_keep = em
 
-    @_on_own_device
+    @on_own_device
     def prefill(self, cond: torch.Tensor, condition: Optional[torch.Tensor], control_strength: float,
                 all_rows: bool) -> torch.Tensor:
         dev = cond.device
@@ -350,7 +290,7 @@ class ARStateHandle(_lib.NativeHandle):
         self._io_keep = (cond, condition)
         return out
 
-    @_on_own_device
+    @on_own_device
     def decode_step(self, tok: torch.Tensor, pos: int) -> torch.Tensor:
         tok = tok.reshape(-1).to(torch.int32).contiguous()
         assert tok.numel() == self.b_eff
@@ -359,7 +299,7 @@ class ARStateHandle(_lib.NativeHandle):
         self._tok_keep = tok
         return out
 
-    @_on_own_device
+    @on_own_device
     def generate(self, sp: CarSampling, n_tokens: int, noise: Optional[torch.Tensor], device) -> torch.Tensor:
         B = self.b_eff // 2 if sp.cfg_scale > 1.0 else self.b_eff
         out = torch.empty((B, n_tokens), dtype=torch.int32, device=device)
@@ -371,7 +311,7 @@ class ARStateHandle(_lib.NativeHandle):
         self._noise_keep = noise
         return out
 
-    @_on_own_device
+    @on_own_device
     def generate_forced(self, sp: CarSampling, forced: torch.Tensor, trace: bool = True, noise: Optional[torch.Tensor] = None):
         """Teacher-forced device-side loop (car_generate_forced): returns (sampler choices int32 [B, n], logits fp32 [n, b_eff, V])."""
         B = self.b_eff // 2 if sp.cfg_scale > 1.0 else self.b_eff
@@ -397,17 +337,6 @@ class ARStateHandle(_lib.NativeHandle):
 
     def step_bytes(self, n_context: int) -> int:
         return int(self.lib.car_decode_step_bytes(self.handle, int(n_context)))
-
-    def close(self):
-        if self.handle:
-            self.lib.car_state_destroy(self.handle)
-            self.handle = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def make_sampling(temperature=1.0, top_k=0, top_p=1.0, sample_logits=True, cfg_scale=1.0, cfg_interval=-1,

@@ -13,7 +13,7 @@ import ctypes as C
 import torch
 
 from .. import _lib
-from .._lib import CAR_BF16, check, cur_stream, _ptr, _ptr_array
+from .._lib import CAR_BF16, check, cur_stream, on_own_device, _ptr, _ptr_array
 
 
 class CarT5Desc(C.Structure):
@@ -43,33 +43,34 @@ class T5EncoderB200:
                 raise NotImplementedError("controlar_b200 T5 encoder: bf16 (or fp32, cast to bf16) checkpoints only")
             return t.detach().to(device=dev, dtype=torch.bfloat16).contiguous()
         emb_key = "shared.weight" if "shared.weight" in sd else "encoder.embed_tokens.weight"
-        self._keep = {"embed": W(emb_key), "rel": W("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"),
-                      "fn": W("encoder.final_layer_norm.weight")}
+        # the library borrows these: they live as long as the encoder (a deep copy gets its own)
+        self._weights = {"embed": W(emb_key), "rel_bias": W("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"),
+                         "final_norm": W("encoder.final_layer_norm.weight")}
         names = {"ln1": "layer.0.layer_norm", "q": "layer.0.SelfAttention.q", "k": "layer.0.SelfAttention.k", "v": "layer.0.SelfAttention.v",
                  "o": "layer.0.SelfAttention.o", "ln2": "layer.1.layer_norm", "wi_0": "layer.1.DenseReluDense.wi_0",
                  "wi_1": "layer.1.DenseReluDense.wi_1", "wo": "layer.1.DenseReluDense.wo"}
-        w = CarT5Weights()
-        w.embed, w.rel_bias, w.final_norm = _ptr(self._keep["embed"]), _ptr(self._keep["rel"]), _ptr(self._keep["fn"])
         for field, sub in names.items():
-            ts = [W(f"encoder.block.{i}.{sub}.weight") for i in range(num_layers)]
-            arr = _ptr_array(ts)
-            self._keep[field] = (ts, arr)
-            setattr(w, field, C.cast(arr, C.POINTER(C.c_void_p)))
+            self._weights[field] = [W(f"encoder.block.{i}.{sub}.weight") for i in range(num_layers)]
         self.d_model = d_model
         self.max_rows = max_rows
-        d = CarT5Desc(CAR_BF16, d_model, d_kv, num_heads, d_ff, num_layers, vocab_size, num_buckets, max_distance, eps)
-        self._desc, self._w = d, w
-        self.handle = C.c_void_p()
-        self._create(max_rows)
+        self._desc = CarT5Desc(CAR_BF16, d_model, d_kv, num_heads, d_ff, num_layers, vocab_size, num_buckets, max_distance, eps)
+        self._h = _lib.NativeHandle("car_t5_destroy")
+        self._handle(max_rows)
 
-    def _create(self, max_rows):
-        lib = _lib.lib()
-        if self.handle:
-            lib.car_t5_destroy(self.handle)
-            self.handle = C.c_void_p()
-        with torch.cuda.device(self.device):
-            check(lib.car_t5_create(C.byref(self._desc), C.byref(self._w), max_rows, cur_stream(), C.byref(self.handle)), "car_t5_create")
-        self.max_rows = max_rows
+    @on_own_device
+    def _handle(self, rows):
+        """The CarT5, created first (after a copy dropped it) or again when `rows` exceeds the capacity it was created for."""
+        if self._h is None:
+            self._h = _lib.NativeHandle("car_t5_destroy")
+        if not self._h.handle or rows > self.max_rows:
+            self._h.close()
+            max_rows = max(rows, self.max_rows)
+            w = CarT5Weights()
+            for field, t in self._weights.items():
+                setattr(w, field, _ptr(t) if torch.is_tensor(t) else C.cast(_ptr_array(t), C.POINTER(C.c_void_p)))
+            check(_lib.lib().car_t5_create(C.byref(self._desc), C.byref(w), max_rows, cur_stream(), C.byref(self._h.handle)), "car_t5_create")
+            self.max_rows = max_rows
+        return self._h.handle
 
     @classmethod
     def from_hf(cls, model, device=None, max_rows=8 * 120):
@@ -84,23 +85,15 @@ class T5EncoderB200:
                    vocab_size=cfg.vocab_size, num_buckets=cfg.relative_attention_num_buckets, max_distance=cfg.relative_attention_max_distance,
                    eps=cfg.layer_norm_epsilon, device=dev, max_rows=max_rows)
 
+    @on_own_device
     def __call__(self, input_ids=None, attention_mask=None, **unused):
         ids = input_ids.to(device=self.device, dtype=torch.int32).contiguous()
         B, L = ids.shape
         mask = (torch.ones_like(ids) if attention_mask is None else attention_mask.to(device=self.device, dtype=torch.int32)).contiguous()
-        if B * L > self.max_rows:
-            self._create(B * L)
+        h = self._handle(B * L)
         out = torch.empty(B, L, self.d_model, dtype=torch.bfloat16, device=self.device)
-        with torch.cuda.device(self.device):
-            check(_lib.lib().car_t5_forward(self.handle, _ptr(ids), _ptr(mask), B, L, _ptr(out), cur_stream()), "car_t5_forward")
+        check(_lib.lib().car_t5_forward(h, _ptr(ids), _ptr(mask), B, L, _ptr(out), cur_stream()), "car_t5_forward")
         return {"last_hidden_state": out}
 
     def eval(self):
         return self
-
-    def __del__(self):
-        try:
-            if self.handle:
-                _lib.lib().car_t5_destroy(self.handle)
-        except Exception:
-            pass

@@ -7,7 +7,7 @@ from typing import List
 import torch
 
 from . import _lib
-from ._lib import check, cur_stream, dtype_code, param_signature, _ptr, _ptr_array
+from ._lib import check, cur_stream, dtype_code, on_own_device, param_signature, _ptr, _ptr_array
 
 
 class CarDinoDesc(C.Structure):
@@ -53,23 +53,6 @@ def _dev_of(module):
     return next(module.parameters()).device
 
 
-def _on_module_device(attr):
-    """Run a handle method with the device of `getattr(self, attr)`'s parameters current (the library launches on the current device
-    and takes its current stream)."""
-    import functools
-
-    def deco(fn):
-        @functools.wraps(fn)
-        def wrapped(self, *a, **k):
-            dev = _dev_of(getattr(self, attr))
-            if dev.type != "cuda":
-                return fn(self, *a, **k)
-            with torch.cuda.device(dev):
-                return fn(self, *a, **k)
-        return wrapped
-    return deco
-
-
 class DinoHandle(_lib.ModuleHandle):
     def __init__(self, adapter, adapter_mlp=None):
         super().__init__("car_dino_destroy")
@@ -77,13 +60,17 @@ class DinoHandle(_lib.ModuleHandle):
         self.adapter, self.adapter_mlp = adapter, adapter_mlp
         self._build()
 
+    @property
+    def device(self):
+        return _dev_of(self.adapter)
+
     def _params(self):
         ps = list(self.adapter.model.parameters())
         if self.adapter_mlp is not None:
             ps += list(self.adapter_mlp.parameters())
         return ps
 
-    @_on_module_device("adapter")
+    @on_own_device
     def _build(self):
         m = self.adapter.model
         dt = m.layernorm.weight.dtype
@@ -144,7 +131,7 @@ class DinoHandle(_lib.ModuleHandle):
         self.dtype, self.hidden, self.out_dim = dt, m.hidden, out_dim
         self.sig = param_signature(self._params())
 
-    @_on_module_device("adapter")
+    @on_own_device
     def forward(self, x: torch.Tensor, apply_mlp: bool) -> torch.Tensor:
         if param_signature(self._params()) != self.sig:
             self._build()
@@ -217,7 +204,11 @@ class VQHandle(_lib.ModuleHandle):
         self.vq = vq
         self._build()
 
-    @_on_module_device("vq")
+    @property
+    def device(self):
+        return _dev_of(self.vq)
+
+    @on_own_device
     def _build(self):
         vq = self.vq
         cfg = vq.config
@@ -240,7 +231,7 @@ class VQHandle(_lib.ModuleHandle):
         if param_signature(vq_tensor_order(self.vq)) != self.sig:
             self._build()
 
-    @_on_module_device("vq")
+    @on_own_device
     def decode_code(self, codes: torch.Tensor, B: int, h: int, w: int) -> torch.Tensor:
         self._fresh()
         codes = codes.reshape(B, h * w).to(torch.int32).contiguous()
@@ -249,7 +240,7 @@ class VQHandle(_lib.ModuleHandle):
         self._keep = codes
         return out
 
-    @_on_module_device("vq")
+    @on_own_device
     def decode(self, quant: torch.Tensor) -> torch.Tensor:
         self._fresh()
         B, e, h, w = quant.shape
@@ -259,7 +250,7 @@ class VQHandle(_lib.ModuleHandle):
         self._keep = quant
         return out
 
-    @_on_module_device("vq")
+    @on_own_device
     def encode(self, img: torch.Tensor):
         self._fresh()
         B, _, H, W = img.shape

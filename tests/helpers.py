@@ -62,3 +62,40 @@ def assert_mismatches_are_near_ties(z_ref_combined, raw_ref, ref_tok, mine_tok, 
         bound = near_tie_bound(float(raw_ref[:, i].abs().max()), cfg_scale)
         assert margin <= bound, f"{what}: token ({b},{i}) differs with margin {margin:.4f} > near-tie bound {bound:.4f}"
     return float(mism.float().mean())
+
+
+class ObservedLib:
+    """The library with the create / destroy entry points of `kinds` observed (e.g. "hed": car_hed_create / car_hed_destroy).
+    `created` and `destroyed` list every handle; a destroy of a handle that is not live is recorded but never reaches the library;
+    while `refuse` is set, creates fail before the library sees them.  Install with
+    `monkeypatch.setattr(_lib, "_lib", ObservedLib(_lib.lib(), kinds))`."""
+
+    def __init__(self, real, kinds):
+        self.real, self.refuse = real, False
+        self.created, self.destroyed, self.live = [], [], set()
+        for k in kinds:
+            setattr(self, f"car_{k}_create", self._create(getattr(real, f"car_{k}_create")))
+            setattr(self, f"car_{k}_destroy", self._destroy(getattr(real, f"car_{k}_destroy")))
+
+    def __getattr__(self, name):
+        return getattr(self.real, name)
+
+    def _create(self, fn):
+        def create(*args):
+            if self.refuse:
+                return -1
+            rc = fn(*args)
+            h = args[-1]._obj.value                      # every create takes `out` last, as byref(c_void_p)
+            self.created.append(h)
+            self.live.add(h)
+            return rc
+        return create
+
+    def _destroy(self, fn):
+        def destroy(h):
+            self.destroyed.append(h.value)
+            if h.value not in self.live:
+                return 0
+            self.live.discard(h.value)
+            return fn(h)
+        return destroy

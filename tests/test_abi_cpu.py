@@ -98,6 +98,51 @@ def test_tensor_list_creates_reject_bad_lists_before_any_cuda_call():
         assert not h, name
 
 
+
+def test_ar_creates_reject_bad_arguments_before_any_cuda_call():
+    """The model, state, training and T5 creates each refuse a null `out`, a null descriptor / model / weight table, and an unsupported
+    shape, before any CUDA call: `out` stays null and the message names the entry point.  No pointer handed over is dereferenced
+    (the stand-in model pointer only reaches a create whose shape check fails first)."""
+    import ctypes as C
+    from controlar_b200 import _lib
+    from controlar_b200.language.t5 import CarT5Desc, CarT5Weights
+    l = _lib.lib()
+    P = 1 << 20
+
+    def desc(dtype, **change):
+        kw = dict(dtype=dtype, dim=128, n_layer=3, n_head=2, ffn_dim=384, vocab_size=64, cls_token_num=1, block_size=16, norm_eps=1e-5,
+                  rope_base=1e4)
+        return C.byref(_lib.CarModelDesc(**{**kw, **change}))
+    bf16, f32 = _lib.CAR_BF16, _lib.CAR_F32
+    w, tw = C.byref(_lib.CarWeights()), C.byref(_lib.CarTrainWeights(adapter_dim=64))
+    t5 = lambda **change: C.byref(CarT5Desc(**{**dict(dtype=bf16, d_model=128, d_kv=64, n_heads=2, d_ff=256, n_layers=2, vocab=64,
+                                                     num_buckets=32, max_distance=128, eps=1e-6), **change}))
+    t5w = C.byref(CarT5Weights())
+    kv = C.byref(C.c_void_p(P))
+    calls = {
+        "car_model_create": lambda out: [lambda: l.car_model_create(desc(bf16), w, None, None), lambda: l.car_model_create(None, w, None, out),
+                                         lambda: l.car_model_create(desc(bf16), None, None, out),
+                                         lambda: l.car_model_create(desc(bf16, n_layer=4), w, None, out)],
+        "car_state_create": lambda out: [lambda: l.car_state_create(P, 2, 32, 16, kv, kv, P, None),
+                                         lambda: l.car_state_create(None, 2, 32, 16, kv, kv, P, out),
+                                         lambda: l.car_state_create(P, 2, 32, 16, None, kv, P, out),
+                                         lambda: l.car_state_create(P, 0, 32, 16, kv, kv, P, out)],
+        "car_train_create": lambda out: [lambda: l.car_train_create(desc(f32), tw, 2, 16, P, None, None),
+                                         lambda: l.car_train_create(None, tw, 2, 16, P, None, out),
+                                         lambda: l.car_train_create(desc(f32), None, 2, 16, P, None, out),
+                                         lambda: l.car_train_create(desc(f32, n_layer=4), tw, 2, 16, P, None, out),
+                                         lambda: l.car_train_create(desc(f32, n_head=0), tw, 2, 16, P, None, out)],
+        "car_t5_create": lambda out: [lambda: l.car_t5_create(t5(), t5w, 64, None, None), lambda: l.car_t5_create(None, t5w, 64, None, out),
+                                      lambda: l.car_t5_create(t5(), None, 64, None, out),
+                                      lambda: l.car_t5_create(t5(d_kv=32), t5w, 64, None, out)],
+    }
+    for name, cases in calls.items():
+        h = C.c_void_p()
+        for i, call in enumerate(cases(C.byref(h))):
+            assert call() < 0, (name, i)
+            assert name.encode() in l.car_last_error(), (name, i, l.car_last_error())
+        assert not h, name
+
 def test_product_fails_loudly_without_gpu():
     import torch
     if torch.cuda.is_available():

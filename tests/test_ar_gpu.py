@@ -242,3 +242,70 @@ def test_sampled_choices_with_torch_noise_bf16_persistent_kernel():
     choice, _ = st.generate_forced(sp, ref.to(dev), trace=False, noise=noise)
     agree = float((choice.cpu() == ref).float().mean())
     assert agree >= 0.9, f"only {agree:.3f} of the sampled choices match the reference"
+
+
+# the smoke test's model: bf16 decodes on the persistent kernel, fp32 on the per-kernel graph chain
+SMALL = GPTSpec(dim=256, n_layer=6, n_head=4, vocab_size=2048, cls_token_num=120, block_size=64, model_type="t2i")
+
+
+def _greedy_grid(model):
+    """generate()'s greedy token grid on fixed inputs (CFG, masks, control tokens given as the control encoder's output)."""
+    from controlar_b200.autoregressive.models.generate import generate
+    dt = model.tok_embeddings.weight.dtype
+    cond, masks = text_inputs(SMALL.cls_token_num, SMALL.caption_dim, 2, 1, dt)
+    ctrl = torch.randn(2, 16, SMALL.dim, generator=torch.Generator().manual_seed(3)) * 0.5
+    model.adapter.forward = lambda x: x
+    model.adapter_mlp.forward = lambda x: x
+    return generate(model, cond.cuda(), 16, emb_masks=masks.cuda(), cfg_scale=4.0, condition=ctrl.to(dt).cuda(), control_strength=0.7,
+                    temperature=1.0, top_k=0, top_p=1.0, sample_logits=False).cpu()
+
+
+def test_weight_update_repacks_the_model():
+    """load_state_dict between two generate() calls: the packed copies are rewritten in place (car_model_repack) and the grid is that
+    of a model built with the new weights."""
+    model, _ = build_product_gpt(SMALL, 0, torch.bfloat16)
+    g0 = _greedy_grid(model)
+    generation = model._car_model.generation
+    fresh, sd5 = build_product_gpt(SMALL, 5, torch.bfloat16)
+    missing, unexpected = model.load_state_dict(sd5, strict=False)
+    assert not unexpected and all(".kv_cache." in k for k in missing)     # the caches setup_caches added are buffers too
+    g5 = _greedy_grid(model)
+    assert model._car_model.generation == generation               # same layout: repacked, not re-created
+    assert torch.equal(g5, _greedy_grid(fresh)) and not torch.equal(g0, g5)
+
+
+def test_replaced_parameter_data_is_picked_up():
+    """`p.data = t` on any weight the library borrows (it changes data_ptr, not _version) takes effect at the next generate()."""
+    model, _ = build_product_gpt(SMALL, 0, torch.bfloat16)
+    fresh, _ = build_product_gpt(SMALL, 0, torch.bfloat16)
+    g0 = _greedy_grid(model)
+    w = model.layers[1].attention.wo.weight
+    new = (torch.randn(w.shape, generator=torch.Generator().manual_seed(7)) * 0.05).to(device=w.device, dtype=w.dtype)
+    w.data = new.clone()
+    fresh.layers[1].attention.wo.weight.data.copy_(new)
+    g1 = _greedy_grid(model)
+    assert torch.equal(g1, _greedy_grid(fresh)) and not torch.equal(g0, g1)
+
+
+def test_failed_model_recreate_leaves_no_stale_handle(monkeypatch):
+    """A new layout (bf16 -> fp32) whose CarModel create is refused leaves no handle behind: the next call builds a new model and
+    state, and every model and state the library created is destroyed exactly once."""
+    import gc
+    from controlar_b200 import _lib
+    from tests.helpers import ObservedLib
+    gc.collect()                                       # earlier tests' handles are destroyed by the library itself, not observed
+    lib = ObservedLib(_lib.lib(), ["model", "state"])
+    monkeypatch.setattr(_lib, "_lib", lib)
+    model, _ = build_product_gpt(SMALL, 0, torch.bfloat16)
+    _greedy_grid(model)
+    model.to(torch.float32)
+    lib.refuse = True
+    with pytest.raises(RuntimeError, match="car_model_create"):
+        _greedy_grid(model)
+    assert not model._car_model.handle
+    lib.refuse = False
+    want = _greedy_grid(build_product_gpt(SMALL, 0, torch.bfloat16)[0].to(torch.float32))
+    assert torch.equal(_greedy_grid(model), want)
+    del model
+    gc.collect()
+    assert len(lib.created) == 6 and sorted(lib.destroyed) == sorted(lib.created), (lib.created, lib.destroyed)

@@ -108,45 +108,76 @@ def test_hed_weight_update_rebuilds_handle():
 def test_hed_failed_recreate_leaves_no_stale_handle(monkeypatch):
     """A weight update whose re-create fails leaves no handle behind: the next call builds a new one, and every handle the library
     created is destroyed exactly once.  The library's own create and destroy run; only the refusal of one create is injected."""
-    import ctypes as C
     import gc
     from controlar_b200 import _lib
     from tests.golden.make_golden import hed_inputs
-    real = _lib.lib()
-    created, destroyed, live, refuse = [], [], set(), [False]
-
-    class Lib:                                             # the library, with car_hed_create / car_hed_destroy observed
-        def __getattr__(self, name):
-            return getattr(real, name)
-
-        def car_hed_create(self, ts, n, stream, out):
-            if refuse[0]:
-                return -1
-            rc = real.car_hed_create(ts, n, stream, out)
-            created.append(out._obj.value)
-            live.add(out._obj.value)
-            return rc
-
-        def car_hed_destroy(self, h):
-            destroyed.append(h.value)
-            if h.value not in live:                        # recorded, but a freed handle never reaches the library
-                return 0
-            live.discard(h.value)
-            return real.car_hed_destroy(h)
-    monkeypatch.setattr(_lib, "_lib", Lib())
+    from tests.helpers import ObservedLib
+    gc.collect()                                       # earlier tests' handles are destroyed by the library itself, not observed
+    lib = ObservedLib(_lib.lib(), ["hed"])
+    monkeypatch.setattr(_lib, "_lib", lib)
     x = next(iter(hed_inputs().values())).cuda()
     m = _hed(0)
     with torch.no_grad():
         m.run(x)
         m.norm.add_(1.0)                                   # an in-place update: the next call rebuilds
-        refuse[0] = True
+        lib.refuse = True
         with pytest.raises(RuntimeError, match="car_hed_create"):
             m.run(x)
-        refuse[0] = False
+        lib.refuse = False
         m.run(x)
     del m
     gc.collect()
-    assert len(created) == 2 and sorted(destroyed) == sorted(created), (created, destroyed)
+    assert len(lib.created) == 2 and sorted(lib.destroyed) == sorted(lib.created), (lib.created, lib.destroyed)
+
+
+def _t5_encoder(max_rows=64):
+    from controlar_b200.language.t5 import T5EncoderB200
+    from oracle.weights import make_t5_state_dict
+    from tests.helpers import load_golden
+    g = load_golden("t5")
+    c = g["config"]
+    sd = {k: v.to(torch.bfloat16) for k, v in make_t5_state_dict(**c, seed=g["seed"]).items()}
+    return T5EncoderB200(sd, d_model=c["d_model"], d_kv=c["d_kv"], num_heads=c["num_heads"], d_ff=c["d_ff"], num_layers=c["num_layers"],
+                         vocab_size=c["vocab"], max_rows=max_rows)
+
+
+def test_t5_encoder_deep_copies():
+    """A used encoder deep-copies: the copy keeps its weights, drops the library handle and builds its own on first call."""
+    import copy
+    from tests.golden.make_golden import t5_inputs
+    ids, mask = t5_inputs()["b2_L120"]
+    enc = _t5_encoder()
+    want = enc(input_ids=ids.cuda(), attention_mask=mask.cuda())["last_hidden_state"]
+    clone = copy.deepcopy(enc)
+    assert clone._h is None and enc._h.handle
+    got = clone(input_ids=ids.cuda(), attention_mask=mask.cuda())["last_hidden_state"]
+    assert torch.equal(got, want)
+
+
+def test_t5_failed_recreate_leaves_no_stale_handle(monkeypatch):
+    """Growing `max_rows` re-creates the encoder; when that create is refused, no handle is left behind, the next call builds a new
+    one, and every handle the library created is destroyed exactly once."""
+    import gc
+    from controlar_b200 import _lib
+    from tests.golden.make_golden import t5_inputs
+    from tests.helpers import ObservedLib
+    gc.collect()                                       # earlier tests' handles are destroyed by the library itself, not observed
+    lib = ObservedLib(_lib.lib(), ["t5"])
+    monkeypatch.setattr(_lib, "_lib", lib)
+    small, big = t5_inputs()["b3_L24"], t5_inputs()["b2_L120"]          # 72 rows, then 240
+    enc = _t5_encoder(max_rows=72)
+    want = enc(input_ids=small[0].cuda(), attention_mask=small[1].cuda())["last_hidden_state"]
+    lib.refuse = True
+    with pytest.raises(RuntimeError, match="car_t5_create"):
+        enc(input_ids=big[0].cuda(), attention_mask=big[1].cuda())
+    assert not enc._h.handle
+    lib.refuse = False
+    enc(input_ids=big[0].cuda(), attention_mask=big[1].cuda())
+    assert enc.max_rows == 240
+    assert torch.equal(enc(input_ids=small[0].cuda(), attention_mask=small[1].cuda())["last_hidden_state"], want)
+    del enc
+    gc.collect()
+    assert len(lib.created) == 2 and sorted(lib.destroyed) == sorted(lib.created), (lib.created, lib.destroyed)
 
 
 def test_t5_encoder_vs_hf_golden():
