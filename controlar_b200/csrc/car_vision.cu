@@ -225,27 +225,22 @@ static int dino_forward_t(CarDino* m, const TI* image, int B, int H, int W, void
     const int C = d.hidden, h = H / 16, w = W / 16, hw = h * w, Tn = hw + 1, heads = d.heads;
     const int Tp = (Tn + 31) & ~31;                      // key axis of V^T, zero padded (vit_attention_kernel reads it in 8-key chunks)
     const long long rows = (long long)B * Tn;
-    // workspace
-    size_t need = 0;
-    auto sz = [&](size_t b) { need += (b + 255) & ~(size_t)255; };
+    // workspace (every buffer is sized for its one use)
     const int KP = m->kpad;
-    sz((size_t)B * hw * KP * 2); sz((size_t)B * hw * C * 2); sz((size_t)hw * C * 2);
-    sz(rows * C * 2); sz(rows * C * 2); sz(rows * 2 * C * 2); sz((size_t)B * C * Tp * 2);
-    sz(rows * C * 2); sz(rows * 4 * C * 2);
-    sz((size_t)B * hw * C * 2); sz((size_t)B * hw * std::max(m->ad_dim, 1) * 2);
-    CAR_TRY(m->ws.reserve(need));
-    m->ws.reset();
-    bf16* patches = (bf16*)m->ws.take((size_t)B * hw * KP * 2);
-    bf16* ptok = (bf16*)m->ws.take((size_t)B * hw * C * 2);
-    bf16* posi = (bf16*)m->ws.take((size_t)hw * C * 2);
-    bf16* x = (bf16*)m->ws.take(rows * C * 2);
-    bf16* xn = (bf16*)m->ws.take(rows * C * 2);
-    bf16* qk = (bf16*)m->ws.take(rows * 2 * C * 2);
-    bf16* vT = (bf16*)m->ws.take((size_t)B * C * Tp * 2);
-    bf16* ctx = (bf16*)m->ws.take(rows * C * 2);
-    bf16* hid = (bf16*)m->ws.take(rows * 4 * C * 2);
-    bf16* feat = (bf16*)m->ws.take((size_t)B * hw * C * 2);
-    bf16* mlp_h = (bf16*)m->ws.take((size_t)B * hw * std::max(m->ad_dim, 1) * 2);
+    bf16 *patches, *ptok, *posi, *x, *xn, *qk, *vT, *ctx, *hid, *feat, *mlp_h;
+    CAR_TRY(m->ws.carve([&](Carve& c) {
+        patches = c.take<bf16>((size_t)B * hw * KP);
+        ptok = c.take<bf16>((size_t)B * hw * C);
+        posi = c.take<bf16>((size_t)hw * C);
+        x = c.take<bf16>(rows * C);
+        xn = c.take<bf16>(rows * C);
+        qk = c.take<bf16>(rows * 2 * C);
+        vT = c.take<bf16>((size_t)B * C * Tp);
+        ctx = c.take<bf16>(rows * C);
+        hid = c.take<bf16>(rows * 4 * C);
+        feat = c.take<bf16>((size_t)B * hw * C);
+        mlp_h = c.take<bf16>((size_t)B * hw * std::max(m->ad_dim, 1));
+    }));
 
     CAR_CUDA(cudaMemsetAsync(vT, 0, (size_t)B * C * Tp * 2, st));   // padded key columns must be finite (x 0 prob)
     // 1. resize to (h*P, w*P) + patchify (dinov2_adapter.py:16-24; ViT: P = 16, no resize), patch projection + bias
@@ -439,11 +434,12 @@ extern "C" int car_vq_destroy(CarVQ* m) {
 // ---- layer helpers on NHWC bf16 activations ----
 struct Act { bf16* p; int B, H, W, C; long long n() const { return (long long)B * H * W * C; } };
 
-static int conv_fwd(cudaStream_t st, const ConvW& c, const Act& x, int ups, int stride2, bf16* out, const bf16* resid, int Ho, int Wo,
+static int conv_fwd(cudaStream_t st, const ConvW& c, const Act& x, int ups, int stride2, Buf<bf16> out, const bf16* resid, int Ho, int Wo,
                     float* out_nchw_f32 = nullptr) {
     if (x.C != c.cin_pad && !(c.k == 1 && x.C == c.cin_pad)) CAR_FAIL(CAR_ERR_STATE, "conv input channel mismatch");
+    if (!out_nchw_f32) CAR_TRY(car_fits(__func__, out, (size_t)x.B * Ho * Wo * c.cout));
     if (c.k == 3 && !stride2 && !ups && !out_nchw_f32 && c.cin_pad % WG_BK == 0 && c.cout % 8 == 0 && Ho == x.H && Wo == x.W && x.H >= WG_TH && x.W >= WG_TW && wg_encoder() != nullptr &&
-        ((uintptr_t)x.p % 16) == 0 && ((uintptr_t)out % 16) == 0 && (!resid || ((uintptr_t)resid % 16) == 0)) {
+        ((uintptr_t)x.p % 16) == 0 && ((uintptr_t)out.p % 16) == 0 && (!resid || ((uintptr_t)resid % 16) == 0)) {
         // 3x3 / pad 1 convolution on the wgmma kernel: one 4-D TMA box per (tap, 64-channel block), padding by TMA zero fill
         alignas(64) CUtensorMap mapA, mapB;
         if (!wg_make_map_nhwc(&mapA, x.p, x.B, x.H, x.W, c.cin_pad) || !wg_make_map(&mapB, c.w, c.cout, 9 * c.cin_pad, 9 * c.cin_pad))
@@ -465,10 +461,11 @@ static int conv_fwd(cudaStream_t st, const ConvW& c, const Act& x, int ups, int 
     else { p.C = out; p.ldc = c.cout; p.resid = resid; p.ldr = c.cout; }
     return dense(st, p);
 }
-static int gn_fwd(cudaStream_t st, const NormW& nw, const Act& x, bf16* y, int swish, float* stats) {
+static int gn_fwd(cudaStream_t st, const NormW& nw, const Act& x, Buf<bf16> y, int swish, float* stats) {
     const int G = 32;
     const int C8 = x.C / 8;
-    if (x.C % 64 == 0 && 256 % C8 == 0 && x.H * x.W >= 4 * GN_CHUNKS && ((uintptr_t)x.p % 16) == 0 && ((uintptr_t)y % 16) == 0 &&
+    CAR_TRY(car_fits(__func__, y, (size_t)x.n()));
+    if (x.C % 64 == 0 && 256 % C8 == 0 && x.H * x.W >= 4 * GN_CHUNKS && ((uintptr_t)x.p % 16) == 0 && ((uintptr_t)y.p % 16) == 0 &&
         ((uintptr_t)nw.w % 16) == 0 && ((uintptr_t)nw.b % 16) == 0) {
         // coalesced two-stage statistics + 16-byte apply (vision.cuh); `stats` has room for the partial sums behind the [B*32][2] block
         float* part = stats + (size_t)x.B * G * 2;
@@ -483,10 +480,10 @@ static int gn_fwd(cudaStream_t st, const NormW& nw, const Act& x, bf16* y, int s
     return CAR_OK;
 }
 
-struct VqScratch { bf16 *t0, *t1, *t2; float* stats; float* S; bf16* P; bf16* vT; };
+struct VqScratch { Buf<bf16> a, b, t0, t1, t2; float* stats; float* S; bf16* P; Buf<bf16> vT; };   // a / b: the ping-pong activations
 
 // ResnetBlock.forward (vq_model.py:300-315): x + conv2(swish(GN(conv1(swish(GN(x))))))  [+ 1x1 shortcut]
-static int res_fwd(cudaStream_t st, const ResW& r, Act& x, bf16* out, VqScratch& s) {
+static int res_fwd(cudaStream_t st, const ResW& r, Act& x, Buf<bf16> out, VqScratch& s) {
     Act a = x;
     CAR_TRY(gn_fwd(st, r.n1, x, s.t0, 1, s.stats));
     a.p = s.t0;
@@ -501,15 +498,15 @@ static int res_fwd(cudaStream_t st, const ResW& r, Act& x, bf16* out, VqScratch&
     return CAR_OK;
 }
 // AttnBlock.forward (vq_model.py:328-352): single head over H*W tokens, scale C^-0.5
-static int attn_fwd(cudaStream_t st, const AttnW& a, Act& x, bf16* out, VqScratch& s) {
+static int attn_fwd(cudaStream_t st, const AttnW& a, Act& x, Buf<bf16> out, VqScratch& s) {
     const int C = x.C, hw = x.H * x.W, B = x.B;
     const int hwp = (hw + 31) & ~31;
     CAR_TRY(gn_fwd(st, a.n, x, s.t0, 0, s.stats));
     Act xn{s.t0, B, x.H, x.W, C};
-    bf16* q = s.t1;
-    bf16* k = s.t2;
+    Buf<bf16> q = s.t1, k = s.t2;
     CAR_TRY(conv_fwd(st, a.q, xn, 0, 0, q, nullptr, x.H, x.W));
     CAR_TRY(conv_fwd(st, a.k, xn, 0, 0, k, nullptr, x.H, x.W));
+    CAR_TRY(car_fits(__func__, s.vT, (size_t)B * C * hwp));
     {   // V^T [B][C][hwp]
         DenseP p = dp_plain(a.v.w, C, xn.p, C, C, hw, C, s.vT, hwp);
         p.sB = (long long)hw * C; p.sC = (long long)C * hwp; p.bias = a.v.b; p.bias_along_m = 1;
@@ -532,22 +529,15 @@ static int attn_fwd(cudaStream_t st, const AttnW& a, Act& x, bf16* out, VqScratc
     return CAR_OK;
 }
 
-static int vq_scratch(cudaStream_t st, CarVQ* m, int B, int Hmax, int Wmax, int h16, int w16, int Cfull, VqScratch& s, bf16** bufA, bf16** bufB,
-                      size_t extra, void** extra_p) {
-    const CarVQDesc& d = m->d;
-    const size_t act = (size_t)B * Hmax * Wmax * Cfull * 2;            // largest activation (ch channels at full res)
+// the decoder's scratch buffers, in carve order
+static void vq_scratch(Carve& c, const CarVQDesc& d, int B, int Hmax, int Wmax, int h16, int w16, int Cfull, VqScratch& s) {
+    const size_t act = (size_t)B * Hmax * Wmax * Cfull;                // largest activation (ch channels at full res)
     const int hw = h16 * w16, hwp = (hw + 31) & ~31, Cmax = d.ch * d.ch_mult[d.n_levels - 1];
-    size_t need = 5 * (act + 256) + (size_t)B * 32 * 2 * 4 * (1 + GN_CHUNKS) + 256 + (size_t)B * hw * hwp * 6 + 512 + (size_t)B * Cmax * hwp * 2 + 256 + extra + 256;
-    CAR_TRY(m->ws.reserve(need));
-    m->ws.reset();
-    *bufA = (bf16*)m->ws.take(act); *bufB = (bf16*)m->ws.take(act);
-    s.t0 = (bf16*)m->ws.take(act); s.t1 = (bf16*)m->ws.take(act); s.t2 = (bf16*)m->ws.take(act);
-    s.stats = (float*)m->ws.take((size_t)B * 32 * 2 * 4 * (1 + GN_CHUNKS));
-    s.S = (float*)m->ws.take((size_t)B * hw * hwp * 4); s.P = (bf16*)m->ws.take((size_t)B * hw * hwp * 2);
-    s.vT = (bf16*)m->ws.take((size_t)B * Cmax * hwp * 2);
-    if (extra_p) *extra_p = m->ws.take(extra);
-    CAR_CUDA(cudaMemsetAsync(s.vT, 0, (size_t)B * Cmax * hwp * 2, st));
-    return CAR_OK;
+    s.a = c.take<bf16>(act); s.b = c.take<bf16>(act);
+    s.t0 = c.take<bf16>(act); s.t1 = c.take<bf16>(act); s.t2 = c.take<bf16>(act);
+    s.stats = c.take<float>((size_t)B * 32 * 2 * (1 + GN_CHUNKS));
+    s.S = c.take<float>((size_t)B * hw * hwp); s.P = c.take<bf16>((size_t)B * hw * hwp);
+    s.vT = c.take<bf16>((size_t)B * Cmax * hwp);
 }
 
 // VQModel.decode_code (vq_model.py:53-56): codes int32 [B][h*w] -> image fp32 NCHW [B][3][16h][16w] (VQ-16)
@@ -557,16 +547,20 @@ static int vq_decode_impl(CarVQ* m, const int32_t* codes, const float* quant, in
     cudaStream_t st = (cudaStream_t)stream;
     const CarVQDesc& d = m->d;
     const int up = 1 << (d.n_levels - 1);
-    VqScratch s; bf16 *bA, *bB; void* zbuf;
-    CAR_TRY(vq_scratch(st, m, B, h * up, w * up, h, w, d.ch, s, &bA, &bB, (size_t)B * h * w * 32 * 2, &zbuf));
+    VqScratch s; bf16* zbuf;
+    CAR_TRY(m->ws.carve([&](Carve& c) {
+        vq_scratch(c, d, B, h * up, w * up, h, w, d.ch, s);
+        zbuf = c.take<bf16>((size_t)B * h * w * 32);
+    }));
+    CAR_CUDA(cudaMemsetAsync(s.vT, 0, s.vT.cap * 2, st));
     // get_codebook_entry (vq_model.py:262-277) + post_quant_conv
-    if (codes) CAR_LAUNCH(codebook_lookup_kernel, gsz((long long)B * h * w * 32), 256, 0, st, m->codebook_n, codes, (bf16*)zbuf, (long long)B * h * w, d.embed_dim, 32, d.codebook_size);
-    else CAR_LAUNCH((nchw_to_nhwc_bf16_kernel<float>), gsz((long long)B * h * w * 32), 256, 0, st, quant, (bf16*)zbuf, B, d.embed_dim, h * w, 32);
-    Act x{(bf16*)zbuf, B, h, w, 32};
-    CAR_TRY(conv_fwd(st, m->post_quant, x, 0, 0, bA, nullptr, h, w));
-    x = Act{bA, B, h, w, d.z_channels};
-    bf16* cur = bB;
-    auto flip = [&](bf16* used) { return used == bA ? bB : bA; };
+    if (codes) CAR_LAUNCH(codebook_lookup_kernel, gsz((long long)B * h * w * 32), 256, 0, st, m->codebook_n, codes, zbuf, (long long)B * h * w, d.embed_dim, 32, d.codebook_size);
+    else CAR_LAUNCH((nchw_to_nhwc_bf16_kernel<float>), gsz((long long)B * h * w * 32), 256, 0, st, quant, zbuf, B, d.embed_dim, h * w, 32);
+    Act x{zbuf, B, h, w, 32};
+    CAR_TRY(conv_fwd(st, m->post_quant, x, 0, 0, s.a, nullptr, h, w));
+    x = Act{s.a, B, h, w, d.z_channels};
+    Buf<bf16> cur = s.b;
+    auto flip = [&](bf16* used) { return used == s.a ? s.b : s.a; };
     CAR_TRY(conv_fwd(st, m->d_conv_in, x, 0, 0, cur, nullptr, h, w));
     x = Act{cur, B, h, w, m->d_conv_in.cout};
     CAR_TRY(res_fwd(st, m->d_mid0, x, flip(x.p), s));
@@ -578,8 +572,9 @@ static int vq_decode_impl(CarVQ* m, const int32_t* codes, const float* quant, in
             if (!m->d_attn[idx].empty()) CAR_TRY(attn_fwd(st, m->d_attn[idx][b], x, flip(x.p), s));
         }
         if (m->d_has_up[idx]) {   // Upsample (vq_model.py:368-379): nearest x2, then the 3x3 convolution
-            bf16* o = flip(x.p);
+            Buf<bf16> o = flip(x.p);
             if (wg_encoder() != nullptr && x.C % WG_BK == 0) {   // materialise the up-sampled tensor (bandwidth-trivial) so the convolution is a plain TMA box walk
+                CAR_TRY(car_fits("upsample2x", s.t2, (size_t)x.n() * 4));
                 CAR_LAUNCH(upsample2x_nhwc_kernel, gsz((long long)B * x.H * 2 * x.W * 2 * (x.C / 8)), 256, 0, st, (const bf16*)x.p, s.t2, B, x.H, x.W, x.C);
                 Act u{s.t2, B, x.H * 2, x.W * 2, x.C};
                 CAR_TRY(conv_fwd(st, m->d_up[idx], u, 0, 0, o, nullptr, u.H, u.W));
@@ -596,7 +591,7 @@ static int vq_decode_impl(CarVQ* m, const int32_t* codes, const float* quant, in
                    (const bf16*)m->d_conv_out.b, out, B, y.H, y.W, y.C);
         return CAR_OK;
     }
-    return conv_fwd(st, m->d_conv_out, y, 0, 0, nullptr, nullptr, x.H, x.W, out);
+    return conv_fwd(st, m->d_conv_out, y, 0, 0, Buf<bf16>{}, nullptr, x.H, x.W, out);
 }
 
 extern "C" int car_vq_decode_code(CarVQ* m, const int32_t* codes, int32_t B, int32_t h, int32_t w, float* out, void* stream) {
@@ -611,16 +606,18 @@ extern "C" int car_vq_decode(CarVQ* m, const float* quant, int32_t B, int32_t h,
 // ---- VQModel.encode (vq_model.py:41-46) at fp32 grade: the "x3" split-bf16 path of vision.cuh ----
 // fp32 NHWC activations; every convolution = one launch of the bf16 implicit-GEMM kernel over tripled K, fp32 output / bias / residual.
 struct ActF { float* p; int B, H, W, C; long long npix() const { return (long long)B * H * W; } long long n() const { return npix() * C; } };
-struct EncScratch { bf16 *t3, *x3; float *h1, *sc; float* stats; float *qf, *kf, *vf, *S, *P, *ctx; bf16 *q3, *k3, *P3, *vT3; };
+struct EncScratch { Buf<bf16> t3, x3; Buf<float> h1, sc; float* stats; Buf<float> qf, kf, vf, ctx; float *S, *P; Buf<bf16> q3, k3, P3, vT3; };
 
-static int split3(cudaStream_t st, const float* x, bf16* y, long long npix, int C, int bside = 0) {
+static int split3(cudaStream_t st, const float* x, Buf<bf16> y, long long npix, int C, int bside = 0) {
+    CAR_TRY(car_fits(__func__, y, (size_t)npix * C * 3));
     CAR_LAUNCH(split3_kernel, gsz(npix * C), 256, 0, st, x, y, npix, C, bside);
     return CAR_OK;
 }
 // a3: S3 activations [B][Hs][Ws][3 cin_pad]; out fp32 [B][Ho][Wo][cout] (+ fp32 residual of the same shape)
-static int conv_x3(cudaStream_t st, const ConvW& c, const bf16* a3, int B, int Hs, int Ws, int stride2, float* out, const float* resid, int Ho, int Wo,
+static int conv_x3(cudaStream_t st, const ConvW& c, const bf16* a3, int B, int Hs, int Ws, int stride2, Buf<float> out, const float* resid, int Ho, int Wo,
                    int act = ACT_NONE) {
     if (!c.w3 || !c.bf) CAR_FAIL(CAR_ERR_STATE, "convolution has no split-bf16 weights (encoder layers only)");
+    CAR_TRY(car_fits(__func__, out, (size_t)B * Ho * Wo * c.cout));
     DenseP p;
     memset(&p, 0, sizeof(p));
     p.A = a3; p.B = c.w3; p.M = B * Ho * Wo; p.N = c.cout; p.K = c.k * c.k * 3 * c.cin_pad; p.ldb = p.K; p.alpha = 1.f;
@@ -630,15 +627,16 @@ static int conv_x3(cudaStream_t st, const ConvW& c, const bf16* a3, int B, int H
     p.bias_f = c.bf; p.C = out; p.ldc = c.cout; p.out_mode = 1; p.resid_f = resid; p.ldr = c.cout; p.act = act;
     return dense(st, p);
 }
-static int gn_x3(cudaStream_t st, const NormW& nw, const ActF& x, bf16* y3, int swish, float* stats) {
+static int gn_x3(cudaStream_t st, const NormW& nw, const ActF& x, Buf<bf16> y3, int swish, float* stats) {
     const int G = 32;
+    CAR_TRY(car_fits(__func__, y3, (size_t)x.n() * 3));
     CAR_LAUNCH(groupnorm_stats_f32_kernel, x.B * G, 512, 0, st, (const float*)x.p, stats, x.H * x.W, x.C, G);
     CAR_LAUNCH(groupnorm_apply_split3_kernel, gsz(x.n()), 256, 0, st, (const float*)x.p, (const float*)stats, (const float*)nw.wf, (const float*)nw.bff, y3,
                x.n(), x.H * x.W, x.C, G, swish);
     return CAR_OK;
 }
 // ResnetBlock.forward (vq_model.py:300-315)
-static int res_x3(cudaStream_t st, const ResW& r, ActF& x, float* out, EncScratch& s) {
+static int res_x3(cudaStream_t st, const ResW& r, ActF& x, Buf<float> out, EncScratch& s) {
     CAR_TRY(gn_x3(st, r.n1, x, s.t3, 1, s.stats));
     CAR_TRY(conv_x3(st, r.c1, s.t3, x.B, x.H, x.W, 0, s.h1, nullptr, x.H, x.W));
     ActF h{s.h1, x.B, x.H, x.W, r.c1.cout};
@@ -654,7 +652,7 @@ static int res_x3(cudaStream_t st, const ResW& r, ActF& x, float* out, EncScratc
     return CAR_OK;
 }
 // AttnBlock.forward (vq_model.py:328-352): single head over H*W tokens, scale C^-0.5, everything fp32-grade
-static int attn_x3(cudaStream_t st, const AttnW& a, ActF& x, float* out, EncScratch& s) {
+static int attn_x3(cudaStream_t st, const AttnW& a, ActF& x, Buf<float> out, EncScratch& s) {
     const int C = x.C, hw = x.H * x.W, B = x.B;
     const int hwp = (hw + 31) & ~31;
     const long long rows = (long long)B * hw;
@@ -671,6 +669,8 @@ static int attn_x3(cudaStream_t st, const AttnW& a, ActF& x, float* out, EncScra
     }
     CAR_LAUNCH(softmax_rows_f32_kernel, (unsigned)rows, 256, 0, st, (const float*)s.S, s.P, hw, hwp);
     CAR_TRY(split3(st, s.P, s.P3, rows, hwp, 0));
+    CAR_TRY(car_fits(__func__, s.vT3, (size_t)B * C * hwp * 3));
+    CAR_TRY(car_fits(__func__, s.ctx, (size_t)rows * C));
     CAR_LAUNCH(transpose_split3b_kernel, gsz((long long)B * C * hwp), 256, 0, st, (const float*)s.vf, s.vT3, B, hw, hwp, C);
     {   // context [B][hw][C] fp32
         DenseP p = dp_plain(s.P3, 3 * hwp, s.vT3, 3 * hwp, hw, C, 3 * hwp, s.ctx, C);
@@ -695,24 +695,21 @@ extern "C" int car_vq_encode(CarVQ* m, const float* img, int32_t B, int32_t H, i
     const size_t npix = (size_t)B * h * w;
     const int hw = h * w, hwp = (hw + 31) & ~31, Cmax = d.ch * d.ch_mult[d.n_levels - 1];
     // workspace: fp32 activations (largest: ch channels at full resolution) and their S3 forms
-    const size_t actf = (size_t)B * H * W * d.ch * 4, act3 = (size_t)B * H * W * d.ch * 3 * 2;
-    const size_t x0 = (size_t)B * H * W * 32 * 3 * 2;
-    const size_t af = npix * Cmax * 4, a3 = npix * Cmax * 3 * 2;
-    const size_t need = 4 * (actf + 256) + 2 * (act3 + 256) + x0 + 256 + (size_t)B * 32 * 2 * 4 + 256 + 4 * (af + 256) + 2 * (a3 + 256) +
-                        2 * ((size_t)B * hw * hwp * 4 + 256) + (size_t)B * hw * hwp * 3 * 2 + 256 + (size_t)B * Cmax * hwp * 3 * 2 + 256 + npix * 8 * 4 * 2 + 1024;
-    CAR_TRY(m->ws.reserve(need));
-    m->ws.reset();
-    float* fA = (float*)m->ws.take(actf); float* fB = (float*)m->ws.take(actf);
-    EncScratch s;
-    s.h1 = (float*)m->ws.take(actf); s.sc = (float*)m->ws.take(actf);
-    s.t3 = (bf16*)m->ws.take(act3); s.x3 = (bf16*)m->ws.take(act3);
-    bf16* img3 = (bf16*)m->ws.take(x0);
-    s.stats = (float*)m->ws.take((size_t)B * 32 * 2 * 4);
-    s.qf = (float*)m->ws.take(af); s.kf = (float*)m->ws.take(af); s.vf = (float*)m->ws.take(af); s.ctx = (float*)m->ws.take(af);
-    s.q3 = (bf16*)m->ws.take(a3); s.k3 = (bf16*)m->ws.take(a3);
-    s.S = (float*)m->ws.take((size_t)B * hw * hwp * 4); s.P = (float*)m->ws.take((size_t)B * hw * hwp * 4);
-    s.P3 = (bf16*)m->ws.take((size_t)B * hw * hwp * 3 * 2); s.vT3 = (bf16*)m->ws.take((size_t)B * Cmax * hwp * 3 * 2);
-    float* zf = (float*)m->ws.take(npix * 8 * 4); float* zq = (float*)m->ws.take(npix * 8 * 4);
+    const size_t actf = (size_t)B * H * W * d.ch, act3 = actf * 3;
+    const size_t af = npix * Cmax, a3 = af * 3;
+    Buf<float> fA, fB, zf; EncScratch s; bf16* img3; float* zq;
+    CAR_TRY(m->ws.carve([&](Carve& c) {
+        fA = c.take<float>(actf); fB = c.take<float>(actf);
+        s.h1 = c.take<float>(actf); s.sc = c.take<float>(actf);
+        s.t3 = c.take<bf16>(act3); s.x3 = c.take<bf16>(act3);
+        img3 = c.take<bf16>((size_t)B * H * W * 32 * 3);
+        s.stats = c.take<float>((size_t)B * 32 * 2);
+        s.qf = c.take<float>(af); s.kf = c.take<float>(af); s.vf = c.take<float>(af); s.ctx = c.take<float>(af);
+        s.q3 = c.take<bf16>(a3); s.k3 = c.take<bf16>(a3);
+        s.S = c.take<float>((size_t)B * hw * hwp); s.P = c.take<float>((size_t)B * hw * hwp);
+        s.P3 = c.take<bf16>((size_t)B * hw * hwp * 3); s.vT3 = c.take<bf16>((size_t)B * Cmax * hwp * 3);
+        zf = c.take<float>(npix * 8); zq = c.take<float>(npix * 8);
+    }));
 
     CAR_LAUNCH(nchw_to_nhwc_split3_kernel, gsz((long long)B * H * W * 32), 256, 0, st, img, img3, B, 3, H * W, 32);
     auto flip = [&](float* used) { return used == fA ? fB : fA; };
@@ -724,7 +721,7 @@ extern "C" int car_vq_encode(CarVQ* m, const float* img, int32_t B, int32_t H, i
             if (!m->e_attn[lvl].empty()) CAR_TRY(attn_x3(st, m->e_attn[lvl][b], x, flip(x.p), s));
         }
         if (m->e_has_down[lvl]) {   // Downsample (vq_model.py:382-397): pad (0,1,0,1), 3x3 stride 2
-            float* o = flip(x.p);
+            Buf<float> o = flip(x.p);
             CAR_TRY(split3(st, x.p, s.x3, x.npix(), x.C));
             CAR_TRY(conv_x3(st, m->e_down[lvl], s.x3, B, x.H, x.W, 1, o, nullptr, x.H / 2, x.W / 2));
             x = ActF{o, B, x.H / 2, x.W / 2, m->e_down[lvl].cout};
@@ -734,7 +731,7 @@ extern "C" int car_vq_encode(CarVQ* m, const float* img, int32_t B, int32_t H, i
     CAR_TRY(attn_x3(st, m->e_mid1, x, flip(x.p), s));
     CAR_TRY(res_x3(st, m->e_mid2, x, flip(x.p), s));
     CAR_TRY(gn_x3(st, m->e_norm_out, x, s.t3, 1, s.stats));
-    float* zc = flip(x.p);
+    Buf<float> zc = flip(x.p);
     CAR_TRY(conv_x3(st, m->e_conv_out, s.t3, B, x.H, x.W, 0, zc, nullptr, x.H, x.W));              // [npix][z_channels]
     CAR_TRY(split3(st, zc, s.x3, (long long)npix, d.z_channels));
     CAR_TRY(conv_x3(st, m->quant_conv, s.x3, B, x.H, x.W, 0, zf, nullptr, x.H, x.W));              // [npix][embed_dim] fp32
@@ -854,13 +851,14 @@ extern "C" int car_hed_forward(CarHED* m, const float* img, int32_t B, int32_t H
     const size_t full = (size_t)B * H * W;
     size_t proj_elems = 0;
     { int h = H, w = W; for (int k = 0; k < 5; ++k) { proj_elems += (size_t)B * h * w; h /= 2; w /= 2; } }
-    const size_t actf = full * 64 * 4, act3 = full * 64 * 3 * 2;                 // largest activation: 64 channels at full resolution
-    CAR_TRY(m->ws.reserve(2 * (actf + 256) + act3 + 256 + full * 32 * 3 * 2 + 256 + proj_elems * 4 + 256));
-    m->ws.reset();
-    float* fA = (float*)m->ws.take(actf); float* fB = (float*)m->ws.take(actf);
-    bf16* s3 = (bf16*)m->ws.take(act3);
-    bf16* img3 = (bf16*)m->ws.take(full * 32 * 3 * 2);
-    float* maps = (float*)m->ws.take(proj_elems * 4);
+    const size_t actf = full * 64, act3 = actf * 3;                             // largest activation: 64 channels at full resolution
+    Buf<float> fA, fB; Buf<bf16> s3; bf16* img3; float* maps;
+    CAR_TRY(m->ws.carve([&](Carve& c) {
+        fA = c.take<float>(actf); fB = c.take<float>(actf);
+        s3 = c.take<bf16>(act3);
+        img3 = c.take<bf16>(full * 32 * 3);
+        maps = c.take<float>(proj_elems);
+    }));
     CAR_LAUNCH(hed_input_split3_kernel, gsz((long long)full * 32), 256, 0, st, img, (const float*)m->norm, img3, B, 3, H * W, 32);
     HedMaps hm;
     int h = H, w = W, ci = 0, curC = 3;
@@ -869,7 +867,8 @@ extern "C" int car_hed_forward(CarHED* m, const float* img, int32_t B, int32_t H
     size_t moff = 0;
     for (int b = 0; b < 5; ++b) {
         if (b > 0) {                                                            // down_sampling=True (:28-30)
-            float* o = other(cur);
+            Buf<float> o = other(cur);
+            CAR_TRY(car_fits("maxpool2", o, (size_t)B * (h / 2) * (w / 2) * curC));
             CAR_LAUNCH(maxpool2_nhwc_f32_kernel, gsz((long long)B * (h / 2) * (w / 2) * curC), 256, 0, st, (const float*)cur, o, B, h, w, curC);
             h /= 2; w /= 2; cur = o;
         }
@@ -877,7 +876,7 @@ extern "C" int car_hed_forward(CarHED* m, const float* img, int32_t B, int32_t H
             const ConvW& c = m->conv[ci];
             const bf16* a3 = img3;
             if (ci > 0) { CAR_TRY(split3(st, cur, s3, (long long)B * h * w, curC)); a3 = s3; }
-            float* o = other(cur);
+            Buf<float> o = other(cur);
             CAR_TRY(conv_x3(st, c, a3, B, h, w, 0, o, nullptr, h, w, ACT_RELU));  // conv + bias, ReLU (:31-33)
             cur = o; curC = c.cout;
         }
@@ -943,7 +942,8 @@ extern "C" int car_lineart_destroy(CarLineArt* m) {
 // one window convolution (gemm_dense.cuh A_WIN): S3 source [B][Hs][Ws][cin3] -> fp32 [B][oH][oW][cout], row (b, oy, ox) of the
 // Ho x Wo grid stored at pixel (osy*oy + oay, osx*ox + oax)
 static int la_conv(cudaStream_t st, const bf16* a3, int B, int Hs, int Ws, int cin3, const bf16* w3, const float* bias, int cout, int kh, int kw,
-                   int stride, int Ho, int Wo, float* out, int oH, int oW, int osy = 1, int osx = 1, int oay = 0, int oax = 0) {
+                   int stride, int Ho, int Wo, Buf<float> out, int oH, int oW, int osy = 1, int osx = 1, int oay = 0, int oax = 0) {
+    CAR_TRY(car_fits(__func__, out, (size_t)B * oH * oW * cout));
     static DevOnce once;
     if (once.first()) CAR_CUDA(cudaFuncSetAttribute(dense_win_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM));
     DenseP p;
@@ -969,15 +969,16 @@ extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, i
     const size_t s_bytes = Bz * std::max({(size_t)(H + 6) * (W + 6) * 24 * 2, (size_t)(H + 2) * (W + 2) * 192 * 2, (size_t)(H1 + 2) * (W1 + 2) * 384 * 2,
                                           (size_t)(H2 + 2) * (W2 + 2) * 768 * 2, (size_t)(H3 + 1) * (W3 + 1) * 384 * 2, (size_t)(Ho + 6) * (Wo + 6) * 64 * 4});
     const size_t x_bytes = Bz * H2 * W2 * 256 * 4, p_bytes = Bz * 64 * 256 * 4, st_bytes = Bz * 256 * 2 * 4;
-    CAR_TRY(m->ws.reserve(f_bytes + s_bytes + 2 * x_bytes + 2 * p_bytes + st_bytes + 6 * 256));
-    m->ws.reset();
-    float* F = (float*)m->ws.take(f_bytes);
-    void* S = m->ws.take(s_bytes);
-    float* X[2] = {(float*)m->ws.take(x_bytes), (float*)m->ws.take(x_bytes)};
-    float* ps = (float*)m->ws.take(p_bytes);
-    float* pq = (float*)m->ws.take(p_bytes);
-    float* stats = (float*)m->ws.take(st_bytes);
-    bf16* S3 = (bf16*)S;
+    Buf<float> F; Buf<char> S; float *X[2], *ps, *pq, *stats;   // S holds S3 (bf16) maps and, for the head, an fp32 map: carved in bytes
+    CAR_TRY(m->ws.carve([&](Carve& c) {
+        F = c.take<float>(f_bytes / 4);
+        S = c.take<char>(s_bytes);
+        X[0] = c.take<float>(x_bytes / 4); X[1] = c.take<float>(x_bytes / 4);
+        ps = c.take<float>(p_bytes / 4);
+        pq = c.take<float>(p_bytes / 4);
+        stats = c.take<float>(st_bytes / 4);
+    }));
+    bf16* S3 = (bf16*)S.p;
     // InstanceNorm of F [B][h][w][C] (+ resid) (ReLU) -> padded S, optional carrier
     auto inorm = [&](int h, int w, int C, const float* resid, float* carrier, InApply a) -> int {
         const int nch = la_nch(h * w);
@@ -985,11 +986,13 @@ extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, i
         CAR_LAUNCH(instnorm_sq_kernel, dim3(C / 32, B, nch), IN_THREADS, 0, st, (const float*)F, (const float*)ps, pq, h * w, C);
         CAR_LAUNCH(instnorm_finish_kernel, (B * C + 255) / 256, 256, 0, st, (const float*)ps, (const float*)pq, stats, B, h * w, C, nch);
         const long long n = (long long)B * (h + a.pt + a.pb) * (w + a.pl + a.pr) * C;
+        CAR_TRY(car_fits("inorm", S, (size_t)n * (a.s3 ? 6 : 4)));
         CAR_LAUNCH(instnorm_apply_pad_kernel, gsz(n), 256, 0, st, (const float*)F, (const float*)stats, resid, carrier, S, B, h, w, C, a);
         return CAR_OK;
     };
     const InApply zero1{1, 1, 1, 1, 0, 1, 1}, refl1{1, 1, 1, 1, 1, 1, 1}, zero_br{0, 0, 1, 1, 0, 1, 1};
     // model0: ReflectionPad2d(3), Conv 7x7 3 -> 64, IN, ReLU
+    CAR_TRY(car_fits("lineart stem split", S, Bz * (H + 6) * (W + 6) * 8 * 3 * 2));
     CAR_LAUNCH(lineart_stem_split3_kernel, gsz(Bz * (H + 6) * (W + 6) * 8), 256, 0, st, img, S3, B, 3, H, W, 3, 8);
     CAR_TRY(la_conv(st, S3, B, H + 6, W + 6, m->stem.cin3, m->stem.w3, m->stem.b, 64, 7, 7, 1, H, W, F, H, W));
     CAR_TRY(inorm(H, W, 64, nullptr, nullptr, zero1));
@@ -1023,7 +1026,7 @@ extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, i
     CAR_TRY(up(m->up[1], H3, W3));
     // model4: ReflectionPad2d(3), Conv 7x7 64 -> 1, Sigmoid (direct fp32 on the padded fp32 map)
     CAR_TRY(inorm(Ho, Wo, 64, nullptr, nullptr, InApply{3, 3, 3, 3, 1, 0, 1}));
-    CAR_LAUNCH(lineart_head_kernel, gsz((long long)B * Ho * Wo * 32), 256, 0, st, (const float*)S, (const float*)m->head_w, (const float*)m->head_b, out, B, Ho, Wo);
+    CAR_LAUNCH(lineart_head_kernel, gsz((long long)B * Ho * Wo * 32), 256, 0, st, (const float*)S.p, (const float*)m->head_w, (const float*)m->head_b, out, B, Ho, Wo);
     return CAR_OK;
 }
 
@@ -1139,7 +1142,8 @@ static int wg_launch_f32(cudaStream_t st, const CUtensorMap& mapA, const CUtenso
     return CAR_OK;
 }
 // out fp32 [M][ldc] = a3 (S3 rows [M][3 w.k]) · W3^T + bias (+ resid [M][ldc])
-static int dpt_gemm(cudaStream_t st, const DptLin& w, const bf16* a3, int M, float* out, int ldc, const float* resid = nullptr) {
+static int dpt_gemm(cudaStream_t st, const DptLin& w, const bf16* a3, int M, Buf<float> out, int ldc, const float* resid = nullptr) {
+    CAR_TRY(car_fits(__func__, out, (size_t)(M - 1) * ldc + w.n));
     alignas(64) CUtensorMap mapA, mapB;
     if (!wg_make_map(&mapA, a3, M, 3 * w.k, 3 * w.k) || !wg_make_map(&mapB, w.w3, w.n, 3 * w.k, 3 * w.k)) CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
     WgP q;
@@ -1151,7 +1155,8 @@ static int dpt_gemm(cudaStream_t st, const DptLin& w, const bf16* a3, int M, flo
 static inline int dpt_fh(int H) { return std::max(H, WG_TH); }
 static inline int dpt_fw(int W) { return std::max(W, WG_TW); }
 // 3x3 / pad 1 / stride 1 convolution: S3 NHWC frame [B][dpt_fh(H)][dpt_fw(W)][3 cin] -> fp32 NHWC [B][H][W][w.n] (+ resid)
-static int dpt_conv3(cudaStream_t st, const DptLin& w, const bf16* s3, int B, int H, int W, float* out, const float* resid = nullptr) {
+static int dpt_conv3(cudaStream_t st, const DptLin& w, const bf16* s3, int B, int H, int W, Buf<float> out, const float* resid = nullptr) {
+    CAR_TRY(car_fits(__func__, out, (size_t)B * H * W * w.n));
     const int cin3 = 3 * (w.k / 9);
     alignas(64) CUtensorMap mapA, mapB;
     if (!wg_make_map_nhwc(&mapA, s3, B, dpt_fh(H), dpt_fw(W), cin3) || !wg_make_map(&mapB, w.w3, w.n, 3 * w.k, 3 * w.k))
@@ -1163,16 +1168,18 @@ static int dpt_conv3(cudaStream_t st, const DptLin& w, const bf16* s3, int B, in
     return wg_launch_f32(st, mapA, mapB, q, B * q.tiles_x * q.tiles_y);
 }
 // S3 image producer (dpt.cuh dpt_image_split_kernel)
-static int dpt_img(cudaStream_t st, const float* a, const float* b, float* sum_out, bf16* y, DptImg q) {
+static int dpt_img(cudaStream_t st, const float* a, const float* b, float* sum_out, Buf<bf16> y, DptImg q) {
+    CAR_TRY(car_fits(__func__, y, (size_t)q.B * q.Hp * q.Wp * 3 * q.C));
     CAR_LAUNCH(dpt_image_split_kernel, gsz((long long)q.B * q.Hp * q.Wp * q.C), 256, 0, st, a, b, sum_out, y, q);
     return CAR_OK;
 }
 static DptImg dpt_frame(int B, int H, int W, int C) { return DptImg{B, H, W, C, dpt_fh(H), dpt_fw(W), 0, 0, 0, 0, 0}; }
 
 // one pre-LN encoder layer over fp32 rows x [B][T][C] -> dst (x may equal dst); S, T0 and X1 are scratch
-static int dpt_layer(cudaStream_t st, const DptLayer& Ly, const float* x, float* dst, int B, int T, int C, int heads, int mlp, float eps, bf16* S,
-                     float* T0, float* X1) {
+static int dpt_layer(cudaStream_t st, const DptLayer& Ly, const float* x, Buf<float> dst, int B, int T, int C, int heads, int mlp, float eps, Buf<bf16> S,
+                     Buf<float> T0, Buf<float> X1) {
     const int M = B * T;
+    CAR_TRY(car_fits(__func__, S, (size_t)M * 3 * std::max(C, mlp)));   // the LayerNorm, attention and GELU rows written below
     CAR_LAUNCH(dpt_layernorm_split_kernel, M, DPT_LN_THREADS, 0, st, x, (const float*)Ly.ln1w, (const float*)Ly.ln1b, S, C, eps);
     CAR_TRY(dpt_gemm(st, Ly.qkv, S, M, T0, 3 * C));
     CAR_LAUNCH(dpt_attention_kernel, dim3((T + DPT_AT_B - 1) / DPT_AT_B, heads, B), 128, 0, st, (const float*)T0, S, T, C);
@@ -1188,8 +1195,8 @@ static int dpt_layer(cudaStream_t st, const DptLayer& Ly, const float* x, float*
 // head: conv 3x3 F -> F/2, x2 bilinear (align_corners=True), conv 3x3 F/2 -> 32, ReLU, conv 1x1 32 -> 1, ReLU.
 // RCU(r) = conv2(ReLU(conv1(ReLU(r)))) + r; the ReLUs, the add and the upsample are fused into the S3 producers.
 // fe[i]: fp32 NHWC [B][sh[i]][sw[i]][F] (i = 0 finest, 2 sh[i] = sh[i-1]); the depth map is [B][H][W] with H = 4 sh[0]
-static int dpt_decode(cudaStream_t st, const DptDecoder& w, float* const fe[4], const int sh[4], const int sw[4], int B, int H, int W, int F,
-                      float* T0, float* T1, float* T2, bf16* S, float* depth) {
+static int dpt_decode(cudaStream_t st, const DptDecoder& w, const Buf<float> fe[4], const int sh[4], const int sw[4], int B, int H, int W, int F,
+                      Buf<float> T0, Buf<float> T1, Buf<float> T2, Buf<bf16> S, float* depth) {
     float* prev = nullptr;                              // fp32 [B][s][s][F], in T1
     for (int j = 0; j < 4; ++j) {
         const int i = 3 - j, s = sh[i], t = sw[i];
@@ -1248,22 +1255,20 @@ extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, 
     }
     ft = std::max({ft, Bz * 64 * h * h * F, Bz * 256 * h * h * 32});
     s3 = std::max({s3, Bz * 64 * h * h * 3 * F, Bz * 256 * h * h * 3 * (F / 2)});
-    size_t feat = 0;
-    for (int i = 0; i < 4; ++i) feat += Bz * dpt_fh(side[i]) * dpt_fw(side[i]) * F * 4 + 256;
-    CAR_TRY(m->ws.reserve(6 * ((size_t)M * C * 4 + 256) + 3 * (ft * 4 + 256) + feat + s3 * 2 + 256));
-    m->ws.reset();
-    float* X = (float*)m->ws.take((size_t)M * C * 4);
-    float* X1 = (float*)m->ws.take((size_t)M * C * 4);
-    float* keep[4];
-    for (int i = 0; i < 4; ++i) keep[i] = (float*)m->ws.take((size_t)M * C * 4);
-    float* T0 = (float*)m->ws.take(ft * 4);
-    float* T1 = (float*)m->ws.take(ft * 4);
-    float* T2 = (float*)m->ws.take(ft * 4);
-    float* fe[4];
-    for (int i = 0; i < 4; ++i) fe[i] = (float*)m->ws.take(Bz * side[i] * side[i] * F * 4);
-    bf16* S = (bf16*)m->ws.take(s3 * 2);
+    Buf<float> X, X1, keep[4], T0, T1, T2, fe[4]; Buf<bf16> S;
+    CAR_TRY(m->ws.carve([&](Carve& c) {
+        X = c.take<float>((size_t)M * C);
+        X1 = c.take<float>((size_t)M * C);
+        for (int i = 0; i < 4; ++i) keep[i] = c.take<float>((size_t)M * C);
+        T0 = c.take<float>(ft);
+        T1 = c.take<float>(ft);
+        T2 = c.take<float>(ft);
+        for (int i = 0; i < 4; ++i) fe[i] = c.take<float>(Bz * side[i] * side[i] * F);
+        S = c.take<bf16>(s3);
+    }));
 
     // ---- embeddings: patch convolution as a GEMM, [CLS], resized position embeddings
+    CAR_TRY(car_fits("dpt patchify", S, (size_t)Mp * 3 * 768));
     CAR_LAUNCH(dpt_patchify_kernel, gsz((long long)Mp * 768), 256, 0, st, pixel_values, S, B, h);
     CAR_TRY(dpt_gemm(st, m->patch, S, Mp, T0, C));
     CAR_LAUNCH(dpt_assemble_kernel, gsz((long long)M * C), 256, 0, st, (const float*)T0, (const float*)m->cls, (const float*)m->pos, X, B, h, h, d.pos_grid,
@@ -1272,7 +1277,7 @@ extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, 
     float* x = X;
     int kept = 0;
     for (int l = 0; l < d.n_layers; ++l) {
-        float* dst = (kept < 4 && d.out_indices[kept] == l) ? keep[kept++] : X;
+        Buf<float> dst = (kept < 4 && d.out_indices[kept] == l) ? keep[kept++] : X;
         CAR_TRY(dpt_layer(st, m->L[l], x, dst, B, T, C, d.n_heads, d.mlp, d.ln_eps, S, T0, X1));
         x = dst;
         if (kept == 4) break;                           // later layers feed nothing the depth map uses
@@ -1280,6 +1285,7 @@ extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, 
     // ---- reassemble: readout projection + GELU, 1x1 projection, resize; then the neck's 3x3 convolution -> fe[i] fp32 NHWC
     for (int i = 0; i < 4; ++i) {
         const int Cn = d.neck[i], f = DPT_FACTOR[i], s = side[i];
+        CAR_TRY(car_fits("dpt readout split", S, (size_t)Mp * 3 * std::max(2 * C, Cn)));   // this and the two row splits below
         CAR_LAUNCH(dpt_readout_split_kernel, gsz((long long)Mp * 2 * C), 256, 0, st, (const float*)keep[i], S, B, h * h, C);
         CAR_TRY(dpt_gemm(st, m->readout[i], S, Mp, T0, C));
         CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)Mp * C), 256, 0, st, (const float*)T0, S, (long long)Mp, C, 1);
@@ -1429,28 +1435,25 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
         const int rn_in[4] = {256, 512, MD_C, MD_C};
         for (int i = 0; i < 4; ++i) s3 = std::max(s3, Bz * dpt_fh(sh[i]) * dpt_fw(sw[i]) * 3 * std::max(rn_in[i], F));
     }
-    size_t feat = 0;
-    for (int i = 0; i < 4; ++i) feat += Bz * sh[i] * sw[i] * F * 4 + 256;
-    const size_t part = Bz * 64 * MD_GROUPS * 4, stb = Bz * MD_GROUPS * 2 * 4;
-    CAR_TRY(m->ws.reserve(4 * ((size_t)M * C * 4 + 256) + 3 * (ft * 4 + 256) + 3 * (car * 4 + 256) + feat + 2 * (part + 256) + 2 * (stb + 256) +
-                          s3 * 2 + 256));
-    m->ws.reset();
-    float* X = (float*)m->ws.take((size_t)M * C * 4);
-    float* X1 = (float*)m->ws.take((size_t)M * C * 4);
-    float* K[2] = {(float*)m->ws.take((size_t)M * C * 4), (float*)m->ws.take((size_t)M * C * 4)};
-    float* T0 = (float*)m->ws.take(ft * 4);
-    float* T1 = (float*)m->ws.take(ft * 4);
-    float* T2 = (float*)m->ws.take(ft * 4);
-    float* Xa = (float*)m->ws.take(car * 4);
-    float* Xb = (float*)m->ws.take(car * 4);
-    float* Td = (float*)m->ws.take(car * 4);
-    float* fe[4];
-    for (int i = 0; i < 4; ++i) fe[i] = (float*)m->ws.take(Bz * sh[i] * sw[i] * F * 4);
-    float* ps = (float*)m->ws.take(part);
-    float* pq = (float*)m->ws.take(part);
-    float* stats = (float*)m->ws.take(stb);
-    float* rstats = (float*)m->ws.take(stb);
-    bf16* S = (bf16*)m->ws.take(s3 * 2);
+    const size_t part = Bz * 64 * MD_GROUPS, stb = Bz * MD_GROUPS * 2;
+    Buf<float> X, X1, K[2], T0, T1, T2, Xa, Xb, Td, fe[4]; float *ps, *pq, *stats, *rstats; Buf<bf16> S;
+    CAR_TRY(m->ws.carve([&](Carve& c) {
+        X = c.take<float>((size_t)M * C);
+        X1 = c.take<float>((size_t)M * C);
+        K[0] = c.take<float>((size_t)M * C); K[1] = c.take<float>((size_t)M * C);
+        T0 = c.take<float>(ft);
+        T1 = c.take<float>(ft);
+        T2 = c.take<float>(ft);
+        Xa = c.take<float>(car);
+        Xb = c.take<float>(car);
+        Td = c.take<float>(car);
+        for (int i = 0; i < 4; ++i) fe[i] = c.take<float>(Bz * sh[i] * sw[i] * F);
+        ps = c.take<float>(part);
+        pq = c.take<float>(part);
+        stats = c.take<float>(stb);
+        rstats = c.take<float>(stb);
+        S = c.take<bf16>(s3);
+    }));
 
     // GroupNorm statistics of fp32 NHWC [B][hh][ww][Cc] -> stt [B][32][2]; chunks of about 4096 elements per (image, group)
     auto gn_stats = [&](const float* src, int hh, int ww, int Cc, float* stt) -> int {
@@ -1462,6 +1465,7 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
     };
     // GN(src) (+ resid, normalised by rn when rn.stats) (ReLU) (max-pool) -> S3 frame in S, fp32 carrier when given
     auto gn_apply = [&](const float* src, const MdNorm& N, const float* resid, GnAffine rn, float* carrier, int hh, int ww, int Cc, GnApply a) -> int {
+        CAR_TRY(car_fits("gn_apply", S, (size_t)B * a.Hp * a.Wp * 3 * Cc));
         CAR_LAUNCH(midas_gn_apply_kernel, gsz((long long)B * a.Hp * a.Wp * Cc), 256, 0, st, src, GnAffine{stats, N.w, N.b}, resid, rn, carrier, S, B, hh,
                    ww, Cc, a);
         return CAR_OK;
@@ -1469,6 +1473,7 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
     const GnAffine none{nullptr, nullptr, nullptr};
 
     // ---- stem: conv 7x7/2 (SAME: 2 before, 3 after) -> GN + ReLU -> max-pool 3x3/2 (SAME: 0 before, 1 after) -> S3 rows
+    CAR_TRY(car_fits("midas stem split", S, Bz * (H + 5) * (W + 5) * 8 * 3));
     CAR_LAUNCH(midas_stem_split3_kernel, gsz((long long)Bz * (H + 5) * (W + 5) * 8), 256, 0, st, x, S, B, H, W);
     CAR_TRY(la_conv(st, S, B, H + 5, W + 5, m->stem.k / 49 * 3, m->stem.w3, m->zero, 64, 7, 7, 2, H / 2, W / 2, T0, H / 2, W / 2));
     CAR_TRY(gn_stats(T0, H / 2, W / 2, 64, stats));
@@ -1502,13 +1507,15 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
             CAR_TRY(gn_apply(T1, k.n2, nullptr, none, nullptr, ho, wo, k.mid, GnApply{0, 0, ho, wo, 1, 0}));
             CAR_TRY(dpt_gemm(st, k.c3, S, Mo, T2, k.out));
             CAR_TRY(gn_stats(T2, ho, wo, k.out, stats));
-            float* xo = xin == Xa ? Xb : Xa;
+            Buf<float> xo = xin == Xa ? Xb : Xa;
+            CAR_TRY(car_fits("midas trunk carrier", xo, (size_t)Mo * k.out));
             CAR_TRY(gn_apply(T2, k.n3, b == 0 ? Td : xin, rn, xo, ho, wo, k.out, GnApply{0, 0, ho, wo, 1, 0}));
             xin = xo; hh = ho; ww = wo;
         }
         if (s < 2) {                                    // stage outputs 0 and 1 are features 1 and 2: scratch.layer{1,2}_rn
             CAR_TRY(dpt_img(st, xin, nullptr, nullptr, S, dpt_frame(B, hh, ww, MD_OUT[s])));
             CAR_TRY(dpt_conv3(st, m->rn[s], S, B, hh, ww, fe[s]));
+            CAR_TRY(car_fits("midas stage split", S, (size_t)B * hh * ww * 3 * MD_OUT[s]));
             CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)B * hh * ww * MD_OUT[s]), 256, 0, st, (const float*)xin, S, (long long)B * hh * ww,
                        MD_OUT[s], 0);
         }
@@ -1519,12 +1526,13 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
     CAR_LAUNCH(dpt_assemble_kernel, gsz((long long)M * C), 256, 0, st, (const float*)T0, (const float*)m->cls, (const float*)m->pos, X, B, h, w, MD_GRID, C);
     float* xv = X;
     for (int l = 0; l < 12; ++l) {
-        float* dst = l == 8 ? K[0] : l == 11 ? K[1] : X;
+        Buf<float> dst = l == 8 ? K[0] : l == 11 ? K[1] : X;
         CAR_TRY(dpt_layer(st, m->L[l], xv, dst, B, T, C, MD_HEADS, MD_MLP, 1e-6f, S, T0, X1));
         xv = dst;
     }
     // ---- reassemble 3 and 4: readout projection + GELU, 1x1 convolution, (3x3/2 convolution); then scratch.layer{3,4}_rn
     for (int i = 0; i < 2; ++i) {
+        CAR_TRY(car_fits("midas readout split", S, (size_t)Mp * 6 * C));   // this and the row split below
         CAR_LAUNCH(dpt_readout_split_kernel, gsz((long long)Mp * 2 * C), 256, 0, st, (const float*)K[i], S, B, P, C);
         CAR_TRY(dpt_gemm(st, m->readout[i], S, Mp, T0, C));
         CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)Mp * C), 256, 0, st, (const float*)T0, S, (long long)Mp, C, 1);

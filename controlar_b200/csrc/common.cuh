@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../include/controlar_b200.h"
+#include "carve.h"
 
 typedef __nv_bfloat16 bf16;
 
@@ -61,7 +62,19 @@ inline int sm_count() {
 inline int gsz(long long total) { return (int)std::min<long long>((total + 255) / 256, sm_count() * 16); }
 
 struct Arena {   // grow-only device workspace, re-used across calls (no allocation in steady state)
-    char* base = nullptr; size_t cap = 0, off = 0;
+    // The scratch buffers of one forward.  `list` names them once, as c.take<T>(count) calls; it runs first on a measuring Carve,
+    // whose end offset is what the arena grows to, then on the real base — so the size is the sum of the takes by construction.
+    template <typename F> int carve(F&& list) {
+        Carve measure(nullptr);
+        list(measure);
+        CAR_TRY(reserve(measure.off));
+        Carve c(base);
+        list(c);
+        return CAR_OK;
+    }
+    void release() { if (base) cudaFree(base); base = nullptr; cap = 0; }
+private:
+    char* base = nullptr; size_t cap = 0;
     int reserve(size_t bytes) {
         if (bytes <= cap) return CAR_OK;
         if (base) cudaFree(base);
@@ -70,10 +83,15 @@ struct Arena {   // grow-only device workspace, re-used across calls (no allocat
         cap = bytes;
         return CAR_OK;
     }
-    void reset() { off = 0; }
-    void* take(size_t bytes) { void* p = base + off; off += (bytes + 255) & ~(size_t)255; return p; }
-    void release() { if (base) cudaFree(base); base = nullptr; cap = 0; }
 };
+
+// In front of every launch that writes a scratch buffer shared between stages (sized as the maximum over its uses): refuse, without
+// launching, a write of `need` elements into a buffer carved for fewer.  `who` names the writer in the message.
+template <typename T> inline int car_fits(const char* who, const Buf<T>& b, size_t need) {
+    if (b.fits(need)) return CAR_OK;
+    g_car_err = std::string(who) + ": writes " + std::to_string(need) + " elements into a scratch buffer carved for " + std::to_string(b.cap);
+    return CAR_ERR_STATE;
+}
 
 // Base of every handle: the device memory its create call allocated and its forward workspace, both freed by `delete`.
 struct CarOwned {
