@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libcontrolar_b200.so")
-SOURCES = ["car_api.cu", "car_vision.cu"]
+SOURCES = ["car_api.cu", "car_vision.cu", "gemm.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC", "-cudart", "static"]
 

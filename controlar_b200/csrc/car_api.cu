@@ -11,8 +11,7 @@
 #include "sampler.cuh"
 #include "misc.cuh"
 #include "decode_persistent.cuh"
-#include "gemm_dense.cuh"
-#include "gemm_wgmma.cuh"
+#include "gemm.h"
 #include "train.cuh"
 #include "train_bwd.cuh"
 #include "t5.cuh"
@@ -464,33 +463,9 @@ static EpiParams epi_base(int kind) {
 // ---------------------------------------------------------------------------------------------------------
 static int dense_linear(cudaStream_t st, const void* A, int lda, const void* W, int M, int N, int K, int act, const void* resid, int ldr,
                         void* out, int ldo) {
-    static DevOnce once;
-    if (once.first()) {
-        CAR_CUDA(cudaFuncSetAttribute(dense_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM));
-    }
-    if (M <= 0 || N <= 0) return CAR_OK;
-    if (K % 8 == 0 && N % 8 == 0 && lda % 8 == 0 && ldo % 8 == 0 && (resid == nullptr || ldr % 8 == 0) &&
-        ((uintptr_t)A % 16) == 0 && ((uintptr_t)W % 16) == 0 && wg_encoder() != nullptr) {
-        // wgmma path (gemm_wgmma.cuh): TMA tensor-map loads, accumulators in registers, persistent warp-specialised CTAs
-        static DevOnce once5;
-        if (once5.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
-        alignas(64) CUtensorMap mapA, mapB;
-        if (!wg_make_map(&mapA, A, M, K, lda) || !wg_make_map(&mapB, W, N, K, K)) CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-        WgP q;
-        memset(&q, 0, sizeof(q));
-        q.M = M; q.N = N; q.K = K;
-        q.resid = (const bf16*)resid; q.ldr = ldr; q.C = (bf16*)out; q.ldc = ldo; q.act = act == ACT_GELU_TANH ? 1 : 0;
-        const int ntiles = ((M + WG_BM - 1) / WG_BM) * ((N + WG_BN - 1) / WG_BN);
-        CAR_LAUNCH(gemm_wgmma_kernel, std::min(ntiles, sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
-        return CAR_OK;
-    }
-    DenseP p;
-    memset(&p, 0, sizeof(p));
-    p.A = (const bf16*)A; p.B = (const bf16*)W; p.M = M; p.N = N; p.K = K; p.lda = lda; p.ldb = K; p.C = out; p.ldc = ldo; p.alpha = 1.f;
-    p.amode = A_PLAIN; p.act = act; p.resid = (const bf16*)resid; p.ldr = ldr; p.out_mode = 0;
-    dim3 grid((N + DG_BN - 1) / DG_BN, (M + DG_BM - 1) / DG_BM, 1);
-    CAR_LAUNCH(dense_gemm_kernel, grid, DG_THREADS, DG_SMEM, st, p);
-    return CAR_OK;
+    DenseP p = dp_plain((const bf16*)A, lda, (const bf16*)W, K, M, N, K, out, ldo);
+    p.act = act; p.resid = (const bf16*)resid; p.ldr = ldr;
+    return gemm(st, p);
 }
 static bool use_dense(const CarState* s, int rows) { return s->m->d.dtype == CAR_BF16 && rows >= 64 && s->qkvP != nullptr; }
 
@@ -912,8 +887,8 @@ extern "C" int car_op_linear(int32_t dtype, const void* x, const void* w, const 
 }
 
 // the dense (M >= 64 rows) tensor-core linear of the prefill / MLP path, exposed for unit tests and micro-benchmarks:
-// y[M,N] = act(x[M,K] · w[N,K]^T) (+ resid), bf16, fp32 accumulate (gemm_wgmma.cuh; the mma.sync kernel of gemm_dense.cuh when the
-// operands are not 16-byte aligned or the TMA tensor-map encoder is unavailable)
+// y[M,N] = act(x[M,K] · w[N,K]^T) (+ resid), bf16, fp32 accumulate, routed by gemm() (gemm.cu): the wgmma kernel when N and K are
+// multiples of 8 and the operands 16-byte aligned, otherwise the mma.sync kernel
 extern "C" int car_op_dense_linear(const void* x, const void* w, const void* resid, void* y, int32_t M, int32_t N, int32_t K, int32_t act,
                                    void* stream) {
     if (!x || !w || !y) CAR_FAIL(CAR_ERR_ARG, "null argument");

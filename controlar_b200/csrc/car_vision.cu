@@ -4,51 +4,13 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "gemm_dense.cuh"
-#include "gemm_wgmma.cuh"
+#include "gemm.h"
 #include "vision.cuh"
 #include "frontend.cuh"
 #include "lineart.cuh"
 #include "dpt.cuh"
 #include "midas.cuh"
 
-// wgmma path of the vision stages (gemm_wgmma.cuh): TMA tensor-map loads, accumulators in registers, persistent warp-specialised CTAs.
-// Used only where the driver provides the TMA tensor-map encoder (wg_encoder() != nullptr).
-static int wg_launch(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, const WgP& q, int tiles_m) {
-    static DevOnce once5;
-    if (once5.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
-    const int ntiles = tiles_m * ((q.N + WG_BN - 1) / WG_BN);
-    CAR_LAUNCH(gemm_wgmma_kernel, std::min(ntiles, sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
-    return CAR_OK;
-}
-
-static int dense(cudaStream_t st, DenseP p, int batch = 1) {
-    static DevOnce once;
-    if (once.first()) CAR_CUDA(cudaFuncSetAttribute(dense_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM));
-    if (p.M <= 0 || p.N <= 0) return CAR_OK;
-    if (p.alpha == 0.f) p.alpha = 1.f;
-    // plain bf16 -> bf16 GEMMs (DINOv2 linears, 1x1 convolutions) go to the wgmma kernel; same epilogue order as below
-    if (batch == 1 && p.amode == A_PLAIN && p.out_mode == 0 && !p.bias_along_m && p.alpha == 1.f && !p.bias_f && !p.resid_f && wg_encoder() != nullptr &&
-        p.K % 8 == 0 && p.N % 8 == 0 && p.lda % 8 == 0 && p.ldb % 8 == 0 && p.ldc % 8 == 0 && (!p.resid || p.ldr % 8 == 0) &&
-        ((uintptr_t)p.A % 16) == 0 && ((uintptr_t)p.B % 16) == 0 && ((uintptr_t)p.C % 16) == 0 && (!p.resid || ((uintptr_t)p.resid % 16) == 0)) {
-        alignas(64) CUtensorMap mapA, mapB;
-        if (!wg_make_map(&mapA, p.A, p.M, p.K, p.lda) || !wg_make_map(&mapB, p.B, p.N, p.K, p.ldb)) CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-        WgP q;
-        memset(&q, 0, sizeof(q));
-        q.M = p.M; q.N = p.N; q.K = p.K; q.resid = p.resid; q.ldr = p.ldr; q.C = (bf16*)p.C; q.ldc = p.ldc;
-        q.act = p.act == ACT_GELU_TANH ? 1 : (p.act == ACT_GELU_ERF ? 2 : 0); q.bias = p.bias; q.scale = p.scale;
-        return wg_launch(st, mapA, mapB, q, (p.M + WG_BM - 1) / WG_BM);
-    }
-    dim3 grid((p.N + DG_BN - 1) / DG_BN, (p.M + DG_BM - 1) / DG_BM, batch);
-    CAR_LAUNCH(dense_gemm_kernel, grid, DG_THREADS, DG_SMEM, st, p);
-    return CAR_OK;
-}
-static DenseP dp_plain(const bf16* A, int lda, const bf16* B, int ldb, int M, int N, int K, void* C, int ldc) {
-    DenseP p;
-    memset(&p, 0, sizeof(p));
-    p.A = A; p.B = B; p.M = M; p.N = N; p.K = K; p.lda = lda; p.ldb = ldb; p.C = C; p.ldc = ldc; p.alpha = 1.f;
-    return p;
-}
 template <typename... KArgs, typename... Args>
 static int launch_on(cudaStream_t st, void (*kernel)(KArgs...), unsigned grid, unsigned block, Args... args) {
     CAR_LAUNCH(kernel, grid, block, 0, st, args...);
@@ -248,7 +210,7 @@ static int dino_forward_t(CarDino* m, const TI* image, int B, int H, int W, void
     {
         DenseP p = dp_plain(patches, KP, m->w_patch, KP, B * hw, C, KP, ptok, C);
         p.bias = (const bf16*)m->b_patch;
-        CAR_TRY(dense(st, p));
+        CAR_TRY(gemm(st, p));
     }
     // 2. CLS + interpolated position embeddings
     CAR_LAUNCH((pos_embed_interp_kernel<TI>), gsz((long long)hw * C), 256, 0, st, (const TI*)m->pos, posi, d.pos_grid, h, w, C);
@@ -261,12 +223,12 @@ static int dino_forward_t(CarDino* m, const TI* image, int B, int H, int W, void
         {   // q | k  : [rows][2C]
             DenseP p = dp_plain(xn, C, Ly.w_qk, C, (int)rows, 2 * C, C, qk, 2 * C);
             p.bias = Ly.b_qk;
-            CAR_TRY(dense(st, p));
+            CAR_TRY(gemm(st, p));
         }
         {   // V^T per image: [C][Tp] = Wv[C][C] · xn_b[Tn][C]^T  (+ bias along M); padded key columns stay 0-weighted
             DenseP p = dp_plain(Ly.w_v, C, xn, C, C, Tn, C, vT, Tp);
             p.sB = (long long)Tn * C; p.sC = (long long)C * Tp; p.bias = (const bf16*)Ly.b_v; p.bias_along_m = 1;
-            CAR_TRY(dense(st, p, B));
+            CAR_TRY(gemm(st, p, B));
         }
         // fused attention (vision.cuh): scores / probabilities never leave the SM.  hidden % 64 == 0 (car_dino_create) and the
         // 256-byte aligned workspace give the kernel its 16-byte aligned rows.
@@ -274,18 +236,18 @@ static int dino_forward_t(CarDino* m, const TI* image, int B, int H, int W, void
         {   // x = x + ls1 * (dense(ctx) + b)
             DenseP p = dp_plain(ctx, C, (const bf16*)Ly.w_o, C, (int)rows, C, C, x, C);
             p.bias = (const bf16*)Ly.b_o; p.scale = (const bf16*)Ly.ls1; p.resid = x; p.ldr = C;
-            CAR_TRY(dense(st, p));
+            CAR_TRY(gemm(st, p));
         }
         CAR_LAUNCH(layernorm_kernel, (unsigned)rows, 128, 0, st, x, (const bf16*)Ly.n2w, (const bf16*)Ly.n2b, xn, C, d.eps, (long long)C, (long long)C);
         {
             DenseP p = dp_plain(xn, C, (const bf16*)Ly.w_fc1, C, (int)rows, 4 * C, C, hid, 4 * C);
             p.bias = (const bf16*)Ly.b_fc1; p.act = ACT_GELU_ERF;
-            CAR_TRY(dense(st, p));
+            CAR_TRY(gemm(st, p));
         }
         {
             DenseP p = dp_plain(hid, 4 * C, (const bf16*)Ly.w_fc2, 4 * C, (int)rows, C, 4 * C, x, C);
             p.bias = (const bf16*)Ly.b_fc2; p.scale = (const bf16*)Ly.ls2; p.resid = x; p.ldr = C;
-            CAR_TRY(dense(st, p));
+            CAR_TRY(gemm(st, p));
         }
     }
     // 4. final LayerNorm, drop CLS (dinov2_adapter.py:29): rows of image b start at token 1
@@ -298,9 +260,9 @@ static int dino_forward_t(CarDino* m, const TI* image, int B, int H, int W, void
         if (!m->ad_fc1) CAR_FAIL(CAR_ERR_STATE, "adapter_mlp weights were not registered");
         DenseP p1 = dp_plain(feat, C, m->ad_fc1, C, B * hw, m->ad_dim, C, mlp_h, m->ad_dim);
         p1.act = ACT_GELU_TANH;
-        CAR_TRY(dense(st, p1));
+        CAR_TRY(gemm(st, p1));
         DenseP p2 = dp_plain(mlp_h, m->ad_dim, m->ad_fc2, m->ad_dim, B * hw, m->ad_dim, m->ad_dim, out, m->ad_dim);
-        CAR_TRY(dense(st, p2));
+        CAR_TRY(gemm(st, p2));
     }
     return CAR_OK;
 }
@@ -438,18 +400,6 @@ static int conv_fwd(cudaStream_t st, const ConvW& c, const Act& x, int ups, int 
                     float* out_nchw_f32 = nullptr) {
     if (x.C != c.cin_pad && !(c.k == 1 && x.C == c.cin_pad)) CAR_FAIL(CAR_ERR_STATE, "conv input channel mismatch");
     if (!out_nchw_f32) CAR_TRY(car_fits(__func__, out, (size_t)x.B * Ho * Wo * c.cout));
-    if (c.k == 3 && !stride2 && !ups && !out_nchw_f32 && c.cin_pad % WG_BK == 0 && c.cout % 8 == 0 && Ho == x.H && Wo == x.W && x.H >= WG_TH && x.W >= WG_TW && wg_encoder() != nullptr &&
-        ((uintptr_t)x.p % 16) == 0 && ((uintptr_t)out.p % 16) == 0 && (!resid || ((uintptr_t)resid % 16) == 0)) {
-        // 3x3 / pad 1 convolution on the wgmma kernel: one 4-D TMA box per (tap, 64-channel block), padding by TMA zero fill
-        alignas(64) CUtensorMap mapA, mapB;
-        if (!wg_make_map_nhwc(&mapA, x.p, x.B, x.H, x.W, c.cin_pad) || !wg_make_map(&mapB, c.w, c.cout, 9 * c.cin_pad, 9 * c.cin_pad))
-            CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-        WgP q;
-        memset(&q, 0, sizeof(q));
-        q.M = x.B * x.H * x.W; q.N = c.cout; q.K = 9 * c.cin_pad; q.resid = resid; q.ldr = c.cout; q.C = out; q.ldc = c.cout; q.bias = c.b;
-        q.conv = 1; q.H = x.H; q.W = x.W; q.tiles_x = (x.W + WG_TW - 1) / WG_TW; q.tiles_y = (x.H + WG_TH - 1) / WG_TH; q.cblks = c.cin_pad / WG_BK;
-        return wg_launch(st, mapA, mapB, q, x.B * q.tiles_x * q.tiles_y);
-    }
     DenseP p;
     memset(&p, 0, sizeof(p));
     p.A = x.p; p.B = c.w; p.M = x.B * Ho * Wo; p.N = c.cout; p.K = c.k * c.k * c.cin_pad; p.ldb = p.K; p.alpha = 1.f;
@@ -459,7 +409,7 @@ static int conv_fwd(cudaStream_t st, const ConvW& c, const Act& x, int ups, int 
     p.bias = c.b;
     if (out_nchw_f32) { p.C = out_nchw_f32; p.out_mode = 2; }
     else { p.C = out; p.ldc = c.cout; p.resid = resid; p.ldr = c.cout; }
-    return dense(st, p);
+    return gemm(st, p);
 }
 static int gn_fwd(cudaStream_t st, const NormW& nw, const Act& x, Buf<bf16> y, int swish, float* stats) {
     const int G = 32;
@@ -510,18 +460,18 @@ static int attn_fwd(cudaStream_t st, const AttnW& a, Act& x, Buf<bf16> out, VqSc
     {   // V^T [B][C][hwp]
         DenseP p = dp_plain(a.v.w, C, xn.p, C, C, hw, C, s.vT, hwp);
         p.sB = (long long)hw * C; p.sC = (long long)C * hwp; p.bias = a.v.b; p.bias_along_m = 1;
-        CAR_TRY(dense(st, p, B));
+        CAR_TRY(gemm(st, p, B));
     }
     {
         DenseP p = dp_plain(q, C, k, C, hw, hw, C, s.S, hwp);
         p.sA = (long long)hw * C; p.sB = (long long)hw * C; p.sC = (long long)hw * hwp; p.alpha = 1.0f / sqrtf((float)C); p.out_mode = 1;
-        CAR_TRY(dense(st, p, B));
+        CAR_TRY(gemm(st, p, B));
     }
     CAR_LAUNCH(softmax_rows_kernel, (unsigned)((long long)B * hw), 256, 0, st, s.S, s.P, hw, hwp, hwp);
     {
         DenseP p = dp_plain(s.P, hwp, s.vT, hwp, hw, C, hwp, q, C);     // ctx overwrites q
         p.sA = (long long)hw * hwp; p.sB = (long long)C * hwp; p.sC = (long long)hw * C;
-        CAR_TRY(dense(st, p, B));
+        CAR_TRY(gemm(st, p, B));
     }
     Act ctx{q, B, x.H, x.W, C};
     CAR_TRY(conv_fwd(st, a.o, ctx, 0, 0, out, x.p, x.H, x.W));
@@ -573,7 +523,7 @@ static int vq_decode_impl(CarVQ* m, const int32_t* codes, const float* quant, in
         }
         if (m->d_has_up[idx]) {   // Upsample (vq_model.py:368-379): nearest x2, then the 3x3 convolution
             Buf<bf16> o = flip(x.p);
-            if (wg_encoder() != nullptr && x.C % WG_BK == 0) {   // materialise the up-sampled tensor (bandwidth-trivial) so the convolution is a plain TMA box walk
+            if (x.C % WG_CBLK == 0) {   // materialise the up-sampled tensor (bandwidth-trivial) so the convolution is a plain TMA box walk
                 CAR_TRY(car_fits("upsample2x", s.t2, (size_t)x.n() * 4));
                 CAR_LAUNCH(upsample2x_nhwc_kernel, gsz((long long)B * x.H * 2 * x.W * 2 * (x.C / 8)), 256, 0, st, (const bf16*)x.p, s.t2, B, x.H, x.W, x.C);
                 Act u{s.t2, B, x.H * 2, x.W * 2, x.C};
@@ -625,7 +575,7 @@ static int conv_x3(cudaStream_t st, const ConvW& c, const bf16* a3, int B, int H
     else { p.amode = stride2 ? A_CONV3x3S2 : A_CONV3x3; p.Hs = Hs; p.Ws = Ws; p.Cin = 3 * c.cin_pad; p.ups = 0; }
     p.Ho = Ho; p.Wo = Wo;
     p.bias_f = c.bf; p.C = out; p.ldc = c.cout; p.out_mode = 1; p.resid_f = resid; p.ldr = c.cout; p.act = act;
-    return dense(st, p);
+    return gemm(st, p);
 }
 static int gn_x3(cudaStream_t st, const NormW& nw, const ActF& x, Buf<bf16> y3, int swish, float* stats) {
     const int G = 32;
@@ -665,7 +615,7 @@ static int attn_x3(cudaStream_t st, const AttnW& a, ActF& x, Buf<float> out, Enc
     {   // scores [B][hw][hwp] fp32
         DenseP p = dp_plain(s.q3, 3 * C, s.k3, 3 * C, hw, hw, 3 * C, s.S, hwp);
         p.sA = (long long)hw * 3 * C; p.sB = (long long)hw * 3 * C; p.sC = (long long)hw * hwp; p.alpha = 1.0f / sqrtf((float)C); p.out_mode = 1;
-        CAR_TRY(dense(st, p, B));
+        CAR_TRY(gemm(st, p, B));
     }
     CAR_LAUNCH(softmax_rows_f32_kernel, (unsigned)rows, 256, 0, st, (const float*)s.S, s.P, hw, hwp);
     CAR_TRY(split3(st, s.P, s.P3, rows, hwp, 0));
@@ -675,7 +625,7 @@ static int attn_x3(cudaStream_t st, const AttnW& a, ActF& x, Buf<float> out, Enc
     {   // context [B][hw][C] fp32
         DenseP p = dp_plain(s.P3, 3 * hwp, s.vT3, 3 * hwp, hw, C, 3 * hwp, s.ctx, C);
         p.sA = (long long)hw * 3 * hwp; p.sB = (long long)C * 3 * hwp; p.sC = (long long)hw * C; p.out_mode = 1;
-        CAR_TRY(dense(st, p, B));
+        CAR_TRY(gemm(st, p, B));
     }
     CAR_TRY(split3(st, s.ctx, s.q3, rows, C, 0));              // (q3 is free again)
     CAR_TRY(conv_x3(st, a.o, s.q3, B, x.H, x.W, 0, out, x.p, x.H, x.W));
@@ -939,22 +889,18 @@ extern "C" int car_lineart_destroy(CarLineArt* m) {
     return CAR_OK;
 }
 
-// one window convolution (gemm_dense.cuh A_WIN): S3 source [B][Hs][Ws][cin3] -> fp32 [B][oH][oW][cout], row (b, oy, ox) of the
+// one window convolution (gemm.h A_WIN): S3 source [B][Hs][Ws][cin3] -> fp32 [B][oH][oW][cout], row (b, oy, ox) of the
 // Ho x Wo grid stored at pixel (osy*oy + oay, osx*ox + oax)
 static int la_conv(cudaStream_t st, const bf16* a3, int B, int Hs, int Ws, int cin3, const bf16* w3, const float* bias, int cout, int kh, int kw,
                    int stride, int Ho, int Wo, Buf<float> out, int oH, int oW, int osy = 1, int osx = 1, int oay = 0, int oax = 0) {
     CAR_TRY(car_fits(__func__, out, (size_t)B * oH * oW * cout));
-    static DevOnce once;
-    if (once.first()) CAR_CUDA(cudaFuncSetAttribute(dense_win_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM));
     DenseP p;
     memset(&p, 0, sizeof(p));
     p.A = a3; p.B = w3; p.M = B * Ho * Wo; p.N = cout; p.K = kh * kw * cin3; p.ldb = p.K; p.alpha = 1.f;
     p.amode = A_WIN; p.Hs = Hs; p.Ws = Ws; p.Cin = cin3; p.Ho = Ho; p.Wo = Wo; p.kh = kh; p.kw = kw; p.ws = stride;
     p.bias_f = bias; p.C = out; p.ldc = cout; p.out_mode = 1;
     p.osy = osy; p.osx = osx; p.oay = oay; p.oax = oax; p.oH = oH; p.oW = oW;
-    dim3 grid((p.N + DG_BN - 1) / DG_BN, (p.M + DG_BM - 1) / DG_BM, 1);
-    CAR_LAUNCH(dense_win_gemm_kernel, grid, DG_THREADS, DG_SMEM, st, p);
-    return CAR_OK;
+    return gemm(st, p);
 }
 static int la_nch(int HW) { return std::max(1, std::min(64, (HW + 2047) / 2048)); }
 
@@ -1134,22 +1080,10 @@ extern "C" int car_dpt_destroy(CarDpt* m) {
     return CAR_OK;
 }
 
-static int wg_launch_f32(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, const WgP& q, int tiles_m) {
-    static DevOnce once;
-    if (once.first()) CAR_CUDA(cudaFuncSetAttribute(gemm_wgmma_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
-    const int ntiles = tiles_m * ((q.N + WG_BN - 1) / WG_BN);
-    CAR_LAUNCH(gemm_wgmma_f32_kernel, std::min(ntiles, sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
-    return CAR_OK;
-}
 // out fp32 [M][ldc] = a3 (S3 rows [M][3 w.k]) · W3^T + bias (+ resid [M][ldc])
 static int dpt_gemm(cudaStream_t st, const DptLin& w, const bf16* a3, int M, Buf<float> out, int ldc, const float* resid = nullptr) {
     CAR_TRY(car_fits(__func__, out, (size_t)(M - 1) * ldc + w.n));
-    alignas(64) CUtensorMap mapA, mapB;
-    if (!wg_make_map(&mapA, a3, M, 3 * w.k, 3 * w.k) || !wg_make_map(&mapB, w.w3, w.n, 3 * w.k, 3 * w.k)) CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-    WgP q;
-    memset(&q, 0, sizeof(q));
-    q.M = M; q.N = w.n; q.K = 3 * w.k; q.bias_f = w.b; q.resid_f = resid; q.ldr = ldc; q.C32 = out; q.ldc = ldc;
-    return wg_launch_f32(st, mapA, mapB, q, (M + WG_BM - 1) / WG_BM);
+    return gemm_f32(st, a3, w.w3, M, w.n, 3 * w.k, w.b, resid, out, ldc);
 }
 // TMA convolution frame: a map smaller than one 16 x 8 pixel box is held in a zero-filled frame of at least that size
 static inline int dpt_fh(int H) { return std::max(H, WG_TH); }
@@ -1157,15 +1091,7 @@ static inline int dpt_fw(int W) { return std::max(W, WG_TW); }
 // 3x3 / pad 1 / stride 1 convolution: S3 NHWC frame [B][dpt_fh(H)][dpt_fw(W)][3 cin] -> fp32 NHWC [B][H][W][w.n] (+ resid)
 static int dpt_conv3(cudaStream_t st, const DptLin& w, const bf16* s3, int B, int H, int W, Buf<float> out, const float* resid = nullptr) {
     CAR_TRY(car_fits(__func__, out, (size_t)B * H * W * w.n));
-    const int cin3 = 3 * (w.k / 9);
-    alignas(64) CUtensorMap mapA, mapB;
-    if (!wg_make_map_nhwc(&mapA, s3, B, dpt_fh(H), dpt_fw(W), cin3) || !wg_make_map(&mapB, w.w3, w.n, 3 * w.k, 3 * w.k))
-        CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-    WgP q;
-    memset(&q, 0, sizeof(q));
-    q.M = B * H * W; q.N = w.n; q.K = 3 * w.k; q.bias_f = w.b; q.resid_f = resid; q.ldr = w.n; q.C32 = out; q.ldc = w.n;
-    q.conv = 1; q.H = H; q.W = W; q.tiles_x = (W + WG_TW - 1) / WG_TW; q.tiles_y = (H + WG_TH - 1) / WG_TH; q.cblks = cin3 / WG_BK;
-    return wg_launch_f32(st, mapA, mapB, q, B * q.tiles_x * q.tiles_y);
+    return gemm_f32_conv3(st, s3, dpt_fh(H), dpt_fw(W), w.w3, B, H, W, 3 * (w.k / 9), w.n, w.b, resid, out);
 }
 // S3 image producer (dpt.cuh dpt_image_split_kernel)
 static int dpt_img(cudaStream_t st, const float* a, const float* b, float* sum_out, Buf<bf16> y, DptImg q) {
@@ -1237,7 +1163,6 @@ static int dpt_decode(cudaStream_t st, const DptDecoder& w, const Buf<float> fe[
 extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, int32_t H, int32_t W, float* depth, void* stream) {
     if (!m || !pixel_values || !depth) CAR_FAIL(CAR_ERR_ARG, "null argument");
     if (B <= 0 || H != W || H % 32 || H < 64) CAR_FAIL(CAR_ERR_ARG, "pixel_values must be square with a side that is a multiple of 32 and at least 64");
-    if (!wg_encoder()) CAR_FAIL(CAR_ERR_UNSUPPORTED, "the DPT detector needs cuTensorMapEncodeTiled (TMA)");
     cudaStream_t st = (cudaStream_t)stream;
     const CarDptDesc& d = m->d;
     const int C = d.hidden, F = d.fusion, h = H / 16, T = 1 + h * h, M = B * T, Mp = B * h * h;
@@ -1413,7 +1338,6 @@ extern "C" int car_midas_destroy(CarMidas* m) {
 extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t H, int32_t W, float* depth, void* stream) {
     if (!m || !x || !depth) CAR_FAIL(CAR_ERR_ARG, "null argument");
     if (B <= 0 || H % 32 || W % 32 || H < 64 || W < 64) CAR_FAIL(CAR_ERR_ARG, "x must be [B][3][H][W] with H and W multiples of 32 and at least 64");
-    if (!wg_encoder()) CAR_FAIL(CAR_ERR_UNSUPPORTED, "the MiDaS detector needs cuTensorMapEncodeTiled (TMA)");
     cudaStream_t st = (cudaStream_t)stream;
     const int C = MD_C, F = MD_F, h = H / 16, w = W / 16, P = h * w, T = 1 + P, M = B * T, Mp = B * P;
     const int sh[4] = {H / 4, H / 8, h, h / 2}, sw[4] = {W / 4, W / 8, w, w / 2};

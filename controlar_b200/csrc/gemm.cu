@@ -1,0 +1,123 @@
+// gemm.cu — the one place a dense tensor-core GEMM picks its kernel, gets its TMA tensor maps, shared-memory opt-in and grid.
+#include "gemm.h"
+#include "gemm_dense.cuh"
+#include "gemm_wgmma.cuh"
+
+static_assert(ACT_GELU_TANH == 1 && ACT_GELU_ERF == 2, "WgP::act takes the ACT_* codes of the activations the wgmma epilogue implements");
+
+// ---- TMA tensor maps (driver entry point fetched through the runtime: the library does not link libcuda) ----
+typedef CUresult (*wg_encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
+                                 const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+static wg_encode_fn wg_encoder() {
+    static wg_encode_fn fn = [] {
+        void* f = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) f = nullptr;
+        return (wg_encode_fn)f;
+    }();
+    return fn;
+}
+// bf16 tensor of `rank` dimensions (innermost first, byte strides of the outer ones), 128-byte swizzle, zero fill out of bounds
+static int wg_encode(CUtensorMap* map, cuuint32_t rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box) {
+    const wg_encode_fn enc = wg_encoder();
+    if (!enc) CAR_FAIL(CAR_ERR_UNSUPPORTED, "the wgmma GEMM needs the driver's TMA tensor-map encoder (cuTensorMapEncodeTiled)");
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    if (enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+        CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
+    return CAR_OK;
+}
+// row-major bf16 matrix [rows][cols] with row pitch ld elements; box = 64 columns x 128 rows
+static int wg_make_map(CUtensorMap* map, const void* base, int rows, int cols, int ld) {
+    const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+    const cuuint32_t box[2] = {WG_BK, WG_BM};
+    return wg_encode(map, 2, base, dims, strides, box);
+}
+// NHWC bf16 tensor [N][H][W][C] as a 4-D map {C, W, H, N}; box = {64 channels, 16 x, 8 y, 1 image}
+static int wg_make_map_nhwc(CUtensorMap* map, const void* base, int N, int H, int W, int C) {
+    const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+    const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+    const cuuint32_t box[4] = {WG_BK, WG_TW, WG_TH, 1};
+    return wg_encode(map, 4, base, dims, strides, box);
+}
+
+// ---- launchers: one shared-memory opt-in and one grid rule per kernel ----
+// wgmma: persistent, at most one CTA per SM over the tiles_m x n-tiles schedule
+template <bool F32>
+static int wg_launch(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, const WgP& q, int tiles_m) {
+    static DevOnce once;
+    const auto kernel = F32 ? gemm_wgmma_f32_kernel : gemm_wgmma_kernel;
+    if (once.first()) CAR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
+    const int ntiles = tiles_m * ((q.N + WG_BN - 1) / WG_BN);
+    CAR_LAUNCH(kernel, std::min(ntiles, sm_count()), WG_THREADS, WG_SMEM, st, mapA, mapB, q);
+    return CAR_OK;
+}
+// wgmma plain GEMM: q holds M, N, K and the epilogue; A [M][lda], B [N][ldb]
+template <bool F32>
+static int wg_plain(cudaStream_t st, const WgP& q, const bf16* A, int lda, const bf16* B, int ldb) {
+    alignas(64) CUtensorMap mapA, mapB;
+    CAR_TRY(wg_make_map(&mapA, A, q.M, q.K, lda));
+    CAR_TRY(wg_make_map(&mapB, B, q.N, q.K, ldb));
+    return wg_launch<F32>(st, mapA, mapB, q, (q.M + WG_BM - 1) / WG_BM);
+}
+// wgmma 3x3 / pad 1 convolution (one 4-D TMA box per (tap, 64-channel block), padding by TMA zero fill): q holds M = nimg H W, N,
+// K = 9 cin and the epilogue; src NHWC frame [nimg][fh][fw][cin] around the H x W map, B [N][ldb]
+template <bool F32>
+static int wg_conv3(cudaStream_t st, WgP q, const bf16* src, int nimg, int fh, int fw, int cin, int H, int W, const bf16* B, int ldb) {
+    alignas(64) CUtensorMap mapA, mapB;
+    CAR_TRY(wg_make_map_nhwc(&mapA, src, nimg, fh, fw, cin));
+    CAR_TRY(wg_make_map(&mapB, B, q.N, q.K, ldb));
+    q.conv = 1; q.H = H; q.W = W; q.tiles_x = (W + WG_TW - 1) / WG_TW; q.tiles_y = (H + WG_TH - 1) / WG_TH; q.cblks = cin / WG_BK;
+    return wg_launch<F32>(st, mapA, mapB, q, nimg * q.tiles_x * q.tiles_y);
+}
+// mma.sync: one CTA per 128 x 128 output tile, blockIdx.z over the batch
+template <bool WIN>
+static int dg_launch(cudaStream_t st, const DenseP& p, int batch) {
+    static DevOnce once;
+    const auto kernel = WIN ? dense_win_gemm_kernel : dense_gemm_kernel;
+    if (once.first()) CAR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM));
+    CAR_LAUNCH(kernel, dim3((p.N + DG_BN - 1) / DG_BN, (p.M + DG_BM - 1) / DG_BM, batch), DG_THREADS, DG_SMEM, st, p);
+    return CAR_OK;
+}
+
+static bool aligned16(const void* p) { return ((uintptr_t)p % 16) == 0; }
+
+int gemm(cudaStream_t st, const DenseP& dp, int batch) {
+    if (dp.M <= 0 || dp.N <= 0) return CAR_OK;
+    DenseP p = dp;
+    if (p.alpha == 0.f) p.alpha = 1.f;
+    if (p.amode == A_WIN) return dg_launch<true>(st, p, batch);
+    // the wgmma epilogue: bf16 bias along n, bf16 rounding, GELU (tanh or erf), LayerScale, bf16 residual, one bf16 [M][ldc] output
+    const bool wg_epi = batch == 1 && p.out_mode == 0 && p.alpha == 1.f && !p.bias_along_m && !p.bias_f && !p.resid_f &&
+                        (p.act == ACT_NONE || p.act == ACT_GELU_TANH || p.act == ACT_GELU_ERF);
+    // its tensor maps and paired stores: 16-byte row pitches and base pointers, whole 8-column groups
+    const bool wg_ok = wg_epi && p.K % 8 == 0 && p.N % 8 == 0 && p.lda % 8 == 0 && p.ldb % 8 == 0 && p.ldc % 8 == 0 &&
+                       (!p.resid || p.ldr % 8 == 0) && aligned16(p.A) && aligned16(p.B) && aligned16(p.C) && (!p.resid || aligned16(p.resid));
+    // the convolution walks whole 64-channel blocks of 16 x 8 pixel boxes over an unscaled map
+    const bool wg_conv = p.amode == A_CONV3x3 && !p.ups && p.Cin % WG_BK == 0 && p.Ho == p.Hs && p.Wo == p.Ws && p.Hs >= WG_TH && p.Ws >= WG_TW;
+    if (wg_ok && (p.amode == A_PLAIN || wg_conv)) {
+        WgP q;
+        memset(&q, 0, sizeof(q));
+        q.M = p.M; q.N = p.N; q.K = p.K; q.resid = p.resid; q.ldr = p.ldr; q.C = (bf16*)p.C; q.ldc = p.ldc;
+        q.act = p.act; q.bias = p.bias; q.scale = p.scale;
+        if (p.amode == A_PLAIN) return wg_plain<false>(st, q, p.A, p.lda, p.B, p.ldb);
+        return wg_conv3<false>(st, q, p.A, p.M / (p.Hs * p.Ws), p.Hs, p.Ws, p.Cin, p.Hs, p.Ws, p.B, p.ldb);
+    }
+    return dg_launch<false>(st, p, batch);
+}
+
+int gemm_f32(cudaStream_t st, const bf16* A, const bf16* B, int M, int N, int K, const float* bias, const float* resid, float* out, int ldc) {
+    WgP q;
+    memset(&q, 0, sizeof(q));
+    q.M = M; q.N = N; q.K = K; q.bias_f = bias; q.resid_f = resid; q.ldr = ldc; q.C32 = out; q.ldc = ldc;
+    return wg_plain<true>(st, q, A, K, B, K);
+}
+
+int gemm_f32_conv3(cudaStream_t st, const bf16* src, int fh, int fw, const bf16* B, int nimg, int H, int W, int cin, int N, const float* bias,
+                   const float* resid, float* out) {
+    WgP q;
+    memset(&q, 0, sizeof(q));
+    q.M = nimg * H * W; q.N = N; q.K = 9 * cin; q.bias_f = bias; q.resid_f = resid; q.ldr = N; q.C32 = out; q.ldc = N;
+    return wg_conv3<true>(st, q, src, nimg, fh, fw, cin, H, W, B, q.K);
+}

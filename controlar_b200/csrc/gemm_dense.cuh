@@ -1,47 +1,12 @@
 // gemm_dense.cuh — tiled bf16 tensor-core GEMM for the dense (M >= 128) stages: DINOv2 linears/attention, VQGAN
 // convolutions as implicit GEMM (NHWC), VQGAN attention.  C[M,N] = epi(A[M,K] · B[N,K]^T), fp32 accumulate.
-//
-//   A operand addressing modes
-//     A_PLAIN   : row-major [M, lda]
-//     A_CONV3x3 : implicit im2col of an NHWC tensor for a 3x3 / pad 1 / stride 1 convolution, optionally reading a
-//                 nearest-2x up-sampled view of the source (Upsample, tokenizer/tokenizer_image/vq_model.py:368-379);
-//                 K index = tap*Cin + c, tap = ky*3+kx; row m = (b*Ho + y)*Wo + x
-//     A_CONV3x3S2: 3x3 / stride 2 on an input padded (0,1,0,1) (Downsample, vq_model.py:382-397)
-//     A_WIN      : kh x kw window, stride s, over an already padded NHWC source [B][Hs][Ws][Cin] (no bounds checks in the
-//                  window): row m = (b*Ho + oy)*Wo + ox reads pixels (s*oy + ky, s*ox + kx), K index = (ky*kw + kx)*Cin + c.
-//                  fp32 output through a pixel map: row (b, oy, ox) is stored at pixel (osy*oy + oay, osx*ox + oax) of an
-//                  [B][oH][oW][ldc] tensor.  Own instantiation (dense_win_gemm_kernel); dense_gemm_kernel does not take it.
-//   B operand: row-major [N, K] (nn.Linear / flattened conv weight [Cout, 9*Cin] in (ky,kx,c) order)
-//   batched via blockIdx.z with element strides.
+// A operand addressing modes and the DenseP fields: gemm.h.
 //
 // Round-1 implementation note: mma.sync m16n8k16 + cp.async 3-stage pipeline + ldmatrix (the robust legacy tensor
-// path).  The plain GEMMs and 3x3 convolutions that fit
-// the TMA tile walk run on gemm_wgmma.cuh instead; this kernel takes the batched, strided and up-sampling cases.
+// path).  gemm() (gemm.cu) sends the plain GEMMs and 3x3 convolutions that fit the TMA tile walk to gemm_wgmma.cuh
+// instead; this kernel takes the batched, strided, up-sampling and fp32-output cases.
 #pragma once
-#include "common.cuh"
-
-enum { A_PLAIN = 0, A_CONV3x3 = 1, A_CONV3x3S2 = 2, A_WIN = 3 };
-enum { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF = 2, ACT_RELU = 3 };
-
-struct DenseP {
-    const bf16* A; const bf16* B;
-    int M, N, K;
-    int lda, ldb;
-    long long sA, sB, sC, sR;          // batch strides (elements) for A, B, C, resid
-    int amode; int Hs, Ws, Cin, Ho, Wo, ups;   // conv source dims (before up-sampling), output dims
-    // epilogue: v = acc*alpha (+bias[n] | bias[m]); v = rnd(v); act; (*scale[n]); (+resid); store
-    float alpha;
-    const bf16* bias; int bias_along_m;
-    const float* bias_f;               // fp32 bias (per n), fp32-output modes
-    const float* resid_f;              // fp32 residual [M, ldr] (+ z * sR), fp32-output modes: added without rounding
-    int act;
-    const bf16* scale;                 // LayerScale lambda (per n), applied after rounding: r(r(v)*scale)
-    const bf16* resid; int ldr;        // residual added last: r(v + resid)
-    void* C; int ldc;
-    int out_mode;                      // 0: bf16 [M, ldc]; 1: fp32 [M, ldc]; 2: fp32 NCHW image: C[(b*N + n)*Ho*Wo + pix]
-    int kh, kw, ws;                    // A_WIN: window and stride
-    int osy, osx, oay, oax, oH, oW;    // A_WIN: output pixel map
-};
+#include "gemm.h"
 
 constexpr int DG_BM = 128, DG_BN = 128, DG_BK = 32, DG_STAGES = 3, DG_THREADS = 256;
 constexpr int DG_SMEM = DG_STAGES * (DG_BM + DG_BN) * DG_BK * 2;   // 48 KB
@@ -218,5 +183,5 @@ __device__ __forceinline__ void dense_gemm_body(const DenseP& p) {
         }
     }
 }
-static __global__ void __launch_bounds__(DG_THREADS) dense_gemm_kernel(DenseP p) { dense_gemm_body<false>(p); }   // (static: one copy per translation unit)
-static __global__ void __launch_bounds__(DG_THREADS) dense_win_gemm_kernel(DenseP p) { dense_gemm_body<true>(p); }
+__global__ void __launch_bounds__(DG_THREADS) dense_gemm_kernel(DenseP p) { dense_gemm_body<false>(p); }
+__global__ void __launch_bounds__(DG_THREADS) dense_win_gemm_kernel(DenseP p) { dense_gemm_body<true>(p); }

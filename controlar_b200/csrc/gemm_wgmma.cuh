@@ -19,10 +19,10 @@
 // Shared-memory descriptors (sm_90 layout): start >> 4 | LBO (unused for swizzled K-major, 1) << 16 | SBO 1024 >> 4 << 32 |
 // layout 1 (128-byte swizzle) << 62; the k16 step inside a 128-byte swizzle atom advances the start address by 32 bytes.
 #pragma once
-#include "common.cuh"
+#include "gemm.h"
 #include <cuda.h>
 
-constexpr int WG_BM = 128, WG_BN = 128, WG_BK = 64, WG_STAGES = 6, WG_THREADS = 384, WG_CONSUMERS = 2;
+constexpr int WG_BM = 128, WG_BN = 128, WG_BK = WG_CBLK, WG_STAGES = 6, WG_THREADS = 384, WG_CONSUMERS = 2;
 constexpr int WG_TILE_BYTES = WG_BM * WG_BK * 2;                               // 16 KB per operand and stage
 constexpr int WG_STAGE_BYTES = 2 * WG_TILE_BYTES;
 constexpr int WG_SMEM = WG_STAGES * WG_STAGE_BYTES + 1024;                     // + 1024-byte alignment slack (swizzle atoms)
@@ -44,7 +44,7 @@ struct WgP {
     // round to bf16 (resid, C, act, bias, scale) are not read there.
     const float* bias_f; const float* resid_f; float* C32;
 };
-constexpr int WG_TW = 16, WG_TH = 8;                                            // output-pixel block of a conv tile (WG_TW * WG_TH = WG_BM)
+static_assert(WG_TW * WG_TH == WG_BM, "a conv tile's output-pixel block is one 128-row A tile");
 
 __device__ __forceinline__ uint32_t wg_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void wg_mbar_init(uint32_t bar, int count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count)); }
@@ -218,46 +218,11 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap& mapA, const C
         }
     }
 }
-static __global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                                                                          const WgP p) {
+__global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                                                                   const WgP p) {
     gemm_wgmma_body<false>(mapA, mapB, p);
 }
-static __global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_f32_kernel(const __grid_constant__ CUtensorMap mapA,
-                                                                              const __grid_constant__ CUtensorMap mapB, const WgP p) {
+__global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_f32_kernel(const __grid_constant__ CUtensorMap mapA,
+                                                                       const __grid_constant__ CUtensorMap mapB, const WgP p) {
     gemm_wgmma_body<true>(mapA, mapB, p);
-}
-
-// ---- host: tensor maps (driver entry point fetched through the runtime: the library does not link libcuda) ----
-typedef CUresult (*wg_encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                 const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static wg_encode_fn wg_encoder() {
-    static wg_encode_fn fn = [] {
-        void* f = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) f = nullptr;
-        return (wg_encode_fn)f;
-    }();
-    return fn;
-}
-// row-major bf16 matrix [rows][cols] with row pitch ld elements; box = 64 columns x 128 rows, 128-byte swizzle, zero fill out of bounds
-static bool wg_make_map(CUtensorMap* map, const void* base, int rows, int cols, int ld) {
-    wg_encode_fn enc = wg_encoder();
-    if (!enc) return false;
-    const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-    const cuuint32_t box[2] = {WG_BK, WG_BM};
-    const cuuint32_t estr[2] = {1, 1};
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-// NHWC bf16 tensor [N][H][W][C] as a 4-D map {C, W, H, N}; box = {64 channels, 16 x, 8 y, 1 image}, 128-byte swizzle, zero fill outside
-static bool wg_make_map_nhwc(CUtensorMap* map, const void* base, int N, int H, int W, int C) {
-    wg_encode_fn enc = wg_encoder();
-    if (!enc) return false;
-    const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-    const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    const cuuint32_t box[4] = {WG_BK, WG_TW, WG_TH, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }

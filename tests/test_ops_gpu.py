@@ -89,10 +89,12 @@ def test_sampler_philox_is_seeded_and_distributional():
 
 
 @pytest.mark.parametrize("M,N,K,act,res", [(1920, 3584, 1280, 0, False), (1920, 1280, 3584, 0, True), (480, 768, 256, 1, False),
-                                            (1000, 1288, 1096, 0, True), (130, 136, 72, 1, True), (16384, 1280, 1280, 1, False)])
-def test_dense_tcgen05_linear_vs_torch(M, N, K, act, res):
-    """gemm_wgmma.cuh (TMA + wgmma, accumulators in registers): y = act(x w^T) (+ resid) against an fp32 torch reference of the same rounding points
-    (bf16 product rounding, GELU-tanh in bf16, residual add in bf16); includes M / N / K tails (K % 64 != 0, partial tiles)."""
+                                            (1000, 1288, 1096, 0, True), (130, 136, 72, 1, True), (16384, 1280, 1280, 1, False),
+                                            (200, 100, 72, 1, True)])
+def test_dense_linear_vs_torch(M, N, K, act, res):
+    """gemm() (gemm.cu): y = act(x w^T) (+ resid) against an fp32 torch reference of the same rounding points (bf16 product rounding,
+    GELU-tanh in bf16, residual add in bf16); includes M / N / K tails (K % 64 != 0, partial tiles).  N % 8 != 0 takes the mma.sync
+    kernel, every other row the wgmma kernel (TMA + wgmma, accumulators in registers)."""
     from controlar_b200 import engine
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     x = (torch.randn(M, K, device="cuda", generator=g) * 0.5).to(torch.bfloat16)
