@@ -33,6 +33,11 @@ class CarTrainWeights(C.Structure):
                 ("adapter_dim", C.c_int32), ("num_classes", C.c_int32), ("cond_uncond", C.c_void_p)]
 
 
+class CarTrainDropout(C.Structure):
+    _fields_ = [("token_p", C.c_float), ("resid_p", C.c_float), ("ffn_p", C.c_float), ("n_layer", C.c_int32),
+                ("drop_path", C.c_void_p), ("seed", C.c_void_p)]
+
+
 class CarSampling(C.Structure):
     _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float),
                 ("sample_logits", C.c_int32), ("cfg_scale", C.c_float), ("cfg_interval", C.c_int32),
@@ -76,6 +81,9 @@ PROTOTYPES = {
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "car_train_backward": (C.c_int, [C.c_void_p, C.POINTER(CarTrainWeights), C.c_void_p, C.c_void_p, C.c_void_p]),
     "car_train_destroy": (C.c_int, [C.c_void_p]),
+    "car_train_set_dropout": (C.c_int, [C.c_void_p, C.POINTER(CarTrainDropout)]),
+    "car_dropout_keep_mask": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p,
+                                        C.c_void_p]),
     "car_canny_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
     "car_canny_u8": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                C.c_void_p, C.c_void_p]),

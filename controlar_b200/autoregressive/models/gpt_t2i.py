@@ -160,10 +160,15 @@ class TransformerBlock(nn.Module):
         self.ffn_norm = RMSNorm(config.dim, eps=config.norm_eps)
 
 
+def _dropout_fields(cfg):
+    return (cfg.token_dropout_p, cfg.attn_dropout_p, cfg.resid_dropout_p, cfg.ffn_dropout_p, cfg.drop_path_rate)
+
+
 class Transformer(nn.Module):
     def __init__(self, config: ModelArgs):
         super().__init__()
         self.config = config
+        self._dropout_built = _dropout_fields(config)      # the reference builds its nn.Dropout / DropPath layers here, once
         self.vocab_size, self.n_layer, self.block_size = config.vocab_size, config.n_layer, config.block_size
         self.num_classes, self.model_type, self.cls_token_num = config.num_classes, config.model_type, config.cls_token_num
         self.layer_internal = config.n_layer // 3
@@ -293,9 +298,13 @@ class Transformer(nn.Module):
         if not self.training:
             raise ValueError("forward(idx, cond_idx) is the training branch: call model.train() first (the reference fails here in eval mode too)")
         cfg = self.config
-        if max(cfg.token_dropout_p, cfg.resid_dropout_p, cfg.ffn_dropout_p, cfg.attn_dropout_p, cfg.drop_path_rate) > 0:
-            raise NotImplementedError("controlar_b200 training forward: dropout layers with p > 0 are not built yet "
-                                      "(construct the model with token/resid/ffn dropout 0, i.e. --dropout-p 0 --token-dropout-p 0)")
+        if _dropout_fields(cfg) != getattr(self, "_dropout_built", _dropout_fields(cfg)):
+            raise NotImplementedError("controlar_b200 training forward: the dropout probabilities of model.config changed after the "
+                                      "model was built; like the reference, whose dropout layers are built from ModelArgs once, they "
+                                      "are fixed at construction: build the model with the ModelArgs to train with")
+        if cfg.attn_dropout_p > 0:
+            raise NotImplementedError("controlar_b200 training forward: attention-probability dropout (attn_dropout_p > 0) is not "
+                                      "supported; token, residual and feed-forward dropout and drop_path_rate are")
         B, n = idx.shape
         th = getattr(self, "_car_train", None)
         key = tuple(p.data_ptr() for p in self.parameters())
@@ -311,14 +320,33 @@ class Transformer(nn.Module):
             drop = torch.rand(B, device=idx.device) < cfg.class_dropout_prob
         else:
             drop = torch.zeros(B, dtype=torch.bool, device=idx.device)
+        dropout = self._train_dropout(idx.device)
         feat = self.adapter(condition) if condition is not None else None      # control encoder (CUDA path of vision.py)
         if targets is not None and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             # loss.backward() works like in the reference's train loop (train_c2i_canny.py:200-211): the library's own backward
             # (car_train_backward) behind a torch.autograd.Function; gradients land in .grad of this module's parameters and, when
             # `feat` is part of an autograd graph, flow on into the control encoder
             names = _engine.ARTrainHandle.grad_params(self)
-            return _TrainStep.apply(self, th, idx, cond_idx, feat, drop, mask, targets, valid, *[p for _, p in names])
-        return th.forward(idx, cond_idx, feat, drop, mask, targets, valid)
+            return _TrainStep.apply(self, th, idx, cond_idx, feat, drop, mask, targets, valid, dropout, *[p for _, p in names])
+        return _handle_forward(th, (idx, cond_idx, feat, drop, mask, targets, valid), dropout)
+
+    def _train_dropout(self, device):
+        """The dropout of this training forward: None when every site is off (no random draw: the dropout-free path is unchanged),
+        else (token_p, resid_p, ffn_p, per-layer drop-path rates or None, seed).  The seed is one 64-bit draw from torch's default
+        generator of the device, kept on the device (no host sync): torch.manual_seed reproduces a step, consecutive steps and
+        differently seeded DDP ranks get different masks.  The rates are the reference's (gpt_t2i.py:347)."""
+        cfg = self.config
+        rates = None
+        if cfg.drop_path_rate > 0:
+            rates = [x.item() for x in torch.linspace(0, cfg.drop_path_rate, cfg.n_layer)]
+        if max(cfg.token_dropout_p, cfg.resid_dropout_p, cfg.ffn_dropout_p) <= 0 and rates is None:
+            return None
+        forced = getattr(self, "_force_dropout_seed", None)
+        if forced is not None:
+            seed = torch.tensor([int(forced) & 0xFFFFFFFFFFFFFFFF], dtype=torch.uint64).view(torch.int64).to(device)
+        else:
+            seed = torch.empty(1, dtype=torch.int64, device=device).random_(-2 ** 63, None)
+        return (float(cfg.token_dropout_p), float(cfg.resid_dropout_p), float(cfg.ffn_dropout_p), rates, seed)
 
     def _n_img_check(self, condition):
         if condition.shape[1] != self._n_img:
@@ -329,13 +357,18 @@ class Transformer(nn.Module):
         return list(self.layers)
 
 
+def _handle_forward(handle, args, dropout):
+    """ARTrainHandle.forward; the dropout settings are passed only when a site is on"""
+    return handle.forward(*args) if dropout is None else handle.forward(*args, dropout=dropout)
+
+
 class _TrainStep(torch.autograd.Function):
     """(logits, loss) = car_train_forward; backward = car_train_backward.  Only `loss` is differentiable (the logits come back
     detached: the train scripts never differentiate through them)."""
 
     @staticmethod
-    def forward(ctx, module, handle, idx, cond_idx, feat, drop, mask, targets, valid, *params):
-        logits, loss = handle.forward(idx, cond_idx, feat, drop, mask, targets, valid)
+    def forward(ctx, module, handle, idx, cond_idx, feat, drop, mask, targets, valid, dropout, *params):
+        logits, loss = _handle_forward(handle, (idx, cond_idx, feat, drop, mask, targets, valid), dropout)
         ctx.module, ctx.handle, ctx.generation = module, handle, handle.generation
         ctx.want_feat = feat is not None and feat.requires_grad
         ctx.n_params = len(params)
@@ -350,7 +383,7 @@ class _TrainStep(torch.autograd.Function):
         grads, dfeat = ctx.handle.backward(ctx.module, loss_grad=g_loss, want_feat_grad=ctx.want_feat)
         names = _engine.ARTrainHandle.grad_params(ctx.module)
         out = [grads.get(k) if p.requires_grad else None for k, p in names]
-        return (None, None, None, None, dfeat if ctx.want_feat else None, None, None, None, None, *out)
+        return (None, None, None, None, dfeat if ctx.want_feat else None, None, None, None, None, None, *out)
 
 
 def _factory(n_layer, n_head, dim):

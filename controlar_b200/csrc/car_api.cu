@@ -14,6 +14,7 @@
 #include "gemm.h"
 #include "train.cuh"
 #include "train_bwd.cuh"
+#include "dropout.cuh"
 #include "t5.cuh"
 #include <algorithm>
 
@@ -972,7 +973,32 @@ struct CarTrain : CarOwned {
     const uint8_t *f_drop = nullptr, *f_mask = nullptr;
     const float* f_valid = nullptr;
     bool fwd_ok = false;
+    // dropout (car_train_set_dropout): the settings the next forward takes, and the ones the last forward ran with (its backward's)
+    struct DropCfg { float tok_p = 0.f, resid_p = 0.f, ffn_p = 0.f; std::vector<float> path; const uint64_t* seed = nullptr; };
+    DropCfg drop_next, drop_fwd;
 };
+
+// keep = fp32(1 - p), scale = fp32(1 / keep): the values ATen's CUDA dropout derives from p (native_dropout -> keep probability in
+// double, cast to the fp32 accumulate type, scale = 1.0 / keep)
+static void tr_keep_scale(float p, float* keep, float* scale) {
+    *keep = (float)(1.0 - (double)p);
+    *scale = (float)(1.0 / (double)*keep);
+}
+// the fused dropout of one site of layer l under the settings c; every part off when its p (or rate) is 0
+static TrDrop tr_drop(const CarTrain::DropCfg& c, int site, int l) {
+    TrDrop r{c.seed, site, l, 1.f, 1.f, 0, 1.f, 1.f};
+    const float p = site == CAR_DROP_TOKEN ? c.tok_p : (site == CAR_DROP_RESID ? c.resid_p : c.ffn_p);
+    if (p > 0.f) tr_keep_scale(p, &r.keep, &r.scale);
+    const float rate = (site != CAR_DROP_TOKEN && !c.path.empty()) ? c.path[l] : 0.f;
+    if (rate > 0.f) {                                          // utils/drop_path.py: bernoulli_(keep).div_(keep) on a bf16 tensor
+        float unused;
+        tr_keep_scale(rate, &r.path_keep, &unused);
+        r.path_site = site == CAR_DROP_RESID ? CAR_DROP_PATH_ATTN : CAR_DROP_PATH_FFN;
+        r.path_mult = __bfloat162float(__float2bfloat16_rn(1.f / r.path_keep));
+    }
+    return r;
+}
+static bool tr_drop_on(const TrDrop& r) { return r.seed != nullptr && (r.keep < 1.f || r.path_keep < 1.f); }
 
 static int tr_cast(cudaStream_t st, const void* src, bf16* dst, long long n) {
     CAR_LAUNCH(tr_cast_bf16_kernel, gsz(n), 256, 0, st, (const float*)src, dst, n);
@@ -1068,6 +1094,23 @@ static int tr_attn_smem(size_t floats_per_warp, const void* fn, size_t* bytes) {
     return CAR_OK;
 }
 
+// h += branch output t->o (fp32 += bf16, gpt_t2i.py:305-306) with the branch's dropout and drop path of the last forward's settings
+static int tr_residual_add(CarTrain* t, cudaStream_t st, int site, int l, int R, int B, int S) {
+    const int dim = t->d.dim;
+    const TrDrop dr = tr_drop(t->drop_fwd, site, l);
+    if (tr_drop_on(dr)) CAR_LAUNCH(tr_add_rows_drop_kernel, gsz((long long)R * dim / 4), 256, 0, st, t->h, (const bf16*)t->o, B, S, dim, dr);
+    else CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)R * dim), 256, 0, st, t->h, (const bf16*)t->o, B, S, S, 0, dim);
+    return CAR_OK;
+}
+// the bf16 gradient of a branch output from the fp32 stream gradient t->dh, through the branch's drop path and dropout
+static int tr_residual_take(CarTrain* t, cudaStream_t st, int site, int l, int R, int B, int S) {
+    const int dim = t->d.dim;
+    const TrDrop dr = tr_drop(t->drop_fwd, site, l);
+    if (tr_drop_on(dr)) CAR_LAUNCH(tr_take_rows_drop_kernel, gsz((long long)R * dim / 4), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim, dr);
+    else CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)R * dim), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim);
+    return CAR_OK;
+}
+
 // One TransformerBlock (gpt_t2i.py:303-307) on the fp32 stream t->h, preceded by the control add of gpt_t2i.py:458-460 when the
 // block opens a third of the stack.  for_bwd: the recompute of car_train_backward — keeps the block input (after the control
 // add) in t->h0, the attention-side norm output in t->x, the feed-forward-side one in t->x2, and stops before w2 (t->h then
@@ -1089,7 +1132,7 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     CAR_LAUNCH(tr_attention_kernel, (unsigned)(((long long)B * H * S + TRA_WARPS - 1) / TRA_WARPS), TRA_WARPS * 32, att_smem, st, (const bf16*)t->q,
                (const bf16*)t->kc, (const bf16*)t->vc, mask, B, H, S, t->att);
     CAR_TRY(dense_linear(st, t->att, dim, t->b_wo[l], R, dim, dim, ACT_NONE, nullptr, 0, t->o, dim));
-    CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)R * dim), 256, 0, st, t->h, (const bf16*)t->o, B, S, S, 0, dim);
+    CAR_TRY(tr_residual_add(t, st, CAR_DROP_RESID, l, R, B, S));
     bf16* xn = for_bwd ? t->x2 : t->x;
     CAR_LAUNCH(tr_rmsnorm_kernel, R, 256, 0, st, (const float*)t->h, (const float*)t->ffn_norm[l], xn, dim, d.norm_eps, S, S, 0);
     CAR_TRY(dense_linear(st, xn, dim, t->b_w1[l], R, F, dim, ACT_NONE, nullptr, 0, t->g, F));
@@ -1097,7 +1140,7 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     CAR_LAUNCH(swiglu_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, t->act, (long long)R * F);
     if (for_bwd) return CAR_OK;
     CAR_TRY(dense_linear(st, t->act, F, t->b_w2[l], R, dim, F, ACT_NONE, nullptr, 0, t->o, dim));
-    CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)R * dim), 256, 0, st, t->h, (const bf16*)t->o, B, S, S, 0, dim);
+    CAR_TRY(tr_residual_add(t, st, CAR_DROP_FFN, l, R, B, S));
     return CAR_OK;
 }
 
@@ -1113,6 +1156,9 @@ extern "C" int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const in
     const int n = n_img - 1, S = T + n, R = B * S, RC = B * n_img;
     if (S > T + d.block_size) CAR_FAIL(CAR_ERR_ARG, "sequence longer than the RoPE table");
     t->fwd_ok = false;
+    t->drop_fwd = t->drop_next;
+    const TrDrop dtok = tr_drop(t->drop_fwd, CAR_DROP_TOKEN, 0);
+    const bool tok_on = tr_drop_on(dtok);
     // 0. autocast: bf16 copies of every nn.Linear weight, re-cast each forward (the fp32 masters may have been stepped)
     for (int l = 0; l < L; ++l) {
         CAR_TRY(tr_cast(st, t->wqkv[l], t->b_wqkv[l], (long long)3 * dim * dim)); CAR_TRY(tr_cast(st, t->wo[l], t->b_wo[l], (long long)dim * dim));
@@ -1126,16 +1172,23 @@ extern "C" int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const in
         for (int j = 0; j < 3; ++j) { CAR_TRY(tr_cast(st, t->w.w.ctl_fc1[j], t->b_ctl1[j], (long long)dim * dim)); CAR_TRY(tr_cast(st, t->w.w.ctl_fc2[j], t->b_ctl2[j], (long long)dim * dim)); }
         CAR_TRY(tr_cast(st, t->w.adapter_fc1, t->b_ad1, (long long)dim * t->w.adapter_dim)); CAR_TRY(tr_cast(st, t->w.adapter_fc2, t->b_ad2, (long long)dim * dim));
     }
-    // 1. prefix rows: CaptionEmbedder (token_drop, cap_proj) gpt_t2i.py:145-162 or LabelEmbedder :78-97; image-token rows :423
+    // 1. prefix rows: CaptionEmbedder (token_drop, cap_proj) gpt_t2i.py:145-162 or LabelEmbedder :78-97; image-token rows :423;
+    //    tok_dropout (:430) fused into the writes of both
     if (d.model_type == 1) {
         CAR_LAUNCH(tr_caption_select_kernel, gsz((long long)B * T * d.caption_dim), 256, 0, st, (const float*)cond, (const float*)t->w.cap_uncond,
                    drop_ids, t->capx, B, T, d.caption_dim);
         CAR_TRY(tr_mlp(st, t->capx, B * T, d.caption_dim, t->b_cap1, t->b_cap2, dim, t->ctmp, t->o));
-        CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const bf16*)t->o, t->h, B, T, S, 0, dim);
+        if (tok_on) CAR_LAUNCH(tr_put_rows_drop_kernel, gsz((long long)B * T * dim / 4), 256, 0, st, (const bf16*)t->o, t->h, B, T, S, 0, dim, dtok);
+        else CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const bf16*)t->o, t->h, B, T, S, 0, dim);
+    } else if (tok_on) {
+        CAR_LAUNCH(tr_embed_rows_drop_kernel, B, 256, 0, st, (const float*)t->w.w.label_table, (const int*)cond, 1, drop_ids, t->w.num_classes, t->h, B, 1, S, 0, dim, dtok);
     } else {
         CAR_LAUNCH(tr_embed_rows_kernel, B, 256, 0, st, (const float*)t->w.w.label_table, (const int*)cond, 1, drop_ids, t->w.num_classes, t->h, B, 1, S, 0, dim);
     }
-    CAR_LAUNCH(tr_embed_rows_kernel, B * n, 256, 0, st, (const float*)t->w.w.tok_embeddings, (const int*)idx, n, (const unsigned char*)nullptr, 0, t->h, B, n, S, T, dim);
+    if (tok_on)
+        CAR_LAUNCH(tr_embed_rows_drop_kernel, B * n, 256, 0, st, (const float*)t->w.w.tok_embeddings, (const int*)idx, n, (const unsigned char*)nullptr, 0, t->h, B, n, S, T, dim, dtok);
+    else
+        CAR_LAUNCH(tr_embed_rows_kernel, B * n, 256, 0, st, (const float*)t->w.w.tok_embeddings, (const int*)idx, n, (const unsigned char*)nullptr, 0, t->h, B, n, S, T, dim);
     // 2. control tokens: adapter_mlp -> token_drop -> condition_mlp  gpt_t2i.py:424-427 (feat = the control encoder's output tokens)
     if (feat) {
         CAR_TRY(tr_mlp(st, (const bf16*)feat, RC, t->w.adapter_dim, t->b_ad1, t->b_ad2, dim, t->ctmp, t->cin));
@@ -1233,8 +1286,8 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
     for (int l = L - 1; l >= 0; --l) {
         CAR_CUDA(cudaMemcpyAsync(t->h, t->hs + (size_t)l * R * dim, (size_t)R * dim * 4, cudaMemcpyDeviceToDevice, st));
         CAR_TRY(tr_block_fwd(t, st, l, B, n_img, mask, has_feat, true));
-        // feed-forward: h_out = h_mid + w2(silu(w1 x2) * w3 x2)
-        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)R * dim), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim);
+        // feed-forward: h_out = h_mid + drop_path(ffn_dropout(w2(silu(w1 x2) * w3 x2)))
+        CAR_TRY(tr_residual_take(t, st, CAR_DROP_FFN, l, R, B, S));
         CAR_TRY(tr_wgrad(t, st, t->db, t->act, R, dim, F, g->w.w2 ? (float*)g->w.w2[l] : nullptr));
         CAR_TRY(tr_dgrad(t, st, t->db, t->b_w2[l], R, dim, F, nullptr, t->dact));
         CAR_LAUNCH(tr_swiglu_bwd_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, (const bf16*)t->dact, t->dg, t->du, (long long)R * F);
@@ -1243,8 +1296,8 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         CAR_TRY(tr_dgrad(t, st, t->dg, t->b_w1[l], R, F, dim, nullptr, t->dx));
         CAR_TRY(tr_dgrad(t, st, t->du, t->b_w3[l], R, F, dim, t->dx, t->dx));
         CAR_TRY(tr_norm_bwd(t, st, t->h, t->ffn_norm[l], t->dx, R, S, S, 0, g->w.ffn_norm ? (float*)g->w.ffn_norm[l] : nullptr));
-        // attention: h_mid = h0 + wo(sdpa(rope(wqkv x1)))
-        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)R * dim), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim);
+        // attention: h_mid = h0 + drop_path(resid_dropout(wo(sdpa(rope(wqkv x1)))))
+        CAR_TRY(tr_residual_take(t, st, CAR_DROP_RESID, l, R, B, S));
         CAR_TRY(tr_wgrad(t, st, t->db, t->att, R, dim, dim, g->w.wo ? (float*)g->w.wo[l] : nullptr));
         CAR_TRY(tr_dgrad(t, st, t->db, t->b_wo[l], R, dim, dim, nullptr, t->datt));
         CAR_LAUNCH(tr_attn_bwd_q_kernel, att_grid, TRA_WARPS * 32, smem_q, st, (const bf16*)t->q, (const bf16*)t->kc, (const bf16*)t->vc, mask,
@@ -1264,19 +1317,30 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
             first_ctl = false;
         }
     }
-    // ---- embeddings and the prefix / control front ends ----
+    // ---- embeddings and the prefix / control front ends; dh is the gradient of tok_dropout's output, its mask applies first ----
+    const TrDrop dtok = tr_drop(t->drop_fwd, CAR_DROP_TOKEN, 0);
+    const bool tok_on = tr_drop_on(dtok);
     if (g->w.tok_embeddings) {
         CAR_CUDA(cudaMemsetAsync((void*)g->w.tok_embeddings, 0, (size_t)V * dim * 4, st));
-        CAR_LAUNCH(tr_embed_grad_kernel, B * n, 256, 0, st, (const float*)t->dh, (const int*)t->f_idx, n, (const unsigned char*)nullptr, 0,
-                   (float*)g->w.tok_embeddings, B, n, S, T, dim);
+        if (tok_on)
+            CAR_LAUNCH(tr_embed_grad_drop_kernel, B * n, 256, 0, st, (const float*)t->dh, (const int*)t->f_idx, n, (const unsigned char*)nullptr, 0,
+                       (float*)g->w.tok_embeddings, B, n, S, T, dim, dtok);
+        else
+            CAR_LAUNCH(tr_embed_grad_kernel, B * n, 256, 0, st, (const float*)t->dh, (const int*)t->f_idx, n, (const unsigned char*)nullptr, 0,
+                       (float*)g->w.tok_embeddings, B, n, S, T, dim);
     }
     if (d.model_type == 1) {
-        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const float*)t->dh, t->dadd, B, T, S, 0, dim);
+        if (tok_on) CAR_LAUNCH(tr_take_rows_drop_kernel, gsz((long long)B * T * dim / 4), 256, 0, st, (const float*)t->dh, t->dadd, B, T, S, 0, dim, dtok);
+        else CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const float*)t->dh, t->dadd, B, T, S, 0, dim);
         CAR_TRY(tr_mlp_bwd(t, st, t->capx, B * T, d.caption_dim, t->b_cap1, t->b_cap2, t->dadd, nullptr, nullptr, (float*)g->w.cap_fc1, (float*)g->w.cap_fc2));
     } else if (g->w.label_table) {
         CAR_CUDA(cudaMemsetAsync((void*)g->w.label_table, 0, (size_t)(t->w.num_classes + 1) * dim * 4, st));
-        CAR_LAUNCH(tr_embed_grad_kernel, B, 256, 0, st, (const float*)t->dh, (const int*)t->f_cond, 1, t->f_drop, t->w.num_classes, (float*)g->w.label_table,
-                   B, 1, S, 0, dim);
+        if (tok_on)
+            CAR_LAUNCH(tr_embed_grad_drop_kernel, B, 256, 0, st, (const float*)t->dh, (const int*)t->f_cond, 1, t->f_drop, t->w.num_classes,
+                       (float*)g->w.label_table, B, 1, S, 0, dim, dtok);
+        else
+            CAR_LAUNCH(tr_embed_grad_kernel, B, 256, 0, st, (const float*)t->dh, (const int*)t->f_cond, 1, t->f_drop, t->w.num_classes, (float*)g->w.label_table,
+                       B, 1, S, 0, dim);
     }
     if (has_feat) {
         CAR_TRY(tr_mlp_bwd(t, st, t->cin, RC, dim, t->b_cond1, t->b_cond2, t->dctok, nullptr, t->dcin, (float*)g->w.cond_fc1, (float*)g->w.cond_fc2));
@@ -1284,6 +1348,44 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         CAR_TRY(tr_mlp_bwd(t, st, (const bf16*)t->f_feat, RC, t->w.adapter_dim, t->b_ad1, t->b_ad2, t->dcin, nullptr, (bf16*)d_feat,
                            (float*)g->adapter_fc1, (float*)g->adapter_fc2));
     }
+    return CAR_OK;
+}
+
+static bool tr_prob_ok(float p) { return p >= 0.f && p < 1.f; }           // (false for NaN)
+
+// dropout settings of the next car_train_forward; every check happens before the handle is touched
+extern "C" int car_train_set_dropout(CarTrain* t, const CarTrainDropout* cfg) {
+    if (!t) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    CarTrain::DropCfg c;
+    if (cfg) {
+        if (!tr_prob_ok(cfg->token_p) || !tr_prob_ok(cfg->resid_p) || !tr_prob_ok(cfg->ffn_p))
+            CAR_FAIL(CAR_ERR_ARG, "dropout probabilities must lie in [0, 1)");
+        if (cfg->n_layer < 0 || (cfg->drop_path == nullptr) != (cfg->n_layer == 0))
+            CAR_FAIL(CAR_ERR_ARG, "drop_path and n_layer go together");
+        bool any = cfg->token_p > 0.f || cfg->resid_p > 0.f || cfg->ffn_p > 0.f;
+        for (int l = 0; l < cfg->n_layer; ++l) {
+            if (!tr_prob_ok(cfg->drop_path[l])) CAR_FAIL(CAR_ERR_ARG, "drop-path rates must lie in [0, 1)");
+            any = any || cfg->drop_path[l] > 0.f;
+        }
+        if (any && cfg->seed == nullptr) CAR_FAIL(CAR_ERR_ARG, "dropout needs a device seed");
+        c.tok_p = cfg->token_p; c.resid_p = cfg->resid_p; c.ffn_p = cfg->ffn_p;
+        if (cfg->drop_path) c.path.assign(cfg->drop_path, cfg->drop_path + cfg->n_layer);
+        c.seed = any ? cfg->seed : nullptr;
+    }
+    if (!c.path.empty() && (int)c.path.size() != t->d.n_layer) CAR_FAIL(CAR_ERR_ARG, "drop_path needs one rate per layer");
+    t->drop_next = c;
+    return CAR_OK;
+}
+
+extern "C" int car_dropout_keep_mask(const uint64_t* seed_dev, int32_t site, int32_t layer, int32_t B, int32_t rows, int32_t cols, float p,
+                                     uint8_t* out, void* stream) {
+    if (!seed_dev || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (site < CAR_DROP_TOKEN || site > CAR_DROP_PATH_FFN) CAR_FAIL(CAR_ERR_ARG, "site must be 0 (token) .. 4 (drop path, feed-forward)");
+    if (layer < 0 || layer > 0xFFFF || B <= 0 || rows <= 0 || cols <= 0) CAR_FAIL(CAR_ERR_ARG, "bad layer or shape");
+    if (!tr_prob_ok(p)) CAR_FAIL(CAR_ERR_ARG, "p must lie in [0, 1)");
+    float keep = 1.f, scale;
+    tr_keep_scale(p, &keep, &scale);
+    CAR_LAUNCH(car_dropout_mask_kernel, gsz((long long)B * rows * cols), 256, 0, (cudaStream_t)stream, seed_dev, site, layer, B, rows, cols, keep, out);
     return CAR_OK;
 }
 

@@ -150,7 +150,8 @@ class ARTrainHandle(_lib.NativeHandle):
         self._keep = (keep, tw)
 
     @on_own_device
-    def forward(self, idx, cond, feat, drop_ids, mask, targets, valid):
+    def forward(self, idx, cond, feat, drop_ids, mask, targets, valid, dropout=None):
+        """dropout: None (every site off) or (token_p, resid_p, ffn_p, per-layer drop-path rates or None, int64 [1] device seed)."""
         B, n = idx.shape
         n_img = n + 1
         dev = idx.device
@@ -166,13 +167,28 @@ class ARTrainHandle(_lib.NativeHandle):
         vf = None if valid is None else valid.to(torch.float32).contiguous()
         logits = torch.empty(B, n_img, self.V, device=dev, dtype=torch.float32)
         loss = torch.empty(1, device=dev, dtype=torch.float32) if tg is not None else None
+        seed = self._set_dropout(dropout, dev)
         check(self.lib.car_train_forward(self.handle, B, n_img, _ptr(idx), _ptr(cond), None if feat is None else _ptr(feat), _ptr(drop),
                                          None if m8 is None else _ptr(m8), None if tg is None else _ptr(tg),
                                          None if vf is None else _ptr(vf), _ptr(logits), None if loss is None else _ptr(loss), cur_stream()),
               "car_train_forward")
-        self._last = (idx, cond, feat, drop, m8, tg, vf)      # car_train_backward reads them again
+        self._last = (idx, cond, feat, drop, m8, tg, vf, seed)      # car_train_backward reads them again
         self.generation += 1
         return logits, (None if loss is None else loss[0])
+
+    def _set_dropout(self, dropout, dev):
+        """car_train_set_dropout for the next forward; returns the device seed the forward and its backward read (kept alive)."""
+        cfg = None
+        seed = None
+        if dropout is not None:
+            tok, resid, ffn, rates, seed = dropout
+            seed = seed.to(device=dev, dtype=torch.int64).reshape(1).contiguous()
+            cfg = _lib.CarTrainDropout(float(tok), float(resid), float(ffn), 0, None, _ptr(seed))
+            if rates is not None:
+                arr = (C.c_float * len(rates))(*rates)
+                cfg.n_layer, cfg.drop_path = len(rates), C.cast(arr, C.c_void_p)
+        check(self.lib.car_train_set_dropout(self.handle, None if cfg is None else C.byref(cfg)), "car_train_set_dropout")
+        return seed
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     @staticmethod
@@ -204,7 +220,7 @@ class ARTrainHandle(_lib.NativeHandle):
         loss_grad: 0-dim / [1] fp32 CUDA tensor (d / d loss) or None = 1."""
         if getattr(self, "_last", None) is None:
             raise RuntimeError("controlar_b200: backward() needs a preceding training forward with targets")
-        idx, cond, feat, drop, m8, tg, vf = self._last
+        idx, cond, feat, drop, m8, tg, vf, _seed = self._last
         if tg is None:
             raise RuntimeError("controlar_b200: the last training forward had no targets / loss")
         names = self.grad_params(module)

@@ -236,8 +236,11 @@ int car_vq_destroy(CarVQ* m);
 /* =====================================================================================================
  * Training forward (SURVEY.md row f1): Transformer.forward(idx, cond_idx, targets, mask, valid, condition) with the module
  * in train mode (autoregressive/models/gpt_t2i.py:420-431,451-484) as the train scripts run it — fp32 parameters under bf16
- * autocast (autoregressive/train/train_t2i_canny.py:166-167, train_c2i_canny.py:200-201).  Dropout layers at p = 0; the CFG
- * drop decision (gpt_t2i.py:83,116,148: torch.rand(B) < class_dropout_prob) is drawn by the caller and passed in.
+ * autocast (autoregressive/train/train_t2i_canny.py:166-167, train_c2i_canny.py:200-201).  The CFG drop decision
+ * (gpt_t2i.py:83,116,148: torch.rand(B) < class_dropout_prob) is drawn by the caller and passed in.  Token, residual and
+ * feed-forward dropout and stochastic depth (drop path) run inside the forward and backward kernels when car_train_set_dropout
+ * turns them on; their keep decisions come from a counter-based generator keyed by a device seed (car_dropout_keep_mask), so the
+ * backward regenerates the forward's masks instead of storing them.  Attention-probability dropout is not supported.
  * car_train_backward gives the gradients of every parameter on this path and of the control tokens.
  * ===================================================================================================== */
 typedef struct CarTrain CarTrain;
@@ -273,6 +276,30 @@ int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const int32_t* idx,
  * itself pinned to gradients the reference produced).  Needs dim, ffn_dim, vocab_size multiples of 64. */
 int car_train_backward(CarTrain* t, const CarTrainWeights* grads, void* d_feat, const float* loss_grad, void* stream);
 int car_train_destroy(CarTrain* t);
+/* Dropout of the training path, applied the way nn.Dropout / DropPath apply it on CUDA under bf16 autocast:
+ *   token_p  tok_dropout on the fp32 stream rows (prefix rows and image tokens) before the first control add (gpt_t2i.py:430);
+ *   resid_p  resid_dropout on wo's bf16 output (gpt_t2i.py:290);  ffn_p  ffn_dropout on w2's bf16 output (gpt_t2i.py:217);
+ *            a kept element becomes x * fp32(1 / keep) rounded once to the tensor's dtype, a dropped one 0 (keep = 1 - p);
+ *   drop_path  per-layer DropPath rates (host fp32 [n_layer], the reference's torch.linspace(0, rate, n_layer) values) or NULL:
+ *            after the branch's dropout, the bf16 branch is multiplied by bf16(bernoulli(keep) / keep), one draw per sample and
+ *            branch (gpt_t2i.py:305-306, utils/drop_path.py);
+ *   seed     DEVICE uint64 [1], read by the kernels (no host synchronisation); required when any site is on.
+ * Every p and rate must lie in [0, 1); 0 turns a site off and the path is then bit for bit the dropout-free one.  The settings
+ * (copied, except the seed, which is borrowed) apply from the next car_train_forward on; car_train_backward uses the settings and
+ * seed of the forward it differentiates, so the seed must stay unchanged until then.  cfg NULL turns every site off. */
+typedef struct CarTrainDropout {
+    float           token_p, resid_p, ffn_p;
+    int32_t         n_layer;        /* entries of drop_path (the model's n_layer), 0 when drop_path is NULL */
+    const float*    drop_path;
+    const uint64_t* seed;
+} CarTrainDropout;
+int car_train_set_dropout(CarTrain* t, const CarTrainDropout* cfg);
+/* Conformance entry point for the dropout generator: out uint8 [B, rows, cols] = 1 where the training kernels keep element
+ * (row, col) of sample b at `site` (0 token, 1 resid, 2 ffn, 3 drop path of the attention branch, 4 drop path of the feed-forward
+ * branch) of `layer` (0 for the token site) with drop probability p.  The drop-path sites decide per sample: every (row, col) of a
+ * sample holds that sample's decision.  Same device function as the training kernels; oracle/dropout_masks.py restates it. */
+int car_dropout_keep_mask(const uint64_t* seed_dev, int32_t site, int32_t layer, int32_t B, int32_t rows, int32_t cols, float p,
+                          uint8_t* out, void* stream);
 
 /* ---- antialiased bilinear resize in front of the online VQ encode of the multi-resolution training scripts (SURVEY.md row f2):
  * F.interpolate(x.float(), size=(OH, OW), mode='bilinear', align_corners=False, antialias=True),

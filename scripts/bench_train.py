@@ -27,6 +27,9 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--no-backward", action="store_true", help="forward + loss only (what config 5 names)")
+    ap.add_argument("--dropout-p", type=float, default=0.0, help="resid / ffn dropout (the train scripts' --dropout-p)")
+    ap.add_argument("--token-dropout-p", type=float, default=0.0, help="token dropout (the train scripts' --token-dropout-p)")
+    ap.add_argument("--drop-path-rate", type=float, default=0.0, help="stochastic depth (the c2i scripts' --drop-path-rate)")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device (no CPU fallback)"
     from controlar_b200.autoregressive.models.gpt_t2i import GPT_models
@@ -36,8 +39,9 @@ def main():
     n = (args.image_size // 16) ** 2
     torch.manual_seed(0)
     model = GPT_models[args.model](vocab_size=16384, block_size=n, num_classes=1000, cls_token_num=1, model_type="c2i",
-                                   condition_type="canny", adapter_size="small", token_dropout_p=0.0, resid_dropout_p=0.0,
-                                   ffn_dropout_p=0.0).to(dev).train()
+                                   condition_type="canny", adapter_size="small", token_dropout_p=args.token_dropout_p,
+                                   resid_dropout_p=args.dropout_p, ffn_dropout_p=args.dropout_p,
+                                   drop_path_rate=args.drop_path_rate).to(dev).train()
     torch.nn.init.normal_(model.output.weight, std=0.02)         # the reference zero-inits it; zeros would make a degenerate step
     trained = {id(p) for _, p in ARTrainHandle.grad_params(model)}
     for p in model.parameters():                                  # the control encoder stays frozen under this library
