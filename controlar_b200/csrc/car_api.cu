@@ -1130,7 +1130,7 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     CAR_TRY(dense_linear(st, t->x, dim, t->b_wqkv[l], R, 3 * dim, dim, ACT_NONE, nullptr, 0, t->qkv, 3 * dim));
     CAR_LAUNCH(rope_kv_write_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->qkv, t->rope, t->q, t->kc, t->vc, R, S, dim, H, S);
     CAR_LAUNCH(tr_attention_kernel, (unsigned)(((long long)B * H * S + TRA_WARPS - 1) / TRA_WARPS), TRA_WARPS * 32, att_smem, st, (const bf16*)t->q,
-               (const bf16*)t->kc, (const bf16*)t->vc, mask, B, H, S, t->att);
+               (const bf16*)t->kc, (const bf16*)t->vc, mask, B, H, S, t->att, 1);
     CAR_TRY(dense_linear(st, t->att, dim, t->b_wo[l], R, dim, dim, ACT_NONE, nullptr, 0, t->o, dim));
     CAR_TRY(tr_residual_add(t, st, CAR_DROP_RESID, l, R, B, S));
     bf16* xn = for_bwd ? t->x2 : t->x;
@@ -1301,9 +1301,9 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         CAR_TRY(tr_wgrad(t, st, t->db, t->att, R, dim, dim, g->w.wo ? (float*)g->w.wo[l] : nullptr));
         CAR_TRY(tr_dgrad(t, st, t->db, t->b_wo[l], R, dim, dim, nullptr, t->datt));
         CAR_LAUNCH(tr_attn_bwd_q_kernel, att_grid, TRA_WARPS * 32, smem_q, st, (const bf16*)t->q, (const bf16*)t->kc, (const bf16*)t->vc, mask,
-                   (const bf16*)t->datt, B, H, S, t->lse, t->dsum, t->dq);
+                   (const bf16*)t->datt, B, H, S, t->lse, t->dsum, t->dq, 1);
         CAR_LAUNCH(tr_attn_bwd_kv_kernel, att_grid, TRA_WARPS * 32, smem_kv, st, (const bf16*)t->q, (const bf16*)t->kc, (const bf16*)t->vc, mask,
-                   (const bf16*)t->datt, (const float*)t->lse, (const float*)t->dsum, B, H, S, t->dk, t->dv);
+                   (const bf16*)t->datt, (const float*)t->lse, (const float*)t->dsum, B, H, S, t->dk, t->dv, 1);
         CAR_LAUNCH(tr_rope_bwd_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->dq, (const bf16*)t->dk, (const bf16*)t->dv, t->rope, t->dqkv, R, S, dim, H, S);
         CAR_TRY(tr_wgrad(t, st, t->dqkv, t->x, R, 3 * dim, dim, g->w.wqkv ? (float*)g->w.wqkv[l] : nullptr));
         CAR_TRY(tr_dgrad(t, st, t->dqkv, t->b_wqkv[l], R, 3 * dim, dim, nullptr, t->dx));

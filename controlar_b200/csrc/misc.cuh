@@ -88,7 +88,7 @@ __global__ void set_int_kernel(int* p, int v) { *p = v; }
 
 // ---- prefill helpers of the dense (M = B_eff * T rows) path ------------------------------------------------
 // qkv [rows][3d] (bf16 GEMM output) -> q [rows][d] with RoPE, K/V cache rows (RoPE on K) — gpt_t2i.py:264-271,227-235.
-// row = b * Tq + t, sequence position = t.
+// row = b * Tq + t, sequence position = t.  rope null: no rotation (the plain head split of the control encoder).
 __global__ void rope_kv_write_kernel(const bf16* __restrict__ qkv, const float* __restrict__ rope, bf16* __restrict__ q,
                                      bf16* __restrict__ kc, bf16* __restrict__ vc, int rows, int Tq, int d, int H, int S) {
     const long long total = (long long)rows * (3 * d / 2);
@@ -98,7 +98,7 @@ __global__ void rope_kv_write_kernel(const bf16* __restrict__ qkv, const float* 
         const int sec = n / d, w = n - sec * d, head = w >> 6, e = w & 63;
         const int b = r / Tq, t = r - b * Tq;
         float v0 = tof(qkv[(size_t)r * 3 * d + n]), v1 = tof(qkv[(size_t)r * 3 * d + n + 1]);
-        if (sec < 2) {
+        if (sec < 2 && rope) {
             const float2 cs2 = *reinterpret_cast<const float2*>(rope + ((size_t)t * 32 + (e >> 1)) * 2);
             const float x0 = v0 * cs2.x - v1 * cs2.y, x1 = v1 * cs2.x + v0 * cs2.y;
             v0 = x0; v1 = x1;

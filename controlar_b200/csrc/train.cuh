@@ -90,12 +90,13 @@ __global__ void tr_rmsnorm_kernel(const float* __restrict__ x, const float* __re
 
 // F.scaled_dot_product_attention over full sequences (gpt_t2i.py:282-286), math semantics: fp32 scores, fp32 soft-max over
 // the allowed keys, fp32 probability-weighted sum, one rounding to bf16.  One warp per (b, h, query i); the row of scores
-// lives in shared memory (S floats per warp).  mask: uint8 [B][S][S] (1 = attend) or null = causal.
+// lives in shared memory (S floats per warp).  mask: uint8 [B][S][S] (1 = attend); without one, causal != 0 attends keys 0 .. i and
+// causal == 0 every key (the bidirectional attention of the control encoder, Dinov2SelfAttention).
 // q [B*S][H*64] (RoPE applied), k / v [B][H][S][64] bf16 (RoPE applied to k), out [B*S][H*64].
 constexpr int TRA_WARPS = 4;
 __global__ void __launch_bounds__(TRA_WARPS * 32)
 tr_attention_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kc, const bf16* __restrict__ vc, const unsigned char* __restrict__ mask,
-                    int B, int H, int S, bf16* __restrict__ out) {
+                    int B, int H, int S, bf16* __restrict__ out, int causal) {
     extern __shared__ float tra_sc[];                         // [TRA_WARPS][S]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long item = (long long)blockIdx.x * TRA_WARPS + warp;
@@ -108,7 +109,7 @@ tr_attention_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kc, con
     const bf16* kb = kc + (((size_t)b * H + hd) * S) * 64;
     const bf16* vb = vc + (((size_t)b * H + hd) * S) * 64;
     const unsigned char* mrow = mask ? mask + ((size_t)b * S + i) * S : nullptr;
-    const int s_end = mask ? S : i + 1;                       // causal: keys 0 .. i
+    const int s_end = (mask || !causal) ? S : i + 1;          // causal: keys 0 .. i
     float qf[64];
 #pragma unroll
     for (int e = 0; e < 64; e += 2) unpack_bf16x2(*reinterpret_cast<const uint32_t*>(qp + e), qf[e], qf[e + 1]);

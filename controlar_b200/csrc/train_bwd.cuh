@@ -122,16 +122,17 @@ __global__ void tr_rmsnorm_bwd_kernel(const float* __restrict__ x, const float* 
     }
 }
 
-// column sums of src [rows][K] in two deterministic passes: part[c][k] = sum of the rows of chunk c (fixed order), then
-// dst[k] = sum_c part[c][k].  block (32, 8); grid (ceil(K/32), TR_COLSUM_CHUNKS).
+// column sums of src [rows][K] (fp32 or bf16, summed in fp32) in two deterministic passes: part[c][k] = sum of the rows of chunk c
+// (fixed order), then dst[k] = sum_c part[c][k].  block (32, 8); grid (ceil(K/32), TR_COLSUM_CHUNKS).
 constexpr int TR_COLSUM_CHUNKS = 32;
-__global__ void tr_colsum_part_kernel(const float* __restrict__ src, float* __restrict__ part, int rows, int K) {
+template <typename T>
+__global__ void tr_colsum_part_kernel(const T* __restrict__ src, float* __restrict__ part, int rows, int K) {
     __shared__ float red[8][32];
     const int k = blockIdx.x * 32 + threadIdx.x;
     const int per = (rows + TR_COLSUM_CHUNKS - 1) / TR_COLSUM_CHUNKS;
     const int lo = blockIdx.y * per, hi = min(rows, lo + per);
     float a = 0.f;
-    if (k < K) for (int r = lo + threadIdx.y; r < hi; r += 8) a += src[(size_t)r * K + k];
+    if (k < K) for (int r = lo + threadIdx.y; r < hi; r += 8) a += tof(src[(size_t)r * K + k]);
     red[threadIdx.y][threadIdx.x] = a;
     __syncthreads();
     if (threadIdx.y == 0 && k < K) {
@@ -180,10 +181,11 @@ __global__ void tr_gelu_bwd_kernel(const bf16* __restrict__ t, const bf16* __res
 // ---- scaled-dot-product attention backward (forward: tr_attention_kernel, gpt_t2i.py:282-286) ---------------------------------
 // P = softmax(Q K^T / 8 + mask), O = P V.  dV = P^T dO, dP = dO V^T, dS = P o (dP - rowsum(dP o P)), dQ = dS K / 8, dK = dS^T Q / 8.
 // Pass 1, one warp per (b, h, query i): recomputes the row of P, writes lse = max + log(sum), D = rowsum(dP o P) and dQ.
-// q / dout / dq: [B*S][H*64]; k / v: [B][H][S][64].  Shared memory: TRA_WARPS * (2 S + 128) floats.
+// q / dout / dq: [B*S][H*64]; k / v: [B][H][S][64]; mask / causal as in tr_attention_kernel.  Shared memory: TRA_WARPS * (2 S + 128) floats.
 __global__ void __launch_bounds__(TRA_WARPS * 32)
 tr_attn_bwd_q_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kc, const bf16* __restrict__ vc, const unsigned char* __restrict__ mask,
-                     const bf16* __restrict__ dout, int B, int H, int S, float* __restrict__ lse, float* __restrict__ dsum, bf16* __restrict__ dq) {
+                     const bf16* __restrict__ dout, int B, int H, int S, float* __restrict__ lse, float* __restrict__ dsum, bf16* __restrict__ dq,
+                     int causal) {
     extern __shared__ float trb_sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long item = (long long)blockIdx.x * TRA_WARPS + warp;
@@ -202,7 +204,7 @@ tr_attn_bwd_q_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kc, co
     unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dout + qoff + 2 * lane), gs[2 * lane], gs[2 * lane + 1]);
     __syncwarp();
     const unsigned char* mrow = mask ? mask + ((size_t)b * S + i) * S : nullptr;
-    const int s_end = mask ? S : i + 1;
+    const int s_end = (mask || !causal) ? S : i + 1;
     float mx = -INFINITY;
     for (int s = lane; s < s_end; s += 32) {
         float v = -INFINITY;
@@ -273,7 +275,7 @@ tr_attn_bwd_q_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kc, co
 __global__ void __launch_bounds__(TRA_WARPS * 32)
 tr_attn_bwd_kv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kc, const bf16* __restrict__ vc, const unsigned char* __restrict__ mask,
                       const bf16* __restrict__ dout, const float* __restrict__ lse, const float* __restrict__ dsum, int B, int H, int S,
-                      bf16* __restrict__ dk, bf16* __restrict__ dv) {
+                      bf16* __restrict__ dk, bf16* __restrict__ dv, int causal) {
     extern __shared__ float trb_sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long item = (long long)blockIdx.x * TRA_WARPS + warp;
@@ -289,7 +291,7 @@ tr_attn_bwd_kv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kc, c
     unpack_bf16x2(*reinterpret_cast<const uint32_t*>(kc + kvoff + 2 * lane), ks[2 * lane], ks[2 * lane + 1]);
     unpack_bf16x2(*reinterpret_cast<const uint32_t*>(vc + kvoff + 2 * lane), vs[2 * lane], vs[2 * lane + 1]);
     __syncwarp();
-    const int i_begin = mask ? 0 : s;                         // causal: queries i >= s
+    const int i_begin = (mask || !causal) ? 0 : s;            // causal: queries i >= s
     const float* lrow = lse + ((size_t)b * H + hd) * S;
     const float* drow = dsum + ((size_t)b * H + hd) * S;
     for (int i = i_begin + lane; i < S; i += 32) {
@@ -336,7 +338,8 @@ tr_attn_bwd_kv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kc, c
 }
 
 // backward of rope_kv_write_kernel (apply_rotary_emb gpt_t2i.py:522-532 + the head split): dq [rows][d], dk / dv [B][H][S][64]
-// -> dqkv [rows][3d]; the rotation of a pair by (cos, sin) is undone on the gradient by the transposed rotation.
+// -> dqkv [rows][3d]; the rotation of a pair by (cos, sin) is undone on the gradient by the transposed rotation (no rotation when
+// rope is null: the plain head merge of the control encoder).
 __global__ void tr_rope_bwd_kernel(const bf16* __restrict__ dq, const bf16* __restrict__ dk, const bf16* __restrict__ dv, const float* __restrict__ rope,
                                    bf16* __restrict__ dqkv, int rows, int Tq, int d, int H, int S) {
     const long long total = (long long)rows * (3 * d / 2);
@@ -347,7 +350,7 @@ __global__ void tr_rope_bwd_kernel(const bf16* __restrict__ dq, const bf16* __re
         const int b = r / Tq, t = r - b * Tq;
         const bf16* src = sec == 0 ? dq + (size_t)r * d + w : (sec == 1 ? dk : dv) + (((size_t)b * H + head) * S + t) * 64 + e;
         float g0 = tof(src[0]), g1 = tof(src[1]);
-        if (sec < 2) {
+        if (sec < 2 && rope) {
             const float2 cs2 = *reinterpret_cast<const float2*>(rope + ((size_t)t * 32 + (e >> 1)) * 2);
             const float x0 = g0 * cs2.x + g1 * cs2.y, x1 = g1 * cs2.x - g0 * cs2.y;
             g0 = x0; g1 = x1;

@@ -523,9 +523,9 @@ __global__ void resize_patchify_kernel(const TI* __restrict__ img, bf16* __restr
 }
 
 // position embeddings: bicubic (align_corners=False, A=-0.75, fp32) resize of the [G,G,C] grid to [h,w,C], cast to
-// the model dtype (modeling_dinov2.py interpolate_pos_encoding); pos: [1 + G*G, C]
-template <typename TI>
-__global__ void pos_embed_interp_kernel(const TI* __restrict__ pos, bf16* __restrict__ out /*[h*w][C]*/, int G, int h, int w, int C) {
+// the model dtype (modeling_dinov2.py interpolate_pos_encoding); pos: [1 + G*G, C].  TO = float: the fp32 table of training.
+template <typename TI, typename TO = bf16>
+__global__ void pos_embed_interp_kernel(const TI* __restrict__ pos, TO* __restrict__ out /*[h*w][C]*/, int G, int h, int w, int C) {
     const long long total = (long long)h * w * C;
     const float sy = (float)G / h, sx = (float)G / w;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -548,7 +548,7 @@ __global__ void pos_embed_interp_kernel(const TI* __restrict__ pos, bf16* __rest
             }
             acc += rowv * wy[a];
         }
-        out[i] = fromf<bf16>(acc);
+        out[i] = fromf<TO>(acc);
     }
 }
 

@@ -35,6 +35,10 @@ _PROTOS = {
     "car_dino_create": (C.c_int, [C.POINTER(CarDinoDesc), C.POINTER(CarDinoWeights), C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_dino_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
     "car_dino_destroy": (C.c_int, [C.c_void_p]),
+    "car_dino_train_create": (C.c_int, [C.POINTER(CarDinoDesc), C.POINTER(CarDinoWeights), C.c_void_p, C.POINTER(C.c_void_p)]),
+    "car_dino_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "car_dino_train_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(CarDinoWeights), C.c_void_p]),
+    "car_dino_train_destroy": (C.c_int, [C.c_void_p]),
     "car_vq_create": (C.c_int, [C.POINTER(CarVQDesc), C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_vq_decode_code": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_vq_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
@@ -51,6 +55,33 @@ _lib.PROTOTYPES.update(_PROTOS)
 # ---------------------------------------------------------------------------------------------------------------
 def _dev_of(module):
     return next(module.parameters()).device
+
+
+def _block_tensors(b, is_vit: bool):
+    """One encoder block's tensors by CarDinoWeights array name: HF ViTModel key names (vit_adapter.py) or Dinov2Model's.  ViT has
+    no LayerScale: ls1 / ls2 are None."""
+    att = b.attention
+    t = {"q_w": att.attention.query.weight, "q_b": att.attention.query.bias, "k_w": att.attention.key.weight,
+         "k_b": att.attention.key.bias, "v_w": att.attention.value.weight, "v_b": att.attention.value.bias,
+         "o_w": att.output.dense.weight, "o_b": att.output.dense.bias}
+    if is_vit:
+        t.update(n1_w=b.layernorm_before.weight, n1_b=b.layernorm_before.bias, n2_w=b.layernorm_after.weight, n2_b=b.layernorm_after.bias,
+                 fc1_w=b.intermediate.dense.weight, fc1_b=b.intermediate.dense.bias, fc2_w=b.output.dense.weight,
+                 fc2_b=b.output.dense.bias, ls1=None, ls2=None)
+    else:
+        t.update(n1_w=b.norm1.weight, n1_b=b.norm1.bias, n2_w=b.norm2.weight, n2_b=b.norm2.bias, fc1_w=b.mlp.fc1.weight,
+                 fc1_b=b.mlp.fc1.bias, fc2_w=b.mlp.fc2.weight, fc2_b=b.mlp.fc2.bias, ls1=b.layer_scale1.lambda1,
+                 ls2=b.layer_scale2.lambda1)
+    return t
+
+
+def _is_vit(m) -> bool:
+    return hasattr(m.encoder.layer[0], "layernorm_before")      # HF ViTModel key names (vit_adapter.py) vs Dinov2Model
+
+
+def _resize_mode(adapter, is_vit: bool) -> int:
+    # dinov2_adapter.py:20-24: nearest for canny / seg, bicubic otherwise; ViT_Adapter does not resize (nearest at P = 16 is the identity)
+    return 0 if (is_vit or adapter.condition_type in ("canny", "seg")) else 1
 
 
 class DinoHandle(_lib.ModuleHandle):
@@ -86,33 +117,14 @@ class DinoHandle(_lib.ModuleHandle):
         w.patch_w, w.patch_b = P(e.patch_embeddings.projection.weight), P(e.patch_embeddings.projection.bias)
         w.ln_w, w.ln_b = P(m.layernorm.weight), P(m.layernorm.bias)
         layers = list(m.encoder.layer)
-        is_vit = hasattr(layers[0], "layernorm_before")      # HF ViTModel key names (vit_adapter.py) vs Dinov2Model
+        is_vit = _is_vit(m)
+        ones = None
         if is_vit:
             ones = torch.ones(m.hidden, dtype=dt, device=m.layernorm.weight.device)     # no LayerScale in ViT: x 1 is exact
             keep.append(ones)
-            get = {
-                "n1_w": lambda b: b.layernorm_before.weight, "n1_b": lambda b: b.layernorm_before.bias,
-                "q_w": lambda b: b.attention.attention.query.weight, "q_b": lambda b: b.attention.attention.query.bias,
-                "k_w": lambda b: b.attention.attention.key.weight, "k_b": lambda b: b.attention.attention.key.bias,
-                "v_w": lambda b: b.attention.attention.value.weight, "v_b": lambda b: b.attention.attention.value.bias,
-                "o_w": lambda b: b.attention.output.dense.weight, "o_b": lambda b: b.attention.output.dense.bias,
-                "ls1": lambda b: ones, "n2_w": lambda b: b.layernorm_after.weight, "n2_b": lambda b: b.layernorm_after.bias,
-                "fc1_w": lambda b: b.intermediate.dense.weight, "fc1_b": lambda b: b.intermediate.dense.bias,
-                "fc2_w": lambda b: b.output.dense.weight, "fc2_b": lambda b: b.output.dense.bias, "ls2": lambda b: ones,
-            }
-        else:
-          get = {
-            "n1_w": lambda b: b.norm1.weight, "n1_b": lambda b: b.norm1.bias,
-            "q_w": lambda b: b.attention.attention.query.weight, "q_b": lambda b: b.attention.attention.query.bias,
-            "k_w": lambda b: b.attention.attention.key.weight, "k_b": lambda b: b.attention.attention.key.bias,
-            "v_w": lambda b: b.attention.attention.value.weight, "v_b": lambda b: b.attention.attention.value.bias,
-            "o_w": lambda b: b.attention.output.dense.weight, "o_b": lambda b: b.attention.output.dense.bias,
-            "ls1": lambda b: b.layer_scale1.lambda1, "n2_w": lambda b: b.norm2.weight, "n2_b": lambda b: b.norm2.bias,
-            "fc1_w": lambda b: b.mlp.fc1.weight, "fc1_b": lambda b: b.mlp.fc1.bias,
-            "fc2_w": lambda b: b.mlp.fc2.weight, "fc2_b": lambda b: b.mlp.fc2.bias, "ls2": lambda b: b.layer_scale2.lambda1,
-          }
         for name in _DINO_ARRAYS:
-            ts = [get[name](b).detach().contiguous() for b in layers]
+            ts = [_block_tensors(b, is_vit)[name] for b in layers]
+            ts = [(ones if t is None else t).detach().contiguous() for t in ts]
             arr = _ptr_array(ts)
             keep.extend(ts)
             keep.append(arr)
@@ -121,8 +133,7 @@ class DinoHandle(_lib.ModuleHandle):
         if self.adapter_mlp is not None:
             w.adapter_fc1, w.adapter_fc2 = P(self.adapter_mlp.fc1.weight), P(self.adapter_mlp.fc2.weight)
             out_dim = self.adapter_mlp.fc2.weight.shape[0]
-        # dinov2_adapter.py:20-24: nearest for canny / seg, bicubic otherwise; ViT_Adapter does not resize (nearest at P = 16 is the identity)
-        mode = 0 if (is_vit or self.adapter.condition_type in ("canny", "seg")) else 1
+        mode = _resize_mode(self.adapter, is_vit)
         d = CarDinoDesc(dtype=dtype_code(dt), hidden=m.hidden, heads=m.heads, layers=m.n_layers, patch=m.patch,
                         pos_grid=m.pos_grid, resize_mode=mode, adapter_out_dim=out_dim, eps=m.eps)
         self.close()
@@ -145,8 +156,123 @@ class DinoHandle(_lib.ModuleHandle):
         return out.to(self.dtype)
 
 
+_TOP = [("cls_token", "embeddings.cls_token"), ("pos_emb", "embeddings.position_embeddings"),
+        ("patch_w", "embeddings.patch_embeddings.projection.weight"), ("patch_b", "embeddings.patch_embeddings.projection.bias"),
+        ("ln_w", "layernorm.weight"), ("ln_b", "layernorm.bias")]
+
+
+def encoder_train_params(m):
+    """The backbone parameters on the path of Dinov2_Adapter.forward / ViT_Adapter.forward, as (CarDinoWeights field, layer or None,
+    parameter).  embeddings.mask_token and ViT's pooler.dense.* are not on it (the reference gives them no gradient)."""
+    names = dict(m.named_parameters())
+    out = [(f, None, names[k]) for f, k in _TOP]
+    is_vit = _is_vit(m)
+    for i, b in enumerate(m.encoder.layer):
+        out += [(f, i, t) for f, t in _block_tensors(b, is_vit).items() if t is not None]
+    return out
+
+
+class DinoTrainHandle(_lib.NativeHandle):
+    """CarDinoTrain: the control encoder's forward with fp32 parameters under bf16-autocast numerics, and its backward.  The fp32
+    parameters are borrowed (re-cast to bf16 inside every forward), so an optimizer step needs no rebuild; replacing a parameter
+    tensor (new storage) does, and `key` tells."""
+
+    def __init__(self, adapter):
+        super().__init__("car_dino_train_destroy")
+        self.lib = _lib.lib()
+        m = adapter.model
+        self.params = encoder_train_params(m)
+        self.is_vit = _is_vit(m)
+        self.key = self.key_of(adapter)
+        self.device = m.layernorm.weight.device
+        self.hidden, self.layers = m.hidden, m.n_layers
+        self.generation = 0          # a backward belongs to the forward that produced its feat
+        self._create(adapter)
+
+    @staticmethod
+    def key_of(adapter):
+        return tuple(p.data_ptr() for _, _, p in encoder_train_params(adapter.model))
+
+    def _weights(self, tensors):
+        """CarDinoWeights over `tensors` (parallel to self.params; None = NULL) and the pointer arrays it needs kept alive"""
+        w, keep = CarDinoWeights(), []
+        per = {}
+        for (f, i, _), t in zip(self.params, tensors):
+            if i is None:
+                setattr(w, f, _ptr(t))
+            else:
+                per.setdefault(f, [None] * self.layers)[i] = t
+        for f, ts in per.items():
+            arr = (C.c_void_p * self.layers)(*[None if t is None else _ptr(t) for t in ts])
+            keep.append(arr)
+            setattr(w, f, C.cast(arr, C.POINTER(C.c_void_p)))
+        return w, keep
+
+    @on_own_device
+    def _create(self, adapter):
+        m = adapter.model
+        w, keep = self._weights([p.detach() for _, _, p in self.params])
+        d = CarDinoDesc(dtype=_lib.CAR_F32, hidden=m.hidden, heads=m.heads, layers=m.n_layers, patch=m.patch, pos_grid=m.pos_grid,
+                        resize_mode=_resize_mode(adapter, self.is_vit), adapter_out_dim=0, eps=m.eps)
+        check(self.lib.car_dino_train_create(C.byref(d), C.byref(w), cur_stream(), C.byref(self.handle)), "car_dino_train_create")
+
+    @on_own_device
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        B, _, H, W = x.shape
+        x = x.to(torch.float32).contiguous()
+        feat = torch.empty((B, (H // 16) * (W // 16), self.hidden), dtype=torch.float32, device=x.device)
+        check(self.lib.car_dino_train_forward(self.handle, _ptr(x), B, H, W, _ptr(feat), cur_stream()), "car_dino_train_forward")
+        self._keep = x
+        self.generation += 1
+        return feat
+
+    @on_own_device
+    def backward(self, dfeat: torch.Tensor, want):
+        """fp32 gradients of the last forward for the parameters flagged in `want` (parallel to self.params; None elsewhere)"""
+        grads = [torch.empty_like(p, dtype=torch.float32) if wnt else None for (_, _, p), wnt in zip(self.params, want)]
+        g, keep = self._weights(grads)
+        dfeat = dfeat.to(torch.float32).contiguous()
+        check(self.lib.car_dino_train_backward(self.handle, _ptr(dfeat), C.byref(g), cur_stream()), "car_dino_train_backward")
+        return grads
+
+
+class _EncoderStep(torch.autograd.Function):
+    """feat = car_dino_train_forward(x); backward = car_dino_train_backward.  The input map is data: it gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, handle, x, *params):
+        feat = handle.forward(x)
+        ctx.handle, ctx.generation = handle, handle.generation
+        return feat
+
+    @staticmethod
+    def backward(ctx, dfeat):
+        if ctx.handle.generation != ctx.generation:
+            raise RuntimeError("controlar_b200: the control encoder ran another trainable forward since this output was computed; its "
+                               "backward recomputes from the LAST forward (call backward before the next forward)")
+        want = [ctx.needs_input_grad[2 + i] for i in range(len(ctx.handle.params))]
+        return (None, None, *ctx.handle.backward(dfeat, want))
+
+
+def _trains(adapter) -> bool:
+    """The trainable path runs when autograd records and the backbone is an fp32 module with a parameter that wants a gradient;
+    every other call (generate(), eval, no_grad, a frozen or bf16 encoder) runs the inference encoder."""
+    if not torch.is_grad_enabled():
+        return False
+    ps = [p for _, _, p in encoder_train_params(adapter.model)]
+    return all(p.dtype == torch.float32 for p in ps) and any(p.requires_grad for p in ps)
+
+
 def dinov2_forward(adapter, x: torch.Tensor) -> torch.Tensor:
     """Dinov2_Adapter.forward: [B,3,H,W] -> [B,(H/16)(W/16),C] (reference dinov2_adapter.py:26-29)."""
+    if _trains(adapter):
+        h = getattr(adapter, "_car_dino_train", None)
+        if h is None or h.key != DinoTrainHandle.key_of(adapter):
+            if h is not None:
+                h.close()
+            h = DinoTrainHandle(adapter)
+            object.__setattr__(adapter, "_car_dino_train", h)
+        return _EncoderStep.apply(h, x, *[p for _, _, p in h.params])
     h = getattr(adapter, "_car_dino", None)
     if h is None:
         h = DinoHandle(adapter)

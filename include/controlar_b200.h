@@ -214,6 +214,19 @@ int car_dino_forward(CarDino* m, const void* image, int32_t B, int32_t H, int32_
                      void* stream);
 int car_dino_destroy(CarDino* m);
 
+/* Trainable control encoder: the same module (Dinov2_Adapter.forward / ViT_Adapter.forward) with fp32 parameters under the train
+ * loop's bf16 autocast (fp32 residual stream, LayerNorm, LayerScale and position embeddings; bf16 patch projection, nn.Linear,
+ * attention and GELU), and its backward.  `w` holds the fp32 master weights (desc->dtype = CAR_F32), BORROWED: they must stay
+ * valid and in place for the handle's life; every forward re-casts them.  ls1 / ls2 NULL: no LayerScale (ViT); adapter_fc* are
+ * not read.  Forward: image fp32 [B,3,H,W] -> feat fp32 [B, (H/16)(W/16), hidden].  Backward of the LAST forward on the handle:
+ * d_feat fp32 of feat's shape -> fp32 gradients, OVERWRITTEN, through the non-NULL pointers of `g` (same layout as the weights;
+ * NULL fields and array entries are skipped). */
+typedef struct CarDinoTrain CarDinoTrain;
+int car_dino_train_create(const CarDinoDesc* desc, const CarDinoWeights* w, void* stream, CarDinoTrain** out);
+int car_dino_train_forward(CarDinoTrain* m, const float* image, int32_t B, int32_t H, int32_t W, float* feat, void* stream);
+int car_dino_train_backward(CarDinoTrain* m, const float* d_feat, const CarDinoWeights* g, void* stream);
+int car_dino_train_destroy(CarDinoTrain* m);
+
 /* =====================================================================================================
  * Image tokenizer: VQModel.decode_code / encode (tokenizer/tokenizer_image/vq_model.py:41-56).
  * tensors: the fp32 state-dict tensors in canonical order = encoder, decoder, quantize.embedding.weight,
