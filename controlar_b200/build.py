@@ -9,9 +9,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libcontrolar_b200.so")
-SOURCES = ["car_api.cu", "car_vision.cu", "gemm.cu"]
+SOURCES = ["car_api.cu", "car_vision.cu", "car_train.cu", "gemm.cu"]
+# --no-undefined: a kernel launched from one translation unit and defined in another (misc.h) must resolve when the library links
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-shared",
-              "-Xcompiler", "-fPIC", "-cudart", "static"]
+              "-Xcompiler", "-fPIC", "-cudart", "static", "-Xlinker", "--no-undefined"]
 
 
 def _source_hash(flags) -> str:

@@ -12,9 +12,6 @@
 #include "misc.cuh"
 #include "decode_persistent.cuh"
 #include "gemm.h"
-#include "train.cuh"
-#include "train_bwd.cuh"
-#include "dropout.cuh"
 #include "t5.cuh"
 #include <algorithm>
 
@@ -945,459 +942,6 @@ extern "C" int car_op_attn_prefill(int32_t dtype, const void* q, const void* k_c
     if (dtype != CAR_BF16) CAR_FAIL(CAR_ERR_UNSUPPORTED, "the tensor-core prefill attention is bf16 only");
     if (((uintptr_t)q | (uintptr_t)out) % 4) CAR_FAIL(CAR_ERR_ARG, "q and out must be 4-byte aligned");
     return launch_attn_prefill_mma(st, q, k_cache, v_cache, emb_mask, mask_ld, B, H, S, Tq, Tpre, out);
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// training forward (SURVEY.md §8 row f1): Transformer.forward(idx, cond_idx, targets, mask, valid, condition) in train mode,
-// fp32 parameters under bf16 autocast — gpt_t2i.py:420-431,451-484.  First correct path: prefill GEMM kernels + train.cuh glue.
-// ---------------------------------------------------------------------------------------------------------
-struct CarTrain : CarOwned {
-    CarModelDesc d;
-    CarTrainWeights w;
-    std::vector<const void*> attention_norm, wqkv, wo, ffn_norm, w1, w3, w2;   // borrowed fp32
-    std::vector<bf16*> b_wqkv, b_wo, b_w1, b_w3, b_w2;                          // owned bf16 casts, refreshed every forward
-    bf16 *b_out, *b_cap1, *b_cap2, *b_cond1, *b_cond2, *b_ctl1[3], *b_ctl2[3], *b_ad1, *b_ad2;
-    int maxB, maxN, maxS;
-    const float* rope;
-    float *h, *nll;
-    bf16 *x, *qkv, *q, *kc, *vc, *att, *g, *u, *act, *o, *cin, *ctmp, *ctok, *cadd, *lg;
-    // ---- backward (car_train_backward): the stream saved at every block input, gradient / transpose workspaces ----
-    float *hs, *dh, *h0, *scr, *part, *lse, *dsum;
-    bf16 *capx, *x2, *db, *dact, *dg, *du, *dx, *datt, *dq, *dk, *dv, *dqkv, *dlg, *wT, *yT, *xT, *dWb;
-    bf16 *m_t, *m_a, *m_da, *m_dt, *dctok, *dcin, *dadd;
-    size_t Rp_max;
-    // arguments of the last car_train_forward (borrowed until car_train_backward returns)
-    int fB = 0, fN = 0;
-    const int32_t *f_idx = nullptr, *f_targets = nullptr;
-    const void *f_cond = nullptr, *f_feat = nullptr;
-    const uint8_t *f_drop = nullptr, *f_mask = nullptr;
-    const float* f_valid = nullptr;
-    bool fwd_ok = false;
-    // dropout (car_train_set_dropout): the settings the next forward takes, and the ones the last forward ran with (its backward's)
-    struct DropCfg { float tok_p = 0.f, resid_p = 0.f, ffn_p = 0.f; std::vector<float> path; const uint64_t* seed = nullptr; };
-    DropCfg drop_next, drop_fwd;
-};
-
-// keep = fp32(1 - p), scale = fp32(1 / keep): the values ATen's CUDA dropout derives from p (native_dropout -> keep probability in
-// double, cast to the fp32 accumulate type, scale = 1.0 / keep)
-static void tr_keep_scale(float p, float* keep, float* scale) {
-    *keep = (float)(1.0 - (double)p);
-    *scale = (float)(1.0 / (double)*keep);
-}
-// the fused dropout of one site of layer l under the settings c; every part off when its p (or rate) is 0
-static TrDrop tr_drop(const CarTrain::DropCfg& c, int site, int l) {
-    TrDrop r{c.seed, site, l, 1.f, 1.f, 0, 1.f, 1.f};
-    const float p = site == CAR_DROP_TOKEN ? c.tok_p : (site == CAR_DROP_RESID ? c.resid_p : c.ffn_p);
-    if (p > 0.f) tr_keep_scale(p, &r.keep, &r.scale);
-    const float rate = (site != CAR_DROP_TOKEN && !c.path.empty()) ? c.path[l] : 0.f;
-    if (rate > 0.f) {                                          // utils/drop_path.py: bernoulli_(keep).div_(keep) on a bf16 tensor
-        float unused;
-        tr_keep_scale(rate, &r.path_keep, &unused);
-        r.path_site = site == CAR_DROP_RESID ? CAR_DROP_PATH_ATTN : CAR_DROP_PATH_FFN;
-        r.path_mult = __bfloat162float(__float2bfloat16_rn(1.f / r.path_keep));
-    }
-    return r;
-}
-static bool tr_drop_on(const TrDrop& r) { return r.seed != nullptr && (r.keep < 1.f || r.path_keep < 1.f); }
-
-static int tr_cast(cudaStream_t st, const void* src, bf16* dst, long long n) {
-    CAR_LAUNCH(tr_cast_bf16_kernel, gsz(n), 256, 0, st, (const float*)src, dst, n);
-    return CAR_OK;
-}
-// MLP.forward gpt_t2i.py:177-181 on bf16 operands: out = fc2(gelu_tanh(fc1 x))
-static int tr_mlp(cudaStream_t st, const bf16* x, int rows, int K, const bf16* fc1, const bf16* fc2, int d, bf16* tmp, bf16* out) {
-    CAR_TRY(dense_linear(st, x, K, fc1, rows, d, K, ACT_GELU_TANH, nullptr, 0, tmp, d));
-    return dense_linear(st, tmp, d, fc2, rows, d, d, ACT_NONE, nullptr, 0, out, d);
-}
-
-// everything car_train_create allocates; on failure the caller deletes the half-built handle
-static int train_init(CarTrain* t) {
-    const CarModelDesc& d = t->d;
-    const int L = d.n_layer, dim = d.dim, F = d.ffn_dim, V = d.vocab_size;
-    auto copyp = [&](std::vector<const void*>& v, const void* const* src) { v.assign(src, src + L); };
-    const CarWeights& w = t->w.w;
-    copyp(t->attention_norm, w.attention_norm); copyp(t->wqkv, w.wqkv); copyp(t->wo, w.wo); copyp(t->ffn_norm, w.ffn_norm);
-    copyp(t->w1, w.w1); copyp(t->w3, w.w3); copyp(t->w2, w.w2);
-    t->b_wqkv.resize(L); t->b_wo.resize(L); t->b_w1.resize(L); t->b_w3.resize(L); t->b_w2.resize(L);
-    for (int l = 0; l < L; ++l) {
-        CAR_TRY(t->alloc(&t->b_wqkv[l], (size_t)3 * dim * dim * 2)); CAR_TRY(t->alloc(&t->b_wo[l], (size_t)dim * dim * 2));
-        CAR_TRY(t->alloc(&t->b_w1[l], (size_t)F * dim * 2)); CAR_TRY(t->alloc(&t->b_w3[l], (size_t)F * dim * 2));
-        CAR_TRY(t->alloc(&t->b_w2[l], (size_t)dim * F * 2));
-    }
-    CAR_TRY(t->alloc(&t->b_out, (size_t)V * dim * 2));
-    if (d.model_type == 1) { CAR_TRY(t->alloc(&t->b_cap1, (size_t)dim * d.caption_dim * 2)); CAR_TRY(t->alloc(&t->b_cap2, (size_t)dim * dim * 2)); }
-    CAR_TRY(t->alloc(&t->b_cond1, (size_t)dim * dim * 2)); CAR_TRY(t->alloc(&t->b_cond2, (size_t)dim * dim * 2));
-    for (int j = 0; j < 3; ++j) { CAR_TRY(t->alloc(&t->b_ctl1[j], (size_t)dim * dim * 2)); CAR_TRY(t->alloc(&t->b_ctl2[j], (size_t)dim * dim * 2)); }
-    CAR_TRY(t->alloc(&t->b_ad1, (size_t)dim * t->w.adapter_dim * 2)); CAR_TRY(t->alloc(&t->b_ad2, (size_t)dim * dim * 2));
-    const size_t R = (size_t)t->maxB * t->maxS, RC = (size_t)t->maxB * t->maxN;
-    CAR_TRY(t->alloc(&t->h, R * dim * 4));
-    CAR_TRY(t->alloc(&t->nll, RC * 4));
-    CAR_TRY(t->alloc(&t->x, std::max(R * dim, (size_t)t->maxB * d.cls_token_num * std::max(d.caption_dim, dim)) * 2));
-    CAR_TRY(t->alloc(&t->qkv, R * 3 * dim * 2)); CAR_TRY(t->alloc(&t->q, R * dim * 2)); CAR_TRY(t->alloc(&t->kc, R * dim * 2));
-    CAR_TRY(t->alloc(&t->vc, R * dim * 2)); CAR_TRY(t->alloc(&t->att, R * dim * 2));
-    CAR_TRY(t->alloc(&t->g, R * F * 2)); CAR_TRY(t->alloc(&t->u, R * F * 2)); CAR_TRY(t->alloc(&t->act, R * F * 2)); CAR_TRY(t->alloc(&t->o, R * dim * 2));
-    CAR_TRY(t->alloc(&t->cin, RC * dim * 2)); CAR_TRY(t->alloc(&t->ctmp, std::max(RC, (size_t)t->maxB * d.cls_token_num) * dim * 2));
-    CAR_TRY(t->alloc(&t->ctok, RC * dim * 2)); CAR_TRY(t->alloc(&t->cadd, RC * dim * 2));
-    CAR_TRY(t->alloc(&t->lg, RC * V * 2));
-    // backward workspaces
-    const size_t cap = (size_t)(d.model_type == 1 ? d.caption_dim : 8), ad = (size_t)t->w.adapter_dim;
-    const size_t rows_mlp = std::max(RC, (size_t)t->maxB * d.cls_token_num);
-    const size_t Rp = (std::max(R, rows_mlp) + 63) / 64 * 64;
-    const size_t maxN = std::max({(size_t)3 * dim, (size_t)F, (size_t)V}), maxK = std::max({(size_t)F, (size_t)dim, cap, ad});
-    const size_t maxW = std::max({(size_t)3 * dim * dim, (size_t)F * dim, (size_t)V * dim, (size_t)dim * cap, (size_t)dim * ad});
-    t->Rp_max = Rp;
-    CAR_TRY(t->alloc(&t->hs, (size_t)L * R * dim * 4)); CAR_TRY(t->alloc(&t->dh, R * dim * 4)); CAR_TRY(t->alloc(&t->h0, R * dim * 4));
-    CAR_TRY(t->alloc(&t->scr, R * dim * 4)); CAR_TRY(t->alloc(&t->part, (size_t)TR_COLSUM_CHUNKS * dim * 4));
-    CAR_TRY(t->alloc(&t->lse, (size_t)t->maxB * d.n_head * t->maxS * 4)); CAR_TRY(t->alloc(&t->dsum, (size_t)t->maxB * d.n_head * t->maxS * 4));
-    CAR_TRY(t->alloc(&t->capx, (size_t)t->maxB * d.cls_token_num * cap * 2));
-    CAR_TRY(t->alloc(&t->x2, R * dim * 2)); CAR_TRY(t->alloc(&t->db, R * dim * 2)); CAR_TRY(t->alloc(&t->dact, R * F * 2));
-    CAR_TRY(t->alloc(&t->dg, R * F * 2)); CAR_TRY(t->alloc(&t->du, R * F * 2)); CAR_TRY(t->alloc(&t->dx, R * dim * 2));
-    CAR_TRY(t->alloc(&t->datt, R * dim * 2)); CAR_TRY(t->alloc(&t->dq, R * dim * 2)); CAR_TRY(t->alloc(&t->dk, R * dim * 2));
-    CAR_TRY(t->alloc(&t->dv, R * dim * 2)); CAR_TRY(t->alloc(&t->dqkv, R * 3 * dim * 2)); CAR_TRY(t->alloc(&t->dlg, RC * V * 2));
-    CAR_TRY(t->alloc(&t->wT, maxW * 2)); CAR_TRY(t->alloc(&t->dWb, maxW * 2)); CAR_TRY(t->alloc(&t->yT, maxN * Rp * 2)); CAR_TRY(t->alloc(&t->xT, maxK * Rp * 2));
-    CAR_TRY(t->alloc(&t->m_t, rows_mlp * dim * 2)); CAR_TRY(t->alloc(&t->m_a, rows_mlp * dim * 2));
-    CAR_TRY(t->alloc(&t->m_da, rows_mlp * dim * 2)); CAR_TRY(t->alloc(&t->m_dt, rows_mlp * dim * 2));
-    CAR_TRY(t->alloc(&t->dctok, RC * dim * 2)); CAR_TRY(t->alloc(&t->dcin, RC * dim * 2)); CAR_TRY(t->alloc(&t->dadd, rows_mlp * dim * 2));
-    return CAR_OK;
-}
-
-extern "C" int car_train_create(const CarModelDesc* desc, const CarTrainWeights* w, int32_t max_batch, int32_t max_img_tokens,
-                                const float* rope_table, void* stream, CarTrain** out) {
-    if (!desc || !w || !out || !rope_table) CAR_FAIL(CAR_ERR_ARG, "null argument");
-    const CarModelDesc& d = *desc;
-    if (d.dtype != CAR_F32) CAR_FAIL(CAR_ERR_UNSUPPORTED, "training forward takes the fp32 master weights (bf16 autocast is applied inside)");
-    if (d.n_head <= 0 || d.dim != d.n_head * 64 || d.n_layer % 3 != 0 || d.ffn_dim % 8 != 0 || d.vocab_size % 8 != 0 || w->adapter_dim % 8 != 0 ||
-        (d.model_type == 1 && d.caption_dim % 8 != 0))
-        CAR_FAIL(CAR_ERR_UNSUPPORTED, "shape not supported (head_dim 64, dims multiple of 8, n_layer multiple of 3)");
-    if (max_batch <= 0 || max_img_tokens <= 0) CAR_FAIL(CAR_ERR_ARG, "bad capacity");
-    (void)stream;
-    CarTrain* t = new CarTrain();
-    t->d = d; t->w = *w; t->rope = rope_table;
-    t->maxB = max_batch; t->maxN = max_img_tokens; t->maxS = d.cls_token_num + max_img_tokens - 1;
-    const int rc = train_init(t);
-    if (rc != CAR_OK) { delete t; return rc; }
-    *out = t;
-    return CAR_OK;
-}
-
-extern "C" int car_train_destroy(CarTrain* t) {
-    delete t;
-    return CAR_OK;
-}
-
-// dynamic shared memory of the plain attention kernels (TRA_WARPS warps x floats_per_warp); above 48 KB the opt-in attribute is set on
-// every call (cheap, and correct on every device of the process — no process-wide "already set" flag)
-static int tr_attn_smem(size_t floats_per_warp, const void* fn, size_t* bytes) {
-    *bytes = (size_t)TRA_WARPS * floats_per_warp * 4;
-    if (*bytes > 200 * 1024) CAR_FAIL(CAR_ERR_UNSUPPORTED, "sequence too long for the plain attention kernels");
-    if (*bytes > 48 * 1024) CAR_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    return CAR_OK;
-}
-
-// h += branch output t->o (fp32 += bf16, gpt_t2i.py:305-306) with the branch's dropout and drop path of the last forward's settings
-static int tr_residual_add(CarTrain* t, cudaStream_t st, int site, int l, int R, int B, int S) {
-    const int dim = t->d.dim;
-    const TrDrop dr = tr_drop(t->drop_fwd, site, l);
-    if (tr_drop_on(dr)) CAR_LAUNCH(tr_add_rows_drop_kernel, gsz((long long)R * dim / 4), 256, 0, st, t->h, (const bf16*)t->o, B, S, dim, dr);
-    else CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)R * dim), 256, 0, st, t->h, (const bf16*)t->o, B, S, S, 0, dim);
-    return CAR_OK;
-}
-// the bf16 gradient of a branch output from the fp32 stream gradient t->dh, through the branch's drop path and dropout
-static int tr_residual_take(CarTrain* t, cudaStream_t st, int site, int l, int R, int B, int S) {
-    const int dim = t->d.dim;
-    const TrDrop dr = tr_drop(t->drop_fwd, site, l);
-    if (tr_drop_on(dr)) CAR_LAUNCH(tr_take_rows_drop_kernel, gsz((long long)R * dim / 4), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim, dr);
-    else CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)R * dim), 256, 0, st, (const float*)t->dh, t->db, B, S, S, 0, dim);
-    return CAR_OK;
-}
-
-// One TransformerBlock (gpt_t2i.py:303-307) on the fp32 stream t->h, preceded by the control add of gpt_t2i.py:458-460 when the
-// block opens a third of the stack.  for_bwd: the recompute of car_train_backward — keeps the block input (after the control
-// add) in t->h0, the attention-side norm output in t->x, the feed-forward-side one in t->x2, and stops before w2 (t->h then
-// holds the stream between the two halves).
-static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, const uint8_t* mask, bool has_feat, bool for_bwd) {
-    const CarModelDesc& d = t->d;
-    const int L = d.n_layer, dim = d.dim, F = d.ffn_dim, T = d.cls_token_num, H = d.n_head;
-    const int n = n_img - 1, S = T + n, R = B * S, RC = B * n_img, step3 = L / 3;
-    if (has_feat && l % step3 == 0) {
-        CAR_TRY(tr_mlp(st, t->ctok, RC, dim, t->b_ctl1[l / step3], t->b_ctl2[l / step3], dim, t->ctmp, t->cadd));
-        CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)RC * dim), 256, 0, st, t->h, (const bf16*)t->cadd, B, n_img, S, T - 1, dim);
-    }
-    if (for_bwd) CAR_CUDA(cudaMemcpyAsync(t->h0, t->h, (size_t)R * dim * 4, cudaMemcpyDeviceToDevice, st));
-    size_t att_smem = 0;
-    CAR_TRY(tr_attn_smem((size_t)S, (const void*)tr_attention_kernel, &att_smem));
-    CAR_LAUNCH(tr_rmsnorm_kernel, R, 256, 0, st, (const float*)t->h, (const float*)t->attention_norm[l], t->x, dim, d.norm_eps, S, S, 0);
-    CAR_TRY(dense_linear(st, t->x, dim, t->b_wqkv[l], R, 3 * dim, dim, ACT_NONE, nullptr, 0, t->qkv, 3 * dim));
-    CAR_LAUNCH(rope_kv_write_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->qkv, t->rope, t->q, t->kc, t->vc, R, S, dim, H, S);
-    CAR_LAUNCH(tr_attention_kernel, (unsigned)(((long long)B * H * S + TRA_WARPS - 1) / TRA_WARPS), TRA_WARPS * 32, att_smem, st, (const bf16*)t->q,
-               (const bf16*)t->kc, (const bf16*)t->vc, mask, B, H, S, t->att, 1);
-    CAR_TRY(dense_linear(st, t->att, dim, t->b_wo[l], R, dim, dim, ACT_NONE, nullptr, 0, t->o, dim));
-    CAR_TRY(tr_residual_add(t, st, CAR_DROP_RESID, l, R, B, S));
-    bf16* xn = for_bwd ? t->x2 : t->x;
-    CAR_LAUNCH(tr_rmsnorm_kernel, R, 256, 0, st, (const float*)t->h, (const float*)t->ffn_norm[l], xn, dim, d.norm_eps, S, S, 0);
-    CAR_TRY(dense_linear(st, xn, dim, t->b_w1[l], R, F, dim, ACT_NONE, nullptr, 0, t->g, F));
-    CAR_TRY(dense_linear(st, xn, dim, t->b_w3[l], R, F, dim, ACT_NONE, nullptr, 0, t->u, F));
-    CAR_LAUNCH(swiglu_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, t->act, (long long)R * F);
-    if (for_bwd) return CAR_OK;
-    CAR_TRY(dense_linear(st, t->act, F, t->b_w2[l], R, dim, F, ACT_NONE, nullptr, 0, t->o, dim));
-    CAR_TRY(tr_residual_add(t, st, CAR_DROP_FFN, l, R, B, S));
-    return CAR_OK;
-}
-
-extern "C" int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const int32_t* idx, const void* cond, const void* feat,
-                                 const uint8_t* drop_ids, const uint8_t* mask, const int32_t* targets, const float* valid,
-                                 float* logits_out, float* loss_out, void* stream) {
-    if (!t || !idx || !cond || !drop_ids) CAR_FAIL(CAR_ERR_ARG, "null argument");
-    if (B <= 0 || B > t->maxB || n_img < 2 || n_img > t->maxN) CAR_FAIL(CAR_ERR_ARG, "batch / token count beyond the capacity given to car_train_create");
-    if ((loss_out != nullptr) != (targets != nullptr)) CAR_FAIL(CAR_ERR_ARG, "loss_out and targets go together");
-    cudaStream_t st = (cudaStream_t)stream;
-    const CarModelDesc& d = t->d;
-    const int L = d.n_layer, dim = d.dim, F = d.ffn_dim, V = d.vocab_size, T = d.cls_token_num;
-    const int n = n_img - 1, S = T + n, R = B * S, RC = B * n_img;
-    if (S > T + d.block_size) CAR_FAIL(CAR_ERR_ARG, "sequence longer than the RoPE table");
-    t->fwd_ok = false;
-    t->drop_fwd = t->drop_next;
-    const TrDrop dtok = tr_drop(t->drop_fwd, CAR_DROP_TOKEN, 0);
-    const bool tok_on = tr_drop_on(dtok);
-    // 0. autocast: bf16 copies of every nn.Linear weight, re-cast each forward (the fp32 masters may have been stepped)
-    for (int l = 0; l < L; ++l) {
-        CAR_TRY(tr_cast(st, t->wqkv[l], t->b_wqkv[l], (long long)3 * dim * dim)); CAR_TRY(tr_cast(st, t->wo[l], t->b_wo[l], (long long)dim * dim));
-        CAR_TRY(tr_cast(st, t->w1[l], t->b_w1[l], (long long)F * dim)); CAR_TRY(tr_cast(st, t->w3[l], t->b_w3[l], (long long)F * dim));
-        CAR_TRY(tr_cast(st, t->w2[l], t->b_w2[l], (long long)dim * F));
-    }
-    CAR_TRY(tr_cast(st, t->w.w.output, t->b_out, (long long)V * dim));
-    if (d.model_type == 1) { CAR_TRY(tr_cast(st, t->w.w.cap_fc1, t->b_cap1, (long long)dim * d.caption_dim)); CAR_TRY(tr_cast(st, t->w.w.cap_fc2, t->b_cap2, (long long)dim * dim)); }
-    if (feat) {
-        CAR_TRY(tr_cast(st, t->w.w.cond_fc1, t->b_cond1, (long long)dim * dim)); CAR_TRY(tr_cast(st, t->w.w.cond_fc2, t->b_cond2, (long long)dim * dim));
-        for (int j = 0; j < 3; ++j) { CAR_TRY(tr_cast(st, t->w.w.ctl_fc1[j], t->b_ctl1[j], (long long)dim * dim)); CAR_TRY(tr_cast(st, t->w.w.ctl_fc2[j], t->b_ctl2[j], (long long)dim * dim)); }
-        CAR_TRY(tr_cast(st, t->w.adapter_fc1, t->b_ad1, (long long)dim * t->w.adapter_dim)); CAR_TRY(tr_cast(st, t->w.adapter_fc2, t->b_ad2, (long long)dim * dim));
-    }
-    // 1. prefix rows: CaptionEmbedder (token_drop, cap_proj) gpt_t2i.py:145-162 or LabelEmbedder :78-97; image-token rows :423;
-    //    tok_dropout (:430) fused into the writes of both
-    if (d.model_type == 1) {
-        CAR_LAUNCH(tr_caption_select_kernel, gsz((long long)B * T * d.caption_dim), 256, 0, st, (const float*)cond, (const float*)t->w.cap_uncond,
-                   drop_ids, t->capx, B, T, d.caption_dim);
-        CAR_TRY(tr_mlp(st, t->capx, B * T, d.caption_dim, t->b_cap1, t->b_cap2, dim, t->ctmp, t->o));
-        if (tok_on) CAR_LAUNCH(tr_put_rows_drop_kernel, gsz((long long)B * T * dim / 4), 256, 0, st, (const bf16*)t->o, t->h, B, T, S, 0, dim, dtok);
-        else CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const bf16*)t->o, t->h, B, T, S, 0, dim);
-    } else if (tok_on) {
-        CAR_LAUNCH(tr_embed_rows_drop_kernel, B, 256, 0, st, (const float*)t->w.w.label_table, (const int*)cond, 1, drop_ids, t->w.num_classes, t->h, B, 1, S, 0, dim, dtok);
-    } else {
-        CAR_LAUNCH(tr_embed_rows_kernel, B, 256, 0, st, (const float*)t->w.w.label_table, (const int*)cond, 1, drop_ids, t->w.num_classes, t->h, B, 1, S, 0, dim);
-    }
-    if (tok_on)
-        CAR_LAUNCH(tr_embed_rows_drop_kernel, B * n, 256, 0, st, (const float*)t->w.w.tok_embeddings, (const int*)idx, n, (const unsigned char*)nullptr, 0, t->h, B, n, S, T, dim, dtok);
-    else
-        CAR_LAUNCH(tr_embed_rows_kernel, B * n, 256, 0, st, (const float*)t->w.w.tok_embeddings, (const int*)idx, n, (const unsigned char*)nullptr, 0, t->h, B, n, S, T, dim);
-    // 2. control tokens: adapter_mlp -> token_drop -> condition_mlp  gpt_t2i.py:424-427 (feat = the control encoder's output tokens)
-    if (feat) {
-        CAR_TRY(tr_mlp(st, (const bf16*)feat, RC, t->w.adapter_dim, t->b_ad1, t->b_ad2, dim, t->ctmp, t->cin));
-        CAR_LAUNCH(tr_select_uncond_kernel, gsz((long long)RC * dim), 256, 0, st, t->cin, (const float*)t->w.cond_uncond, drop_ids, B, (long long)n_img * dim);
-        CAR_TRY(tr_mlp(st, t->cin, RC, dim, t->b_cond1, t->b_cond2, dim, t->ctmp, t->ctok));
-    }
-    // 3. blocks  gpt_t2i.py:456-468; the stream at every block input is kept for the backward's recompute
-    for (int l = 0; l < L; ++l) {
-        CAR_CUDA(cudaMemcpyAsync(t->hs + (size_t)l * R * dim, t->h, (size_t)R * dim * 4, cudaMemcpyDeviceToDevice, st));
-        CAR_TRY(tr_block_fwd(t, st, l, B, n_img, mask, feat != nullptr, false));
-    }
-    // 4. head on rows T-1 .. S-1 of every sample (gpt_t2i.py:469-473), loss :474-481
-    CAR_LAUNCH(tr_rmsnorm_kernel, RC, 256, 0, st, (const float*)t->h, (const float*)t->w.w.norm, t->x, dim, d.norm_eps, n_img, S, T - 1);
-    CAR_TRY(dense_linear(st, t->x, dim, t->b_out, RC, V, dim, ACT_NONE, nullptr, 0, t->lg, V));
-    if (targets) {
-        CAR_LAUNCH(tr_ce_rows_kernel, RC, 256, 0, st, (const bf16*)t->lg, (const int*)targets, logits_out, t->nll, V);
-        CAR_LAUNCH(tr_ce_reduce_kernel, 1, 1024, 0, st, (const float*)t->nll, valid, B, n_img, loss_out);
-    } else if (logits_out) {
-        CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)RC * V), 256, 0, st, (const bf16*)t->lg, logits_out, 1, RC, RC, 0, V);
-    }
-    t->fB = B; t->fN = n_img; t->f_idx = idx; t->f_cond = cond; t->f_feat = feat; t->f_drop = drop_ids; t->f_mask = mask; t->f_targets = targets;
-    t->f_valid = valid;
-    t->fwd_ok = targets != nullptr;
-    return CAR_OK;
-}
-
-// ---- backward helpers: the two GEMMs of a linear layer's backward on the [N][K] x [M][K]^T tensor-core kernels ----------------
-// dX [rows][K] = bf16(dY [rows][N] . W [N][K] (+ resid)): needs W^T as the K-major operand
-static int tr_dgrad(CarTrain* t, cudaStream_t st, const bf16* dY, const bf16* Wb, int rows, int N, int K, const bf16* resid, bf16* dX) {
-    CAR_LAUNCH(tr_transpose_pad_kernel, dim3((N + 31) / 32, (K + 31) / 32), dim3(32, 8), 0, st, Wb, t->wT, N, K, N);
-    return dense_linear(st, dY, N, t->wT, rows, K, N, ACT_NONE, resid, K, dX, K);
-}
-// grad [N][K] fp32 = float(bf16(dY^T . X)), dY [rows][N], X [rows][K]: both operands transposed, the row extent zero-padded to 64
-static int tr_wgrad(CarTrain* t, cudaStream_t st, const bf16* dY, const bf16* X, int rows, int N, int K, float* grad) {
-    if (!grad) return CAR_OK;
-    const int Rp = (rows + 63) / 64 * 64;
-    if ((size_t)Rp > t->Rp_max) CAR_FAIL(CAR_ERR_ARG, "row count beyond the transpose workspace");
-    CAR_LAUNCH(tr_transpose_pad_kernel, dim3(Rp / 32, (N + 31) / 32), dim3(32, 8), 0, st, dY, t->yT, rows, N, Rp);
-    CAR_LAUNCH(tr_transpose_pad_kernel, dim3(Rp / 32, (K + 31) / 32), dim3(32, 8), 0, st, X, t->xT, rows, K, Rp);
-    CAR_TRY(dense_linear(st, t->yT, Rp, t->xT, N, K, Rp, ACT_NONE, nullptr, 0, t->dWb, K));
-    CAR_LAUNCH(tr_bf16_to_f32_kernel, gsz((long long)N * K), 256, 0, st, (const bf16*)t->dWb, grad, (long long)N * K);
-    return CAR_OK;
-}
-// RMSNorm backward on `rows` output rows (row map like tr_rmsnorm_kernel) + the weight gradient
-static int tr_norm_bwd(CarTrain* t, cudaStream_t st, const float* h, const void* w, const bf16* dy, int rows, int nrows, int S, int row0, float* gw) {
-    const int dim = t->d.dim;
-    CAR_LAUNCH(tr_rmsnorm_bwd_kernel, rows, 256, 0, st, h, (const float*)w, dy, t->dh, t->scr, dim, t->d.norm_eps, nrows, S, row0);
-    if (gw) {
-        CAR_LAUNCH(tr_colsum_part_kernel, dim3((dim + 31) / 32, TR_COLSUM_CHUNKS), dim3(32, 8), 0, st, (const float*)t->scr, t->part, rows, dim);
-        CAR_LAUNCH(tr_colsum_final_kernel, (dim + 255) / 256, 256, 0, st, (const float*)t->part, gw, dim);
-    }
-    return CAR_OK;
-}
-// MLP backward (gpt_t2i.py:177-181: fc2(gelu_tanh(fc1 x)), no bias), recomputing the two intermediates.  dX (optional) = bf16(dT . fc1 (+ resid))
-static int tr_mlp_bwd(CarTrain* t, cudaStream_t st, const bf16* x, int rows, int K, const bf16* fc1, const bf16* fc2, const bf16* dY,
-                      const bf16* resid, bf16* dX, float* g1, float* g2) {
-    const int dim = t->d.dim;
-    CAR_TRY(dense_linear(st, x, K, fc1, rows, dim, K, ACT_NONE, nullptr, 0, t->m_t, dim));
-    CAR_LAUNCH(tr_gelu_kernel, gsz((long long)rows * dim), 256, 0, st, (const bf16*)t->m_t, t->m_a, (long long)rows * dim);
-    CAR_TRY(tr_wgrad(t, st, dY, t->m_a, rows, dim, dim, g2));
-    CAR_TRY(tr_dgrad(t, st, dY, fc2, rows, dim, dim, nullptr, t->m_da));
-    CAR_LAUNCH(tr_gelu_bwd_kernel, gsz((long long)rows * dim), 256, 0, st, (const bf16*)t->m_t, (const bf16*)t->m_da, t->m_dt, (long long)rows * dim);
-    CAR_TRY(tr_wgrad(t, st, t->m_dt, x, rows, dim, K, g1));
-    if (dX) CAR_TRY(tr_dgrad(t, st, t->m_dt, fc1, rows, dim, K, resid, dX));
-    return CAR_OK;
-}
-
-// Backward of the last car_train_forward(targets != NULL) on this handle: writes d loss / d parameter (fp32, OVERWRITTEN, scaled
-// by *loss_grad when given) through the non-NULL pointers of `g` (a CarTrainWeights whose fields point at gradient buffers of the
-// parameters' shapes) and d loss / d feat (bf16 [B, n_img, adapter_dim]) when d_feat is given.
-extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d_feat, const float* loss_grad, void* stream) {
-    if (!t || !g) CAR_FAIL(CAR_ERR_ARG, "null argument");
-    if (!t->fwd_ok) CAR_FAIL(CAR_ERR_ARG, "car_train_backward needs a preceding car_train_forward with targets on the same handle");
-    cudaStream_t st = (cudaStream_t)stream;
-    const CarModelDesc& d = t->d;
-    const int L = d.n_layer, dim = d.dim, F = d.ffn_dim, V = d.vocab_size, T = d.cls_token_num, H = d.n_head;
-    if (dim % 64 != 0 || F % 64 != 0 || V % 64 != 0) CAR_FAIL(CAR_ERR_UNSUPPORTED, "backward: dim, ffn_dim and vocab_size must be multiples of 64");
-    const int B = t->fB, n_img = t->fN, n = n_img - 1, S = T + n, R = B * S, RC = B * n_img, step3 = L / 3;
-    const bool has_feat = t->f_feat != nullptr;
-    const uint8_t* mask = t->f_mask;
-    size_t smem_q = 0, smem_kv = 0;
-    CAR_TRY(tr_attn_smem((size_t)2 * S + 128, (const void*)tr_attn_bwd_q_kernel, &smem_q));
-    CAR_TRY(tr_attn_smem((size_t)2 * S + 128, (const void*)tr_attn_bwd_kv_kernel, &smem_kv));
-    const unsigned att_grid = (unsigned)(((long long)B * H * S + TRA_WARPS - 1) / TRA_WARPS);
-    t->fwd_ok = false;                                         // the recompute below overwrites the forward's buffers
-    // ---- head: loss -> logits -> output projection -> final norm (gpt_t2i.py:469-481) ----
-    CAR_LAUNCH(tr_rmsnorm_kernel, RC, 256, 0, st, (const float*)t->h, (const float*)t->w.w.norm, t->x, dim, d.norm_eps, n_img, S, T - 1);
-    CAR_LAUNCH(tr_ce_grad_kernel, RC, 256, 0, st, (const bf16*)t->lg, (const int*)t->f_targets, t->f_valid, loss_grad, B, n_img, t->dlg, V);
-    CAR_TRY(tr_wgrad(t, st, t->dlg, t->x, RC, V, dim, (float*)g->w.output));
-    CAR_TRY(tr_dgrad(t, st, t->dlg, t->b_out, RC, V, dim, nullptr, t->dx));
-    CAR_CUDA(cudaMemsetAsync(t->dh, 0, (size_t)R * dim * 4, st));
-    CAR_TRY(tr_norm_bwd(t, st, t->h, t->w.w.norm, t->dx, RC, n_img, S, T - 1, (float*)g->w.norm));
-    // ---- blocks, last to first: recompute from the saved input stream, then feed-forward half, attention half, control add ----
-    bool first_ctl = true;
-    for (int l = L - 1; l >= 0; --l) {
-        CAR_CUDA(cudaMemcpyAsync(t->h, t->hs + (size_t)l * R * dim, (size_t)R * dim * 4, cudaMemcpyDeviceToDevice, st));
-        CAR_TRY(tr_block_fwd(t, st, l, B, n_img, mask, has_feat, true));
-        // feed-forward: h_out = h_mid + drop_path(ffn_dropout(w2(silu(w1 x2) * w3 x2)))
-        CAR_TRY(tr_residual_take(t, st, CAR_DROP_FFN, l, R, B, S));
-        CAR_TRY(tr_wgrad(t, st, t->db, t->act, R, dim, F, g->w.w2 ? (float*)g->w.w2[l] : nullptr));
-        CAR_TRY(tr_dgrad(t, st, t->db, t->b_w2[l], R, dim, F, nullptr, t->dact));
-        CAR_LAUNCH(tr_swiglu_bwd_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, (const bf16*)t->dact, t->dg, t->du, (long long)R * F);
-        CAR_TRY(tr_wgrad(t, st, t->dg, t->x2, R, F, dim, g->w.w1 ? (float*)g->w.w1[l] : nullptr));
-        CAR_TRY(tr_wgrad(t, st, t->du, t->x2, R, F, dim, g->w.w3 ? (float*)g->w.w3[l] : nullptr));
-        CAR_TRY(tr_dgrad(t, st, t->dg, t->b_w1[l], R, F, dim, nullptr, t->dx));
-        CAR_TRY(tr_dgrad(t, st, t->du, t->b_w3[l], R, F, dim, t->dx, t->dx));
-        CAR_TRY(tr_norm_bwd(t, st, t->h, t->ffn_norm[l], t->dx, R, S, S, 0, g->w.ffn_norm ? (float*)g->w.ffn_norm[l] : nullptr));
-        // attention: h_mid = h0 + drop_path(resid_dropout(wo(sdpa(rope(wqkv x1)))))
-        CAR_TRY(tr_residual_take(t, st, CAR_DROP_RESID, l, R, B, S));
-        CAR_TRY(tr_wgrad(t, st, t->db, t->att, R, dim, dim, g->w.wo ? (float*)g->w.wo[l] : nullptr));
-        CAR_TRY(tr_dgrad(t, st, t->db, t->b_wo[l], R, dim, dim, nullptr, t->datt));
-        CAR_LAUNCH(tr_attn_bwd_q_kernel, att_grid, TRA_WARPS * 32, smem_q, st, (const bf16*)t->q, (const bf16*)t->kc, (const bf16*)t->vc, mask,
-                   (const bf16*)t->datt, B, H, S, t->lse, t->dsum, t->dq, 1);
-        CAR_LAUNCH(tr_attn_bwd_kv_kernel, att_grid, TRA_WARPS * 32, smem_kv, st, (const bf16*)t->q, (const bf16*)t->kc, (const bf16*)t->vc, mask,
-                   (const bf16*)t->datt, (const float*)t->lse, (const float*)t->dsum, B, H, S, t->dk, t->dv, 1);
-        CAR_LAUNCH(tr_rope_bwd_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->dq, (const bf16*)t->dk, (const bf16*)t->dv, t->rope, t->dqkv, R, S, dim, H, S);
-        CAR_TRY(tr_wgrad(t, st, t->dqkv, t->x, R, 3 * dim, dim, g->w.wqkv ? (float*)g->w.wqkv[l] : nullptr));
-        CAR_TRY(tr_dgrad(t, st, t->dqkv, t->b_wqkv[l], R, 3 * dim, dim, nullptr, t->dx));
-        CAR_TRY(tr_norm_bwd(t, st, t->h0, t->attention_norm[l], t->dx, R, S, S, 0, g->w.attention_norm ? (float*)g->w.attention_norm[l] : nullptr));
-        // control add h[:, T-1:] += condition_layers[j](condition_token)
-        if (has_feat && l % step3 == 0) {
-            const int j = l / step3;
-            CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)RC * dim), 256, 0, st, (const float*)t->dh, t->dadd, B, n_img, S, T - 1, dim);
-            CAR_TRY(tr_mlp_bwd(t, st, t->ctok, RC, dim, t->b_ctl1[j], t->b_ctl2[j], t->dadd, first_ctl ? nullptr : t->dctok, t->dctok,
-                               (float*)g->w.ctl_fc1[j], (float*)g->w.ctl_fc2[j]));
-            first_ctl = false;
-        }
-    }
-    // ---- embeddings and the prefix / control front ends; dh is the gradient of tok_dropout's output, its mask applies first ----
-    const TrDrop dtok = tr_drop(t->drop_fwd, CAR_DROP_TOKEN, 0);
-    const bool tok_on = tr_drop_on(dtok);
-    if (g->w.tok_embeddings) {
-        CAR_CUDA(cudaMemsetAsync((void*)g->w.tok_embeddings, 0, (size_t)V * dim * 4, st));
-        if (tok_on)
-            CAR_LAUNCH(tr_embed_grad_drop_kernel, B * n, 256, 0, st, (const float*)t->dh, (const int*)t->f_idx, n, (const unsigned char*)nullptr, 0,
-                       (float*)g->w.tok_embeddings, B, n, S, T, dim, dtok);
-        else
-            CAR_LAUNCH(tr_embed_grad_kernel, B * n, 256, 0, st, (const float*)t->dh, (const int*)t->f_idx, n, (const unsigned char*)nullptr, 0,
-                       (float*)g->w.tok_embeddings, B, n, S, T, dim);
-    }
-    if (d.model_type == 1) {
-        if (tok_on) CAR_LAUNCH(tr_take_rows_drop_kernel, gsz((long long)B * T * dim / 4), 256, 0, st, (const float*)t->dh, t->dadd, B, T, S, 0, dim, dtok);
-        else CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const float*)t->dh, t->dadd, B, T, S, 0, dim);
-        CAR_TRY(tr_mlp_bwd(t, st, t->capx, B * T, d.caption_dim, t->b_cap1, t->b_cap2, t->dadd, nullptr, nullptr, (float*)g->w.cap_fc1, (float*)g->w.cap_fc2));
-    } else if (g->w.label_table) {
-        CAR_CUDA(cudaMemsetAsync((void*)g->w.label_table, 0, (size_t)(t->w.num_classes + 1) * dim * 4, st));
-        if (tok_on)
-            CAR_LAUNCH(tr_embed_grad_drop_kernel, B, 256, 0, st, (const float*)t->dh, (const int*)t->f_cond, 1, t->f_drop, t->w.num_classes,
-                       (float*)g->w.label_table, B, 1, S, 0, dim, dtok);
-        else
-            CAR_LAUNCH(tr_embed_grad_kernel, B, 256, 0, st, (const float*)t->dh, (const int*)t->f_cond, 1, t->f_drop, t->w.num_classes, (float*)g->w.label_table,
-                       B, 1, S, 0, dim);
-    }
-    if (has_feat) {
-        CAR_TRY(tr_mlp_bwd(t, st, t->cin, RC, dim, t->b_cond1, t->b_cond2, t->dctok, nullptr, t->dcin, (float*)g->w.cond_fc1, (float*)g->w.cond_fc2));
-        CAR_LAUNCH(tr_zero_dropped_kernel, gsz((long long)RC * dim), 256, 0, st, t->dcin, t->f_drop, B, (long long)n_img * dim);
-        CAR_TRY(tr_mlp_bwd(t, st, (const bf16*)t->f_feat, RC, t->w.adapter_dim, t->b_ad1, t->b_ad2, t->dcin, nullptr, (bf16*)d_feat,
-                           (float*)g->adapter_fc1, (float*)g->adapter_fc2));
-    }
-    return CAR_OK;
-}
-
-static bool tr_prob_ok(float p) { return p >= 0.f && p < 1.f; }           // (false for NaN)
-
-// dropout settings of the next car_train_forward; every check happens before the handle is touched
-extern "C" int car_train_set_dropout(CarTrain* t, const CarTrainDropout* cfg) {
-    if (!t) CAR_FAIL(CAR_ERR_ARG, "null argument");
-    CarTrain::DropCfg c;
-    if (cfg) {
-        if (!tr_prob_ok(cfg->token_p) || !tr_prob_ok(cfg->resid_p) || !tr_prob_ok(cfg->ffn_p))
-            CAR_FAIL(CAR_ERR_ARG, "dropout probabilities must lie in [0, 1)");
-        if (cfg->n_layer < 0 || (cfg->drop_path == nullptr) != (cfg->n_layer == 0))
-            CAR_FAIL(CAR_ERR_ARG, "drop_path and n_layer go together");
-        bool any = cfg->token_p > 0.f || cfg->resid_p > 0.f || cfg->ffn_p > 0.f;
-        for (int l = 0; l < cfg->n_layer; ++l) {
-            if (!tr_prob_ok(cfg->drop_path[l])) CAR_FAIL(CAR_ERR_ARG, "drop-path rates must lie in [0, 1)");
-            any = any || cfg->drop_path[l] > 0.f;
-        }
-        if (any && cfg->seed == nullptr) CAR_FAIL(CAR_ERR_ARG, "dropout needs a device seed");
-        c.tok_p = cfg->token_p; c.resid_p = cfg->resid_p; c.ffn_p = cfg->ffn_p;
-        if (cfg->drop_path) c.path.assign(cfg->drop_path, cfg->drop_path + cfg->n_layer);
-        c.seed = any ? cfg->seed : nullptr;
-    }
-    if (!c.path.empty() && (int)c.path.size() != t->d.n_layer) CAR_FAIL(CAR_ERR_ARG, "drop_path needs one rate per layer");
-    t->drop_next = c;
-    return CAR_OK;
-}
-
-extern "C" int car_dropout_keep_mask(const uint64_t* seed_dev, int32_t site, int32_t layer, int32_t B, int32_t rows, int32_t cols, float p,
-                                     uint8_t* out, void* stream) {
-    if (!seed_dev || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
-    if (site < CAR_DROP_TOKEN || site > CAR_DROP_PATH_FFN) CAR_FAIL(CAR_ERR_ARG, "site must be 0 (token) .. 4 (drop path, feed-forward)");
-    if (layer < 0 || layer > 0xFFFF || B <= 0 || rows <= 0 || cols <= 0) CAR_FAIL(CAR_ERR_ARG, "bad layer or shape");
-    if (!tr_prob_ok(p)) CAR_FAIL(CAR_ERR_ARG, "p must lie in [0, 1)");
-    float keep = 1.f, scale;
-    tr_keep_scale(p, &keep, &scale);
-    CAR_LAUNCH(car_dropout_mask_kernel, gsz((long long)B * rows * cols), 256, 0, (cudaStream_t)stream, seed_dev, site, layer, B, rows, cols, keep, out);
-    return CAR_OK;
-}
-
-// fused AdamW step over a device-resident tensor table (train.cuh); bias corrections from the step count (1-based)
-extern "C" int car_adamw_step(const void* tensors_dev, const void* chunks_dev, int32_t n_chunks, float lr, float beta1, float beta2, float eps,
-                              int32_t step, void* stream) {
-    if (!tensors_dev || !chunks_dev) CAR_FAIL(CAR_ERR_ARG, "null argument");
-    if (n_chunks <= 0 || step < 1) CAR_FAIL(CAR_ERR_ARG, "n_chunks must be positive and step 1-based");
-    const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
-    CAR_LAUNCH(adamw_multi_kernel, n_chunks, 256, 0, (cudaStream_t)stream, (const CarAdamWTensorDev*)tensors_dev, (const int2*)chunks_dev, lr, beta1, beta2,
-               eps, bc1, sqrtf(bc2));
-    return CAR_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -11,14 +11,6 @@
 #include "dpt.cuh"
 #include "midas.cuh"
 
-// The trainable encoder reuses the transformer training path's kernels, which car_api.cu also compiles; this translation unit takes
-// its own internal-linkage copies so that the two objects do not both define them.
-namespace {
-#include "misc.cuh"
-#include "train_bwd.cuh"
-#include "dino_train.cuh"
-}
-
 template <typename... KArgs, typename... Args>
 static int launch_on(cudaStream_t st, void (*kernel)(KArgs...), unsigned grid, unsigned block, Args... args) {
     CAR_LAUNCH(kernel, grid, block, 0, st, args...);
@@ -281,316 +273,6 @@ extern "C" int car_dino_forward(CarDino* m, const void* image, int32_t B, int32_
     if (H % 16 || W % 16 || B <= 0) CAR_FAIL(CAR_ERR_ARG, "H and W must be multiples of 16");
     if (m->d.dtype == CAR_BF16) return dino_forward_t<bf16>(m, (const bf16*)image, B, H, W, out_bf16, apply_mlp, (cudaStream_t)stream);
     return dino_forward_t<float>(m, (const float*)image, B, H, W, out_bf16, apply_mlp, (cudaStream_t)stream);
-}
-
-// =========================================================================================================
-// Trainable control encoder (dino_train.cuh): Dinov2_Adapter / ViT_Adapter forward with fp32 parameters under bf16 autocast, and
-// its backward to every encoder parameter.  The fp32 masters are borrowed and re-cast to bf16 by every forward (an optimizer step
-// changes them in place); the forward keeps the fp32 stream at every block input, the backward recomputes each block from it.
-// =========================================================================================================
-struct CarDinoTrain : CarOwned {
-    CarDinoDesc d;
-    int kpatch, kpad;
-    const float *cls, *pos, *patch_w, *patch_b, *ln_w, *ln_b;
-    struct Layer { const float *n1w, *n1b, *qw, *qb, *kw, *kb, *vw, *vb, *ow, *ob, *ls1, *n2w, *n2b, *f1w, *f1b, *f2w, *f2b, *ls2;
-                   bf16 *w_qkv, *b_qkv, *w_o, *b_o, *w_fc1, *b_fc1, *w_fc2, *b_fc2; };
-    std::vector<Layer> L;
-    bf16 *w_patch, *b_patch;                 // owned bf16 casts, refreshed by every forward
-    int fB = 0, fH = 0, fW = 0;              // shape of the last forward; its backward carves the same workspace
-    bool fwd_ok = false;
-};
-
-struct DtBufs {
-    Buf<bf16> patches, ptok, xn, qkv, q, kc, vc, ctx, o, xn2, pre, act, y2, db, dact, dctx, dq, dk, dv, dqkv, dxn, yT, xT, wT, dWb;
-    Buf<float> posi, hs, xm, dx, scr, part, colv, lse, dsum, dposi, ptmp;
-};
-
-// the one list of takes of a forward and of its backward (same shape => same offsets: the saved streams survive in between)
-static int dt_carve(CarDinoTrain* m, int B, int h, int w, DtBufs& s) {
-    const CarDinoDesc& d = m->d;
-    const size_t C = d.hidden, F = 4 * C, hw = (size_t)h * w, rows = (size_t)B * (hw + 1), Rp = (rows + 63) / 64 * 64;
-    const size_t KP = m->kpad, BHT = (size_t)B * d.heads * (hw + 1), maxK = std::max(F, KP);
-    return m->ws.carve([&](Carve& c) {
-        s.patches = c.take<bf16>((size_t)B * hw * KP); s.ptok = c.take<bf16>((size_t)B * hw * C);
-        s.posi = c.take<float>(hw * C); s.hs = c.take<float>((size_t)(d.layers + 1) * rows * C); s.xm = c.take<float>(rows * C);
-        s.xn = c.take<bf16>(rows * C); s.qkv = c.take<bf16>(rows * 3 * C); s.q = c.take<bf16>(rows * C);
-        s.kc = c.take<bf16>(rows * C); s.vc = c.take<bf16>(rows * C); s.ctx = c.take<bf16>(rows * C); s.o = c.take<bf16>(rows * C);
-        s.xn2 = c.take<bf16>(rows * C); s.pre = c.take<bf16>(rows * F); s.act = c.take<bf16>(rows * F); s.y2 = c.take<bf16>(rows * C);
-        // backward
-        s.dx = c.take<float>(rows * C); s.scr = c.take<float>(rows * C); s.part = c.take<float>((size_t)TR_COLSUM_CHUNKS * F);
-        s.colv = c.take<float>(F); s.lse = c.take<float>(BHT); s.dsum = c.take<float>(BHT);
-        s.dposi = c.take<float>(hw * C); s.ptmp = c.take<float>((size_t)d.pos_grid * w * C);
-        s.db = c.take<bf16>(rows * C); s.dact = c.take<bf16>(rows * F); s.dctx = c.take<bf16>(rows * C);
-        s.dq = c.take<bf16>(rows * C); s.dk = c.take<bf16>(rows * C); s.dv = c.take<bf16>(rows * C);
-        s.dqkv = c.take<bf16>(rows * 3 * C); s.dxn = c.take<bf16>(rows * C);
-        s.yT = c.take<bf16>(F * Rp); s.xT = c.take<bf16>(maxK * Rp); s.wT = c.take<bf16>(F * C); s.dWb = c.take<bf16>(std::max(F * C, C * KP));
-    });
-}
-
-// dynamic shared memory of the plain attention kernels (TRA_WARPS warps x floats_per_warp), opting in above 48 KB
-static int dt_attn_smem(size_t floats_per_warp, const void* fn, size_t* bytes) {
-    *bytes = (size_t)TRA_WARPS * floats_per_warp * 4;
-    if (*bytes > 200 * 1024) CAR_FAIL(CAR_ERR_UNSUPPORTED, "too many tokens for the encoder's attention kernels");
-    if (*bytes > 48 * 1024) CAR_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    return CAR_OK;
-}
-static int dt_cast(cudaStream_t st, const float* src, bf16* dst, long long n) {
-    CAR_LAUNCH(tr_cast_bf16_kernel, gsz(n), 256, 0, st, src, dst, n);
-    return CAR_OK;
-}
-// Y [rows][N] bf16 = X [rows][K] . W [N][K]^T + bias (nn.Linear on autocast's bf16 operands)
-static int dt_linear(cudaStream_t st, const bf16* X, const bf16* W, const bf16* bias, int rows, int N, int K, bf16* Y) {
-    DenseP p = dp_plain(X, K, W, K, rows, N, K, Y, N);
-    p.bias = bias;
-    return gemm(st, p);
-}
-// dX [rows][K] = bf16(dY [rows][N] . W [N][K]) through W^T as the K-major operand (as the transformer backward does)
-static int dt_dgrad(cudaStream_t st, DtBufs& s, const bf16* dY, const bf16* W, int rows, int N, int K, bf16* dX) {
-    CAR_TRY(car_fits("dt_dgrad", s.wT, (size_t)N * K));
-    CAR_LAUNCH(tr_transpose_pad_kernel, dim3((N + 31) / 32, (K + 31) / 32), dim3(32, 8), 0, st, W, (bf16*)s.wT, N, K, N);
-    return gemm(st, dp_plain(dY, N, s.wT, N, rows, K, N, dX, K));
-}
-// s.dWb [N][K] = bf16(dY^T . X), dY [rows][N], X [rows][K]: both operands transposed, the row extent zero-padded to 64
-static int dt_wgrad(cudaStream_t st, DtBufs& s, const bf16* dY, const bf16* X, int rows, int N, int K) {
-    const int Rp = (rows + 63) / 64 * 64;
-    CAR_TRY(car_fits("dt_wgrad", s.yT, (size_t)N * Rp)); CAR_TRY(car_fits("dt_wgrad", s.xT, (size_t)K * Rp));
-    CAR_TRY(car_fits("dt_wgrad", s.dWb, (size_t)N * K));
-    CAR_LAUNCH(tr_transpose_pad_kernel, dim3(Rp / 32, (N + 31) / 32), dim3(32, 8), 0, st, dY, (bf16*)s.yT, rows, N, Rp);
-    CAR_LAUNCH(tr_transpose_pad_kernel, dim3(Rp / 32, (K + 31) / 32), dim3(32, 8), 0, st, X, (bf16*)s.xT, rows, K, Rp);
-    return gemm(st, dp_plain(s.yT, Rp, s.xT, Rp, N, K, Rp, (bf16*)s.dWb, K));
-}
-// dst[k] = sum_r src[r][k] (fp32 or bf16 rows, deterministic two-pass column sum)
-template <typename T> static int dt_colsum(cudaStream_t st, DtBufs& s, const T* src, int rows, int K, float* dst) {
-    CAR_TRY(car_fits("dt_colsum", s.part, (size_t)TR_COLSUM_CHUNKS * K));
-    CAR_LAUNCH(tr_colsum_part_kernel, dim3((K + 31) / 32, TR_COLSUM_CHUNKS), dim3(32, 8), 0, st, src, (float*)s.part, rows, K);
-    CAR_LAUNCH(tr_colsum_final_kernel, (K + 255) / 256, 256, 0, st, (const float*)s.part, dst, K);
-    return CAR_OK;
-}
-// the bias gradients of nn.Linear layers whose bf16 output gradients are the `parts` column blocks of dY [rows][parts * N]
-static int dt_bias_grad(cudaStream_t st, DtBufs& s, const bf16* dY, int rows, int N, int parts, float* const* dst) {
-    bool any = false;
-    for (int j = 0; j < parts; ++j) any = any || dst[j];
-    if (!any) return CAR_OK;
-    CAR_TRY(dt_colsum(st, s, dY, rows, parts * N, (float*)s.colv));
-    for (int j = 0; j < parts; ++j)
-        if (dst[j]) CAR_LAUNCH(dt_round_bf16_kernel, (N + 255) / 256, 256, 0, st, (const float*)s.colv + (size_t)j * N, dst[j], N);
-    return CAR_OK;
-}
-// the fp32 gradient of an autocast weight copy from s.dWb [N][ld] (columns >= K are padding)
-static int dt_weight_grad(cudaStream_t st, DtBufs& s, size_t off, int N, int K, int ld, float* dst) {
-    if (dst) CAR_LAUNCH(dt_bf16_to_f32_2d_kernel, gsz((long long)N * K), 256, 0, st, (const bf16*)s.dWb + off, ld, dst, N, K);
-    return CAR_OK;
-}
-
-extern "C" int car_dino_train_create(const CarDinoDesc* desc, const CarDinoWeights* w, void* stream, CarDinoTrain** out) {
-    if (!desc || !w || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
-    const CarDinoDesc& d = *desc;
-    if (d.dtype != CAR_F32) CAR_FAIL(CAR_ERR_UNSUPPORTED, "the trainable encoder takes the fp32 master weights (bf16 autocast is applied inside)");
-    if (d.hidden <= 0 || d.hidden % 64 || d.heads * 64 != d.hidden) CAR_FAIL(CAR_ERR_UNSUPPORTED, "head_dim must be 64");
-    if (d.patch != 14 && d.patch != 16) CAR_FAIL(CAR_ERR_UNSUPPORTED, "patch size must be 14 (DINOv2) or 16 (ViT-S/16)");
-    if (d.layers <= 0 || d.pos_grid <= 0 || (d.resize_mode != 0 && d.resize_mode != 1)) CAR_FAIL(CAR_ERR_ARG, "bad layers, pos_grid or resize_mode");
-    if (!w->cls_token || !w->pos_emb || !w->patch_w || !w->patch_b || !w->ln_w || !w->ln_b) CAR_FAIL(CAR_ERR_ARG, "null weight");
-    const void* const* arrays[] = {w->n1_w, w->n1_b, w->q_w, w->q_b, w->k_w, w->k_b, w->v_w, w->v_b, w->o_w, w->o_b, w->n2_w, w->n2_b,
-                                   w->fc1_w, w->fc1_b, w->fc2_w, w->fc2_b};
-    for (const void* const* a : arrays) {
-        if (!a) CAR_FAIL(CAR_ERR_ARG, "null weight array");
-        for (int l = 0; l < d.layers; ++l) if (!a[l]) CAR_FAIL(CAR_ERR_ARG, "null weight");
-    }
-    if ((w->ls1 == nullptr) != (w->ls2 == nullptr)) CAR_FAIL(CAR_ERR_ARG, "ls1 and ls2 go together (both NULL: no LayerScale, ViT)");
-    for (int l = 0; w->ls1 && l < d.layers; ++l) if (!w->ls1[l] || !w->ls2[l]) CAR_FAIL(CAR_ERR_ARG, "null weight");
-    (void)stream;
-    CarDinoTrain* m = new CarDinoTrain();
-    m->d = d;
-    const size_t C = d.hidden;
-    m->kpatch = 3 * d.patch * d.patch;
-    m->kpad = (m->kpatch + 31) & ~31;
-    m->cls = (const float*)w->cls_token; m->pos = (const float*)w->pos_emb; m->patch_w = (const float*)w->patch_w;
-    m->patch_b = (const float*)w->patch_b; m->ln_w = (const float*)w->ln_w; m->ln_b = (const float*)w->ln_b;
-    int r = m->alloc(&m->w_patch, C * m->kpad * 2);
-    if (r == CAR_OK) r = m->alloc(&m->b_patch, C * 2);
-    m->L.resize(d.layers);
-    for (int l = 0; l < d.layers && r == CAR_OK; ++l) {
-        CarDinoTrain::Layer& Ly = m->L[l];
-        auto f = [&](const void* const* a) { return a ? (const float*)a[l] : nullptr; };
-        Ly.n1w = f(w->n1_w); Ly.n1b = f(w->n1_b); Ly.qw = f(w->q_w); Ly.qb = f(w->q_b); Ly.kw = f(w->k_w); Ly.kb = f(w->k_b);
-        Ly.vw = f(w->v_w); Ly.vb = f(w->v_b); Ly.ow = f(w->o_w); Ly.ob = f(w->o_b); Ly.ls1 = f(w->ls1); Ly.n2w = f(w->n2_w);
-        Ly.n2b = f(w->n2_b); Ly.f1w = f(w->fc1_w); Ly.f1b = f(w->fc1_b); Ly.f2w = f(w->fc2_w); Ly.f2b = f(w->fc2_b); Ly.ls2 = f(w->ls2);
-        r = m->alloc(&Ly.w_qkv, 3 * C * C * 2);
-        if (r == CAR_OK) r = m->alloc(&Ly.b_qkv, 3 * C * 2);
-        if (r == CAR_OK) r = m->alloc(&Ly.w_o, C * C * 2);
-        if (r == CAR_OK) r = m->alloc(&Ly.b_o, C * 2);
-        if (r == CAR_OK) r = m->alloc(&Ly.w_fc1, 4 * C * C * 2);
-        if (r == CAR_OK) r = m->alloc(&Ly.b_fc1, 4 * C * 2);
-        if (r == CAR_OK) r = m->alloc(&Ly.w_fc2, 4 * C * C * 2);
-        if (r == CAR_OK) r = m->alloc(&Ly.b_fc2, C * 2);
-    }
-    if (r != CAR_OK) { delete m; return r; }
-    *out = m;
-    return CAR_OK;
-}
-
-extern "C" int car_dino_train_destroy(CarDinoTrain* m) {
-    delete m;
-    return CAR_OK;
-}
-
-// One encoder block (Dinov2Layer.forward / ViTLayer.forward) on the fp32 stream x [B*Tn][C].  for_bwd: the backward's recompute —
-// stops after fc2, before the second residual add (x then holds the stream between the two halves).
-static int dt_block(CarDinoTrain* m, cudaStream_t st, DtBufs& s, int l, int B, int Tn, float* x, bool for_bwd) {
-    const CarDinoDesc& d = m->d;
-    const CarDinoTrain::Layer& Ly = m->L[l];
-    const int C = d.hidden, F = 4 * C, H = d.heads, rows = B * Tn;
-    size_t smem = 0;
-    CAR_TRY(dt_attn_smem((size_t)Tn, (const void*)tr_attention_kernel, &smem));
-    CAR_LAUNCH(dt_layernorm_kernel, rows, 128, 0, st, (const float*)x, Ly.n1w, Ly.n1b, (bf16*)s.xn, (float*)nullptr, C, d.eps, Tn, Tn, 0);
-    CAR_TRY(dt_linear(st, s.xn, Ly.w_qkv, Ly.b_qkv, rows, 3 * C, C, s.qkv));
-    CAR_LAUNCH(rope_kv_write_kernel, sm_count() * 8, 256, 0, st, (const bf16*)s.qkv, (const float*)nullptr, (bf16*)s.q, (bf16*)s.kc, (bf16*)s.vc,
-               rows, Tn, C, H, Tn);
-    CAR_LAUNCH(tr_attention_kernel, (unsigned)(((long long)B * H * Tn + TRA_WARPS - 1) / TRA_WARPS), TRA_WARPS * 32, smem, st, (const bf16*)s.q,
-               (const bf16*)s.kc, (const bf16*)s.vc, (const unsigned char*)nullptr, B, H, Tn, (bf16*)s.ctx, 0);
-    CAR_TRY(dt_linear(st, s.ctx, Ly.w_o, Ly.b_o, rows, C, C, s.o));
-    CAR_LAUNCH(dt_layerscale_add_kernel, gsz((long long)rows * C), 256, 0, st, x, (const bf16*)s.o, Ly.ls1, (long long)rows * C, C);
-    CAR_LAUNCH(dt_layernorm_kernel, rows, 128, 0, st, (const float*)x, Ly.n2w, Ly.n2b, (bf16*)s.xn2, (float*)nullptr, C, d.eps, Tn, Tn, 0);
-    CAR_TRY(dt_linear(st, s.xn2, Ly.w_fc1, Ly.b_fc1, rows, F, C, s.pre));
-    CAR_LAUNCH(dt_gelu_erf_kernel, gsz((long long)rows * F), 256, 0, st, (const bf16*)s.pre, (bf16*)s.act, (long long)rows * F);
-    CAR_TRY(dt_linear(st, s.act, Ly.w_fc2, Ly.b_fc2, rows, C, F, s.y2));
-    if (!for_bwd) CAR_LAUNCH(dt_layerscale_add_kernel, gsz((long long)rows * C), 256, 0, st, x, (const bf16*)s.y2, Ly.ls2, (long long)rows * C, C);
-    return CAR_OK;
-}
-
-// image fp32 [B,3,H,W] -> feat fp32 [B, (H/16)(W/16), hidden] (last_hidden_state without the CLS row)
-extern "C" int car_dino_train_forward(CarDinoTrain* m, const float* image, int32_t B, int32_t H, int32_t W, float* feat, void* stream) {
-    if (!m || !image || !feat) CAR_FAIL(CAR_ERR_ARG, "null argument");
-    if (B <= 0 || H <= 0 || W <= 0 || H % 16 || W % 16) CAR_FAIL(CAR_ERR_ARG, "B must be positive, H and W positive multiples of 16");
-    cudaStream_t st = (cudaStream_t)stream;
-    const CarDinoDesc& d = m->d;
-    const int C = d.hidden, F = 4 * C, h = H / 16, w = W / 16, hw = h * w, Tn = hw + 1, rows = B * Tn, KP = m->kpad;
-    m->fwd_ok = false;
-    DtBufs s;
-    CAR_TRY(dt_carve(m, B, h, w, s));
-    // 0. autocast: bf16 copies of the patch projection and of every nn.Linear (weights and biases), re-cast every forward
-    CAR_LAUNCH(dt_cast_pad_kernel, gsz((long long)C * KP), 256, 0, st, m->patch_w, m->w_patch, C, m->kpatch, KP);
-    CAR_TRY(dt_cast(st, m->patch_b, m->b_patch, C));
-    const long long CC = (long long)C * C;
-    for (const CarDinoTrain::Layer& Ly : m->L) {
-        CAR_TRY(dt_cast(st, Ly.qw, Ly.w_qkv, CC)); CAR_TRY(dt_cast(st, Ly.kw, Ly.w_qkv + CC, CC)); CAR_TRY(dt_cast(st, Ly.vw, Ly.w_qkv + 2 * CC, CC));
-        CAR_TRY(dt_cast(st, Ly.qb, Ly.b_qkv, C)); CAR_TRY(dt_cast(st, Ly.kb, Ly.b_qkv + C, C)); CAR_TRY(dt_cast(st, Ly.vb, Ly.b_qkv + 2 * C, C));
-        CAR_TRY(dt_cast(st, Ly.ow, Ly.w_o, CC)); CAR_TRY(dt_cast(st, Ly.ob, Ly.b_o, C));
-        CAR_TRY(dt_cast(st, Ly.f1w, Ly.w_fc1, 4 * CC)); CAR_TRY(dt_cast(st, Ly.f1b, Ly.b_fc1, F));
-        CAR_TRY(dt_cast(st, Ly.f2w, Ly.w_fc2, 4 * CC)); CAR_TRY(dt_cast(st, Ly.f2b, Ly.b_fc2, C));
-    }
-    // 1. resize (fp32) + patchify, patch projection on bf16 operands (dinov2_adapter.py:16-24, Dinov2PatchEmbeddings)
-    CAR_LAUNCH((resize_patchify_kernel<float>), gsz((long long)B * hw * KP), 256, 0, st, image, (bf16*)s.patches, B, H, W, h, w, KP, d.resize_mode, d.patch);
-    {
-        DenseP p = dp_plain(s.patches, KP, m->w_patch, KP, B * hw, C, KP, (bf16*)s.ptok, C);
-        p.bias = m->b_patch;
-        CAR_TRY(gemm(st, p));
-    }
-    // 2. CLS row + fp32 bicubic position embeddings -> the fp32 stream hs[0]
-    CAR_LAUNCH((pos_embed_interp_kernel<float, float>), gsz((long long)hw * C), 256, 0, st, m->pos, (float*)s.posi, d.pos_grid, h, w, C);
-    CAR_LAUNCH(dt_assemble_kernel, gsz((long long)rows * C), 256, 0, st, (const bf16*)s.ptok, m->cls, m->pos, (const float*)s.posi, (float*)s.hs, B, hw, C);
-    // 3. blocks: hs[l + 1] = block_l(hs[l])
-    const size_t RC = (size_t)rows * C;
-    for (int l = 0; l < d.layers; ++l) {
-        float* x = s.hs + (size_t)(l + 1) * RC;
-        CAR_CUDA(cudaMemcpyAsync(x, s.hs + (size_t)l * RC, RC * 4, cudaMemcpyDeviceToDevice, st));
-        CAR_TRY(dt_block(m, st, s, l, B, Tn, x, false));
-    }
-    // 4. final LayerNorm on the patch rows (dinov2_adapter.py:29 drops the CLS row)
-    CAR_LAUNCH(dt_layernorm_kernel, B * hw, 128, 0, st, (const float*)(s.hs + (size_t)d.layers * RC), m->ln_w, m->ln_b, (bf16*)nullptr, feat, C, d.eps,
-               hw, Tn, 1);
-    m->fB = B; m->fH = h; m->fW = w;
-    m->fwd_ok = true;
-    return CAR_OK;
-}
-
-// Backward of the last car_dino_train_forward on this handle from d_feat (fp32, the forward's feat shape): writes d loss / d parameter
-// (fp32, OVERWRITTEN) through the non-NULL pointers of `g` (a CarDinoWeights whose fields point at gradient buffers of the
-// parameters' shapes; NULL skips a tensor).
-extern "C" int car_dino_train_backward(CarDinoTrain* m, const float* d_feat, const CarDinoWeights* g, void* stream) {
-    if (!m || !d_feat || !g) CAR_FAIL(CAR_ERR_ARG, "null argument");
-    if (!m->fwd_ok) CAR_FAIL(CAR_ERR_STATE, "car_dino_train_backward needs a preceding car_dino_train_forward on the same handle");
-    cudaStream_t st = (cudaStream_t)stream;
-    const CarDinoDesc& d = m->d;
-    const int B = m->fB, h = m->fH, w = m->fW, C = d.hidden, F = 4 * C, H = d.heads, hw = h * w, Tn = hw + 1, rows = B * Tn, G = d.pos_grid;
-    const size_t RC = (size_t)rows * C, CC = (size_t)C * C;
-    DtBufs s;
-    CAR_TRY(dt_carve(m, B, h, w, s));
-    m->fwd_ok = false;                                          // the recompute below overwrites the forward's buffers
-    size_t smem_q = 0, smem_kv = 0;
-    CAR_TRY(dt_attn_smem((size_t)2 * Tn + 128, (const void*)tr_attn_bwd_q_kernel, &smem_q));
-    CAR_TRY(dt_attn_smem((size_t)2 * Tn + 128, (const void*)tr_attn_bwd_kv_kernel, &smem_kv));
-    const unsigned att_grid = (unsigned)(((long long)B * H * Tn + TRA_WARPS - 1) / TRA_WARPS);
-    auto at = [](const void* const* a, int l) { return a ? (float*)a[l] : (float*)nullptr; };
-    // final LayerNorm
-    CAR_CUDA(cudaMemsetAsync(s.dx, 0, RC * 4, st));
-    CAR_LAUNCH(dt_layernorm_bwd_kernel<float>, B * hw, 128, 0, st, (const float*)(s.hs + (size_t)d.layers * RC), m->ln_w, d_feat, (float*)s.dx,
-               (float*)s.scr, C, d.eps, hw, Tn, 1);
-    if (g->ln_w) CAR_TRY(dt_colsum(st, s, (const float*)s.scr, B * hw, C, (float*)g->ln_w));
-    if (g->ln_b) CAR_TRY(dt_colsum(st, s, d_feat, B * hw, C, (float*)g->ln_b));
-    for (int l = d.layers - 1; l >= 0; --l) {
-        const CarDinoTrain::Layer& Ly = m->L[l];
-        const float* x0 = s.hs + (size_t)l * RC;
-        CAR_CUDA(cudaMemcpyAsync(s.xm, x0, RC * 4, cudaMemcpyDeviceToDevice, st));
-        CAR_TRY(dt_block(m, st, s, l, B, Tn, s.xm, true));
-        // feed-forward half: x_out = x_mid + ls2 * fc2(gelu(fc1(norm2(x_mid))))
-        CAR_LAUNCH(dt_layerscale_bwd_kernel, gsz((long long)RC), 256, 0, st, (const float*)s.dx, (const bf16*)s.y2, Ly.ls2, (bf16*)s.db,
-                   at(g->ls2, l) ? (float*)s.scr : (float*)nullptr, (long long)RC, C);
-        if (at(g->ls2, l)) CAR_TRY(dt_colsum(st, s, (const float*)s.scr, rows, C, at(g->ls2, l)));
-        if (at(g->fc2_w, l)) { CAR_TRY(dt_wgrad(st, s, s.db, s.act, rows, C, F)); CAR_TRY(dt_weight_grad(st, s, 0, C, F, F, at(g->fc2_w, l))); }
-        { float* b[1] = {at(g->fc2_b, l)}; CAR_TRY(dt_bias_grad(st, s, s.db, rows, C, 1, b)); }
-        CAR_TRY(dt_dgrad(st, s, s.db, Ly.w_fc2, rows, C, F, s.dact));
-        CAR_LAUNCH(dt_gelu_erf_bwd_kernel, gsz((long long)rows * F), 256, 0, st, (const bf16*)s.pre, (const bf16*)s.dact, (bf16*)s.dact, (long long)rows * F);
-        if (at(g->fc1_w, l)) { CAR_TRY(dt_wgrad(st, s, s.dact, s.xn2, rows, F, C)); CAR_TRY(dt_weight_grad(st, s, 0, F, C, C, at(g->fc1_w, l))); }
-        { float* b[1] = {at(g->fc1_b, l)}; CAR_TRY(dt_bias_grad(st, s, s.dact, rows, F, 1, b)); }
-        CAR_TRY(dt_dgrad(st, s, s.dact, Ly.w_fc1, rows, F, C, s.dxn));
-        CAR_LAUNCH(dt_layernorm_bwd_kernel<bf16>, rows, 128, 0, st, (const float*)s.xm, Ly.n2w, (const bf16*)s.dxn, (float*)s.dx, (float*)s.scr, C, d.eps,
-                   Tn, Tn, 0);
-        if (at(g->n2_w, l)) CAR_TRY(dt_colsum(st, s, (const float*)s.scr, rows, C, at(g->n2_w, l)));
-        if (at(g->n2_b, l)) CAR_TRY(dt_colsum(st, s, (const bf16*)s.dxn, rows, C, at(g->n2_b, l)));
-        // attention half: x_mid = x0 + ls1 * o(sdpa(q, k, v)(norm1(x0)))
-        CAR_LAUNCH(dt_layerscale_bwd_kernel, gsz((long long)RC), 256, 0, st, (const float*)s.dx, (const bf16*)s.o, Ly.ls1, (bf16*)s.db,
-                   at(g->ls1, l) ? (float*)s.scr : (float*)nullptr, (long long)RC, C);
-        if (at(g->ls1, l)) CAR_TRY(dt_colsum(st, s, (const float*)s.scr, rows, C, at(g->ls1, l)));
-        if (at(g->o_w, l)) { CAR_TRY(dt_wgrad(st, s, s.db, s.ctx, rows, C, C)); CAR_TRY(dt_weight_grad(st, s, 0, C, C, C, at(g->o_w, l))); }
-        { float* b[1] = {at(g->o_b, l)}; CAR_TRY(dt_bias_grad(st, s, s.db, rows, C, 1, b)); }
-        CAR_TRY(dt_dgrad(st, s, s.db, Ly.w_o, rows, C, C, s.dctx));
-        CAR_LAUNCH(tr_attn_bwd_q_kernel, att_grid, TRA_WARPS * 32, smem_q, st, (const bf16*)s.q, (const bf16*)s.kc, (const bf16*)s.vc,
-                   (const unsigned char*)nullptr, (const bf16*)s.dctx, B, H, Tn, (float*)s.lse, (float*)s.dsum, (bf16*)s.dq, 0);
-        CAR_LAUNCH(tr_attn_bwd_kv_kernel, att_grid, TRA_WARPS * 32, smem_kv, st, (const bf16*)s.q, (const bf16*)s.kc, (const bf16*)s.vc,
-                   (const unsigned char*)nullptr, (const bf16*)s.dctx, (const float*)s.lse, (const float*)s.dsum, B, H, Tn, (bf16*)s.dk, (bf16*)s.dv, 0);
-        CAR_LAUNCH(tr_rope_bwd_kernel, sm_count() * 8, 256, 0, st, (const bf16*)s.dq, (const bf16*)s.dk, (const bf16*)s.dv, (const float*)nullptr,
-                   (bf16*)s.dqkv, rows, Tn, C, H, Tn);
-        if (at(g->q_w, l) || at(g->k_w, l) || at(g->v_w, l)) {
-            CAR_TRY(dt_wgrad(st, s, s.dqkv, s.xn, rows, 3 * C, C));
-            CAR_TRY(dt_weight_grad(st, s, 0, C, C, C, at(g->q_w, l)));
-            CAR_TRY(dt_weight_grad(st, s, CC, C, C, C, at(g->k_w, l)));
-            CAR_TRY(dt_weight_grad(st, s, 2 * CC, C, C, C, at(g->v_w, l)));
-        }
-        { float* b[3] = {at(g->q_b, l), at(g->k_b, l), at(g->v_b, l)}; CAR_TRY(dt_bias_grad(st, s, s.dqkv, rows, C, 3, b)); }
-        CAR_TRY(dt_dgrad(st, s, s.dqkv, Ly.w_qkv, rows, 3 * C, C, s.dxn));
-        CAR_LAUNCH(dt_layernorm_bwd_kernel<bf16>, rows, 128, 0, st, x0, Ly.n1w, (const bf16*)s.dxn, (float*)s.dx, (float*)s.scr, C, d.eps, Tn, Tn, 0);
-        if (at(g->n1_w, l)) CAR_TRY(dt_colsum(st, s, (const float*)s.scr, rows, C, at(g->n1_w, l)));
-        if (at(g->n1_b, l)) CAR_TRY(dt_colsum(st, s, (const bf16*)s.dxn, rows, C, at(g->n1_b, l)));
-    }
-    // embeddings: CLS row and position table (fp32), patch tokens (bf16 gradient of the cast) -> patch projection
-    float* dpos = (float*)g->pos_emb;
-    CAR_LAUNCH(dt_embed_bwd_kernel, gsz((long long)Tn * C), 256, 0, st, (const float*)s.dx, (float*)g->cls_token, dpos,
-               dpos ? (float*)s.dposi : (float*)nullptr, B, Tn, C);
-    if (dpos) {
-        CAR_LAUNCH(dt_cubic_t_kernel, gsz((long long)G * w * C), 256, 0, st, (const float*)s.dposi, (float*)s.ptmp, G, h, 1, w * C);
-        CAR_LAUNCH(dt_cubic_t_kernel, gsz((long long)G * G * C), 256, 0, st, (const float*)s.ptmp, dpos + C, G, w, G, C);
-    }
-    if (g->patch_w || g->patch_b) {
-        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)B * hw * C), 256, 0, st, (const float*)s.dx, (bf16*)s.db, B, hw, Tn, 1, C);
-        if (g->patch_w) {
-            CAR_TRY(dt_wgrad(st, s, s.db, s.patches, B * hw, C, m->kpad));
-            CAR_TRY(dt_weight_grad(st, s, 0, C, m->kpatch, m->kpad, (float*)g->patch_w));
-        }
-        float* b[1] = {(float*)g->patch_b};
-        CAR_TRY(dt_bias_grad(st, s, s.db, B * hw, C, 1, b));
-    }
-    return CAR_OK;
 }
 
 // =========================================================================================================

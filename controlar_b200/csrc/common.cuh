@@ -191,6 +191,26 @@ __device__ __forceinline__ float warp_max(float v) {
     return v;
 }
 
+// ---- block reduce helpers (blockDim.x multiple of 32, <= 1024)
+__device__ __forceinline__ float block_sum(float v, float* red) {
+    v = warp_sum(v);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float s = 0.f;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += red[i];
+    __syncthreads();
+    return s;
+}
+__device__ __forceinline__ float block_max(float v, float* red) {
+    v = warp_max(v);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float s = red[0];
+    for (int i = 1; i < (int)(blockDim.x >> 5); ++i) s = fmaxf(s, red[i]);
+    __syncthreads();
+    return s;
+}
+
 // streaming 128-bit load that does not allocate in L1 (weights / KV are read once per step)
 __device__ __forceinline__ uint4 ldg_stream(const void* p) {
     uint4 r;

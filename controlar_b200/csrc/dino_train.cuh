@@ -5,10 +5,10 @@
 // nn.Linear take bf16 operands and return bf16; attention and GELU-erf run on bf16 tensors.  The inference encoder of
 // car_dino_forward keeps a bf16 stream instead and is a different arithmetic.
 // The GEMMs, the attention kernels, the head split / merge, the transposes and the column sums are the transformer training
-// path's (train.cuh, train_bwd.cuh, misc.cuh); what is here is the encoder-only glue.
+// path's (train.cuh, train_bwd.cuh, misc.h); what is here is the encoder-only glue.  dt_cubic_t_kernel takes the bicubic weights
+// cubic1 / cubic2 of patch_embed.cuh, which car_train.cu includes first.
 #pragma once
 #include "common.cuh"
-#include "vision.cuh"
 
 // nn.LayerNorm on the fp32 stream (fp32 statistics, eps inside the sqrt, fp32 affine).  Output row r reads stream row
 // (r / nrows) * S + row0 + r % nrows; writes yb = bf16(y) (the cast in front of the next nn.Linear) or, when yb is null, yf = y.
@@ -156,12 +156,6 @@ __global__ void dt_cast_pad_kernel(const float* __restrict__ src, bf16* __restri
         const long long r = i / ld;
         dst[i] = __float2bfloat16_rn(c < cols ? src[r * cols + c] : 0.f);
     }
-}
-// dst [rows][cols] fp32 = src [rows][lds] bf16 (the weight gradient of an autocast copy, padding columns dropped)
-__global__ void dt_bf16_to_f32_2d_kernel(const bf16* __restrict__ src, int lds, float* __restrict__ dst, int rows, int cols) {
-    const long long total = (long long)rows * cols;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
-        dst[i] = __bfloat162float(src[(i / cols) * lds + i % cols]);
 }
 // dst = float(bf16(src)): the bias gradient of an nn.Linear under autocast is the bf16 column sum of its bf16 output gradient
 __global__ void dt_round_bf16_kernel(const float* __restrict__ src, float* __restrict__ dst, int n) {

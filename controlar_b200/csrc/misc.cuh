@@ -1,6 +1,7 @@
 // misc.cuh — weight packing and the small gather / element-wise kernels around the GEMMs.
 #pragma once
 #include "common.cuh"
+#include "misc.h"
 
 // Pack nn.Linear weight W[N][K] (bf16, row-major) into the fragment-streaming layout of gemm_skinny.cuh:
 // chunk (nb, s) = 8 rows x 32 k, stored as 32 lanes x 16 B with lane (g = l>>2, t = l&3) holding

@@ -25,10 +25,12 @@ __global__ void tr_transpose_pad_kernel(const bf16* __restrict__ src, bf16* __re
     }
 }
 
-// the cast at the end of a weight-gradient GEMM: autograd's bf16 gradient of the autocast copy -> fp32 .grad of the master
-__global__ void tr_bf16_to_f32_kernel(const bf16* __restrict__ src, float* __restrict__ dst, long long n) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        dst[i] = __bfloat162float(src[i]);
+// the cast at the end of a weight-gradient GEMM: autograd's bf16 gradient of the autocast copy -> fp32 .grad of the master.
+// dst [rows][cols] fp32 = src [rows][lds] bf16 (columns >= cols of src are padding, dropped)
+__global__ void tr_bf16_to_f32_2d_kernel(const bf16* __restrict__ src, int lds, float* __restrict__ dst, int rows, int cols) {
+    const long long total = (long long)rows * cols;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
+        dst[i] = __bfloat162float(src[(i / cols) * lds + i % cols]);
 }
 
 // out[b][j][:] = bf16(h[b][row0 + j][:]) — the bf16 gradient a bf16 branch receives from the fp32 stream (fp32 + bf16 add)
@@ -371,8 +373,4 @@ __global__ void tr_embed_grad_kernel(const float* __restrict__ dh, const int* __
     const float* src = dh + ((size_t)b * S + row0 + j) * d;
     float* dst = grad + (size_t)id * d;
     for (int k = threadIdx.x; k < d; k += blockDim.x) atomicAdd(dst + k, src[k]);
-}
-
-__global__ void tr_scale_f32_kernel(float* __restrict__ p, float s, long long n) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) p[i] *= s;
 }

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE — the hand-derived backward of the teacher-forced training forward (SURVEY.md §8 row f1), written out
-op by op in the decomposition `car_train_backward` (controlar_b200/csrc/car_api.cu, train_bwd.cuh) uses: layer-wise recompute
+op by op in the decomposition `car_train_backward` (controlar_b200/csrc/car_train.cu, train_bwd.cuh) uses: layer-wise recompute
 from the saved fp32 residual stream, bf16 gradients wherever autograd under bf16 autocast produces bf16 ones (every nn.Linear
 operand / result, SDPA, GELU / SiLU), fp32 on the residual stream, RMSNorm and the loss.  Never shipped or called by the product.
 
