@@ -1,7 +1,7 @@
 """HED soft-edge control-map detector on the GPU — same surface as the reference's `condition/hed.py`: `ControlNetHED_Apache2` (an
 nn.Module with the reference's state-dict keys: `norm`, `block{1..5}.convs.{i}.{weight,bias}`, `block{k}.projection.{weight,bias}`)
 and `HEDdetector()(input_image)` (tensor (B, C, H, W) in 0..255 -> tensor (B, H, W) in [0, 255]).  The reference runs fp32; the
-13 ReLU convolutions here run on the fp32-grade split-bf16 tensor-core path (csrc/vision.cuh "x3"), pooling / projections / resize /
+13 ReLU convolutions here run on the fp32-grade split-bf16 tensor-core path (csrc/split3.cuh "x3"), pooling / projections / resize /
 sigmoid in fp32 (csrc/frontend.cuh).  Weights come from the caller (`load_state_dict`) — there is no network to download
 ControlNetHED.pth from; `HEDdetector(modelpath=...)` loads a local copy like the reference does."""
 from __future__ import annotations

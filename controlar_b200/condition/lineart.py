@@ -3,7 +3,7 @@
 state-dict keys (`model0.1`, `model1.{0,3}`, `model2.{0,1,2}.conv_block.{1,5}`, `model3.{0,3}`, `model4.1`, each `.weight` / `.bias`),
 so `load_state_dict(torch.load('condition/ckpts/model.pth'))` of the released checkpoint works unchanged.  `forward(x)` takes
 (B, 3, H, W) pixels in 0..255 and returns (B, 1, Ho, Wo) in [0, 1], Ho = 4 * ceil(ceil(H / 2) / 2) (likewise Wo).  The reference runs
-fp32; here every convolution but the head runs on the fp32-grade split-bf16 tensor-core path (csrc/vision.cuh "x3", csrc/lineart.cuh)
+fp32; here every convolution but the head runs on the fp32-grade split-bf16 tensor-core path (csrc/split3.cuh "x3", csrc/lineart.cuh)
 with instance norm, padding and the head in fp32.  No autograd: the reference calls it under no_grad."""
 from __future__ import annotations
 

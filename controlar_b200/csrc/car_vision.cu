@@ -17,6 +17,10 @@ static int launch_on(cudaStream_t st, void (*kernel)(KArgs...), unsigned grid, u
     return CAR_OK;
 }
 
+// A split-bf16 weight of the fp32-grade networks (split3.cuh): W3 bf16 [n][kh][kw][cin3] = [ w_hi | w_hi | w_lo ] per tap, cin3 =
+// 3 x the padded input channels (the channels per pixel of its S3 source), and the fp32 bias [n] (null: none)
+struct X3W { bf16* w; const float* b; int n, cin3, kh, kw; };
+
 // Reader of the flat tensor list a create call takes (device pointers in state-dict order, fp32), copying and packing each tensor
 // into memory the handle owns.  The list comes from the caller: the constructor refuses a null entry before any CUDA call, and every
 // read is bounds-checked.  The first error sticks — later calls allocate, copy and launch nothing, and return null — and finish()
@@ -75,14 +79,19 @@ struct TensorReader {
         if (ok()) cuda(cudaMemsetAsync(p, 0, (size_t)count * 4, st), "memset");
         return p;
     }
-    // split-bf16 weight of the x3 GEMMs: [cout][cin][k][k] -> [cout][k][k][3 cin_pad] = [ w_hi | w_hi | w_lo ] per tap
-    bf16* x3(const float* src, int cout, int cin, int k, int cin_pad) {
-        const long long n3 = (long long)cout * k * k * cin_pad;
-        bf16* w3 = (bf16*)alloc((size_t)n3 * 3 * 2);
-        pack(conv_weight_pack_x3_kernel, n3, src, w3, cout, cin, k, k, cin_pad);
-        return w3;
+    // split-bf16 weight: fp32 [n][cin][k][k] at src -> W3 [n][k][k][3 cin_pad], with the fp32 bias b
+    X3W x3(const float* src, int n, int cin, int k, int cin_pad, const float* b) {
+        const long long n3 = (long long)n * k * k * cin_pad;
+        X3W w{(bf16*)alloc((size_t)n3 * 3 * 2), b, n, 3 * cin_pad, k, k};
+        pack(conv_weight_pack_x3_kernel, n3, src, w.w, n, cin, k, k, cin_pad);
+        return w;
     }
-    bf16* x3(int cout, int cin, int k, int cin_pad) { return x3(next(), cout, cin, k, cin_pad); }
+    // the next tensor as a split-bf16 weight, then (bias) the one after it as its bias
+    X3W x3(int n, int cin, int k, int cin_pad, bool bias = true) {
+        X3W w = x3(next(), n, cin, k, cin_pad, nullptr);
+        if (bias) w.b = f32(n);
+        return w;
+    }
     // the create's last step: the whole list was read and nothing failed
     int finish() {
         if (ok() && i != n) fail(CAR_ERR_ARG, "tensor list length does not match the architecture");
@@ -278,10 +287,15 @@ extern "C" int car_dino_forward(CarDino* m, const void* image, int32_t B, int32_
 // =========================================================================================================
 // VQGAN tokenizer
 // =========================================================================================================
-struct ConvW { bf16* w; bf16* b; int cin, cin_pad, cout, k; bf16* w3; float* bf; };     // w3 / bf: split-bf16 weights + fp32 bias (encoder)
-struct NormW { bf16 *w, *b; int c; float *wf, *bff; };                                   // wf / bff: fp32 copies (encoder)
-struct ResW { NormW n1, n2; ConvW c1, c2, nin; bool has_nin; };
-struct AttnW { NormW n; ConvW q, k, v, o; };
+struct ConvW { bf16* w; bf16* b; int cin, cin_pad, cout, k; };
+struct NormW { bf16 *w, *b; int c; };
+struct NormF { float *w, *b; };                                          // fp32 affine of a norm in the fp32-grade networks
+template <typename Conv, typename Norm> struct ResT { Norm n1, n2; Conv c1, c2, nin; bool has_nin; };
+template <typename Conv, typename Norm> struct AttnT { Norm n; Conv q, k, v, o; };
+using ResW = ResT<ConvW, NormW>;                                         // decoder: bf16
+using AttnW = AttnT<ConvW, NormW>;
+using ResX3 = ResT<X3W, NormF>;                                          // encoder: fp32 grade
+using AttnX3 = AttnT<X3W, NormF>;
 
 struct CarVQ : CarOwned {
     CarVQDesc d;
@@ -291,9 +305,9 @@ struct CarVQ : CarOwned {
     ResW d_mid0, d_mid2; AttnW d_mid1;
     std::vector<std::vector<ResW>> d_res; std::vector<std::vector<AttnW>> d_attn; std::vector<ConvW> d_up; std::vector<bool> d_has_up;
     // encoder
-    ConvW quant_conv, e_conv_in, e_conv_out; NormW e_norm_out;
-    ResW e_mid0, e_mid2; AttnW e_mid1;
-    std::vector<std::vector<ResW>> e_res; std::vector<std::vector<AttnW>> e_attn; std::vector<ConvW> e_down; std::vector<bool> e_has_down;
+    X3W quant_conv, e_conv_in, e_conv_out; NormF e_norm_out;
+    ResX3 e_mid0, e_mid2; AttnX3 e_mid1;
+    std::vector<std::vector<ResX3>> e_res; std::vector<std::vector<AttnX3>> e_attn; std::vector<X3W> e_down; std::vector<bool> e_has_down;
 };
 
 static bf16* take_bf16(TensorReader& tc, const float* src, long long n) {
@@ -301,38 +315,32 @@ static bf16* take_bf16(TensorReader& tc, const float* src, long long n) {
     tc.pack(cast_to_bf16_kernel<float>, n, src, p, n);
     return p;
 }
-static void take_conv(TensorReader& tc, int cout, int cin, int k, ConvW* c, bool x3 = false) {
-    c->cin = cin; c->cout = cout; c->k = k; c->cin_pad = (cin + 31) & ~31; c->w3 = nullptr; c->bf = nullptr;
+static void take_conv(TensorReader& tc, int cout, int cin, int k, ConvW* c) {
+    c->cin = cin; c->cout = cout; c->k = k; c->cin_pad = (cin + 31) & ~31;
     const float* w = tc.next();
-    const float* b = tc.next();
-    if (x3) {   // fp32-grade encoder path (vision.cuh "x3"): [w_hi | w_hi | w_lo] per tap + the fp32 bias
-        c->w3 = tc.x3(w, cout, cin, k, c->cin_pad);
-        c->bf = tc.f32(b, cout);
-    }
     const long long n = (long long)cout * k * k * c->cin_pad;
     c->w = (bf16*)tc.alloc((size_t)n * 2);
     tc.pack(conv_weight_pack_kernel<float>, n, w, c->w, cout, cin, k, k, c->cin_pad);
-    c->b = take_bf16(tc, b, cout);
+    c->b = take_bf16(tc, tc.next(), cout);
 }
-static void take_norm(TensorReader& tc, int c, NormW* nw, bool x3 = false) {
-    nw->c = c; nw->wf = nullptr; nw->bff = nullptr;
-    const float* w = tc.next();
-    const float* b = tc.next();
-    if (x3) { nw->wf = tc.f32(w, c); nw->bff = tc.f32(b, c); }
-    nw->w = take_bf16(tc, w, c);
-    nw->b = take_bf16(tc, b, c);
+static void take_conv(TensorReader& tc, int cout, int cin, int k, X3W* c) { *c = tc.x3(cout, cin, k, (cin + 31) & ~31); }
+static void take_norm(TensorReader& tc, int c, NormW* nw) {
+    nw->c = c;
+    nw->w = take_bf16(tc, tc.next(), c);
+    nw->b = take_bf16(tc, tc.next(), c);
 }
+static void take_norm(TensorReader& tc, int c, NormF* nf) { nf->w = tc.f32(c); nf->b = tc.f32(c); }
 // canonical order inside a ResnetBlock: norm1.{w,b} conv1.{w,b} norm2.{w,b} conv2.{w,b} [nin_shortcut.{w,b}]
-static void take_res(TensorReader& tc, int cin, int cout, ResW* r, bool x3 = false) {
-    take_norm(tc, cin, &r->n1, x3); take_conv(tc, cout, cin, 3, &r->c1, x3);
-    take_norm(tc, cout, &r->n2, x3); take_conv(tc, cout, cout, 3, &r->c2, x3);
+template <typename Conv, typename Norm> static void take_res(TensorReader& tc, int cin, int cout, ResT<Conv, Norm>* r) {
+    take_norm(tc, cin, &r->n1); take_conv(tc, cout, cin, 3, &r->c1);
+    take_norm(tc, cout, &r->n2); take_conv(tc, cout, cout, 3, &r->c2);
     r->has_nin = cin != cout;
-    if (r->has_nin) take_conv(tc, cout, cin, 1, &r->nin, x3);
+    if (r->has_nin) take_conv(tc, cout, cin, 1, &r->nin);
 }
 // AttnBlock: norm.{w,b} q.{w,b} k.{w,b} v.{w,b} proj_out.{w,b}
-static void take_attn(TensorReader& tc, int c, AttnW* a, bool x3 = false) {
-    take_norm(tc, c, &a->n, x3); take_conv(tc, c, c, 1, &a->q, x3); take_conv(tc, c, c, 1, &a->k, x3);
-    take_conv(tc, c, c, 1, &a->v, x3); take_conv(tc, c, c, 1, &a->o, x3);
+template <typename Conv, typename Norm> static void take_attn(TensorReader& tc, int c, AttnT<Conv, Norm>* a) {
+    take_norm(tc, c, &a->n); take_conv(tc, c, c, 1, &a->q); take_conv(tc, c, c, 1, &a->k);
+    take_conv(tc, c, c, 1, &a->v); take_conv(tc, c, c, 1, &a->o);
 }
 
 extern "C" int car_vq_create(const CarVQDesc* desc, const void* const* tensors, int32_t n_tensors, void* stream, CarVQ** out) {
@@ -344,22 +352,22 @@ extern "C" int car_vq_create(const CarVQDesc* desc, const void* const* tensors, 
     TensorReader tc(__func__, tensors, n_tensors, stream, m);
     const int ch = d.ch, nres = d.n_levels, nrb = d.num_res_blocks;
     // ---- encoder (vq_model.py:65-125)
-    take_conv(tc, ch, 3, 3, &m->e_conv_in, true);
+    take_conv(tc, ch, 3, 3, &m->e_conv_in);
     m->e_res.resize(nres); m->e_attn.resize(nres); m->e_down.resize(nres); m->e_has_down.assign(nres, false);
     int block_in = ch;
     for (int lvl = 0; lvl < nres; ++lvl) {
         block_in = ch * (lvl == 0 ? 1 : d.ch_mult[lvl - 1]);
         const int block_out = ch * d.ch_mult[lvl];
         for (int b = 0; b < nrb; ++b) {
-            ResW r; take_res(tc, block_in, block_out, &r, true); m->e_res[lvl].push_back(r);
+            ResX3 r; take_res(tc, block_in, block_out, &r); m->e_res[lvl].push_back(r);
             block_in = block_out;
-            if (lvl == nres - 1) { AttnW a; take_attn(tc, block_in, &a, true); m->e_attn[lvl].push_back(a); }
+            if (lvl == nres - 1) { AttnX3 a; take_attn(tc, block_in, &a); m->e_attn[lvl].push_back(a); }
         }
-        if (lvl != nres - 1) { take_conv(tc, block_in, block_in, 3, &m->e_down[lvl], true); m->e_has_down[lvl] = true; }
+        if (lvl != nres - 1) { take_conv(tc, block_in, block_in, 3, &m->e_down[lvl]); m->e_has_down[lvl] = true; }
     }
-    take_res(tc, block_in, block_in, &m->e_mid0, true); take_attn(tc, block_in, &m->e_mid1, true);
-    take_res(tc, block_in, block_in, &m->e_mid2, true);
-    take_norm(tc, block_in, &m->e_norm_out, true); take_conv(tc, d.z_channels, block_in, 3, &m->e_conv_out, true);
+    take_res(tc, block_in, block_in, &m->e_mid0); take_attn(tc, block_in, &m->e_mid1);
+    take_res(tc, block_in, block_in, &m->e_mid2);
+    take_norm(tc, block_in, &m->e_norm_out); take_conv(tc, d.z_channels, block_in, 3, &m->e_conv_out);
     // ---- decoder (vq_model.py:129-195)
     block_in = ch * d.ch_mult[nres - 1];
     take_conv(tc, block_in, d.z_channels, 3, &m->d_conv_in);
@@ -381,7 +389,7 @@ extern "C" int car_vq_create(const CarVQDesc* desc, const void* const* tensors, 
     const float* codebook = tc.next();
     m->codebook_n = (float*)tc.alloc((size_t)d.codebook_size * d.embed_dim * 4);
     tc.launch(codebook_normalize_kernel, (d.codebook_size + 255) / 256, 256, codebook, m->codebook_n, d.codebook_size, d.embed_dim);
-    take_conv(tc, d.embed_dim, d.z_channels, 1, &m->quant_conv, true);
+    take_conv(tc, d.embed_dim, d.z_channels, 1, &m->quant_conv);
     take_conv(tc, d.z_channels, d.embed_dim, 1, &m->post_quant);
     const int rc = tc.finish();
     if (rc != CAR_OK) { delete m; return rc; }
@@ -553,72 +561,80 @@ extern "C" int car_vq_decode(CarVQ* m, const float* quant, int32_t B, int32_t h,
     return vq_decode_impl(m, nullptr, quant, B, h, w, out, stream);
 }
 
-// ---- VQModel.encode (vq_model.py:41-46) at fp32 grade: the "x3" split-bf16 path of vision.cuh ----
+// ---- VQModel.encode (vq_model.py:41-46) at fp32 grade: the split-bf16 ("x3") path of split3.cuh ----
 // fp32 NHWC activations; every convolution = one launch of the bf16 implicit-GEMM kernel over tripled K, fp32 output / bias / residual.
 struct ActF { float* p; int B, H, W, C; long long npix() const { return (long long)B * H * W; } long long n() const { return npix() * C; } };
 struct EncScratch { Buf<bf16> t3, x3; Buf<float> h1, sc; float* stats; Buf<float> qf, kf, vf, ctx; float *S, *P; Buf<bf16> q3, k3, P3, vT3; };
 
-static int split3(cudaStream_t st, const float* x, Buf<bf16> y, long long npix, int C, int bside = 0) {
-    CAR_TRY(car_fits(__func__, y, (size_t)npix * C * 3));
-    CAR_LAUNCH(split3_kernel, gsz(npix * C), 256, 0, st, x, y, npix, C, bside);
+// fp32 rows x [M][N] -> S3 rows (mode X3_ROWS_A, X3_ROWS_A_GELU) or W3 rows (X3_ROWS_B) [M][3N]
+static int split3_rows(cudaStream_t st, const float* x, Buf<bf16> y, long long M, int N, int mode = X3_ROWS_A) {
+    CAR_TRY(car_fits(__func__, y, (size_t)M * N * 3));
+    CAR_LAUNCH(split3_rows_kernel, gsz(M * N), 256, 0, st, x, y, M, N, mode);
     return CAR_OK;
 }
-// a3: S3 activations [B][Hs][Ws][3 cin_pad]; out fp32 [B][Ho][Wo][cout] (+ fp32 residual of the same shape)
-static int conv_x3(cudaStream_t st, const ConvW& c, const bf16* a3, int B, int Hs, int Ws, int stride2, Buf<float> out, const float* resid, int Ho, int Wo,
-                   int act = ACT_NONE) {
-    if (!c.w3 || !c.bf) CAR_FAIL(CAR_ERR_STATE, "convolution has no split-bf16 weights (encoder layers only)");
-    CAR_TRY(car_fits(__func__, out, (size_t)B * Ho * Wo * c.cout));
+// image fp32 NCHW (- sub[c]) -> padded S3 NHWC frame (split3.cuh image_split3_kernel)
+static int image_split3(cudaStream_t st, const float* x, const float* sub, Buf<bf16> y, X3Image q) {
+    const long long n = (long long)q.B * (q.pt + q.H + q.pb) * (q.pl + q.W + q.pr) * q.Cpad;
+    CAR_TRY(car_fits(__func__, y, (size_t)n * 3));
+    CAR_LAUNCH(image_split3_kernel, gsz(n), 256, 0, st, x, sub, y, q);
+    return CAR_OK;
+}
+// mma.sync implicit GEMM (gemm.h A_PLAIN for a 1x1 weight, else A_CONV3x3 or, with stride2, A_CONV3x3S2): S3 activations
+// [B][Hs][Ws][w.cin3] -> out fp32 [B][Ho][Wo][w.n] = conv + bias (+ fp32 residual of the same shape), then act
+static int x3_mma(cudaStream_t st, const X3W& w, const bf16* a3, int B, int Hs, int Ws, int stride2, Buf<float> out, const float* resid, int Ho, int Wo,
+                  int act = ACT_NONE) {
+    CAR_TRY(car_fits(__func__, out, (size_t)B * Ho * Wo * w.n));
     DenseP p;
     memset(&p, 0, sizeof(p));
-    p.A = a3; p.B = c.w3; p.M = B * Ho * Wo; p.N = c.cout; p.K = c.k * c.k * 3 * c.cin_pad; p.ldb = p.K; p.alpha = 1.f;
-    if (c.k == 1) { p.amode = A_PLAIN; p.lda = 3 * c.cin_pad; }
-    else { p.amode = stride2 ? A_CONV3x3S2 : A_CONV3x3; p.Hs = Hs; p.Ws = Ws; p.Cin = 3 * c.cin_pad; p.ups = 0; }
+    p.A = a3; p.B = w.w; p.M = B * Ho * Wo; p.N = w.n; p.K = w.kh * w.kw * w.cin3; p.ldb = p.K; p.alpha = 1.f;
+    if (w.kh == 1) { p.amode = A_PLAIN; p.lda = w.cin3; }
+    else { p.amode = stride2 ? A_CONV3x3S2 : A_CONV3x3; p.Hs = Hs; p.Ws = Ws; p.Cin = w.cin3; p.ups = 0; }
     p.Ho = Ho; p.Wo = Wo;
-    p.bias_f = c.bf; p.C = out; p.ldc = c.cout; p.out_mode = 1; p.resid_f = resid; p.ldr = c.cout; p.act = act;
+    p.bias_f = w.b; p.C = out; p.ldc = w.n; p.out_mode = 1; p.resid_f = resid; p.ldr = w.n; p.act = act;
     return gemm(st, p);
 }
-static int gn_x3(cudaStream_t st, const NormW& nw, const ActF& x, Buf<bf16> y3, int swish, float* stats) {
+static int gn_x3(cudaStream_t st, const NormF& nw, const ActF& x, Buf<bf16> y3, int swish, float* stats) {
     const int G = 32;
     CAR_TRY(car_fits(__func__, y3, (size_t)x.n() * 3));
     CAR_LAUNCH(groupnorm_stats_f32_kernel, x.B * G, 512, 0, st, (const float*)x.p, stats, x.H * x.W, x.C, G);
-    CAR_LAUNCH(groupnorm_apply_split3_kernel, gsz(x.n()), 256, 0, st, (const float*)x.p, (const float*)stats, (const float*)nw.wf, (const float*)nw.bff, y3,
+    CAR_LAUNCH(groupnorm_apply_split3_kernel, gsz(x.n()), 256, 0, st, (const float*)x.p, (const float*)stats, (const float*)nw.w, (const float*)nw.b, y3,
                x.n(), x.H * x.W, x.C, G, swish);
     return CAR_OK;
 }
 // ResnetBlock.forward (vq_model.py:300-315)
-static int res_x3(cudaStream_t st, const ResW& r, ActF& x, Buf<float> out, EncScratch& s) {
+static int res_x3(cudaStream_t st, const ResX3& r, ActF& x, Buf<float> out, EncScratch& s) {
     CAR_TRY(gn_x3(st, r.n1, x, s.t3, 1, s.stats));
-    CAR_TRY(conv_x3(st, r.c1, s.t3, x.B, x.H, x.W, 0, s.h1, nullptr, x.H, x.W));
-    ActF h{s.h1, x.B, x.H, x.W, r.c1.cout};
+    CAR_TRY(x3_mma(st, r.c1, s.t3, x.B, x.H, x.W, 0, s.h1, nullptr, x.H, x.W));
+    ActF h{s.h1, x.B, x.H, x.W, r.c1.n};
     CAR_TRY(gn_x3(st, r.n2, h, s.t3, 1, s.stats));
     const float* sc = x.p;
     if (r.has_nin) {
-        CAR_TRY(split3(st, x.p, s.x3, x.npix(), x.C));
-        CAR_TRY(conv_x3(st, r.nin, s.x3, x.B, x.H, x.W, 0, s.sc, nullptr, x.H, x.W));
+        CAR_TRY(split3_rows(st, x.p, s.x3, x.npix(), x.C));
+        CAR_TRY(x3_mma(st, r.nin, s.x3, x.B, x.H, x.W, 0, s.sc, nullptr, x.H, x.W));
         sc = s.sc;
     }
-    CAR_TRY(conv_x3(st, r.c2, s.t3, x.B, x.H, x.W, 0, out, sc, x.H, x.W));
-    x.p = out; x.C = r.c2.cout;
+    CAR_TRY(x3_mma(st, r.c2, s.t3, x.B, x.H, x.W, 0, out, sc, x.H, x.W));
+    x.p = out; x.C = r.c2.n;
     return CAR_OK;
 }
 // AttnBlock.forward (vq_model.py:328-352): single head over H*W tokens, scale C^-0.5, everything fp32-grade
-static int attn_x3(cudaStream_t st, const AttnW& a, ActF& x, Buf<float> out, EncScratch& s) {
+static int attn_x3(cudaStream_t st, const AttnX3& a, ActF& x, Buf<float> out, EncScratch& s) {
     const int C = x.C, hw = x.H * x.W, B = x.B;
     const int hwp = (hw + 31) & ~31;
     const long long rows = (long long)B * hw;
     CAR_TRY(gn_x3(st, a.n, x, s.t3, 0, s.stats));
-    CAR_TRY(conv_x3(st, a.q, s.t3, B, x.H, x.W, 0, s.qf, nullptr, x.H, x.W));
-    CAR_TRY(conv_x3(st, a.k, s.t3, B, x.H, x.W, 0, s.kf, nullptr, x.H, x.W));
-    CAR_TRY(conv_x3(st, a.v, s.t3, B, x.H, x.W, 0, s.vf, nullptr, x.H, x.W));
-    CAR_TRY(split3(st, s.qf, s.q3, rows, C, 0));
-    CAR_TRY(split3(st, s.kf, s.k3, rows, C, 1));
+    CAR_TRY(x3_mma(st, a.q, s.t3, B, x.H, x.W, 0, s.qf, nullptr, x.H, x.W));
+    CAR_TRY(x3_mma(st, a.k, s.t3, B, x.H, x.W, 0, s.kf, nullptr, x.H, x.W));
+    CAR_TRY(x3_mma(st, a.v, s.t3, B, x.H, x.W, 0, s.vf, nullptr, x.H, x.W));
+    CAR_TRY(split3_rows(st, s.qf, s.q3, rows, C));
+    CAR_TRY(split3_rows(st, s.kf, s.k3, rows, C, X3_ROWS_B));
     {   // scores [B][hw][hwp] fp32
         DenseP p = dp_plain(s.q3, 3 * C, s.k3, 3 * C, hw, hw, 3 * C, s.S, hwp);
         p.sA = (long long)hw * 3 * C; p.sB = (long long)hw * 3 * C; p.sC = (long long)hw * hwp; p.alpha = 1.0f / sqrtf((float)C); p.out_mode = 1;
         CAR_TRY(gemm(st, p, B));
     }
     CAR_LAUNCH(softmax_rows_f32_kernel, (unsigned)rows, 256, 0, st, (const float*)s.S, s.P, hw, hwp);
-    CAR_TRY(split3(st, s.P, s.P3, rows, hwp, 0));
+    CAR_TRY(split3_rows(st, s.P, s.P3, rows, hwp));
     CAR_TRY(car_fits(__func__, s.vT3, (size_t)B * C * hwp * 3));
     CAR_TRY(car_fits(__func__, s.ctx, (size_t)rows * C));
     CAR_LAUNCH(transpose_split3b_kernel, gsz((long long)B * C * hwp), 256, 0, st, (const float*)s.vf, s.vT3, B, hw, hwp, C);
@@ -627,8 +643,8 @@ static int attn_x3(cudaStream_t st, const AttnW& a, ActF& x, Buf<float> out, Enc
         p.sA = (long long)hw * 3 * hwp; p.sB = (long long)C * 3 * hwp; p.sC = (long long)hw * C; p.out_mode = 1;
         CAR_TRY(gemm(st, p, B));
     }
-    CAR_TRY(split3(st, s.ctx, s.q3, rows, C, 0));              // (q3 is free again)
-    CAR_TRY(conv_x3(st, a.o, s.q3, B, x.H, x.W, 0, out, x.p, x.H, x.W));
+    CAR_TRY(split3_rows(st, s.ctx, s.q3, rows, C));             // (q3 is free again)
+    CAR_TRY(x3_mma(st, a.o, s.q3, B, x.H, x.W, 0, out, x.p, x.H, x.W));
     x.p = out;
     return CAR_OK;
 }
@@ -647,7 +663,7 @@ extern "C" int car_vq_encode(CarVQ* m, const float* img, int32_t B, int32_t H, i
     // workspace: fp32 activations (largest: ch channels at full resolution) and their S3 forms
     const size_t actf = (size_t)B * H * W * d.ch, act3 = actf * 3;
     const size_t af = npix * Cmax, a3 = af * 3;
-    Buf<float> fA, fB, zf; EncScratch s; bf16* img3; float* zq;
+    Buf<float> fA, fB, zf; EncScratch s; Buf<bf16> img3; float* zq;
     CAR_TRY(m->ws.carve([&](Carve& c) {
         fA = c.take<float>(actf); fB = c.take<float>(actf);
         s.h1 = c.take<float>(actf); s.sc = c.take<float>(actf);
@@ -661,10 +677,10 @@ extern "C" int car_vq_encode(CarVQ* m, const float* img, int32_t B, int32_t H, i
         zf = c.take<float>(npix * 8); zq = c.take<float>(npix * 8);
     }));
 
-    CAR_LAUNCH(nchw_to_nhwc_split3_kernel, gsz((long long)B * H * W * 32), 256, 0, st, img, img3, B, 3, H * W, 32);
+    CAR_TRY(image_split3(st, img, nullptr, img3, X3Image{B, 3, H, W, 32, 0, 0, 0, 0, 0}));
     auto flip = [&](float* used) { return used == fA ? fB : fA; };
-    CAR_TRY(conv_x3(st, m->e_conv_in, img3, B, H, W, 0, fA, nullptr, H, W));
-    ActF x{fA, B, H, W, m->e_conv_in.cout};
+    CAR_TRY(x3_mma(st, m->e_conv_in, img3, B, H, W, 0, fA, nullptr, H, W));
+    ActF x{fA, B, H, W, m->e_conv_in.n};
     for (int lvl = 0; lvl < d.n_levels; ++lvl) {
         for (size_t b = 0; b < m->e_res[lvl].size(); ++b) {
             CAR_TRY(res_x3(st, m->e_res[lvl][b], x, flip(x.p), s));
@@ -672,9 +688,9 @@ extern "C" int car_vq_encode(CarVQ* m, const float* img, int32_t B, int32_t H, i
         }
         if (m->e_has_down[lvl]) {   // Downsample (vq_model.py:382-397): pad (0,1,0,1), 3x3 stride 2
             Buf<float> o = flip(x.p);
-            CAR_TRY(split3(st, x.p, s.x3, x.npix(), x.C));
-            CAR_TRY(conv_x3(st, m->e_down[lvl], s.x3, B, x.H, x.W, 1, o, nullptr, x.H / 2, x.W / 2));
-            x = ActF{o, B, x.H / 2, x.W / 2, m->e_down[lvl].cout};
+            CAR_TRY(split3_rows(st, x.p, s.x3, x.npix(), x.C));
+            CAR_TRY(x3_mma(st, m->e_down[lvl], s.x3, B, x.H, x.W, 1, o, nullptr, x.H / 2, x.W / 2));
+            x = ActF{o, B, x.H / 2, x.W / 2, m->e_down[lvl].n};
         }
     }
     CAR_TRY(res_x3(st, m->e_mid0, x, flip(x.p), s));
@@ -682,9 +698,9 @@ extern "C" int car_vq_encode(CarVQ* m, const float* img, int32_t B, int32_t H, i
     CAR_TRY(res_x3(st, m->e_mid2, x, flip(x.p), s));
     CAR_TRY(gn_x3(st, m->e_norm_out, x, s.t3, 1, s.stats));
     Buf<float> zc = flip(x.p);
-    CAR_TRY(conv_x3(st, m->e_conv_out, s.t3, B, x.H, x.W, 0, zc, nullptr, x.H, x.W));              // [npix][z_channels]
-    CAR_TRY(split3(st, zc, s.x3, (long long)npix, d.z_channels));
-    CAR_TRY(conv_x3(st, m->quant_conv, s.x3, B, x.H, x.W, 0, zf, nullptr, x.H, x.W));              // [npix][embed_dim] fp32
+    CAR_TRY(x3_mma(st, m->e_conv_out, s.t3, B, x.H, x.W, 0, zc, nullptr, x.H, x.W));               // [npix][z_channels]
+    CAR_TRY(split3_rows(st, zc, s.x3, (long long)npix, d.z_channels));
+    CAR_TRY(x3_mma(st, m->quant_conv, s.x3, B, x.H, x.W, 0, zf, nullptr, x.H, x.W));               // [npix][embed_dim] fp32
     CAR_LAUNCH(vq_argmin_kernel, (unsigned)((npix + 127) / 128), 128, 0, st, (const float*)zf, m->codebook_n, idx_out, quant_out ? zq : nullptr, (long long)npix, d.embed_dim, d.codebook_size);
     if (quant_out) CAR_LAUNCH(nhwc_to_nchw_f32_kernel, gsz((long long)npix * d.embed_dim), 256, 0, st, zq, quant_out, B, h * w, d.embed_dim);
     return CAR_OK;
@@ -756,7 +772,7 @@ extern "C" int car_left_pad_captions(const void* embs, const int64_t* masks, int
 // them, a 1x1 projection per block, bilinear resize of the five maps, mean, sigmoid.  fp32 in the reference => fp32-grade here.
 // ---------------------------------------------------------------------------------------------------------
 struct CarHED : CarOwned {
-    std::vector<ConvW> conv;           // 13, in forward order
+    std::vector<X3W> conv;             // 13, in forward order
     float* norm;                       // [3]
     float* pw[5]; float* pb[5];        // projection weights [C] / bias [1]
 };
@@ -773,12 +789,7 @@ extern "C" int car_hed_create(const void* const* tensors, int32_t n_tensors, voi
         int cin = HED_BLK[b][0];
         const int cout = HED_BLK[b][1];
         for (int i = 0; i < HED_BLK[b][2]; ++i) {
-            ConvW c;
-            memset(&c, 0, sizeof(c));
-            c.cin = cin; c.cout = cout; c.k = 3; c.cin_pad = (cin + 31) & ~31;
-            c.w3 = tc.x3(cout, cin, 3, c.cin_pad);
-            c.bf = tc.f32(cout);
-            m->conv.push_back(c);
+            m->conv.push_back(tc.x3(cout, cin, 3, (cin + 31) & ~31));
             cin = cout;
         }
         m->pw[b] = tc.f32(cout); m->pb[b] = tc.f32(1);
@@ -802,14 +813,14 @@ extern "C" int car_hed_forward(CarHED* m, const float* img, int32_t B, int32_t H
     size_t proj_elems = 0;
     { int h = H, w = W; for (int k = 0; k < 5; ++k) { proj_elems += (size_t)B * h * w; h /= 2; w /= 2; } }
     const size_t actf = full * 64, act3 = actf * 3;                             // largest activation: 64 channels at full resolution
-    Buf<float> fA, fB; Buf<bf16> s3; bf16* img3; float* maps;
+    Buf<float> fA, fB; Buf<bf16> s3, img3; float* maps;
     CAR_TRY(m->ws.carve([&](Carve& c) {
         fA = c.take<float>(actf); fB = c.take<float>(actf);
         s3 = c.take<bf16>(act3);
         img3 = c.take<bf16>(full * 32 * 3);
         maps = c.take<float>(proj_elems);
     }));
-    CAR_LAUNCH(hed_input_split3_kernel, gsz((long long)full * 32), 256, 0, st, img, (const float*)m->norm, img3, B, 3, H * W, 32);
+    CAR_TRY(image_split3(st, img, m->norm, img3, X3Image{B, 3, H, W, 32, 0, 0, 0, 0, 0}));
     HedMaps hm;
     int h = H, w = W, ci = 0, curC = 3;
     float* cur = nullptr;                                                       // the one live fp32 activation (NHWC); ping-pong fA / fB
@@ -823,12 +834,12 @@ extern "C" int car_hed_forward(CarHED* m, const float* img, int32_t B, int32_t H
             h /= 2; w /= 2; cur = o;
         }
         for (int i = 0; i < HED_BLK[b][2]; ++i, ++ci) {
-            const ConvW& c = m->conv[ci];
+            const X3W& c = m->conv[ci];
             const bf16* a3 = img3;
-            if (ci > 0) { CAR_TRY(split3(st, cur, s3, (long long)B * h * w, curC)); a3 = s3; }
+            if (ci > 0) { CAR_TRY(split3_rows(st, cur, s3, (long long)B * h * w, curC)); a3 = s3; }
             Buf<float> o = other(cur);
-            CAR_TRY(conv_x3(st, c, a3, B, h, w, 0, o, nullptr, h, w, ACT_RELU));  // conv + bias, ReLU (:31-33)
-            cur = o; curC = c.cout;
+            CAR_TRY(x3_mma(st, c, a3, B, h, w, 0, o, nullptr, h, w, ACT_RELU));   // conv + bias, ReLU (:31-33)
+            cur = o; curC = c.n;
         }
         float* mp = maps + moff;
         CAR_LAUNCH(hed_proj_kernel, (unsigned)(((long long)B * h * w * 32 + 255) / 256), 256, 0, st, (const float*)cur, (const float*)m->pw[b], (const float*)m->pb[b], mp,
@@ -846,11 +857,25 @@ extern "C" int car_hed_forward(CarHED* m, const float* img, int32_t B, int32_t H
 // two transposed convolutions, 7x7 head + sigmoid, InstanceNorm2d (no parameters) after every convolution but the head.  fp32 in
 // the reference => fp32-grade here: fp32 activations, every convolution but the head on the split-bf16 window GEMM (lineart.cuh).
 // ---------------------------------------------------------------------------------------------------------
-struct LaConv { bf16* w3; float* b; int cin3, cout; };   // cin3 = 3 * Cin_pad (channels per pixel of the S3 source)
 struct CarLineArt : CarOwned {
-    LaConv stem, down[2], res[6], up[2];              // up[i].w3: the four parity classes back to back (lineart.cuh)
+    X3W stem, down[2], res[6], up[2][4];              // up[i][(a, b)]: parity class (a, b), the four back to back in one allocation (lineart.cuh)
     float *head_w, *head_b;                           // [64][7][7], [1]
 };
+
+// ConvTranspose2d(3, stride 2, pad 1, output_padding 1) weight [cin][cout][3][3] -> the W3 of its four parity classes (a, b), each
+// a (1 + a) x (1 + b) window, packed back to back in one allocation (lineart.cuh); then the bias
+static void la_convT(TensorReader& tc, X3W (&up)[4], int cin, int cout) {
+    const long long n3 = 9LL * cout * cin;
+    const float* w = tc.next();
+    bf16* w3 = (bf16*)tc.alloc((size_t)n3 * 3 * 2);
+    tc.pack(convT_weight_pack_x3_kernel, n3, w, w3, cin, cout, cin);
+    const float* b = tc.f32(cout);
+    size_t off = 0;
+    for (int cls = 0; cls < 4; ++cls) {
+        up[cls] = X3W{w3 ? w3 + off : nullptr, b, cout, 3 * cin, 1 + (cls >> 1), 1 + (cls & 1)};
+        off += (size_t)cout * up[cls].kh * up[cls].kw * 3 * cin;
+    }
+}
 
 // tensors (fp32, device), state-dict order: model0.1, model1.0, model1.3, model2.{0,1,2}.conv_block.{1,5}, model3.0, model3.3,
 // model4.1 — each weight then bias
@@ -859,25 +884,12 @@ extern "C" int car_lineart_create(const void* const* tensors, int32_t n_tensors,
     if (n_tensors != 24) CAR_FAIL(CAR_ERR_ARG, "LineArt expects 24 tensors (12 x (weight, bias) in state-dict order)");
     CarLineArt* m = new CarLineArt();
     TensorReader tc(__func__, tensors, n_tensors, stream, m);
-    auto conv = [&](LaConv& c, int cin, int cin_pad, int cout, int k) {
-        c.cin3 = 3 * cin_pad; c.cout = cout;
-        c.w3 = tc.x3(cout, cin, k, cin_pad);
-        c.b = tc.f32(cout);
-    };
-    auto convT = [&](LaConv& c, int cin, int cout) {
-        c.cin3 = 3 * cin; c.cout = cout;
-        const long long n3 = 9LL * cout * cin;
-        const float* w = tc.next();
-        c.w3 = (bf16*)tc.alloc((size_t)n3 * 3 * 2);
-        tc.pack(convT_weight_pack_x3_kernel, n3, w, c.w3, cin, cout, cin);
-        c.b = tc.f32(cout);
-    };
-    conv(m->stem, 3, 8, 64, 7);                       // 3 input channels padded to 8 (16-byte chunks), not 32
-    conv(m->down[0], 64, 64, 128, 3);
-    conv(m->down[1], 128, 128, 256, 3);
-    for (int i = 0; i < 6; ++i) conv(m->res[i], 256, 256, 256, 3);
-    convT(m->up[0], 256, 128);
-    convT(m->up[1], 128, 64);
+    m->stem = tc.x3(64, 3, 7, 8);                     // 3 input channels padded to 8 (16-byte chunks), not 32
+    m->down[0] = tc.x3(128, 64, 3, 64);
+    m->down[1] = tc.x3(256, 128, 3, 128);
+    for (int i = 0; i < 6; ++i) m->res[i] = tc.x3(256, 256, 3, 256);
+    la_convT(tc, m->up[0], 256, 128);
+    la_convT(tc, m->up[1], 128, 64);
     m->head_w = tc.f32(64 * 49); m->head_b = tc.f32(1);
     const int rc = tc.finish();
     if (rc != CAR_OK) { delete m; return rc; }
@@ -889,16 +901,18 @@ extern "C" int car_lineart_destroy(CarLineArt* m) {
     return CAR_OK;
 }
 
-// one window convolution (gemm.h A_WIN): S3 source [B][Hs][Ws][cin3] -> fp32 [B][oH][oW][cout], row (b, oy, ox) of the
-// Ho x Wo grid stored at pixel (osy*oy + oay, osx*ox + oax)
-static int la_conv(cudaStream_t st, const bf16* a3, int B, int Hs, int Ws, int cin3, const bf16* w3, const float* bias, int cout, int kh, int kw,
-                   int stride, int Ho, int Wo, Buf<float> out, int oH, int oW, int osy = 1, int osx = 1, int oay = 0, int oax = 0) {
-    CAR_TRY(car_fits(__func__, out, (size_t)B * oH * oW * cout));
+// one window convolution (gemm.h A_WIN) with the weight's w.kh x w.kw window: S3 source [B][Hs][Ws][w.cin3] -> fp32
+// [B][oH][oW][w.n], row (b, oy, ox) of the Ho x Wo grid stored at pixel (osy*oy + oay, osx*ox + oax).  The window kernel reads the
+// bias unconditionally: a bias-free weight carries a zero bias.
+static int x3_win(cudaStream_t st, const X3W& w, const bf16* a3, int B, int Hs, int Ws, int stride, int Ho, int Wo, Buf<float> out, int oH, int oW,
+                  int osy = 1, int osx = 1, int oay = 0, int oax = 0) {
+    if (!w.b) CAR_FAIL(CAR_ERR_STATE, "window convolution without a bias");
+    CAR_TRY(car_fits(__func__, out, (size_t)B * oH * oW * w.n));
     DenseP p;
     memset(&p, 0, sizeof(p));
-    p.A = a3; p.B = w3; p.M = B * Ho * Wo; p.N = cout; p.K = kh * kw * cin3; p.ldb = p.K; p.alpha = 1.f;
-    p.amode = A_WIN; p.Hs = Hs; p.Ws = Ws; p.Cin = cin3; p.Ho = Ho; p.Wo = Wo; p.kh = kh; p.kw = kw; p.ws = stride;
-    p.bias_f = bias; p.C = out; p.ldc = cout; p.out_mode = 1;
+    p.A = a3; p.B = w.w; p.M = B * Ho * Wo; p.N = w.n; p.K = w.kh * w.kw * w.cin3; p.ldb = p.K; p.alpha = 1.f;
+    p.amode = A_WIN; p.Hs = Hs; p.Ws = Ws; p.Cin = w.cin3; p.Ho = Ho; p.Wo = Wo; p.kh = w.kh; p.kw = w.kw; p.ws = stride;
+    p.bias_f = w.b; p.C = out; p.ldc = w.n; p.out_mode = 1;
     p.osy = osy; p.osx = osx; p.oay = oay; p.oax = oax; p.oH = oH; p.oW = oW;
     return gemm(st, p);
 }
@@ -938,33 +952,26 @@ extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, i
     };
     const InApply zero1{1, 1, 1, 1, 0, 1, 1}, refl1{1, 1, 1, 1, 1, 1, 1}, zero_br{0, 0, 1, 1, 0, 1, 1};
     // model0: ReflectionPad2d(3), Conv 7x7 3 -> 64, IN, ReLU
-    CAR_TRY(car_fits("lineart stem split", S, Bz * (H + 6) * (W + 6) * 8 * 3 * 2));
-    CAR_LAUNCH(lineart_stem_split3_kernel, gsz(Bz * (H + 6) * (W + 6) * 8), 256, 0, st, img, S3, B, 3, H, W, 3, 8);
-    CAR_TRY(la_conv(st, S3, B, H + 6, W + 6, m->stem.cin3, m->stem.w3, m->stem.b, 64, 7, 7, 1, H, W, F, H, W));
+    CAR_TRY(image_split3(st, img, nullptr, Buf<bf16>{S3, S.cap / 2}, X3Image{B, 3, H, W, 8, 3, 3, 3, 3, 1}));
+    CAR_TRY(x3_win(st, m->stem, S3, B, H + 6, W + 6, 1, H, W, F, H, W));
     CAR_TRY(inorm(H, W, 64, nullptr, nullptr, zero1));
     // model1: 2 x [Conv 3x3 stride 2 pad 1 (zeros), IN, ReLU]
-    CAR_TRY(la_conv(st, S3, B, H + 2, W + 2, m->down[0].cin3, m->down[0].w3, m->down[0].b, 128, 3, 3, 2, H1, W1, F, H1, W1));
+    CAR_TRY(x3_win(st, m->down[0], S3, B, H + 2, W + 2, 2, H1, W1, F, H1, W1));
     CAR_TRY(inorm(H1, W1, 128, nullptr, nullptr, zero1));
-    CAR_TRY(la_conv(st, S3, B, H1 + 2, W1 + 2, m->down[1].cin3, m->down[1].w3, m->down[1].b, 256, 3, 3, 2, H2, W2, F, H2, W2));
+    CAR_TRY(x3_win(st, m->down[1], S3, B, H1 + 2, W1 + 2, 2, H2, W2, F, H2, W2));
     CAR_TRY(inorm(H2, W2, 256, nullptr, X[0], refl1));
     // model2: 3 x ResidualBlock: x + [ReflPad 1, Conv, IN, ReLU, ReflPad 1, Conv, IN](x); the fp32 carrier x ping-pongs X[0] / X[1]
     for (int r = 0; r < 3; ++r) {
-        const LaConv &c1 = m->res[2 * r], &c2 = m->res[2 * r + 1];
-        CAR_TRY(la_conv(st, S3, B, H2 + 2, W2 + 2, c1.cin3, c1.w3, c1.b, 256, 3, 3, 1, H2, W2, F, H2, W2));
+        CAR_TRY(x3_win(st, m->res[2 * r], S3, B, H2 + 2, W2 + 2, 1, H2, W2, F, H2, W2));
         CAR_TRY(inorm(H2, W2, 256, nullptr, nullptr, refl1));
-        CAR_TRY(la_conv(st, S3, B, H2 + 2, W2 + 2, c2.cin3, c2.w3, c2.b, 256, 3, 3, 1, H2, W2, F, H2, W2));
+        CAR_TRY(x3_win(st, m->res[2 * r + 1], S3, B, H2 + 2, W2 + 2, 1, H2, W2, F, H2, W2));
         InApply a = r < 2 ? refl1 : zero_br;          // the last block feeds the transposed convolution
         a.relu = 0;
         CAR_TRY(inorm(H2, W2, 256, X[r & 1], r < 2 ? X[(r + 1) & 1] : nullptr, a));
     }
     // model3: 2 x [ConvTranspose2d 3x3 stride 2 pad 1 output_padding 1, IN, ReLU], four parity classes each
-    auto up = [&](const LaConv& c, int h, int w) -> int {
-        const bf16* wc = c.w3;
-        for (int cls = 0; cls < 4; ++cls) {
-            const int a = cls >> 1, b = cls & 1, kh = 1 + a, kw = 1 + b;
-            CAR_TRY(la_conv(st, S3, B, h + 1, w + 1, c.cin3, wc, c.b, c.cout, kh, kw, 1, h, w, F, 2 * h, 2 * w, 2, 2, a, b));
-            wc += (size_t)c.cout * kh * kw * c.cin3;
-        }
+    auto up = [&](const X3W (&c)[4], int h, int w) -> int {
+        for (int cls = 0; cls < 4; ++cls) CAR_TRY(x3_win(st, c[cls], S3, B, h + 1, w + 1, 1, h, w, F, 2 * h, 2 * w, 2, 2, cls >> 1, cls & 1));
         return CAR_OK;
     };
     CAR_TRY(up(m->up[0], H2, W2));
@@ -982,23 +989,36 @@ extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, i
 // GEMM and 3x3 stride-1 convolution on the fp32-output wgmma instantiation over split-bf16 operands, the stride-2 convolution on
 // the window GEMM (gemm_dense.cuh A_WIN), attention fused (dpt.cuh).  No eager or mma.sync fall-back for the wgmma stages.
 // ---------------------------------------------------------------------------------------------------------
-struct DptLin { bf16* w3; float* b; int n, k; };      // W3 [n][3k] (k = 9 cin for a 3x3 convolution), fp32 bias or null
-struct DptLayer { DptLin qkv, o, fc1, fc2; float *ln1w, *ln1b, *ln2w, *ln2b; };
+struct DptLayer { X3W qkv, o, fc1, fc2; float *ln1w, *ln1b, *ln2w, *ln2b; };
 struct DptDecoder {                                     // fusion stages and depth head (shared with MiDaS DPT-Hybrid)
-    DptLin fproj[4], rcu[4][2][2];                      // fusion layer j: projection, residual_layer{1,2}.convolution{1,2}
-    DptLin head0, head2;
+    X3W fproj[4], rcu[4][2][2];                         // fusion layer j: projection, residual_layer{1,2}.convolution{1,2}
+    X3W head0, head2;
     float *head4w, *head4b;
 };
 struct CarDpt : CarOwned {
     CarDptDesc d;
-    DptLin patch;
+    X3W patch;
     float *cls, *pos;                                   // [C], [1 + g^2][C]
     using Layer = DptLayer;
     std::vector<Layer> L;
-    DptLin proj[4], resize[4], readout[4], neck[4];     // resize: ConvTranspose2d GEMM (stages 0, 1), 3x3 stride-2 convolution (3)
+    X3W proj[4], resize[4], readout[4], neck[4];        // resize: ConvTranspose2d GEMM (stages 0, 1), 3x3 stride-2 convolution (3)
     DptDecoder dec;
 };
 static const int DPT_FACTOR[4] = {4, 2, 1, 0};         // 0: the 0.5 stage (3x3 stride-2 convolution)
+
+// ConvTranspose2d(k = s = f): weight [cin][cin][f][f] -> W3 [f^2 cin][3 cin] (dpt.cuh dpt_convT_pack_kernel); the bias repeated per
+// (ky, kx)
+static X3W dpt_convT(TensorReader& tc, int cin, int f) {
+    const int n = f * f * cin;
+    const float* w = tc.next();
+    X3W L{(bf16*)tc.alloc((size_t)n * cin * 3 * 2), nullptr, n, 3 * cin, 1, 1};
+    tc.pack(dpt_convT_pack_kernel, (long long)n * cin, w, L.w, cin, cin, f);
+    const float* b = tc.next();
+    float* bias = (float*)tc.alloc((size_t)n * 4);
+    for (int t = 0; t < f * f; ++t) tc.copy(bias + (size_t)t * cin, b, cin);
+    L.b = bias;
+    return L;
+}
 
 extern "C" int car_dpt_create(const CarDptDesc* desc, const void* const* tensors, int32_t n_tensors, void* stream, CarDpt** out) {
     if (!desc || !tensors || !out) CAR_FAIL(CAR_ERR_ARG, "null argument");
@@ -1016,59 +1036,44 @@ extern "C" int car_dpt_create(const CarDptDesc* desc, const void* const* tensors
     m->d = d;
     const int C = d.hidden, F = d.fusion;
     TensorReader tc(__func__, tensors, n_tensors, stream, m);
-    // weight [n][cin][kh][kw] (kh = kw = 1: nn.Linear) -> W3 [n][kh][kw][3 cin]; then the bias when `bias`
-    auto lin = [&](DptLin& L, int n, int cin, int k, bool bias) {
-        L.n = n; L.k = k * k * cin;
-        L.w3 = tc.x3(n, cin, k, cin);
-        L.b = bias ? tc.f32(n) : nullptr;
-    };
-    // ConvTranspose2d(k = s = f): weight [cin][cin][f][f] -> W3 [f^2 cin][3 cin]; the bias repeated per (ky, kx)
-    auto convT = [&](DptLin& L, int cin, int f) {
-        L.n = f * f * cin; L.k = cin;
-        const float* w = tc.next();
-        L.w3 = (bf16*)tc.alloc((size_t)L.n * L.k * 3 * 2);
-        tc.pack(dpt_convT_pack_kernel, (long long)L.n * L.k, w, L.w3, cin, cin, f);
-        const float* b = tc.next();
-        L.b = (float*)tc.alloc((size_t)L.n * 4);
-        for (int t = 0; t < f * f; ++t) tc.copy(L.b + (size_t)t * cin, b, cin);
-    };
+    // weights [n][cin][kh][kw] (kh = kw = 1: nn.Linear) -> W3 [n][kh][kw][3 cin]
     // dpt.embeddings
     m->cls = tc.f32(C);
     m->pos = tc.f32((long long)(1 + d.pos_grid * d.pos_grid) * C);
-    lin(m->patch, C, 3 * 256, 1, true);                 // [C][3][16][16] read as [C][768]
+    m->patch = tc.x3(C, 3 * 256, 1, 3 * 256);           // [C][3][16][16] read as [C][768]
     // dpt.encoder.layer.{i}: query, key, value (one [3C][3C] GEMM), output.dense, intermediate.dense, output.dense, LN before / after
     m->L.resize(d.n_layers);
     for (int l = 0; l < d.n_layers; ++l) {
         CarDpt::Layer& Ly = m->L[l];
-        Ly.qkv.n = 3 * C; Ly.qkv.k = C;
-        Ly.qkv.w3 = (bf16*)tc.alloc((size_t)3 * C * C * 3 * 2);
-        Ly.qkv.b = (float*)tc.alloc((size_t)3 * C * 4);
+        bf16* qkv = (bf16*)tc.alloc((size_t)3 * C * C * 3 * 2);
+        float* qkv_b = (float*)tc.alloc((size_t)3 * C * 4);
         for (int j = 0; j < 3 && tc.ok(); ++j) {
             const float* w = tc.next();
-            tc.pack(conv_weight_pack_x3_kernel, (long long)C * C, w, Ly.qkv.w3 + (size_t)j * C * 3 * C, C, C, 1, 1, C);
-            tc.copy(Ly.qkv.b + (size_t)j * C, tc.next(), C);
+            tc.pack(conv_weight_pack_x3_kernel, (long long)C * C, w, qkv + (size_t)j * C * 3 * C, C, C, 1, 1, C);
+            tc.copy(qkv_b + (size_t)j * C, tc.next(), C);
         }
-        lin(Ly.o, C, C, 1, true);
-        lin(Ly.fc1, d.mlp, C, 1, true);
-        lin(Ly.fc2, C, d.mlp, 1, true);
+        Ly.qkv = X3W{qkv, qkv_b, 3 * C, 3 * C, 1, 1};
+        Ly.o = tc.x3(C, C, 1, C);
+        Ly.fc1 = tc.x3(d.mlp, C, 1, C);
+        Ly.fc2 = tc.x3(C, d.mlp, 1, d.mlp);
         Ly.ln1w = tc.f32(C); Ly.ln1b = tc.f32(C); Ly.ln2w = tc.f32(C); Ly.ln2b = tc.f32(C);
     }
     tc.skip(2);                                         // dpt.layernorm: applied to last_hidden_state only, which depth does not use
     // neck.reassemble_stage.layers.{i}: projection (1x1), resize
     for (int i = 0; i < 4; ++i) {
-        lin(m->proj[i], d.neck[i], C, 1, true);
-        if (DPT_FACTOR[i] > 1) convT(m->resize[i], d.neck[i], DPT_FACTOR[i]);
-        else if (DPT_FACTOR[i] == 0) lin(m->resize[i], d.neck[i], d.neck[i], 3, true);
+        m->proj[i] = tc.x3(d.neck[i], C, 1, C);
+        if (DPT_FACTOR[i] > 1) m->resize[i] = dpt_convT(tc, d.neck[i], DPT_FACTOR[i]);
+        else if (DPT_FACTOR[i] == 0) m->resize[i] = tc.x3(d.neck[i], d.neck[i], 3, d.neck[i]);
     }
-    for (int i = 0; i < 4; ++i) lin(m->readout[i], C, 2 * C, 1, true);
-    for (int i = 0; i < 4; ++i) lin(m->neck[i], F, d.neck[i], 3, false);
+    for (int i = 0; i < 4; ++i) m->readout[i] = tc.x3(C, 2 * C, 1, 2 * C);
+    for (int i = 0; i < 4; ++i) m->neck[i] = tc.x3(F, d.neck[i], 3, d.neck[i], false);
     for (int j = 0; j < 4; ++j) {
-        lin(m->dec.fproj[j], F, F, 1, true);
+        m->dec.fproj[j] = tc.x3(F, F, 1, F);
         for (int r = 0; r < 2; ++r)
-            for (int c = 0; c < 2; ++c) lin(m->dec.rcu[j][r][c], F, F, 3, true);
+            for (int c = 0; c < 2; ++c) m->dec.rcu[j][r][c] = tc.x3(F, F, 3, F);
     }
-    lin(m->dec.head0, F / 2, F, 3, true);
-    lin(m->dec.head2, 32, F / 2, 3, true);
+    m->dec.head0 = tc.x3(F / 2, F, 3, F);
+    m->dec.head2 = tc.x3(32, F / 2, 3, F / 2);
     m->dec.head4w = tc.f32(32); m->dec.head4b = tc.f32(1);
     const int rc = tc.finish();
     if (rc != CAR_OK) { delete m; return rc; }
@@ -1080,18 +1085,19 @@ extern "C" int car_dpt_destroy(CarDpt* m) {
     return CAR_OK;
 }
 
-// out fp32 [M][ldc] = a3 (S3 rows [M][3 w.k]) · W3^T + bias (+ resid [M][ldc])
-static int dpt_gemm(cudaStream_t st, const DptLin& w, const bf16* a3, int M, Buf<float> out, int ldc, const float* resid = nullptr) {
+// wgmma GEMM (gemm.h gemm_f32): out fp32 [M][ldc] = a3 (S3 rows [M][w.cin3]) · W3^T + bias (+ resid [M][ldc])
+static int x3_gemm(cudaStream_t st, const X3W& w, const bf16* a3, int M, Buf<float> out, int ldc, const float* resid = nullptr) {
     CAR_TRY(car_fits(__func__, out, (size_t)(M - 1) * ldc + w.n));
-    return gemm_f32(st, a3, w.w3, M, w.n, 3 * w.k, w.b, resid, out, ldc);
+    return gemm_f32(st, a3, w.w, M, w.n, w.kh * w.kw * w.cin3, w.b, resid, out, ldc);
 }
 // TMA convolution frame: a map smaller than one 16 x 8 pixel box is held in a zero-filled frame of at least that size
-static inline int dpt_fh(int H) { return std::max(H, WG_TH); }
-static inline int dpt_fw(int W) { return std::max(W, WG_TW); }
-// 3x3 / pad 1 / stride 1 convolution: S3 NHWC frame [B][dpt_fh(H)][dpt_fw(W)][3 cin] -> fp32 NHWC [B][H][W][w.n] (+ resid)
-static int dpt_conv3(cudaStream_t st, const DptLin& w, const bf16* s3, int B, int H, int W, Buf<float> out, const float* resid = nullptr) {
+static inline int x3_fh(int H) { return std::max(H, WG_TH); }
+static inline int x3_fw(int W) { return std::max(W, WG_TW); }
+// wgmma 3x3 / pad 1 / stride 1 convolution (gemm.h gemm_f32_conv3): S3 NHWC frame [B][x3_fh(H)][x3_fw(W)][w.cin3] -> fp32 NHWC
+// [B][H][W][w.n] (+ resid)
+static int x3_conv3(cudaStream_t st, const X3W& w, const bf16* s3, int B, int H, int W, Buf<float> out, const float* resid = nullptr) {
     CAR_TRY(car_fits(__func__, out, (size_t)B * H * W * w.n));
-    return gemm_f32_conv3(st, s3, dpt_fh(H), dpt_fw(W), w.w3, B, H, W, 3 * (w.k / 9), w.n, w.b, resid, out);
+    return gemm_f32_conv3(st, s3, x3_fh(H), x3_fw(W), w.w, B, H, W, w.cin3, w.n, w.b, resid, out);
 }
 // S3 image producer (dpt.cuh dpt_image_split_kernel)
 static int dpt_img(cudaStream_t st, const float* a, const float* b, float* sum_out, Buf<bf16> y, DptImg q) {
@@ -1099,7 +1105,7 @@ static int dpt_img(cudaStream_t st, const float* a, const float* b, float* sum_o
     CAR_LAUNCH(dpt_image_split_kernel, gsz((long long)q.B * q.Hp * q.Wp * q.C), 256, 0, st, a, b, sum_out, y, q);
     return CAR_OK;
 }
-static DptImg dpt_frame(int B, int H, int W, int C) { return DptImg{B, H, W, C, dpt_fh(H), dpt_fw(W), 0, 0, 0, 0, 0}; }
+static DptImg dpt_frame(int B, int H, int W, int C) { return DptImg{B, H, W, C, x3_fh(H), x3_fw(W), 0, 0, 0, 0, 0}; }
 
 // one pre-LN encoder layer over fp32 rows x [B][T][C] -> dst (x may equal dst); S, T0 and X1 are scratch
 static int dpt_layer(cudaStream_t st, const DptLayer& Ly, const float* x, Buf<float> dst, int B, int T, int C, int heads, int mlp, float eps, Buf<bf16> S,
@@ -1107,13 +1113,13 @@ static int dpt_layer(cudaStream_t st, const DptLayer& Ly, const float* x, Buf<fl
     const int M = B * T;
     CAR_TRY(car_fits(__func__, S, (size_t)M * 3 * std::max(C, mlp)));   // the LayerNorm, attention and GELU rows written below
     CAR_LAUNCH(dpt_layernorm_split_kernel, M, DPT_LN_THREADS, 0, st, x, (const float*)Ly.ln1w, (const float*)Ly.ln1b, S, C, eps);
-    CAR_TRY(dpt_gemm(st, Ly.qkv, S, M, T0, 3 * C));
+    CAR_TRY(x3_gemm(st, Ly.qkv, S, M, T0, 3 * C));
     CAR_LAUNCH(dpt_attention_kernel, dim3((T + DPT_AT_B - 1) / DPT_AT_B, heads, B), 128, 0, st, (const float*)T0, S, T, C);
-    CAR_TRY(dpt_gemm(st, Ly.o, S, M, X1, C, x));
+    CAR_TRY(x3_gemm(st, Ly.o, S, M, X1, C, x));
     CAR_LAUNCH(dpt_layernorm_split_kernel, M, DPT_LN_THREADS, 0, st, (const float*)X1, (const float*)Ly.ln2w, (const float*)Ly.ln2b, S, C, eps);
-    CAR_TRY(dpt_gemm(st, Ly.fc1, S, M, T0, mlp));
-    CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)M * mlp), 256, 0, st, (const float*)T0, S, (long long)M, mlp, 1);
-    CAR_TRY(dpt_gemm(st, Ly.fc2, S, M, dst, C, X1));
+    CAR_TRY(x3_gemm(st, Ly.fc1, S, M, T0, mlp));
+    CAR_TRY(split3_rows(st, T0, S, M, mlp, X3_ROWS_A_GELU));
+    CAR_TRY(x3_gemm(st, Ly.fc2, S, M, dst, C, X1));
     return CAR_OK;
 }
 
@@ -1131,29 +1137,29 @@ static int dpt_decode(cudaStream_t st, const DptDecoder& w, const Buf<float> fe[
         const float* xin = fe[i];                       // input of residual_layer2
         if (prev) {
             CAR_TRY(dpt_img(st, fe[i], nullptr, nullptr, S, rq));
-            CAR_TRY(dpt_conv3(st, w.rcu[j][0][0], S, B, s, t, T0));
+            CAR_TRY(x3_conv3(st, w.rcu[j][0][0], S, B, s, t, T0));
             CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, rq));
-            CAR_TRY(dpt_conv3(st, w.rcu[j][0][1], S, B, s, t, T0, fe[i]));
+            CAR_TRY(x3_conv3(st, w.rcu[j][0][1], S, B, s, t, T0, fe[i]));
             CAR_TRY(dpt_img(st, prev, T0, prev, S, rq));                             // prev += RCU1(feature), ReLU'd S3 of it
             xin = prev;
         } else {
             CAR_TRY(dpt_img(st, fe[i], nullptr, nullptr, S, rq));
         }
-        CAR_TRY(dpt_conv3(st, w.rcu[j][1][0], S, B, s, t, T0));
+        CAR_TRY(x3_conv3(st, w.rcu[j][1][0], S, B, s, t, T0));
         CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, rq));
-        CAR_TRY(dpt_conv3(st, w.rcu[j][1][1], S, B, s, t, T2, xin));
+        CAR_TRY(x3_conv3(st, w.rcu[j][1][1], S, B, s, t, T2, xin));
         DptImg uq{B, 2 * s, 2 * t, F, 2 * s, 2 * t, 0, 0, 0, 1, 0};
         CAR_TRY(dpt_img(st, T2, nullptr, nullptr, S, uq));
-        CAR_TRY(dpt_gemm(st, w.fproj[j], S, B * 4 * s * t, T1, F));
+        CAR_TRY(x3_gemm(st, w.fproj[j], S, B * 4 * s * t, T1, F));
         prev = T1;
     }
     const int h2 = H / 2, w2 = W / 2;
     CAR_TRY(dpt_img(st, prev, nullptr, nullptr, S, dpt_frame(B, h2, w2, F)));
-    CAR_TRY(dpt_conv3(st, w.head0, S, B, h2, w2, T0));
+    CAR_TRY(x3_conv3(st, w.head0, S, B, h2, w2, T0));
     DptImg uq = dpt_frame(B, H, W, F / 2);
     uq.up = 1;
     CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, uq));
-    CAR_TRY(dpt_conv3(st, w.head2, S, B, H, W, T2));
+    CAR_TRY(x3_conv3(st, w.head2, S, B, H, W, T2));
     CAR_LAUNCH(dpt_head_kernel, gsz((long long)B * H * W * 32), 256, 0, st, (const float*)T2, (const float*)w.head4w, (const float*)w.head4b, depth,
                (long long)B * H * W);
     return CAR_OK;
@@ -1176,7 +1182,7 @@ extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, 
         const int f = DPT_FACTOR[i];
         ft = std::max({ft, (size_t)Mp * C, (size_t)Mp * (f > 1 ? f * f : 1) * d.neck[i]});
         s3 = std::max({s3, (size_t)Mp * 3 * d.neck[i], Bz * (h + 2) * (h + 2) * 3 * d.neck[i],
-                       Bz * dpt_fh(side[i]) * dpt_fw(side[i]) * 3 * std::max(d.neck[i], F)});
+                       Bz * x3_fh(side[i]) * x3_fw(side[i]) * 3 * std::max(d.neck[i], F)});
     }
     ft = std::max({ft, Bz * 64 * h * h * F, Bz * 256 * h * h * 32});
     s3 = std::max({s3, Bz * 64 * h * h * 3 * F, Bz * 256 * h * h * 3 * (F / 2)});
@@ -1195,7 +1201,7 @@ extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, 
     // ---- embeddings: patch convolution as a GEMM, [CLS], resized position embeddings
     CAR_TRY(car_fits("dpt patchify", S, (size_t)Mp * 3 * 768));
     CAR_LAUNCH(dpt_patchify_kernel, gsz((long long)Mp * 768), 256, 0, st, pixel_values, S, B, h);
-    CAR_TRY(dpt_gemm(st, m->patch, S, Mp, T0, C));
+    CAR_TRY(x3_gemm(st, m->patch, S, Mp, T0, C));
     CAR_LAUNCH(dpt_assemble_kernel, gsz((long long)M * C), 256, 0, st, (const float*)T0, (const float*)m->cls, (const float*)m->pos, X, B, h, h, d.pos_grid,
                C);
     // ---- encoder: pre-LN layers; the residual stream stays fp32, the out-index layers write their output into keep[]
@@ -1212,23 +1218,23 @@ extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, 
         const int Cn = d.neck[i], f = DPT_FACTOR[i], s = side[i];
         CAR_TRY(car_fits("dpt readout split", S, (size_t)Mp * 3 * std::max(2 * C, Cn)));   // this and the two row splits below
         CAR_LAUNCH(dpt_readout_split_kernel, gsz((long long)Mp * 2 * C), 256, 0, st, (const float*)keep[i], S, B, h * h, C);
-        CAR_TRY(dpt_gemm(st, m->readout[i], S, Mp, T0, C));
-        CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)Mp * C), 256, 0, st, (const float*)T0, S, (long long)Mp, C, 1);
-        CAR_TRY(dpt_gemm(st, m->proj[i], S, Mp, T1, Cn));                           // [B][h][h][Cn]
+        CAR_TRY(x3_gemm(st, m->readout[i], S, Mp, T0, C));
+        CAR_TRY(split3_rows(st, T0, S, Mp, C, X3_ROWS_A_GELU));
+        CAR_TRY(x3_gemm(st, m->proj[i], S, Mp, T1, Cn));                            // [B][h][h][Cn]
         DptImg q = dpt_frame(B, s, s, Cn);
         if (f > 1) {
-            CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)Mp * Cn), 256, 0, st, (const float*)T1, S, (long long)Mp, Cn, 0);
-            CAR_TRY(dpt_gemm(st, m->resize[i], S, Mp, T0, f * f * Cn));          // [B][h][h][f][f][Cn]
+            CAR_TRY(split3_rows(st, T1, S, Mp, Cn));
+            CAR_TRY(x3_gemm(st, m->resize[i], S, Mp, T0, f * f * Cn));           // [B][h][h][f][f][Cn]
             q.shuf = f;
             CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, q));
         } else if (f == 0) {
             CAR_TRY(dpt_img(st, T1, nullptr, nullptr, S, DptImg{B, h, h, Cn, h + 2, h + 2, 1, 1, 0, 0, 0}));
-            CAR_TRY(la_conv(st, S, B, h + 2, h + 2, 3 * Cn, m->resize[i].w3, m->resize[i].b, Cn, 3, 3, 2, s, s, T0, s, s));
+            CAR_TRY(x3_win(st, m->resize[i], S, B, h + 2, h + 2, 2, s, s, T0, s, s));
             CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, q));
         } else {
             CAR_TRY(dpt_img(st, T1, nullptr, nullptr, S, q));
         }
-        CAR_TRY(dpt_conv3(st, m->neck[i], S, B, s, s, fe[i]));
+        CAR_TRY(x3_conv3(st, m->neck[i], S, B, s, s, fe[i]));
     }
     // ---- fusion and head
     return dpt_decode(st, m->dec, fe, side, side, B, H, W, F, T0, T1, T2, S, depth);
@@ -1240,22 +1246,21 @@ extern "C" int car_dpt_forward(CarDpt* m, const float* pixel_values, int32_t B, 
 // stage-2 map is the token grid of a ViT-B/16 (1x1 projection, [CLS], position embeddings resized to h x w), then reassemble
 // (stage outputs 0 and 1 as they are; readout "project" of blocks 8 and 11, 1x1 convolution, and a 3x3/2 convolution for the
 // last), the neck's 3x3 convolutions and the DPT fusion and head (dpt_decode).  fp32 in the reference => fp32-grade here: 1x1
-// convolutions and GEMMs on dpt_gemm, 3x3 stride-1 convolutions on dpt_conv3 (wgmma), the stem and the stride-2 convolutions on
-// the window GEMM (la_conv), GroupNorm in midas.cuh.  Token grids need not be square.
+// convolutions and GEMMs on x3_gemm, 3x3 stride-1 convolutions on x3_conv3 (wgmma), the stem and the stride-2 convolutions on
+// the window GEMM (x3_win), GroupNorm in midas.cuh.  Token grids need not be square.
 // ---------------------------------------------------------------------------------------------------------
-struct MdNorm { float *w, *b; };
-struct MdBlock { DptLin dn, c1, c2, c3; MdNorm dnn, n1, n2, n3; int cin, mid, out, stride; };
+struct MdBlock { X3W dn, c1, c2, c3; NormF dnn, n1, n2, n3; int cin, mid, out, stride; };
 static const int MD_DEPTH[3] = {3, 4, 9}, MD_OUT[3] = {256, 512, 1024};
 constexpr int MD_BLOCKS = 16, MD_C = 768, MD_HEADS = 12, MD_MLP = 3072, MD_F = 256, MD_GRID = 24, MD_NT = 368;
 struct CarMidas : CarOwned {
     float* zero;                                        // [1024] zeros: the bias of the bias-free window convolutions
-    DptLin stem;
-    MdNorm stem_n;
+    X3W stem;
+    NormF stem_n;
     MdBlock blk[MD_BLOCKS];
-    DptLin patch;                                       // patch_embed.proj: 1x1 convolution 1024 -> 768 with bias
+    X3W patch;                                          // patch_embed.proj: 1x1 convolution 1024 -> 768 with bias
     float *cls, *pos;                                   // [768], [1 + 24^2][768]
     DptLayer L[12];
-    DptLin readout[2], proj[2], resize4, rn[4];         // act_postprocess{3,4}: readout, 1x1, (3x3/2); scratch.layer{1..4}_rn
+    X3W readout[2], proj[2], resize4, rn[4];            // act_postprocess{3,4}: readout, 1x1, (3x3/2); scratch.layer{1..4}_rn
     DptDecoder dec;
 };
 
@@ -1267,62 +1272,56 @@ extern "C" int car_midas_create(const void* const* tensors, int32_t n_tensors, v
     if (n_tensors != MD_NT) CAR_FAIL(CAR_ERR_ARG, "MiDaS DPT-Hybrid expects 368 tensors in state-dict order");
     CarMidas* m = new CarMidas();
     TensorReader tc(__func__, tensors, n_tensors, stream, m);
-    auto lin = [&](DptLin& L, int n, int cin, int k, bool bias) {
-        L.n = n; L.k = k * k * cin;
-        L.w3 = tc.x3(n, cin, k, cin);
-        L.b = bias ? tc.f32(n) : nullptr;
-    };
-    // weight-standardised convolution [n][cin][k][k] -> W3 [n][k][k][3 cin_pad]; the standardised fp32 weight goes through `wsd`,
-    // re-used in stream order (its largest user is a 3x3 256 -> 256 convolution)
+    // weight-standardised bias-free convolution [n][cin][k][k] -> W3 [n][k][k][3 cin_pad]; the standardised fp32 weight goes through
+    // `wsd`, re-used in stream order (its largest user is a 3x3 256 -> 256 convolution).  A window convolution (7x7/2 stem, stride-2
+    // 1x1 and 3x3) takes the zero bias.
     float* wsd = (float*)tc.alloc((size_t)256 * 256 * 9 * 4);
-    auto sconv = [&](DptLin& L, int n, int cin, int k, int cin_pad) {
-        L.n = n; L.k = k * k * cin_pad; L.b = nullptr;
-        tc.launch(midas_ws_kernel, n, MD_THREADS, tc.next(), wsd, cin * k * k, 1e-8);
-        L.w3 = tc.x3(wsd, n, cin, k, cin_pad);
-    };
-    auto norm = [&](MdNorm& N, int c) { N.w = tc.f32(c); N.b = tc.f32(c); };
     m->zero = tc.zeros(1024);
+    auto sconv = [&](int n, int cin, int k, int cin_pad, bool window) {
+        tc.launch(midas_ws_kernel, n, MD_THREADS, tc.next(), wsd, cin * k * k, 1e-8);
+        return tc.x3(wsd, n, cin, k, cin_pad, window ? m->zero : nullptr);
+    };
     m->cls = tc.f32(MD_C);
     m->pos = tc.f32((long long)(1 + MD_GRID * MD_GRID) * MD_C);
-    sconv(m->stem, 64, 3, 7, 8);                        // 3 input channels padded to 8 (16-byte chunks)
-    norm(m->stem_n, 64);
+    m->stem = sconv(64, 3, 7, 8, true);                 // 3 input channels padded to 8 (16-byte chunks)
+    take_norm(tc, 64, &m->stem_n);
     int cin = 64, bi = 0;
     for (int s = 0; s < 3; ++s)
         for (int b = 0; b < MD_DEPTH[s]; ++b, ++bi) {
             MdBlock& k = m->blk[bi];
             k.cin = cin; k.out = MD_OUT[s]; k.mid = k.out / 4; k.stride = (s > 0 && b == 0) ? 2 : 1;
-            if (b == 0) { sconv(k.dn, k.out, cin, 1, cin); norm(k.dnn, k.out); }
-            sconv(k.c1, k.mid, cin, 1, cin); norm(k.n1, k.mid);
-            sconv(k.c2, k.mid, k.mid, 3, k.mid); norm(k.n2, k.mid);
-            sconv(k.c3, k.out, k.mid, 1, k.mid); norm(k.n3, k.out);
+            if (b == 0) { k.dn = sconv(k.out, cin, 1, cin, k.stride == 2); take_norm(tc, k.out, &k.dnn); }
+            k.c1 = sconv(k.mid, cin, 1, cin, false); take_norm(tc, k.mid, &k.n1);
+            k.c2 = sconv(k.mid, k.mid, 3, k.mid, k.stride == 2); take_norm(tc, k.mid, &k.n2);
+            k.c3 = sconv(k.out, k.mid, 1, k.mid, false); take_norm(tc, k.out, &k.n3);
             cin = k.out;
         }
-    lin(m->patch, MD_C, 1024, 1, true);
+    m->patch = tc.x3(MD_C, 1024, 1, 1024);
     for (int l = 0; l < 12; ++l) {                      // blocks.{l}: norm1, attn.qkv (fused), attn.proj, norm2, mlp.fc1, mlp.fc2
         DptLayer& Ly = m->L[l];
         Ly.ln1w = tc.f32(MD_C); Ly.ln1b = tc.f32(MD_C);
-        lin(Ly.qkv, 3 * MD_C, MD_C, 1, true);
-        lin(Ly.o, MD_C, MD_C, 1, true);
+        Ly.qkv = tc.x3(3 * MD_C, MD_C, 1, MD_C);
+        Ly.o = tc.x3(MD_C, MD_C, 1, MD_C);
         Ly.ln2w = tc.f32(MD_C); Ly.ln2b = tc.f32(MD_C);
-        lin(Ly.fc1, MD_MLP, MD_C, 1, true);
-        lin(Ly.fc2, MD_C, MD_MLP, 1, true);
+        Ly.fc1 = tc.x3(MD_MLP, MD_C, 1, MD_C);
+        Ly.fc2 = tc.x3(MD_C, MD_MLP, 1, MD_MLP);
     }
     tc.skip(4);                                         // norm, head: the ViT's final norm and classifier, unused by the depth map
     for (int i = 0; i < 2; ++i) {
-        lin(m->readout[i], MD_C, 2 * MD_C, 1, true);
-        lin(m->proj[i], MD_C, MD_C, 1, true);
+        m->readout[i] = tc.x3(MD_C, 2 * MD_C, 1, 2 * MD_C);
+        m->proj[i] = tc.x3(MD_C, MD_C, 1, MD_C);
     }
-    lin(m->resize4, MD_C, MD_C, 3, true);
+    m->resize4 = tc.x3(MD_C, MD_C, 3, MD_C);
     const int rn_in[4] = {256, 512, MD_C, MD_C};
-    for (int i = 0; i < 4; ++i) lin(m->rn[i], MD_F, rn_in[i], 3, false);
+    for (int i = 0; i < 4; ++i) m->rn[i] = tc.x3(MD_F, rn_in[i], 3, rn_in[i], false);
     for (int r = 1; r <= 4; ++r) {                      // refinenet{r} is fusion layer 4 - r (the coarsest runs first)
         const int j = 4 - r;
-        lin(m->dec.fproj[j], MD_F, MD_F, 1, true);
+        m->dec.fproj[j] = tc.x3(MD_F, MD_F, 1, MD_F);
         for (int u = 0; u < 2; ++u)
-            for (int c = 0; c < 2; ++c) lin(m->dec.rcu[j][u][c], MD_F, MD_F, 3, true);
+            for (int c = 0; c < 2; ++c) m->dec.rcu[j][u][c] = tc.x3(MD_F, MD_F, 3, MD_F);
     }
-    lin(m->dec.head0, MD_F / 2, MD_F, 3, true);
-    lin(m->dec.head2, 32, MD_F / 2, 3, true);
+    m->dec.head0 = tc.x3(MD_F / 2, MD_F, 3, MD_F);
+    m->dec.head2 = tc.x3(32, MD_F / 2, 3, MD_F / 2);
     m->dec.head4w = tc.f32(32); m->dec.head4b = tc.f32(1);
     const int rc = tc.finish();
     if (rc != CAR_OK) { delete m; return rc; }
@@ -1347,17 +1346,17 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
     const size_t ft = std::max({(size_t)M * MD_MLP, Bz * HW / 4 * F, Bz * HW * 32, Bz * HW / 4 * 64});
     const size_t car = Bz * HW / 16 * 256;              // the widest trunk map: stage 0, 256 channels at H/4
     size_t s3 = std::max({Bz * (H + 5) * (W + 5) * 24, (size_t)M * 3 * MD_MLP, (size_t)Mp * 6 * C, Bz * (h + 2) * (w + 2) * 3 * C,
-                          Bz * 4 * sh[0] * sw[0] * 3 * F, Bz * dpt_fh(H / 2) * dpt_fw(W / 2) * 3 * F, Bz * HW * 3 * (F / 2)});
+                          Bz * 4 * sh[0] * sw[0] * 3 * F, Bz * x3_fh(H / 2) * x3_fw(W / 2) * 3 * F, Bz * HW * 3 * (F / 2)});
     {
         int hh = H / 4, ww = W / 4, ci = 64;
         for (int s = 0; s < 3; ++s) {
             const int mid = MD_OUT[s] / 4, ho = s ? hh / 2 : hh, wo = s ? ww / 2 : ww;
-            s3 = std::max({s3, Bz * hh * ww * 3 * ci, Bz * (hh + 1) * (ww + 1) * 3 * mid, Bz * dpt_fh(hh) * dpt_fw(ww) * 3 * mid,
+            s3 = std::max({s3, Bz * hh * ww * 3 * ci, Bz * (hh + 1) * (ww + 1) * 3 * mid, Bz * x3_fh(hh) * x3_fw(ww) * 3 * mid,
                            Bz * ho * wo * 3 * MD_OUT[s]});
             ci = MD_OUT[s]; hh = ho; ww = wo;
         }
         const int rn_in[4] = {256, 512, MD_C, MD_C};
-        for (int i = 0; i < 4; ++i) s3 = std::max(s3, Bz * dpt_fh(sh[i]) * dpt_fw(sw[i]) * 3 * std::max(rn_in[i], F));
+        for (int i = 0; i < 4; ++i) s3 = std::max(s3, Bz * x3_fh(sh[i]) * x3_fw(sw[i]) * 3 * std::max(rn_in[i], F));
     }
     const size_t part = Bz * 64 * MD_GROUPS, stb = Bz * MD_GROUPS * 2;
     Buf<float> X, X1, K[2], T0, T1, T2, Xa, Xb, Td, fe[4]; float *ps, *pq, *stats, *rstats; Buf<bf16> S;
@@ -1388,7 +1387,7 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
         return CAR_OK;
     };
     // GN(src) (+ resid, normalised by rn when rn.stats) (ReLU) (max-pool) -> S3 frame in S, fp32 carrier when given
-    auto gn_apply = [&](const float* src, const MdNorm& N, const float* resid, GnAffine rn, float* carrier, int hh, int ww, int Cc, GnApply a) -> int {
+    auto gn_apply = [&](const float* src, const NormF& N, const float* resid, GnAffine rn, float* carrier, int hh, int ww, int Cc, GnApply a) -> int {
         CAR_TRY(car_fits("gn_apply", S, (size_t)B * a.Hp * a.Wp * 3 * Cc));
         CAR_LAUNCH(midas_gn_apply_kernel, gsz((long long)B * a.Hp * a.Wp * Cc), 256, 0, st, src, GnAffine{stats, N.w, N.b}, resid, rn, carrier, S, B, hh,
                    ww, Cc, a);
@@ -1397,9 +1396,8 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
     const GnAffine none{nullptr, nullptr, nullptr};
 
     // ---- stem: conv 7x7/2 (SAME: 2 before, 3 after) -> GN + ReLU -> max-pool 3x3/2 (SAME: 0 before, 1 after) -> S3 rows
-    CAR_TRY(car_fits("midas stem split", S, Bz * (H + 5) * (W + 5) * 8 * 3));
-    CAR_LAUNCH(midas_stem_split3_kernel, gsz((long long)Bz * (H + 5) * (W + 5) * 8), 256, 0, st, x, S, B, H, W);
-    CAR_TRY(la_conv(st, S, B, H + 5, W + 5, m->stem.k / 49 * 3, m->stem.w3, m->zero, 64, 7, 7, 2, H / 2, W / 2, T0, H / 2, W / 2));
+    CAR_TRY(image_split3(st, x, nullptr, S, X3Image{B, 3, H, W, 8, 2, 2, 3, 3, 0}));
+    CAR_TRY(x3_win(st, m->stem, S, B, H + 5, W + 5, 2, H / 2, W / 2, T0, H / 2, W / 2));
     CAR_TRY(gn_stats(T0, H / 2, W / 2, 64, stats));
     int hh = H / 4, ww = W / 4;
     CAR_TRY(gn_apply(T0, m->stem_n, nullptr, none, nullptr, H / 2, W / 2, 64, GnApply{0, 0, hh, ww, 1, 1}));
@@ -1413,23 +1411,23 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
             const int ho = hh / k.stride, wo = ww / k.stride, Min = B * hh * ww, Mo = B * ho * wo;
             GnAffine rn = none;
             if (b == 0) {
-                if (k.stride == 1) CAR_TRY(dpt_gemm(st, k.dn, S, Min, Td, k.out));
-                else CAR_TRY(la_conv(st, S, B, hh, ww, 3 * k.cin, k.dn.w3, m->zero, k.out, 1, 1, 2, ho, wo, Td, ho, wo));
+                if (k.stride == 1) CAR_TRY(x3_gemm(st, k.dn, S, Min, Td, k.out));
+                else CAR_TRY(x3_win(st, k.dn, S, B, hh, ww, 2, ho, wo, Td, ho, wo));
                 CAR_TRY(gn_stats(Td, ho, wo, k.out, rstats));
                 rn = GnAffine{rstats, k.dnn.w, k.dnn.b};
             }
-            CAR_TRY(dpt_gemm(st, k.c1, S, Min, T0, k.mid));
+            CAR_TRY(x3_gemm(st, k.c1, S, Min, T0, k.mid));
             CAR_TRY(gn_stats(T0, hh, ww, k.mid, stats));
             if (k.stride == 1) {
-                CAR_TRY(gn_apply(T0, k.n1, nullptr, none, nullptr, hh, ww, k.mid, GnApply{0, 0, dpt_fh(hh), dpt_fw(ww), 1, 0}));
-                CAR_TRY(dpt_conv3(st, k.c2, S, B, hh, ww, T1));
+                CAR_TRY(gn_apply(T0, k.n1, nullptr, none, nullptr, hh, ww, k.mid, GnApply{0, 0, x3_fh(hh), x3_fw(ww), 1, 0}));
+                CAR_TRY(x3_conv3(st, k.c2, S, B, hh, ww, T1));
             } else {                                    // SAME for 3x3/2 on an even map: no padding before, one after
                 CAR_TRY(gn_apply(T0, k.n1, nullptr, none, nullptr, hh, ww, k.mid, GnApply{0, 0, hh + 1, ww + 1, 1, 0}));
-                CAR_TRY(la_conv(st, S, B, hh + 1, ww + 1, 3 * k.mid, k.c2.w3, m->zero, k.mid, 3, 3, 2, ho, wo, T1, ho, wo));
+                CAR_TRY(x3_win(st, k.c2, S, B, hh + 1, ww + 1, 2, ho, wo, T1, ho, wo));
             }
             CAR_TRY(gn_stats(T1, ho, wo, k.mid, stats));
             CAR_TRY(gn_apply(T1, k.n2, nullptr, none, nullptr, ho, wo, k.mid, GnApply{0, 0, ho, wo, 1, 0}));
-            CAR_TRY(dpt_gemm(st, k.c3, S, Mo, T2, k.out));
+            CAR_TRY(x3_gemm(st, k.c3, S, Mo, T2, k.out));
             CAR_TRY(gn_stats(T2, ho, wo, k.out, stats));
             Buf<float> xo = xin == Xa ? Xb : Xa;
             CAR_TRY(car_fits("midas trunk carrier", xo, (size_t)Mo * k.out));
@@ -1438,15 +1436,13 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
         }
         if (s < 2) {                                    // stage outputs 0 and 1 are features 1 and 2: scratch.layer{1,2}_rn
             CAR_TRY(dpt_img(st, xin, nullptr, nullptr, S, dpt_frame(B, hh, ww, MD_OUT[s])));
-            CAR_TRY(dpt_conv3(st, m->rn[s], S, B, hh, ww, fe[s]));
-            CAR_TRY(car_fits("midas stage split", S, (size_t)B * hh * ww * 3 * MD_OUT[s]));
-            CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)B * hh * ww * MD_OUT[s]), 256, 0, st, (const float*)xin, S, (long long)B * hh * ww,
-                       MD_OUT[s], 0);
+            CAR_TRY(x3_conv3(st, m->rn[s], S, B, hh, ww, fe[s]));
+            CAR_TRY(split3_rows(st, xin, S, (long long)B * hh * ww, MD_OUT[s]));
         }
     }
     // ---- ViT-B/16: tokens = 1x1 projection of the stage-2 map, [CLS], position embeddings resized 24 x 24 -> h x w; blocks 8 and 11
     // write their outputs into K[]
-    CAR_TRY(dpt_gemm(st, m->patch, S, Mp, T0, C));
+    CAR_TRY(x3_gemm(st, m->patch, S, Mp, T0, C));
     CAR_LAUNCH(dpt_assemble_kernel, gsz((long long)M * C), 256, 0, st, (const float*)T0, (const float*)m->cls, (const float*)m->pos, X, B, h, w, MD_GRID, C);
     float* xv = X;
     for (int l = 0; l < 12; ++l) {
@@ -1458,17 +1454,17 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
     for (int i = 0; i < 2; ++i) {
         CAR_TRY(car_fits("midas readout split", S, (size_t)Mp * 6 * C));   // this and the row split below
         CAR_LAUNCH(dpt_readout_split_kernel, gsz((long long)Mp * 2 * C), 256, 0, st, (const float*)K[i], S, B, P, C);
-        CAR_TRY(dpt_gemm(st, m->readout[i], S, Mp, T0, C));
-        CAR_LAUNCH(dpt_split_rows_kernel, gsz((long long)Mp * C), 256, 0, st, (const float*)T0, S, (long long)Mp, C, 1);
-        CAR_TRY(dpt_gemm(st, m->proj[i], S, Mp, T1, C));                            // [B][h][w][C]
+        CAR_TRY(x3_gemm(st, m->readout[i], S, Mp, T0, C));
+        CAR_TRY(split3_rows(st, T0, S, Mp, C, X3_ROWS_A_GELU));
+        CAR_TRY(x3_gemm(st, m->proj[i], S, Mp, T1, C));                             // [B][h][w][C]
         if (i == 0) {
             CAR_TRY(dpt_img(st, T1, nullptr, nullptr, S, dpt_frame(B, h, w, C)));
         } else {
             CAR_TRY(dpt_img(st, T1, nullptr, nullptr, S, DptImg{B, h, w, C, h + 2, w + 2, 1, 1, 0, 0, 0}));
-            CAR_TRY(la_conv(st, S, B, h + 2, w + 2, 3 * C, m->resize4.w3, m->resize4.b, C, 3, 3, 2, sh[3], sw[3], T0, sh[3], sw[3]));
+            CAR_TRY(x3_win(st, m->resize4, S, B, h + 2, w + 2, 2, sh[3], sw[3], T0, sh[3], sw[3]));
             CAR_TRY(dpt_img(st, T0, nullptr, nullptr, S, dpt_frame(B, sh[3], sw[3], C)));
         }
-        CAR_TRY(dpt_conv3(st, m->rn[2 + i], S, B, sh[2 + i], sw[2 + i], fe[2 + i]));
+        CAR_TRY(x3_conv3(st, m->rn[2 + i], S, B, sh[2 + i], sw[2 + i], fe[2 + i]));
     }
     // ---- fusion (refinenet4 .. 1) and head (output_conv)
     return dpt_decode(st, m->dec, fe, sh, sw, B, H, W, F, T0, T1, T2, S, depth);

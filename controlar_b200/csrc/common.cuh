@@ -192,12 +192,13 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // ---- block reduce helpers (blockDim.x multiple of 32, <= 1024)
-__device__ __forceinline__ float block_sum(float v, float* red) {
+// NW: the block's warp count when the kernel fixes it at compile time (the final loop is then unrolled), 0: blockDim.x / 32
+template <int NW = 0> __device__ __forceinline__ float block_sum(float v, float* red) {
     v = warp_sum(v);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
     __syncthreads();
     float s = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += red[i];
+    for (int i = 0; i < (NW ? NW : (int)(blockDim.x >> 5)); ++i) s += red[i];
     __syncthreads();
     return s;
 }

@@ -1,11 +1,11 @@
 // dpt.cuh — the DPT depth detector (HF transformers DPTForDepthEstimation, non-hybrid ViT backbone), fp32 in the reference =>
 // fp32-grade here.  Every GEMM and 3x3 stride-1 convolution runs on the fp32-output wgmma instantiation (gemm_wgmma.cuh) over
-// split-bf16 "x3" operands (vision.cuh): activations S3 = [ hi | lo | hi ], weights W3 = [ w_hi | w_hi | w_lo ].  The kernels below
-// are the fp32 glue that writes each S3 operand, plus the fused attention and the 1x1 output head:
+// split-bf16 "x3" operands (split3.cuh): activations S3 = [ hi | lo | hi ], weights W3 = [ w_hi | w_hi | w_lo ].  The kernels below
+// are the fp32 glue that writes each S3 operand, plus the fused attention and the 1x1 output head (fp32 rows, optionally through
+// exact GELU, go through split3_rows_kernel):
 //   patchify       image NCHW -> S3 rows of the 16x16/16 patch convolution, K index c * 256 + ky * 16 + kx (the weight's order)
 //   assemble       [CLS] + patch tokens + position embeddings bilinearly resized (align_corners=False) from the stored grid
 //   layernorm      two-pass fp32 row statistics (mean, then centred squares) -> S3 row
-//   split rows     fp32 rows -> S3 rows, optionally through exact GELU (the MLP and the readout projection)
 //   readout        S3 of cat(token, [CLS]) per patch token (readout_type "project")
 //   image          fp32 NHWC (or the GEMM output of a k = s ConvTranspose2d, pixel shuffle folded in) -> S3 NHWC image, optionally
 //                  + a second map (the fusion add, also written back in fp32), ReLU, or a x2 bilinear upsample (align_corners=True);
@@ -14,17 +14,7 @@
 //   attention      fused multi-head attention for 64-dim heads: scores and probabilities stay in registers (online soft-max)
 //   head           ReLU -> 1x1 convolution to one channel + bias -> ReLU, direct fp32
 #pragma once
-#include "common.cuh"
-
-__device__ __forceinline__ void dpt_split(float v, bf16& hi, bf16& lo) {
-    hi = __float2bfloat16_rn(v);
-    lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-}
-__device__ __forceinline__ void dpt_put3(bf16* o, int C, float v) {      // A side: hi | lo | hi
-    bf16 hi, lo;
-    dpt_split(v, hi, lo);
-    o[0] = hi; o[C] = lo; o[2 * C] = hi;
-}
+#include "split3.cuh"
 
 // ConvTranspose2d(k = s = f) weight fp32 [Cin][Cout][f][f] -> W3 [(ky f + kx) Cout + o][3 Cin]: the transposed convolution is one
 // GEMM whose output row is an input pixel and whose column is (ky, kx, o) of its f x f output block
@@ -34,10 +24,7 @@ __global__ void dpt_convT_pack_kernel(const float* __restrict__ w, bf16* __restr
         const int c = (int)(i % Cin);
         const long long n = i / Cin;
         const int o = (int)(n % Cout), tap = (int)(n / Cout), ky = tap / f, kx = tap - ky * f;
-        bf16 hi, lo;
-        dpt_split(w[(((size_t)c * Cout + o) * f + ky) * f + kx], hi, lo);
-        bf16* q = y + n * 3 * Cin + c;
-        q[0] = hi; q[Cin] = hi; q[2 * Cin] = lo;
+        x3_put_w3(y + n * 3 * Cin + c, Cin, w[(((size_t)c * Cout + o) * f + ky) * f + kx]);
     }
 }
 
@@ -50,7 +37,7 @@ __global__ void dpt_patchify_kernel(const float* __restrict__ x, bf16* __restric
         const long long row = i / K;
         const int p = (int)(row % (h * h)), b = (int)(row / (h * h));
         const int c = k >> 8, ky = (k >> 4) & 15, kx = k & 15, py = p / h, px = p - py * h;
-        dpt_put3(y + row * 3 * K + k, K, x[(((size_t)b * 3 + c) * H + 16 * py + ky) * H + 16 * px + kx]);
+        x3_put_s3(y + row * 3 * K + k, K, x[(((size_t)b * 3 + c) * H + 16 * py + ky) * H + 16 * px + kx]);
     }
 }
 
@@ -80,39 +67,18 @@ __global__ void dpt_assemble_kernel(const float* __restrict__ patch, const float
 
 // LayerNorm (biased variance, eps) of each row of X [M][C] -> S3 rows [M][3C]; one block per row, fixed reduction order
 constexpr int DPT_LN_THREADS = 256;
-__device__ __forceinline__ float dpt_block_sum(float v, float* red) {
-    v = warp_sum(v);
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    __syncthreads();
-    if (lane == 0) red[w] = v;
-    __syncthreads();
-    float s = 0.f;
-    for (int k = 0; k < DPT_LN_THREADS / 32; ++k) s += red[k];
-    return s;
-}
 __global__ void __launch_bounds__(DPT_LN_THREADS) dpt_layernorm_split_kernel(const float* __restrict__ X, const float* __restrict__ w,
                                                                             const float* __restrict__ bias, bf16* __restrict__ y, int C, float eps) {
     __shared__ float red[DPT_LN_THREADS / 32];
     const float* x = X + (size_t)blockIdx.x * C;
     float s = 0.f;
     for (int c = threadIdx.x; c < C; c += DPT_LN_THREADS) s += x[c];
-    const float mean = dpt_block_sum(s, red) / (float)C;
+    const float mean = block_sum<DPT_LN_THREADS / 32>(s, red) / (float)C;
     float q = 0.f;
     for (int c = threadIdx.x; c < C; c += DPT_LN_THREADS) { const float d = x[c] - mean; q = fmaf(d, d, q); }
-    const float rstd = 1.0f / sqrtf(dpt_block_sum(q, red) / (float)C + eps);
+    const float rstd = 1.0f / sqrtf(block_sum<DPT_LN_THREADS / 32>(q, red) / (float)C + eps);
     bf16* o = y + (size_t)blockIdx.x * 3 * C;
-    for (int c = threadIdx.x; c < C; c += DPT_LN_THREADS) dpt_put3(o + c, C, (x[c] - mean) * rstd * w[c] + bias[c]);
-}
-
-// fp32 rows x [M][N] -> S3 rows [M][3N], optionally through exact GELU
-__global__ void dpt_split_rows_kernel(const float* __restrict__ x, bf16* __restrict__ y, long long M, int N, int gelu) {
-    const long long total = M * N;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const long long r = i / N;
-        const int n = (int)(i - r * N);
-        const float v = x[i];
-        dpt_put3(y + r * 3 * N + n, N, gelu ? gelu_erf_f(v) : v);
-    }
+    for (int c = threadIdx.x; c < C; c += DPT_LN_THREADS) x3_put_s3(o + c, C, (x[c] - mean) * rstd * w[c] + bias[c]);
 }
 
 // readout "project": S3 rows [B h^2][3 * 2C] of cat(X[b, 1 + p], X[b, 0])
@@ -124,7 +90,7 @@ __global__ void dpt_readout_split_kernel(const float* __restrict__ X, bf16* __re
         const long long row = i / K;
         const int p = (int)(row % hh), b = (int)(row / hh);
         const float v = k < C ? X[((size_t)b * T + 1 + p) * C + k] : X[(size_t)b * T * C + (k - C)];
-        dpt_put3(y + row * 3 * K + k, K, v);
+        x3_put_s3(y + row * 3 * K + k, K, v);
     }
 }
 
@@ -167,7 +133,7 @@ __global__ void dpt_image_split_kernel(const float* __restrict__ a, const float*
             }
             if (q.relu) v = fmaxf(v, 0.f);
         }
-        dpt_put3(y + bp * 3 * q.C + c, q.C, v);
+        x3_put_s3(y + bp * 3 * q.C + c, q.C, v);
     }
 }
 
@@ -181,7 +147,7 @@ __device__ __forceinline__ uint32_t dpt_pack(bf16 a, bf16 b) {
 }
 __device__ __forceinline__ void dpt_split2(float x, float y, uint32_t& hi, uint32_t& lo) {
     bf16 xh, xl, yh, yl;
-    dpt_split(x, xh, xl); dpt_split(y, yh, yl);
+    x3_split(x, xh, xl); x3_split(y, yh, yl);
     hi = dpt_pack(xh, yh); lo = dpt_pack(xl, yl);
 }
 __device__ __forceinline__ void dpt_mma3(float (&c)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint32_t bh0, uint32_t bh1, uint32_t bl0,
@@ -227,8 +193,8 @@ __global__ void __launch_bounds__(128) dpt_attention_kernel(const float* __restr
             const float ke[4] = {kv.x, kv.y, kv.z, kv.w}, ve[4] = {vv.x, vv.y, vv.z, vv.w};
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                dpt_split(ke[e], sk[0][key][d + e], sk[1][key][d + e]);
-                dpt_split(ve[e], sv[0][d + e][key], sv[1][d + e][key]);
+                x3_split(ke[e], sk[0][key][d + e], sk[1][key][d + e]);
+                x3_split(ve[e], sv[0][d + e][key], sv[1][d + e][key]);
             }
         }
         __syncthreads();

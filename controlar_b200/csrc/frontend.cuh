@@ -119,21 +119,8 @@ __global__ void left_pad_pack_kernel(const uint4* __restrict__ in, const long lo
 }
 
 // ---- HED soft-edge detector (condition/hed.py:17-84), fp32 in the reference: the convolutions run on the fp32-grade split-bf16
-// path of vision.cuh ("x3"); the kernels below are the glue around them ----
-// image fp32 NCHW [B][3][HW] minus the per-channel `norm` -> S3 NHWC with Cpad channels per part (ControlNetHED_Apache2.__call__ :47)
-__global__ void hed_input_split3_kernel(const float* __restrict__ x, const float* __restrict__ norm, bf16* __restrict__ y, int B, int C, int HW, int Cpad) {
-    const long long total = (long long)B * HW * Cpad;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int c = (int)(i % Cpad);
-        const long long bp = i / Cpad;
-        const int pix = (int)(bp % HW), b = (int)(bp / HW);
-        const float v = c < C ? x[((size_t)b * C + c) * HW + pix] - norm[c] : 0.f;
-        const bf16 hi = __float2bfloat16_rn(v);
-        const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        bf16* o = y + bp * 3 * Cpad + c;
-        o[0] = hi; o[Cpad] = lo; o[2 * Cpad] = hi;
-    }
-}
+// path ("x3", split3.cuh; the input minus the per-channel `norm` of ControlNetHED_Apache2.__call__ :47 is written by
+// image_split3_kernel); the kernels below are the glue around them ----
 // F.max_pool2d(kernel 2, stride 2) on NHWC fp32 (floor: odd trailing rows / columns are dropped), :29-30
 __global__ void maxpool2_nhwc_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W, int C) {
     const int Ho = H / 2, Wo = W / 2;

@@ -1,7 +1,7 @@
 // lineart.cuh — the LineArt control-map detector (reference condition/lineart.py:8-86), fp32 in the reference => fp32-grade here.
-// Every wide convolution is one A_WIN launch of the split-bf16 ("x3", vision.cuh) implicit GEMM over an S3 source whose padding was
-// written by the kernel that produced it; the kernels below are that glue:
-//   stem input     NCHW fp32 -> reflect-pad 3 -> S3 NHWC with 8 channels per part
+// Every wide convolution is one A_WIN launch of the split-bf16 ("x3", split3.cuh) implicit GEMM over an S3 source whose padding was
+// written by the kernel that produced it (the stem's input: image_split3_kernel, reflect-pad 3, 8 channels per part); the kernels
+// below are the rest of that glue:
 //   instance norm  InstanceNorm2d defaults (affine=False, eps 1e-5, biased variance per (sample, channel)): deterministic two-pass
 //                  statistics over NHWC fp32, then one apply kernel that adds the residual, applies ReLU and writes the next
 //                  convolution's padded input (reflect or zero, S3 or fp32) plus, where asked, the fp32 carrier
@@ -10,28 +10,7 @@
 //                  i and tap 0 of input i+1 (a zero row / column is appended at the bottom / right) -> windows of 1x1, 1x2, 2x1, 2x2
 //   head           7x7 convolution to one channel + bias + sigmoid, direct fp32
 #pragma once
-#include "common.cuh"
-
-// image fp32 NCHW [B][3][H][W] -> S3 NHWC [B][H+2p][W+2p][3*Cpad], reflection padding p (ReflectionPad2d(3), lineart.py:31)
-__global__ void lineart_stem_split3_kernel(const float* __restrict__ x, bf16* __restrict__ y, int B, int C, int H, int W, int pad, int Cpad) {
-    const int Hp = H + 2 * pad, Wp = W + 2 * pad;
-    const long long total = (long long)B * Hp * Wp * Cpad;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int c = (int)(i % Cpad);
-        const long long bp = i / Cpad;
-        const int px = (int)(bp % Wp);
-        const long long r = bp / Wp;
-        const int py = (int)(r % Hp), b = (int)(r / Hp);
-        int sy = py - pad, sx = px - pad;
-        sy = sy < 0 ? -sy : (sy >= H ? 2 * H - 2 - sy : sy);
-        sx = sx < 0 ? -sx : (sx >= W ? 2 * W - 2 - sx : sx);
-        const float v = c < C ? x[(((size_t)b * C + c) * H + sy) * W + sx] : 0.f;
-        const bf16 hi = __float2bfloat16_rn(v);
-        const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        bf16* o = y + bp * 3 * Cpad + c;
-        o[0] = hi; o[Cpad] = lo; o[2 * Cpad] = hi;
-    }
-}
+#include "split3.cuh"
 
 // ConvTranspose2d weight fp32 [Cin][Cout][3][3] -> W3 of the four parity classes back to back, class (a, b) in the order (0,0) (0,1)
 // (1,0) (1,1), each [Cout][ty < 1+a][tx < 1+b][3 Cin_pad] = [ w_hi | w_hi | w_lo ]; window tap t of an odd class reads kernel tap 2 - 2t
@@ -53,10 +32,7 @@ __global__ void convT_weight_pack_x3_kernel(const float* __restrict__ w, bf16* _
         const int ty = tap / ntx, tx = tap - ty * ntx;
         const int ky = a ? 2 - 2 * ty : 1, kx = bb ? 2 - 2 * tx : 1;
         const float v = c < Cin ? w[(((size_t)c * Cout + o) * 3 + ky) * 3 + kx] : 0.f;
-        const bf16 hi = __float2bfloat16_rn(v);
-        const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        bf16* d = y + (i - c) * 3 + c;                   // (i - c) = index of this (class, o, tap) row times Cin_pad
-        d[0] = hi; d[Cin_pad] = hi; d[2 * Cin_pad] = lo;
+        x3_put_w3(y + (i - c) * 3 + c, Cin_pad, v);     // (i - c) = index of this (class, o, tap) row times Cin_pad
     }
 }
 
@@ -137,14 +113,8 @@ __global__ void instnorm_apply_pad_kernel(const float* __restrict__ x, const flo
             if (a.relu) v = fmaxf(v, 0.f);
             if (carrier && inside) carrier[src] = v;
         }
-        if (a.s3) {
-            const bf16 hi = __float2bfloat16_rn(v);
-            const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-            bf16* o = (bf16*)y + bp * 3 * C + c;
-            o[0] = hi; o[C] = lo; o[2 * C] = hi;
-        } else {
-            ((float*)y)[i] = v;
-        }
+        if (a.s3) x3_put_s3((bf16*)y + bp * 3 * C + c, C, v);
+        else ((float*)y)[i] = v;
     }
 }
 

@@ -1,16 +1,15 @@
 // midas.cuh — the ResNet-50 trunk of MiDaS DPT-Hybrid (reference condition/midas/midas/vit.py, timm ResNetV2 with preact=False and
-// stem_type "same"), fp32 in the reference => fp32-grade here.  The convolutions run on the split-bf16 ("x3", vision.cuh) GEMMs of
-// car_vision.cu; the kernels below are the glue:
+// stem_type "same"), fp32 in the reference => fp32-grade here.  The convolutions run on the split-bf16 ("x3", split3.cuh) GEMMs of
+// car_vision.cu, the stem's input written by image_split3_kernel with TF "SAME" padding of the 7x7/2 stem (2 before, 3 after; the
+// sides are even); the kernels below are the rest of the glue:
 //   weight standardisation  per output channel (w - mean) / sqrt(biased var + 1e-8), statistics in fp64, once at create time
-//   stem input              image NCHW fp32 -> S3 NHWC with 8 channels per part, TF "SAME" padding of the 7x7/2 stem (2 before, 3
-//                           after; the sides are even)
 //   group norm              GroupNorm(32, eps 1e-5) statistics in two deterministic passes (group mean, then centred squares) over
 //                           NHWC fp32, reduced in an order that depends on the map size only, never on the batch; one apply kernel
 //                           fuses the affine, the residual (optionally group-normalised itself: the downsample shortcut), ReLU, the
 //                           stem's 3x3/2 max-pool and the padded S3 write of the next convolution's operand
 // The ViT, reassemble, fusion and head stages are the DPT kernels (dpt.cuh).
 #pragma once
-#include "common.cuh"
+#include "split3.cuh"
 
 constexpr int MD_GROUPS = 32;
 constexpr int MD_THREADS = 256;
@@ -41,39 +40,9 @@ __global__ void __launch_bounds__(MD_THREADS) midas_ws_kernel(const float* __res
     for (int k = threadIdx.x; k < K; k += MD_THREADS) y[(size_t)blockIdx.x * K + k] = (float)(((double)x[k] - mean) * inv);
 }
 
-// image fp32 NCHW [B][3][H][W] -> S3 NHWC [B][H+5][W+5][3*8], the image at (2, 2), zeros elsewhere
-__global__ void midas_stem_split3_kernel(const float* __restrict__ x, bf16* __restrict__ y, int B, int H, int W) {
-    constexpr int CP = 8;
-    const int Hp = H + 5, Wp = W + 5;
-    const long long total = (long long)B * Hp * Wp * CP;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int c = (int)(i % CP);
-        const long long bp = i / CP;
-        const int px = (int)(bp % Wp);
-        const long long r = bp / Wp;
-        const int py = (int)(r % Hp), b = (int)(r / Hp);
-        const int sy = py - 2, sx = px - 2;
-        const float v = (c < 3 && sy >= 0 && sy < H && sx >= 0 && sx < W) ? x[(((size_t)b * 3 + c) * H + sy) * W + sx] : 0.f;
-        const bf16 hi = __float2bfloat16_rn(v);
-        const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        bf16* o = y + bp * 3 * CP + c;
-        o[0] = hi; o[CP] = lo; o[2 * CP] = hi;
-    }
-}
-
 // ---- group-norm statistics over NHWC fp32 [B][HW][C], 32 groups of cpg = C / 32 channels.  grid (32, B, nch), 256 threads; pixel
 // chunk j of nch covers [j*per, (j+1)*per); element e of a chunk is (pixel p0 + e / cpg, channel g*cpg + e % cpg).  Every sum has a
 // fixed order that depends on (HW, C) only.
-__device__ __forceinline__ float md_block_sum(float v, float* red) {
-    v = warp_sum(v);
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    __syncthreads();
-    if (lane == 0) red[w] = v;
-    __syncthreads();
-    float s = 0.f;
-    for (int k = 0; k < MD_THREADS / 32; ++k) s += red[k];
-    return s;
-}
 __device__ __forceinline__ float md_chunk_sum(const float* __restrict__ xb, int HW, int C, int g, int nch, int j, float mean, bool centred,
                                               float* red) {
     const int cpg = C / MD_GROUPS, per = (HW + nch - 1) / nch;
@@ -86,7 +55,7 @@ __device__ __forceinline__ float md_chunk_sum(const float* __restrict__ xb, int 
         const float v = base[(size_t)p * C + k];
         if (centred) { const float d = v - mean; s = fmaf(d, d, s); } else s += v;
     }
-    return md_block_sum(s, red);
+    return block_sum<MD_THREADS / 32>(s, red);
 }
 __device__ __forceinline__ float md_mean(const float* __restrict__ part_s, int b, int nch, int g, int HW, int C) {
     float s = 0.f;
@@ -155,9 +124,6 @@ __global__ void midas_gn_apply_kernel(const float* __restrict__ x, GnAffine n, c
             }
             if (carrier) carrier[(((size_t)b * Ho + oy) * Wo + ox) * C + c] = v;
         }
-        const bf16 hi = __float2bfloat16_rn(v);
-        const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        bf16* o = y + bp * 3 * C + c;
-        o[0] = hi; o[C] = lo; o[2 * C] = hi;
+        x3_put_s3(y + bp * 3 * C + c, C, v);
     }
 }

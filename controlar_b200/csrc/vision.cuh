@@ -4,6 +4,7 @@
 #pragma once
 #include "common.cuh"
 #include "patch_embed.cuh"
+#include "split3.cuh"
 
 // nn.LayerNorm over the last dim (fp32 statistics, eps inside the sqrt), bf16 in/out.  one block per row.
 __global__ void layernorm_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const bf16* __restrict__ b,
@@ -337,40 +338,8 @@ __global__ void upsample2x_nhwc_kernel(const bf16* __restrict__ x, bf16* __restr
     }
 }
 
-// ---- fp32-grade path of the VQGAN encoder ("x3": split-bf16 operands, three partial products, fp32 accumulate) ----
-// VQModel.encode runs in fp32 in the reference (vq_model.py:41-46; sample / extract scripts keep the tokenizer in fp32) and its
-// arg-min indices must come out the same (SURVEY.md §8 a18: index work is bit-exact), which a bf16 encoder cannot deliver: the
-// latent then carries ~1e-2 relative noise and 6-7 % of the indices flip.  Here every fp32 value x travels as the pair
-// hi = bf16(x), lo = bf16(x - hi) (x = hi + lo to 2^-17) and a product x·w is evaluated as hi·w_hi + lo·w_hi + hi·w_lo on the
-// tensor cores with fp32 accumulation, by tripling the GEMM's K dimension:
-//   activations "S3" : NHWC bf16 with 3C channels per pixel  [ hi(C) | lo(C) | hi(C) ]   (A side)
-//   weights     "W3" : [Cout][tap][3 Cin_pad]                [ w_hi  | w_hi  | w_lo  ]   (B side)
-// so the bf16 implicit-GEMM kernel (gemm_dense.cuh) is used unchanged, with fp32 output, fp32 bias and fp32 residual.
-__global__ void split3_kernel(const float* __restrict__ x, bf16* __restrict__ y, long long npix, int C, int bside) {
-    const long long total = npix * C;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const long long pix = i / C; const int c = (int)(i - pix * C);
-        const float v = x[i];
-        const bf16 hi = __float2bfloat16_rn(v);
-        const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        bf16* o = y + pix * 3 * C + c;
-        o[0] = hi; o[C] = bside ? hi : lo; o[2 * C] = bside ? lo : hi;       // A side: hi | lo | hi ; B side: hi | hi | lo
-    }
-}
-// image fp32 NCHW [B][C][HW] -> S3 NHWC with Cpad channels per part (zero padded)
-__global__ void nchw_to_nhwc_split3_kernel(const float* __restrict__ x, bf16* __restrict__ y, int B, int C, int HW, int Cpad) {
-    const long long total = (long long)B * HW * Cpad;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int c = (int)(i % Cpad);
-        const long long bp = i / Cpad;
-        const int pix = (int)(bp % HW), b = (int)(bp / HW);
-        const float v = c < C ? x[((size_t)b * C + c) * HW + pix] : 0.f;
-        const bf16 hi = __float2bfloat16_rn(v);
-        const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        bf16* o = y + bp * 3 * Cpad + c;
-        o[0] = hi; o[Cpad] = lo; o[2 * Cpad] = hi;
-    }
-}
+// ---- fp32-grade path of the VQGAN encoder (split-bf16 "x3" operands, split3.cuh).  VQModel.encode runs in fp32 in the reference
+// (vq_model.py:41-46; sample / extract scripts keep the tokenizer in fp32) and its arg-min indices must come out the same.
 // conv weight fp32 [Cout][Cin][kh][kw] -> W3 bf16 [Cout][kh][kw][3 Cin_pad] = [ w_hi | w_hi | w_lo ] per tap
 __global__ void conv_weight_pack_x3_kernel(const float* __restrict__ w, bf16* __restrict__ y, int Cout, int Cin, int KH, int KW, int Cin_pad) {
     const long long total = (long long)Cout * KH * KW * Cin_pad;
@@ -382,10 +351,7 @@ __global__ void conv_weight_pack_x3_kernel(const float* __restrict__ w, bf16* __
         const int ky = (int)(r % KH);
         const int o = (int)(r / KH);
         const float v = c < Cin ? w[(((size_t)o * Cin + c) * KH + ky) * KW + kx] : 0.f;
-        const bf16 hi = __float2bfloat16_rn(v);
-        const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        bf16* q = y + tapidx * 3 * Cin_pad + c;
-        q[0] = hi; q[Cin_pad] = hi; q[2 * Cin_pad] = lo;
+        x3_put_w3(y + tapidx * 3 * Cin_pad + c, Cin_pad, v);
     }
 }
 // GroupNorm(32, eps 1e-6) statistics over NHWC fp32 (two-pass mean / variance in fp64-free fp32: mean first, then centred squares)
@@ -406,7 +372,7 @@ __global__ void groupnorm_stats_f32_kernel(const float* __restrict__ x, float* _
     ss = block_sum(ss, red);
     if (threadIdx.x == 0) { stats[blockIdx.x * 2] = mean; stats[blockIdx.x * 2 + 1] = rsqrtf(ss / n + 1e-6f); }
 }
-// y = GN(x) (*swish) in fp32, written as S3 (or plain fp32 when y3 is null)
+// y = GN(x) (*swish) in fp32, written as S3
 __global__ void groupnorm_apply_split3_kernel(const float* __restrict__ x, const float* __restrict__ stats, const float* __restrict__ w,
                                               const float* __restrict__ bsh, bf16* __restrict__ y3, long long total, int HW, int C, int G, int swish) {
     const int cg = C / G;
@@ -416,10 +382,7 @@ __global__ void groupnorm_apply_split3_kernel(const float* __restrict__ x, const
         const float* st = stats + ((size_t)b * G + c / cg) * 2;
         float v = (x[i] - st[0]) * st[1] * w[c] + bsh[c];
         if (swish) v = v / (1.0f + expf(-v));
-        const bf16 hi = __float2bfloat16_rn(v);
-        const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        bf16* o = y3 + pix * 3 * C + c;
-        o[0] = hi; o[C] = lo; o[2 * C] = hi;
+        x3_put_s3(y3 + pix * 3 * C + c, C, v);
     }
 }
 // soft-max over rows of fp32 scores, fp32 out (columns >= n of the padded row are zeroed)
@@ -443,10 +406,7 @@ __global__ void transpose_split3b_kernel(const float* __restrict__ v, bf16* __re
         const long long bc = i / hwp;
         const int c = (int)(bc % C), b = (int)(bc / C);
         const float x = t < hw ? v[((size_t)b * hw + t) * C + c] : 0.f;
-        const bf16 hi = __float2bfloat16_rn(x);
-        const bf16 lo = __float2bfloat16_rn(x - __bfloat162float(hi));
-        bf16* o = y + bc * 3 * hwp + t;
-        o[0] = hi; o[hwp] = hi; o[2 * hwp] = lo;
+        x3_put_w3(y + bc * 3 * hwp + t, hwp, x);
     }
 }
 

@@ -71,7 +71,7 @@ def test_vq_encode_vs_reference_golden():
         bad = (idx.cpu() != ref_idx).nonzero().flatten().tolist()
         for i in bad:
             gap = float(d[i, idx[i].item()] - d[i, ref_idx[i]])
-            assert gap < 1e-4, (tag, i, gap)        # fp32-grade encoder (csrc/vision.cuh "x3"): only genuine ties may differ
+            assert gap < 1e-4, (tag, i, gap)        # fp32-grade encoder (csrc/split3.cuh "x3"): only genuine ties may differ
         assert agree >= 0.98, (tag, agree)
         assert quant.shape == v[f"enc_quant_{tag}"].shape
         # round trip through the product path

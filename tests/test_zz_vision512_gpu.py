@@ -84,7 +84,7 @@ def test_vq_encode_512_indices_vs_reference_golden():
     worst_gap = max(gaps) if gaps else 0.0
     _log(case="vq_encode_512", agree=agree, n_bad=len(gaps), worst_gap=worst_gap, median_ref_margin=float(margin.median()),
          frac_ref_margin_below_1e_3=float((margin < 1e-3).float().mean()))
-    # The encoder runs at fp32 grade (split-bf16 operands, three partial products, fp32 accumulate: csrc/vision.cuh "x3"), like the
+    # The encoder runs at fp32 grade (split-bf16 operands, three partial products, fp32 accumulate: csrc/split3.cuh "x3"), like the
     # reference's fp32 VQModel.  (With the bf16 encoder of round 1: 93.4 % agreement, worst mismatch 2.1e-2 further than the reference's
     # best code — the reference's own median best-vs-second margin is 2.2e-2.)  Measured on an H100 80GB HBM3 with the fp32-grade
     # path: 1024 of 1024 indices identical.  Bar: >= 99.9 % identical and every mismatch a near-tie of the reference's own distances (gap < 1e-4;
