@@ -50,6 +50,17 @@ class CarDptDesc(C.Structure):
                 ("ln_eps", C.c_float)]
 
 
+class CarGemmDesc(C.Structure):
+    """gemm.h's DenseP, field for field (include/controlar_b200.h)."""
+    _fields_ = [("A", C.c_void_p), ("B", C.c_void_p), ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32),
+                ("lda", C.c_int32), ("ldb", C.c_int32), ("sA", C.c_int64), ("sB", C.c_int64), ("sC", C.c_int64), ("sR", C.c_int64),
+                ("amode", C.c_int32), ("Hs", C.c_int32), ("Ws", C.c_int32), ("Cin", C.c_int32), ("Ho", C.c_int32), ("Wo", C.c_int32),
+                ("ups", C.c_int32), ("alpha", C.c_float), ("bias", C.c_void_p), ("bias_along_m", C.c_int32), ("bias_f", C.c_void_p),
+                ("resid_f", C.c_void_p), ("act", C.c_int32), ("scale", C.c_void_p), ("resid", C.c_void_p), ("ldr", C.c_int32),
+                ("C", C.c_void_p), ("ldc", C.c_int32), ("out_mode", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32), ("ws", C.c_int32),
+                ("osy", C.c_int32), ("osx", C.c_int32), ("oay", C.c_int32), ("oax", C.c_int32), ("oH", C.c_int32), ("oW", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/controlar_b200.h
 PROTOTYPES = {
     "car_last_error": (C.c_char_p, []),
@@ -104,6 +115,12 @@ PROTOTYPES = {
     "car_t5_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_t5_destroy": (C.c_int, [C.c_void_p]),
     "car_adamw_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32, C.c_void_p]),
+    "car_op_gemm_route": (C.c_int, [C.POINTER(CarGemmDesc), C.c_int32]),
+    "car_op_gemm": (C.c_int, [C.POINTER(CarGemmDesc), C.c_int32, C.c_void_p]),
+    "car_op_gemm_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                  C.c_void_p]),
+    "car_op_gemm_f32_conv3": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "car_op_rmsnorm": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float,
                                  C.c_void_p]),
     "car_op_attn_decode": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,

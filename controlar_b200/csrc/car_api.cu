@@ -885,12 +885,42 @@ extern "C" int car_op_linear(int32_t dtype, const void* x, const void* w, const 
 }
 
 // the dense (M >= 64 rows) tensor-core linear of the prefill / MLP path, exposed for unit tests and micro-benchmarks:
-// y[M,N] = act(x[M,K] · w[N,K]^T) (+ resid), bf16, fp32 accumulate, routed by gemm() (gemm.cu): the wgmma kernel when N and K are
-// multiples of 8 and the operands 16-byte aligned, otherwise the mma.sync kernel
+// y[M,N] = act(x[M,K] · w[N,K]^T) (+ resid), bf16, fp32 accumulate, routed by gemm() (gemm.cu): the wgmma kernel when N is a
+// multiple of 8 and y, resid 16-byte aligned, otherwise the mma.sync kernel; K % 8 != 0 or misaligned x, w are refused (gemm.h)
 extern "C" int car_op_dense_linear(const void* x, const void* w, const void* resid, void* y, int32_t M, int32_t N, int32_t K, int32_t act,
                                    void* stream) {
     if (!x || !w || !y) CAR_FAIL(CAR_ERR_ARG, "null argument");
     return dense_linear((cudaStream_t)stream, x, K, w, M, N, K, act ? ACT_GELU_TANH : ACT_NONE, resid, N, y, N);
+}
+
+// the library's GEMM front end (gemm.h), for conformance tests: the descriptor is copied field by field into a DenseP
+static DenseP dense_p(const CarGemmDesc& d) {
+    DenseP p;
+    memset(&p, 0, sizeof(p));
+    p.A = (const bf16*)d.A; p.B = (const bf16*)d.B; p.M = d.M; p.N = d.N; p.K = d.K; p.lda = d.lda; p.ldb = d.ldb;
+    p.sA = d.sA; p.sB = d.sB; p.sC = d.sC; p.sR = d.sR;
+    p.amode = d.amode; p.Hs = d.Hs; p.Ws = d.Ws; p.Cin = d.Cin; p.Ho = d.Ho; p.Wo = d.Wo; p.ups = d.ups;
+    p.alpha = d.alpha; p.bias = (const bf16*)d.bias; p.bias_along_m = d.bias_along_m; p.bias_f = d.bias_f; p.resid_f = d.resid_f;
+    p.act = d.act; p.scale = (const bf16*)d.scale; p.resid = (const bf16*)d.resid; p.ldr = d.ldr; p.C = d.C; p.ldc = d.ldc;
+    p.out_mode = d.out_mode; p.kh = d.kh; p.kw = d.kw; p.ws = d.ws;
+    p.osy = d.osy; p.osx = d.osx; p.oay = d.oay; p.oax = d.oax; p.oH = d.oH; p.oW = d.oW;
+    return p;
+}
+extern "C" int car_op_gemm_route(const CarGemmDesc* d, int32_t batch) {
+    if (!d) CAR_FAIL(CAR_ERR_ARG, "null descriptor");
+    return gemm_route(dense_p(*d), batch);
+}
+extern "C" int car_op_gemm(const CarGemmDesc* d, int32_t batch, void* stream) {
+    if (!d) CAR_FAIL(CAR_ERR_ARG, "null descriptor");
+    return gemm((cudaStream_t)stream, dense_p(*d), batch);
+}
+extern "C" int car_op_gemm_f32(const void* A, const void* B, int32_t M, int32_t N, int32_t K, const float* bias, const float* resid, float* out,
+                               int32_t ldc, void* stream) {
+    return gemm_f32((cudaStream_t)stream, (const bf16*)A, (const bf16*)B, M, N, K, bias, resid, out, ldc);
+}
+extern "C" int car_op_gemm_f32_conv3(const void* src, int32_t fh, int32_t fw, const void* B, int32_t nimg, int32_t H, int32_t W, int32_t cin,
+                                     int32_t N, const float* bias, const float* resid, float* out, void* stream) {
+    return gemm_f32_conv3((cudaStream_t)stream, (const bf16*)src, fh, fw, (const bf16*)B, nimg, H, W, cin, N, bias, resid, out);
 }
 
 extern "C" int car_op_rmsnorm(int32_t dtype, const void* x, const void* w, void* y, int32_t M, int32_t K, float eps, void* stream) {

@@ -81,33 +81,99 @@ static int dg_launch(cudaStream_t st, const DenseP& p, int batch) {
     return CAR_OK;
 }
 
-static bool aligned16(const void* p) { return ((uintptr_t)p % 16) == 0; }
+static bool aligned(const void* p, int bytes) { return ((uintptr_t)p % bytes) == 0; }
+static bool aligned16(const void* p) { return aligned(p, 16); }
 
-int gemm(cudaStream_t st, const DenseP& dp, int batch) {
-    if (dp.M <= 0 || dp.N <= 0) return CAR_OK;
-    DenseP p = dp;
-    if (p.alpha == 0.f) p.alpha = 1.f;
-    if (p.amode == A_WIN) return dg_launch<true>(st, p, batch);
+// the contract of gemm.h, field by field, then the route
+int gemm_route(const DenseP& p, int batch) {
+    if (!p.A || !p.B || !p.C) CAR_FAIL(CAR_ERR_ARG, "A, B and C must be non-null");
+    if (p.M < 0 || p.N < 0) CAR_FAIL(CAR_ERR_ARG, "M and N must be >= 0");
+    if (p.K <= 0) CAR_FAIL(CAR_ERR_ARG, "K must be > 0");
+    if (batch < 1 || batch > 65535) CAR_FAIL(CAR_ERR_ARG, "batch must be in [1, 65535]");
+    if (p.amode < A_PLAIN || p.amode > A_WIN) CAR_FAIL(CAR_ERR_ARG, "unknown amode");
+    if (p.act < ACT_NONE || p.act > ACT_RELU) CAR_FAIL(CAR_ERR_ARG, "unknown act");
+    if (p.out_mode < 0 || p.out_mode > 2) CAR_FAIL(CAR_ERR_ARG, "out_mode must be 0, 1 or 2");
+    // the mma.sync loader: 16-byte cp.async chunks along K
+    if (p.K % 8 || p.ldb % 8) CAR_FAIL(CAR_ERR_ARG, "K and ldb must be multiples of 8");
+    if (p.ldb < p.K) CAR_FAIL(CAR_ERR_ARG, "ldb must be >= K");
+    if (!aligned16(p.A) || !aligned16(p.B)) CAR_FAIL(CAR_ERR_ARG, "A and B must be 16-byte aligned");
+    if (batch > 1 && (p.sA % 8 || p.sB % 8)) CAR_FAIL(CAR_ERR_ARG, "sA and sB must be multiples of 8");
+    if (p.bias_along_m && !p.bias) CAR_FAIL(CAR_ERR_ARG, "bias_along_m needs a bf16 bias");
+    if ((p.resid || p.resid_f) && p.ldr < p.N) CAR_FAIL(CAR_ERR_ARG, "ldr must be >= N");
+    const bool gelu = p.act == ACT_GELU_TANH || p.act == ACT_GELU_ERF;
+    if (p.out_mode != 0 && (p.scale || p.resid || gelu)) CAR_FAIL(CAR_ERR_ARG, "scale, resid and GELU round to bf16: they need out_mode 0");
+    if (p.out_mode == 2) {
+        if (batch != 1) CAR_FAIL(CAR_ERR_ARG, "out_mode 2 (NCHW) needs batch 1");
+        if (p.ldc != 0) CAR_FAIL(CAR_ERR_ARG, "out_mode 2 (NCHW) has no ldc: it must be 0");
+        if (p.Ho <= 0 || p.Wo <= 0 || p.M % (p.Ho * p.Wo)) CAR_FAIL(CAR_ERR_ARG, "out_mode 2 (NCHW) needs Ho, Wo > 0 and M a multiple of Ho Wo");
+    } else if (p.ldc < p.N) {
+        CAR_FAIL(CAR_ERR_ARG, "ldc must be >= N");
+    }
+    if (p.amode == A_PLAIN) {
+        if (p.lda < p.K || p.lda % 8) CAR_FAIL(CAR_ERR_ARG, "lda must be >= K and a multiple of 8");
+    } else {
+        if (p.Cin <= 0 || p.Cin % 8) CAR_FAIL(CAR_ERR_ARG, "Cin must be a positive multiple of 8");
+        if (p.Hs <= 0 || p.Ws <= 0 || p.Ho <= 0 || p.Wo <= 0) CAR_FAIL(CAR_ERR_ARG, "Hs, Ws, Ho and Wo must be > 0");
+        if (p.M % (p.Ho * p.Wo)) CAR_FAIL(CAR_ERR_ARG, "M must be a multiple of Ho Wo");
+        if (p.ups != 0 && !(p.ups == 1 && p.amode == A_CONV3x3)) CAR_FAIL(CAR_ERR_ARG, "ups must be 0, or 1 with A_CONV3x3");
+    }
+    if (p.amode == A_CONV3x3 || p.amode == A_CONV3x3S2) {
+        if (p.K != 9 * p.Cin) CAR_FAIL(CAR_ERR_ARG, "a 3x3 convolution needs K == 9 Cin");
+    }
+    if (p.amode == A_WIN) {
+        if (!p.bias_f) CAR_FAIL(CAR_ERR_ARG, "A_WIN needs bias_f");
+        if (p.out_mode != 1) CAR_FAIL(CAR_ERR_ARG, "A_WIN stores fp32: out_mode must be 1");
+        if (batch != 1) CAR_FAIL(CAR_ERR_ARG, "A_WIN needs batch 1");
+        if ((p.alpha != 0.f && p.alpha != 1.f) || p.bias || p.act != ACT_NONE || p.resid_f)
+            CAR_FAIL(CAR_ERR_ARG, "A_WIN does not apply alpha, bias, act or resid_f");
+        if (p.kh < 1 || p.kw < 1 || p.ws < 1) CAR_FAIL(CAR_ERR_ARG, "kh, kw and ws must be >= 1");
+        if (p.K != p.kh * p.kw * p.Cin) CAR_FAIL(CAR_ERR_ARG, "A_WIN needs K == kh kw Cin");
+        if ((long long)p.ws * (p.Ho - 1) + p.kh > p.Hs || (long long)p.ws * (p.Wo - 1) + p.kw > p.Ws)
+            CAR_FAIL(CAR_ERR_ARG, "A_WIN windows must lie inside the Hs x Ws source");
+        if (p.osy < 1 || p.osx < 1 || p.oay < 0 || p.oax < 0) CAR_FAIL(CAR_ERR_ARG, "A_WIN needs osy, osx >= 1 and oay, oax >= 0");
+        if ((long long)p.osy * (p.Ho - 1) + p.oay >= p.oH || (long long)p.osx * (p.Wo - 1) + p.oax >= p.oW)
+            CAR_FAIL(CAR_ERR_ARG, "A_WIN pixel map must land inside oH x oW");
+        return GEMM_MMA_WIN;
+    }
     // the wgmma epilogue: bf16 bias along n, bf16 rounding, GELU (tanh or erf), LayerScale, bf16 residual, one bf16 [M][ldc] output
-    const bool wg_epi = batch == 1 && p.out_mode == 0 && p.alpha == 1.f && !p.bias_along_m && !p.bias_f && !p.resid_f &&
-                        (p.act == ACT_NONE || p.act == ACT_GELU_TANH || p.act == ACT_GELU_ERF);
-    // its tensor maps and paired stores: 16-byte row pitches and base pointers, whole 8-column groups
-    const bool wg_ok = wg_epi && p.K % 8 == 0 && p.N % 8 == 0 && p.lda % 8 == 0 && p.ldb % 8 == 0 && p.ldc % 8 == 0 &&
-                       (!p.resid || p.ldr % 8 == 0) && aligned16(p.A) && aligned16(p.B) && aligned16(p.C) && (!p.resid || aligned16(p.resid));
+    const bool wg_epi = batch == 1 && p.out_mode == 0 && (p.alpha == 0.f || p.alpha == 1.f) && !p.bias_along_m && !p.bias_f && !p.resid_f &&
+                        (p.act == ACT_NONE || gelu);
+    // its paired stores: 16-byte row pitches and base pointers, whole 8-column groups (A and B are checked above)
+    const bool wg_ok = wg_epi && p.N % 8 == 0 && p.ldc % 8 == 0 && aligned16(p.C) && (!p.resid || (p.ldr % 8 == 0 && aligned16(p.resid)));
     // the convolution walks whole 64-channel blocks of 16 x 8 pixel boxes over an unscaled map
     const bool wg_conv = p.amode == A_CONV3x3 && !p.ups && p.Cin % WG_BK == 0 && p.Ho == p.Hs && p.Wo == p.Ws && p.Hs >= WG_TH && p.Ws >= WG_TW;
-    if (wg_ok && (p.amode == A_PLAIN || wg_conv)) {
-        WgP q;
-        memset(&q, 0, sizeof(q));
-        q.M = p.M; q.N = p.N; q.K = p.K; q.resid = p.resid; q.ldr = p.ldr; q.C = (bf16*)p.C; q.ldc = p.ldc;
-        q.act = p.act; q.bias = p.bias; q.scale = p.scale;
-        if (p.amode == A_PLAIN) return wg_plain<false>(st, q, p.A, p.lda, p.B, p.ldb);
-        return wg_conv3<false>(st, q, p.A, p.M / (p.Hs * p.Ws), p.Hs, p.Ws, p.Cin, p.Hs, p.Ws, p.B, p.ldb);
-    }
-    return dg_launch<false>(st, p, batch);
+    if (wg_ok && p.amode == A_PLAIN) return GEMM_WGMMA;
+    if (wg_ok && wg_conv) return GEMM_WGMMA_CONV3;
+    return GEMM_MMA;
+}
+
+int gemm(cudaStream_t st, const DenseP& dp, int batch) {
+    const int route = gemm_route(dp, batch);
+    if (route < 0) return route;
+    if (dp.M == 0 || dp.N == 0) return CAR_OK;
+    DenseP p = dp;
+    if (p.alpha == 0.f) p.alpha = 1.f;
+    if (route == GEMM_MMA_WIN) return dg_launch<true>(st, p, batch);
+    if (route == GEMM_MMA) return dg_launch<false>(st, p, batch);
+    WgP q;
+    memset(&q, 0, sizeof(q));
+    q.M = p.M; q.N = p.N; q.K = p.K; q.resid = p.resid; q.ldr = p.ldr; q.C = (bf16*)p.C; q.ldc = p.ldc;
+    q.act = p.act; q.bias = p.bias; q.scale = p.scale;
+    if (route == GEMM_WGMMA) return wg_plain<false>(st, q, p.A, p.lda, p.B, p.ldb);
+    return wg_conv3<false>(st, q, p.A, p.M / (p.Hs * p.Ws), p.Hs, p.Ws, p.Cin, p.Hs, p.Ws, p.B, p.ldb);
 }
 
 int gemm_f32(cudaStream_t st, const bf16* A, const bf16* B, int M, int N, int K, const float* bias, const float* resid, float* out, int ldc) {
+    if (!A || !B) CAR_FAIL(CAR_ERR_ARG, "A and B must be non-null");
+    if (!out) CAR_FAIL(CAR_ERR_ARG, "out must be non-null");
+    // the fp32 epilogue's paired float2 stores and loads
+    if (!aligned(out, 8) || (resid && !aligned(resid, 8))) CAR_FAIL(CAR_ERR_ARG, "out and resid must be 8-byte aligned");
+    if (M < 0) CAR_FAIL(CAR_ERR_ARG, "M must be >= 0");
+    if (N <= 0 || N % 8) CAR_FAIL(CAR_ERR_ARG, "N must be a positive multiple of 8");
+    if (K <= 0 || K % 8) CAR_FAIL(CAR_ERR_ARG, "K must be a positive multiple of 8");
+    if (ldc < N || ldc % 2) CAR_FAIL(CAR_ERR_ARG, "ldc must be >= N and even");
+    if (!aligned16(A) || !aligned16(B)) CAR_FAIL(CAR_ERR_ARG, "A and B must be 16-byte aligned");
+    if (M == 0) return CAR_OK;
     WgP q;
     memset(&q, 0, sizeof(q));
     q.M = M; q.N = N; q.K = K; q.bias_f = bias; q.resid_f = resid; q.ldr = ldc; q.C32 = out; q.ldc = ldc;
@@ -116,6 +182,15 @@ int gemm_f32(cudaStream_t st, const bf16* A, const bf16* B, int M, int N, int K,
 
 int gemm_f32_conv3(cudaStream_t st, const bf16* src, int fh, int fw, const bf16* B, int nimg, int H, int W, int cin, int N, const float* bias,
                    const float* resid, float* out) {
+    if (!src || !B) CAR_FAIL(CAR_ERR_ARG, "src and B must be non-null");
+    if (!out) CAR_FAIL(CAR_ERR_ARG, "out must be non-null");
+    // the fp32 epilogue's paired float2 stores and loads
+    if (!aligned(out, 8) || (resid && !aligned(resid, 8))) CAR_FAIL(CAR_ERR_ARG, "out and resid must be 8-byte aligned");
+    if (nimg <= 0 || H <= 0 || W <= 0) CAR_FAIL(CAR_ERR_ARG, "nimg, H and W must be > 0");
+    if (cin <= 0 || cin % WG_CBLK) CAR_FAIL(CAR_ERR_ARG, "cin must be a positive multiple of 64");
+    if (N <= 0 || N % 8) CAR_FAIL(CAR_ERR_ARG, "N must be a positive multiple of 8");
+    if (fh < H || fw < W || fh < WG_TH || fw < WG_TW) CAR_FAIL(CAR_ERR_ARG, "the frame must hold the H x W map and one 16 x 8 pixel box");
+    if (!aligned16(src) || !aligned16(B)) CAR_FAIL(CAR_ERR_ARG, "src and B must be 16-byte aligned");
     WgP q;
     memset(&q, 0, sizeof(q));
     q.M = nimg * H * W; q.N = N; q.K = 9 * cin; q.bias_f = bias; q.resid_f = resid; q.ldr = N; q.C32 = out; q.ldc = N;

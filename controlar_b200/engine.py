@@ -11,7 +11,7 @@ from typing import List, Optional
 import torch
 
 from . import _lib
-from ._lib import (CarModelDesc, CarSampling, CarTrainWeights, CarWeights, check, cur_stream, dtype_code, on_own_device,
+from ._lib import (CarGemmDesc, CarModelDesc, CarSampling, CarTrainWeights, CarWeights, check, cur_stream, dtype_code, on_own_device,
                    param_signature, _ptr, _ptr_array)
 
 
@@ -412,6 +412,39 @@ def op_dense_linear(x: torch.Tensor, w: torch.Tensor, resid: Optional[torch.Tens
         check(lib.car_op_dense_linear(_ptr(x.contiguous()), _ptr(w.detach().contiguous()), _ptr(resid.contiguous()) if resid is not None else None,
                                       _ptr(y), M, N, K, int(act), cur_stream()), "car_op_dense_linear")
     return y
+
+
+def gemm_desc(**fields) -> CarGemmDesc:
+    """A CarGemmDesc (gemm.h's DenseP) from keyword fields; tensors are replaced by their data pointers, alpha defaults to 1."""
+    d = CarGemmDesc(alpha=1.0)
+    for k, v in fields.items():
+        setattr(d, k, v.data_ptr() if torch.is_tensor(v) else v)
+    return d
+
+
+def op_gemm_route(desc: CarGemmDesc, batch: int = 1) -> int:
+    """The route gemm() takes for (desc, batch) (car_op_gemm_route): 0 wgmma plain, 1 wgmma 3x3 convolution, 2 mma.sync, 3 mma.sync
+    window, or a negative error code when gemm() would refuse it (message in car_last_error).  Host only."""
+    return _lib.lib().car_op_gemm_route(C.byref(desc), int(batch))
+
+
+def op_gemm(desc: CarGemmDesc, batch: int = 1) -> None:
+    """gemm() on the current device's current stream (car_op_gemm); raises when the descriptor is refused."""
+    check(_lib.lib().car_op_gemm(C.byref(desc), int(batch), cur_stream()), "car_op_gemm")
+
+
+def op_gemm_f32(A, B, M: int, N: int, K: int, bias, resid, out, ldc: int) -> None:
+    """gemm_f32 (car_op_gemm_f32): out fp32 [M][ldc] = A [M][K] . B [N][K]^T + bias (+ resid).  Tensors or raw device pointers."""
+    p = lambda t: t.data_ptr() if torch.is_tensor(t) else t
+    check(_lib.lib().car_op_gemm_f32(p(A), p(B), M, N, K, p(bias), p(resid), p(out), ldc, cur_stream()), "car_op_gemm_f32")
+
+
+def op_gemm_f32_conv3(src, fh: int, fw: int, B, nimg: int, H: int, W: int, cin: int, N: int, bias, resid, out) -> None:
+    """gemm_f32_conv3 (car_op_gemm_f32_conv3): 3x3 / pad 1 convolution of the NHWC frame src [nimg][fh][fw][cin] -> out fp32
+    [nimg][H][W][N] (+ bias, + resid).  Tensors or raw device pointers."""
+    p = lambda t: t.data_ptr() if torch.is_tensor(t) else t
+    check(_lib.lib().car_op_gemm_f32_conv3(p(src), fh, fw, p(B), nimg, H, W, cin, N, p(bias), p(resid), p(out), cur_stream()),
+          "car_op_gemm_f32_conv3")
 
 
 def op_rmsnorm(x: torch.Tensor, w: torch.Tensor, eps: float) -> torch.Tensor:

@@ -160,10 +160,42 @@ int64_t car_launch_count(int32_t reset);
 /* y[M,N] = act(x[M,K] @ W[N,K]^T (+bias)); act: 0 none, 1 GELU-tanh (gpt_t2i.py:171), 2 GELU-erf. */
 int car_op_linear(int32_t dtype, const void* x, const void* w, const void* bias, void* y, int32_t M, int32_t N,
                   int32_t K, int32_t act, void* stream);
-/* y[M,N] = act(x[M,K] w[N,K]^T) (+ resid[M,N]) on the dense tensor-core path of the prefill (bf16, fp32 accumulate; act 1 = GELU-tanh);
- * K, N multiples of 8.  Unit-test / micro-benchmark hook for csrc/gemm_tc5.cuh. */
+/* y[M,N] = act(x[M,K] w[N,K]^T) (+ resid[M,N]) on the dense tensor-core path of the prefill (bf16, fp32 accumulate; act 1 = GELU-tanh),
+ * through gemm() (csrc/gemm.cu): K a multiple of 8, x and w 16-byte aligned.  Unit-test / micro-benchmark hook. */
 int car_op_dense_linear(const void* x, const void* w, const void* resid, void* y, int32_t M, int32_t N, int32_t K, int32_t act,
                         void* stream);
+
+/* The dense GEMM front end (csrc/gemm.h), exposed for conformance tests.  CarGemmDesc mirrors gemm.h's DenseP field for field
+ * (pointers are device pointers; bf16 operands, fp32 bias_f / resid_f); the contract, the epilogue order and the routes are
+ * documented there.
+ * car_op_gemm_route: the route gemm() takes for (desc, batch): 0 wgmma plain, 1 wgmma 3x3 convolution, 2 mma.sync, 3 mma.sync
+ *   window; < 0 (CAR_ERR_ARG, message in car_last_error) when the descriptor is refused.  Host only: never touches the device.
+ * car_op_gemm: gemm() itself, the code path every library caller takes.
+ * car_op_gemm_f32 / car_op_gemm_f32_conv3: gemm.h's gemm_f32 and gemm_f32_conv3 (fp32 output over split-bf16 operands). */
+typedef struct CarGemmDesc {
+    const void *A, *B;
+    int32_t M, N, K;
+    int32_t lda, ldb;
+    int64_t sA, sB, sC, sR;
+    int32_t amode, Hs, Ws, Cin, Ho, Wo, ups;
+    float alpha;
+    const void* bias; int32_t bias_along_m;
+    const float* bias_f;
+    const float* resid_f;
+    int32_t act;
+    const void* scale;
+    const void* resid; int32_t ldr;
+    void* C; int32_t ldc;
+    int32_t out_mode;
+    int32_t kh, kw, ws;
+    int32_t osy, osx, oay, oax, oH, oW;
+} CarGemmDesc;
+int car_op_gemm_route(const CarGemmDesc* desc, int32_t batch);
+int car_op_gemm(const CarGemmDesc* desc, int32_t batch, void* stream);
+int car_op_gemm_f32(const void* A, const void* B, int32_t M, int32_t N, int32_t K, const float* bias, const float* resid, float* out,
+                    int32_t ldc, void* stream);
+int car_op_gemm_f32_conv3(const void* src, int32_t fh, int32_t fw, const void* B, int32_t nimg, int32_t H, int32_t W, int32_t cin,
+                          int32_t N, const float* bias, const float* resid, float* out, void* stream);
 
 /* RMSNorm.forward (gpt_t2i.py:193-198). */
 int car_op_rmsnorm(int32_t dtype, const void* x, const void* w, void* y, int32_t M, int32_t K, float eps,
