@@ -107,9 +107,9 @@ static void tr_keep_scale(float p, float* keep, float* scale) {
     *keep = (float)(1.0 - (double)p);
     *scale = (float)(1.0 / (double)*keep);
 }
-// the fused dropout of one site of layer l under the settings c; every part off when its p (or rate) is 0
+// the dropout of one site of layer l under the settings c; every part off when its p (or rate) is 0
 static TrDrop tr_drop(const CarTrain::DropCfg& c, int site, int l) {
-    TrDrop r{c.seed, site, l, 1.f, 1.f, 0, 1.f, 1.f};
+    TrDrop r{c.seed, site, l};
     const float p = site == CAR_DROP_TOKEN ? c.tok_p : (site == CAR_DROP_RESID ? c.resid_p : c.ffn_p);
     if (p > 0.f) tr_keep_scale(p, &r.keep, &r.scale);
     const float rate = (site != CAR_DROP_TOKEN && !c.path.empty()) ? c.path[l] : 0.f;
@@ -121,7 +121,6 @@ static TrDrop tr_drop(const CarTrain::DropCfg& c, int site, int l) {
     }
     return r;
 }
-static bool tr_drop_on(const TrDrop& r) { return r.seed != nullptr && (r.keep < 1.f || r.path_keep < 1.f); }
 
 // MLP.forward gpt_t2i.py:177-181 on bf16 operands: out = fc2(gelu_tanh(fc1 x))
 static int tr_mlp(cudaStream_t st, const bf16* x, int rows, int K, const bf16* fc1, const bf16* fc2, int d, Buf<bf16> tmp, Buf<bf16> out) {
@@ -205,23 +204,6 @@ extern "C" int car_train_destroy(CarTrain* t) {
     return CAR_OK;
 }
 
-// h += branch output t->o (fp32 += bf16, gpt_t2i.py:305-306) with the branch's dropout and drop path of the last forward's settings
-static int tr_residual_add(CarTrain* t, cudaStream_t st, int site, int l, int R, int B, int S) {
-    const int dim = t->d.dim;
-    const TrDrop dr = tr_drop(t->drop_fwd, site, l);
-    if (tr_drop_on(dr)) CAR_LAUNCH(tr_add_rows_drop_kernel, gsz((long long)R * dim / 4), 256, 0, st, (float*)t->h, (const bf16*)t->o, B, S, dim, dr);
-    else CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)R * dim), 256, 0, st, (float*)t->h, (const bf16*)t->o, B, S, S, 0, dim);
-    return CAR_OK;
-}
-// the bf16 gradient of a branch output from the fp32 stream gradient t->dh, through the branch's drop path and dropout
-static int tr_residual_take(CarTrain* t, cudaStream_t st, int site, int l, int R, int B, int S) {
-    const int dim = t->d.dim;
-    const TrDrop dr = tr_drop(t->drop_fwd, site, l);
-    if (tr_drop_on(dr)) CAR_LAUNCH(tr_take_rows_drop_kernel, gsz((long long)R * dim / 4), 256, 0, st, (const float*)t->dh, (bf16*)t->db, B, S, S, 0, dim, dr);
-    else CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)R * dim), 256, 0, st, (const float*)t->dh, (bf16*)t->db, B, S, S, 0, dim);
-    return CAR_OK;
-}
-
 // One TransformerBlock (gpt_t2i.py:303-307) on the fp32 stream t->h, preceded by the control add of gpt_t2i.py:458-460 when the
 // block opens a third of the stack.  for_bwd: the recompute of car_train_backward — keeps the block input (after the control
 // add) in t->h0, the attention-side norm output in t->x, the feed-forward-side one in t->x2, and stops before w2 (t->h then
@@ -232,7 +214,7 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     const int n = n_img - 1, S = T + n, R = B * S, RC = B * n_img, step3 = L / 3;
     if (has_feat && l % step3 == 0) {
         CAR_TRY(tr_mlp(st, t->ctok, RC, dim, t->b_ctl1[l / step3], t->b_ctl2[l / step3], dim, t->ctmp, t->cadd));
-        CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)RC * dim), 256, 0, st, (float*)t->h, (const bf16*)t->cadd, B, n_img, S, T - 1, dim);
+        CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)RC * dim / 4), 256, 0, st, (float*)t->h, (const bf16*)t->cadd, B, n_img, S, T - 1, dim, TrDrop{});
     }
     if (for_bwd) CAR_CUDA(cudaMemcpyAsync(t->h0, t->h, (size_t)R * dim * 4, cudaMemcpyDeviceToDevice, st));
     size_t att_smem = 0;
@@ -243,7 +225,9 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     CAR_LAUNCH(tr_attention_kernel, (unsigned)(((long long)B * H * S + TRA_WARPS - 1) / TRA_WARPS), TRA_WARPS * 32, att_smem, st, (const bf16*)t->q,
                (const bf16*)t->kc, (const bf16*)t->vc, mask, B, H, S, (bf16*)t->att, 1);
     CAR_TRY(gemm(st, dp_plain(t->att, dim, t->b_wo[l], dim, R, dim, dim, t->o, dim)));
-    CAR_TRY(tr_residual_add(t, st, CAR_DROP_RESID, l, R, B, S));
+    // h += branch output (gpt_t2i.py:305-306) through the branch's dropout and drop path of the last forward's settings
+    CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)R * dim / 4), 256, 0, st, (float*)t->h, (const bf16*)t->o, B, S, S, 0, dim,
+               tr_drop(t->drop_fwd, CAR_DROP_RESID, l));
     bf16* xn = for_bwd ? t->x2 : t->x;
     CAR_LAUNCH(tr_rmsnorm_kernel, R, 256, 0, st, (const float*)t->h, (const float*)t->ffn_norm[l], xn, dim, d.norm_eps, S, S, 0);
     CAR_TRY(gemm(st, dp_plain(xn, dim, t->b_w1[l], dim, R, F, dim, t->g, F)));
@@ -251,7 +235,8 @@ static int tr_block_fwd(CarTrain* t, cudaStream_t st, int l, int B, int n_img, c
     CAR_LAUNCH(swiglu_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, (bf16*)t->act, (long long)R * F);
     if (for_bwd) return CAR_OK;
     CAR_TRY(gemm(st, dp_plain(t->act, F, t->b_w2[l], F, R, dim, F, t->o, dim)));
-    CAR_TRY(tr_residual_add(t, st, CAR_DROP_FFN, l, R, B, S));
+    CAR_LAUNCH(tr_add_rows_kernel, gsz((long long)R * dim / 4), 256, 0, st, (float*)t->h, (const bf16*)t->o, B, S, S, 0, dim,
+               tr_drop(t->drop_fwd, CAR_DROP_FFN, l));
     return CAR_OK;
 }
 
@@ -269,7 +254,6 @@ extern "C" int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const in
     t->fwd_ok = false;
     t->drop_fwd = t->drop_next;
     const TrDrop dtok = tr_drop(t->drop_fwd, CAR_DROP_TOKEN, 0);
-    const bool tok_on = tr_drop_on(dtok);
     // 0. autocast: bf16 copies of every nn.Linear weight, re-cast each forward (the fp32 masters may have been stepped)
     for (int l = 0; l < L; ++l) {
         CAR_TRY(tr_cast(st, t->wqkv[l], t->b_wqkv[l], (long long)3 * dim * dim)); CAR_TRY(tr_cast(st, t->wo[l], t->b_wo[l], (long long)dim * dim));
@@ -284,22 +268,16 @@ extern "C" int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const in
         CAR_TRY(tr_cast(st, t->w.adapter_fc1, t->b_ad1, (long long)dim * t->w.adapter_dim)); CAR_TRY(tr_cast(st, t->w.adapter_fc2, t->b_ad2, (long long)dim * dim));
     }
     // 1. prefix rows: CaptionEmbedder (token_drop, cap_proj) gpt_t2i.py:145-162 or LabelEmbedder :78-97; image-token rows :423;
-    //    tok_dropout (:430) fused into the writes of both
+    //    tok_dropout (:430) applied by the writes of both
     if (d.model_type == 1) {
         CAR_LAUNCH(tr_caption_select_kernel, gsz((long long)B * T * d.caption_dim), 256, 0, st, (const float*)cond, (const float*)t->w.cap_uncond,
                    drop_ids, (bf16*)t->capx, B, T, d.caption_dim);
         CAR_TRY(tr_mlp(st, t->capx, B * T, d.caption_dim, t->b_cap1, t->b_cap2, dim, t->ctmp, t->o));
-        if (tok_on) CAR_LAUNCH(tr_put_rows_drop_kernel, gsz((long long)B * T * dim / 4), 256, 0, st, (const bf16*)t->o, (float*)t->h, B, T, S, 0, dim, dtok);
-        else CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const bf16*)t->o, (float*)t->h, B, T, S, 0, dim);
-    } else if (tok_on) {
-        CAR_LAUNCH(tr_embed_rows_drop_kernel, B, 256, 0, st, (const float*)t->w.w.label_table, (const int*)cond, 1, drop_ids, t->w.num_classes, (float*)t->h, B, 1, S, 0, dim, dtok);
+        CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)B * T * dim / 4), 256, 0, st, (const bf16*)t->o, (float*)t->h, B, T, S, 0, dim, dtok);
     } else {
-        CAR_LAUNCH(tr_embed_rows_kernel, B, 256, 0, st, (const float*)t->w.w.label_table, (const int*)cond, 1, drop_ids, t->w.num_classes, (float*)t->h, B, 1, S, 0, dim);
+        CAR_LAUNCH(tr_embed_rows_kernel, B, 256, 0, st, (const float*)t->w.w.label_table, (const int*)cond, 1, drop_ids, t->w.num_classes, (float*)t->h, B, 1, S, 0, dim, dtok);
     }
-    if (tok_on)
-        CAR_LAUNCH(tr_embed_rows_drop_kernel, B * n, 256, 0, st, (const float*)t->w.w.tok_embeddings, (const int*)idx, n, (const unsigned char*)nullptr, 0, (float*)t->h, B, n, S, T, dim, dtok);
-    else
-        CAR_LAUNCH(tr_embed_rows_kernel, B * n, 256, 0, st, (const float*)t->w.w.tok_embeddings, (const int*)idx, n, (const unsigned char*)nullptr, 0, (float*)t->h, B, n, S, T, dim);
+    CAR_LAUNCH(tr_embed_rows_kernel, B * n, 256, 0, st, (const float*)t->w.w.tok_embeddings, (const int*)idx, n, (const unsigned char*)nullptr, 0, (float*)t->h, B, n, S, T, dim, dtok);
     // 2. control tokens: adapter_mlp -> token_drop -> condition_mlp  gpt_t2i.py:424-427 (feat = the control encoder's output tokens)
     if (feat) {
         CAR_TRY(tr_mlp(st, (const bf16*)feat, RC, t->w.adapter_dim, t->b_ad1, t->b_ad2, dim, t->ctmp, t->cin));
@@ -318,7 +296,7 @@ extern "C" int car_train_forward(CarTrain* t, int32_t B, int32_t n_img, const in
         CAR_LAUNCH(tr_ce_rows_kernel, RC, 256, 0, st, (const bf16*)t->lg, (const int*)targets, logits_out, (float*)t->nll, V);
         CAR_LAUNCH(tr_ce_reduce_kernel, 1, 1024, 0, st, (const float*)t->nll, valid, B, n_img, loss_out);
     } else if (logits_out) {
-        CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)RC * V), 256, 0, st, (const bf16*)t->lg, logits_out, 1, RC, RC, 0, V);
+        CAR_LAUNCH(tr_put_rows_bf16_kernel, gsz((long long)RC * V / 4), 256, 0, st, (const bf16*)t->lg, logits_out, 1, RC, RC, 0, V, TrDrop{});
     }
     t->fB = B; t->fN = n_img; t->f_idx = idx; t->f_cond = cond; t->f_feat = feat; t->f_drop = drop_ids; t->f_mask = mask; t->f_targets = targets;
     t->f_valid = valid;
@@ -380,7 +358,8 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         CAR_CUDA(cudaMemcpyAsync(t->h, t->hs + (size_t)l * R * dim, (size_t)R * dim * 4, cudaMemcpyDeviceToDevice, st));
         CAR_TRY(tr_block_fwd(t, st, l, B, n_img, mask, has_feat, true));
         // feed-forward: h_out = h_mid + drop_path(ffn_dropout(w2(silu(w1 x2) * w3 x2)))
-        CAR_TRY(tr_residual_take(t, st, CAR_DROP_FFN, l, R, B, S));
+        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)R * dim / 4), 256, 0, st, (const float*)t->dh, (bf16*)t->db, B, S, S, 0, dim,
+                   tr_drop(t->drop_fwd, CAR_DROP_FFN, l));
         CAR_TRY(tr_wgrad_f32(st, sc, t->db, t->act, R, dim, F, g->w.w2 ? (float*)g->w.w2[l] : nullptr));
         CAR_TRY(tr_dgrad(st, sc, t->db, t->b_w2[l], R, dim, F, nullptr, t->dact));
         CAR_LAUNCH(tr_swiglu_bwd_kernel, sm_count() * 8, 256, 0, st, (const bf16*)t->g, (const bf16*)t->u, (const bf16*)t->dact, (bf16*)t->dg, (bf16*)t->du, (long long)R * F);
@@ -390,7 +369,8 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         CAR_TRY(tr_dgrad(st, sc, t->du, t->b_w3[l], R, F, dim, t->dx, t->dx));
         CAR_TRY(tr_norm_bwd(t, st, t->h, t->ffn_norm[l], t->dx, R, S, S, 0, g->w.ffn_norm ? (float*)g->w.ffn_norm[l] : nullptr));
         // attention: h_mid = h0 + drop_path(resid_dropout(wo(sdpa(rope(wqkv x1)))))
-        CAR_TRY(tr_residual_take(t, st, CAR_DROP_RESID, l, R, B, S));
+        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)R * dim / 4), 256, 0, st, (const float*)t->dh, (bf16*)t->db, B, S, S, 0, dim,
+                   tr_drop(t->drop_fwd, CAR_DROP_RESID, l));
         CAR_TRY(tr_wgrad_f32(st, sc, t->db, t->att, R, dim, dim, g->w.wo ? (float*)g->w.wo[l] : nullptr));
         CAR_TRY(tr_dgrad(st, sc, t->db, t->b_wo[l], R, dim, dim, nullptr, t->datt));
         CAR_LAUNCH(tr_attn_bwd_q_kernel, att_grid, TRA_WARPS * 32, smem_q, st, (const bf16*)t->q, (const bf16*)t->kc, (const bf16*)t->vc, mask,
@@ -405,7 +385,8 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
         if (has_feat && l % step3 == 0) {
             const int j = l / step3;
             CAR_TRY(car_fits("car_train_backward", t->dadd, (size_t)RC * dim));
-            CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)RC * dim), 256, 0, st, (const float*)t->dh, (bf16*)t->dadd, B, n_img, S, T - 1, dim);
+            CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)RC * dim / 4), 256, 0, st, (const float*)t->dh, (bf16*)t->dadd, B, n_img, S, T - 1, dim,
+                       TrDrop{});
             CAR_TRY(tr_mlp_bwd(t, st, t->ctok, RC, dim, t->b_ctl1[j], t->b_ctl2[j], t->dadd, first_ctl ? nullptr : (const bf16*)t->dctok, t->dctok,
                                (float*)g->w.ctl_fc1[j], (float*)g->w.ctl_fc2[j]));
             first_ctl = false;
@@ -413,29 +394,19 @@ extern "C" int car_train_backward(CarTrain* t, const CarTrainWeights* g, void* d
     }
     // ---- embeddings and the prefix / control front ends; dh is the gradient of tok_dropout's output, its mask applies first ----
     const TrDrop dtok = tr_drop(t->drop_fwd, CAR_DROP_TOKEN, 0);
-    const bool tok_on = tr_drop_on(dtok);
     if (g->w.tok_embeddings) {
         CAR_CUDA(cudaMemsetAsync((void*)g->w.tok_embeddings, 0, (size_t)V * dim * 4, st));
-        if (tok_on)
-            CAR_LAUNCH(tr_embed_grad_drop_kernel, B * n, 256, 0, st, (const float*)t->dh, (const int*)t->f_idx, n, (const unsigned char*)nullptr, 0,
-                       (float*)g->w.tok_embeddings, B, n, S, T, dim, dtok);
-        else
-            CAR_LAUNCH(tr_embed_grad_kernel, B * n, 256, 0, st, (const float*)t->dh, (const int*)t->f_idx, n, (const unsigned char*)nullptr, 0,
-                       (float*)g->w.tok_embeddings, B, n, S, T, dim);
+        CAR_LAUNCH(tr_embed_grad_kernel, B * n, 256, 0, st, (const float*)t->dh, (const int*)t->f_idx, n, (const unsigned char*)nullptr, 0,
+                   (float*)g->w.tok_embeddings, B, n, S, T, dim, dtok);
     }
     if (d.model_type == 1) {
         CAR_TRY(car_fits("car_train_backward", t->dadd, (size_t)B * T * dim));
-        if (tok_on) CAR_LAUNCH(tr_take_rows_drop_kernel, gsz((long long)B * T * dim / 4), 256, 0, st, (const float*)t->dh, (bf16*)t->dadd, B, T, S, 0, dim, dtok);
-        else CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)B * T * dim), 256, 0, st, (const float*)t->dh, (bf16*)t->dadd, B, T, S, 0, dim);
+        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)B * T * dim / 4), 256, 0, st, (const float*)t->dh, (bf16*)t->dadd, B, T, S, 0, dim, dtok);
         CAR_TRY(tr_mlp_bwd(t, st, t->capx, B * T, d.caption_dim, t->b_cap1, t->b_cap2, t->dadd, nullptr, nullptr, (float*)g->w.cap_fc1, (float*)g->w.cap_fc2));
     } else if (g->w.label_table) {
         CAR_CUDA(cudaMemsetAsync((void*)g->w.label_table, 0, (size_t)(t->w.num_classes + 1) * dim * 4, st));
-        if (tok_on)
-            CAR_LAUNCH(tr_embed_grad_drop_kernel, B, 256, 0, st, (const float*)t->dh, (const int*)t->f_cond, 1, t->f_drop, t->w.num_classes,
-                       (float*)g->w.label_table, B, 1, S, 0, dim, dtok);
-        else
-            CAR_LAUNCH(tr_embed_grad_kernel, B, 256, 0, st, (const float*)t->dh, (const int*)t->f_cond, 1, t->f_drop, t->w.num_classes, (float*)g->w.label_table,
-                       B, 1, S, 0, dim);
+        CAR_LAUNCH(tr_embed_grad_kernel, B, 256, 0, st, (const float*)t->dh, (const int*)t->f_cond, 1, t->f_drop, t->w.num_classes,
+                   (float*)g->w.label_table, B, 1, S, 0, dim, dtok);
     }
     if (has_feat) {
         CAR_TRY(tr_mlp_bwd(t, st, t->cin, RC, dim, t->b_cond1, t->b_cond2, t->dctok, nullptr, t->dcin, (float*)g->w.cond_fc1, (float*)g->w.cond_fc2));
@@ -760,7 +731,7 @@ extern "C" int car_dino_train_backward(CarDinoTrain* m, const float* d_feat, con
         CAR_LAUNCH(dt_cubic_t_kernel, gsz((long long)G * G * C), 256, 0, st, (const float*)s.ptmp, dpos + C, G, w, G, C);
     }
     if (g->patch_w || g->patch_b) {
-        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)B * hw * C), 256, 0, st, (const float*)s.dx, (bf16*)s.db, B, hw, Tn, 1, C);
+        CAR_LAUNCH(tr_take_rows_bf16_kernel, gsz((long long)B * hw * C / 4), 256, 0, st, (const float*)s.dx, (bf16*)s.db, B, hw, Tn, 1, C, TrDrop{});
         if (g->patch_w) {
             CAR_TRY(tr_wgrad(st, sc, s.db, s.patches, B * hw, C, m->kpad));
             CAR_TRY(tr_weight_grad(st, sc, 0, C, m->kpatch, m->kpad, (float*)g->patch_w));

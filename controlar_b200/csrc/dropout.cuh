@@ -1,6 +1,6 @@
 // dropout.cuh — the keep decisions of the training path's dropout layers (reference gpt_t2i.py:217,290,430 nn.Dropout and the
-// stochastic depth of utils/drop_path.py, TransformerBlock gpt_t2i.py:305-306) and the kernels that fuse them into the existing
-// passes of the training forward / backward.
+// stochastic depth of utils/drop_path.py, TransformerBlock gpt_t2i.py:305-306).  The row passes of the training forward / backward
+// (train.cuh, train_bwd.cuh) take a TrDrop and apply the masks as they write; a site that is off skips its mask steps.
 //
 // Generator: Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011), stateless and counter based.
 // Key = the 64-bit seed, counter = (column / 4, row, sample, site << 16 | layer); the four output words are the decisions of the
@@ -39,129 +39,27 @@ __device__ __forceinline__ uint4 car_dropout_bits(uint64_t seed, int site, int l
 
 __device__ __forceinline__ float car_keep_bit(uint32_t r, float keep) { return (float)(r >> 8) * 0x1p-24f < keep ? 1.f : 0.f; }
 
-// What one fused pass applies.  Element dropout (nn.Dropout on CUDA): x * mask * scale in fp32, scale = fp32(1 / keep), one
+// What one row pass applies.  Element dropout (nn.Dropout on CUDA): x * mask * scale in fp32, scale = fp32(1 / keep), one
 // rounding to the tensor's dtype; off when keep >= 1.  Drop path: x * bf16(bernoulli(keep) / keep) on the bf16 branch, one draw
-// per sample; off when path_keep >= 1.  seed == nullptr: both off.
+// per sample; off when path_keep >= 1.  TrDrop{} is both off; seed is read only when one of them is on.
 struct TrDrop {
-    const uint64_t* seed;
-    int site, layer;
-    float keep, scale;
-    int path_site;
-    float path_keep, path_mult;
+    const uint64_t* seed = nullptr;
+    int site = CAR_DROP_TOKEN, layer = 0;
+    float keep = 1.f, scale = 1.f;
+    int path_site = 0;
+    float path_keep = 1.f, path_mult = 1.f;
 };
+
+__device__ __forceinline__ uint64_t tr_drop_seed(const TrDrop& dr) { return dr.keep < 1.f || dr.path_keep < 1.f ? *dr.seed : 0; }
+
+// the keep words of columns 4 c4 .. 4 c4 + 3 of (sample b, row); zeros when element dropout is off (then nothing reads them)
+__device__ __forceinline__ uint4 tr_drop_words(const TrDrop& dr, uint64_t seed, int b, int row, int c4) {
+    return dr.keep < 1.f ? car_dropout_bits(seed, dr.site, dr.layer, b, row, c4) : make_uint4(0, 0, 0, 0);
+}
 
 __device__ __forceinline__ float tr_path_mult(const TrDrop& dr, uint64_t seed, int b) {
     if (dr.path_keep >= 1.f) return 1.f;
     return car_keep_bit(car_dropout_bits(seed, dr.path_site, dr.layer, b, 0, 0).x, dr.path_keep) * dr.path_mult;
-}
-
-// forward of a residual branch: h[b][s][:] += float(bf16(bf16(o * m * scale) * path)), o = add[b][s][:] bf16 (the wo / w2 output),
-// every step skipped when its site is off.  Four columns per thread (one generator call); d % 4 == 0.
-__global__ void tr_add_rows_drop_kernel(float* __restrict__ h, const bf16* __restrict__ add, int B, int S, int d, TrDrop dr) {
-    const uint64_t seed = *dr.seed;
-    const int d4 = d / 4;
-    const long long total = (long long)B * S * d4;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int c4 = (int)(i % d4);
-        const long long rs = i / d4;
-        const int s = (int)(rs % S), b = (int)(rs / S);
-        const uint4 r = dr.keep < 1.f ? car_dropout_bits(seed, dr.site, dr.layer, b, s, c4) : make_uint4(0, 0, 0, 0);
-        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-        const float pm = tr_path_mult(dr, seed, b);
-        const size_t o = (size_t)rs * d + 4 * c4;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            float v = __bfloat162float(add[o + e]);
-            if (dr.keep < 1.f) v = rnd<bf16>(v * car_keep_bit(rr[e], dr.keep) * dr.scale);
-            if (dr.path_keep < 1.f) v = rnd<bf16>(v * pm);
-            h[o + e] = h[o + e] + v;
-        }
-    }
-}
-
-// backward of the same branch, as autograd orders it: out = bf16(bf16(bf16(dh) * path) * m * scale) — the bf16 gradient the
-// wo / w2 output receives from the fp32 stream through drop path and then dropout.
-// Token site (the prefix rows of the caption MLP): out[b][j][:] = bf16(dh[b][row0 + j][:] * m * scale), fp32 product first.
-__global__ void tr_take_rows_drop_kernel(const float* __restrict__ dh, bf16* __restrict__ out, int B, int nrows, int S, int row0, int d, TrDrop dr) {
-    const uint64_t seed = *dr.seed;
-    const int d4 = d / 4;
-    const long long total = (long long)B * nrows * d4;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int c4 = (int)(i % d4);
-        const long long rj = i / d4;
-        const int j = (int)(rj % nrows), b = (int)(rj / nrows);
-        const int s = row0 + j;
-        const uint4 r = dr.keep < 1.f ? car_dropout_bits(seed, dr.site, dr.layer, b, s, c4) : make_uint4(0, 0, 0, 0);
-        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-        const float pm = tr_path_mult(dr, seed, b);
-        const float* src = dh + ((size_t)b * S + s) * d + 4 * c4;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            float g = src[e];
-            if (dr.site == CAR_DROP_TOKEN) {
-                g = g * car_keep_bit(rr[e], dr.keep) * dr.scale;
-            } else {
-                g = rnd<bf16>(g);
-                if (dr.path_keep < 1.f) g = rnd<bf16>(g * pm);
-                if (dr.keep < 1.f) g = g * car_keep_bit(rr[e], dr.keep) * dr.scale;
-            }
-            out[(size_t)rj * d + 4 * c4 + e] = __float2bfloat16_rn(g);
-        }
-    }
-}
-
-// token dropout on the fp32 rows the embedding gathers write (tok_dropout gpt_t2i.py:430, after the cat that promotes to fp32):
-// h[b][row0 + j][:] = table[index(b, j)][:] * m * scale — tr_embed_rows_kernel with the mask fused.  One CTA per row.
-__global__ void tr_embed_rows_drop_kernel(const float* __restrict__ table, const int* __restrict__ idx, int ld, const unsigned char* __restrict__ drop,
-                                          int drop_to, float* __restrict__ h, int B, int nrows, int S, int row0, int d, TrDrop dr) {
-    const uint64_t seed = *dr.seed;
-    const int bj = blockIdx.x;
-    const int b = bj / nrows, j = bj - b * nrows;
-    int id = idx[(size_t)b * ld + j];
-    if (drop != nullptr && drop[b]) id = drop_to;
-    const float* src = table + (size_t)id * d;
-    float* dst = h + ((size_t)b * S + row0 + j) * d;
-    for (int c4 = threadIdx.x; c4 < d / 4; c4 += blockDim.x) {
-        const uint4 r = car_dropout_bits(seed, dr.site, dr.layer, b, row0 + j, c4);
-        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) dst[4 * c4 + e] = src[4 * c4 + e] * car_keep_bit(rr[e], dr.keep) * dr.scale;
-    }
-}
-
-// the same on the caption MLP's bf16 prefix rows: h[b][row0 + j][:] = float(src[b][j][:]) * m * scale (tr_put_rows_bf16_kernel + mask)
-__global__ void tr_put_rows_drop_kernel(const bf16* __restrict__ src, float* __restrict__ h, int B, int nrows, int S, int row0, int d, TrDrop dr) {
-    const uint64_t seed = *dr.seed;
-    const int d4 = d / 4;
-    const long long total = (long long)B * nrows * d4;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int c4 = (int)(i % d4);
-        const long long rj = i / d4;
-        const int j = (int)(rj % nrows), b = (int)(rj / nrows);
-        const uint4 r = car_dropout_bits(seed, dr.site, dr.layer, b, row0 + j, c4);
-        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-            h[((size_t)b * S + row0 + j) * d + 4 * c4 + e] = __bfloat162float(src[(size_t)rj * d + 4 * c4 + e]) * car_keep_bit(rr[e], dr.keep) * dr.scale;
-    }
-}
-
-// embedding-table gradient through the token dropout: grad[index(b, j)][:] += dh[b][row0 + j][:] * m * scale (tr_embed_grad_kernel + mask)
-__global__ void tr_embed_grad_drop_kernel(const float* __restrict__ dh, const int* __restrict__ idx, int ld, const unsigned char* __restrict__ drop,
-                                          int drop_to, float* __restrict__ grad, int B, int nrows, int S, int row0, int d, TrDrop dr) {
-    const uint64_t seed = *dr.seed;
-    const int bj = blockIdx.x;
-    const int b = bj / nrows, j = bj - b * nrows;
-    int id = idx[(size_t)b * ld + j];
-    if (drop != nullptr && drop[b]) id = drop_to;
-    const float* src = dh + ((size_t)b * S + row0 + j) * d;
-    float* dst = grad + (size_t)id * d;
-    for (int c4 = threadIdx.x; c4 < d / 4; c4 += blockDim.x) {
-        const uint4 r = car_dropout_bits(seed, dr.site, dr.layer, b, row0 + j, c4);
-        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) atomicAdd(dst + 4 * c4 + e, src[4 * c4 + e] * car_keep_bit(rr[e], dr.keep) * dr.scale);
-    }
 }
 
 // conformance view of the generator: out[b][r][c] = keep decision of (site, layer, b, r, c); drop-path sites give every (r, c) of a

@@ -4,9 +4,11 @@
 // embeddings and the RMSNorm stay fp32; every nn.Linear takes bf16 operands (cast of the fp32 tensor) and returns bf16;
 // fp32 + bf16 adds promote to fp32; GELU / SiLU / the SwiGLU product run on the bf16 tensors; cross-entropy is fp32.
 // First correct path: the GEMMs are the dense tensor-core kernels of the prefill (gemm_wgmma.cuh / gemm_dense.cuh), everything
-// here is bandwidth-trivial glue plus a plain attention kernel; fusing them is the next step of this row.
+// here is bandwidth-trivial glue plus a plain attention kernel; fusing them is the next step of this row.  The row passes that
+// write the fp32 stream take a TrDrop (dropout.cuh): token, residual and feed-forward dropout and drop path apply as they write.
 #pragma once
 #include "common.cuh"
+#include "dropout.cuh"
 
 // dst[i] = bf16(src[i]) — autocast's per-forward cast of an fp32 weight (or activation) to the GEMM operand type
 __global__ void tr_cast_bf16_kernel(const float* __restrict__ src, bf16* __restrict__ dst, long long n) {
@@ -25,28 +27,50 @@ __global__ void tr_caption_select_kernel(const float* __restrict__ cap, const fl
     }
 }
 
-// h[b][row0 + j][:] = src[b][j][:]  (bf16 -> fp32), j < nrows — the cls_embedding rows of torch.cat (gpt_t2i.py:428)
-__global__ void tr_put_rows_bf16_kernel(const bf16* __restrict__ src, float* __restrict__ h, int B, int nrows, int S, int row0, int d) {
-    const long long total = (long long)B * nrows * d;
+// h[b][row0 + j][:] = float(src[b][j][:]) * m * scale, j < nrows — the cls_embedding rows of torch.cat (gpt_t2i.py:428) through
+// tok_dropout (:430, after the cat that promotes to fp32); also the fp32 copy of the logits (TrDrop{}).  Four columns per thread
+// (one generator call); d % 4 == 0.
+__global__ void tr_put_rows_bf16_kernel(const bf16* __restrict__ src, float* __restrict__ h, int B, int nrows, int S, int row0, int d, TrDrop dr) {
+    const uint64_t seed = tr_drop_seed(dr);
+    const int d4 = d / 4;
+    const long long total = (long long)B * nrows * d4;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int k = (int)(i % d);
-        const long long rj = i / d;
+        const int c4 = (int)(i % d4);
+        const long long rj = i / d4;
         const int j = (int)(rj % nrows), b = (int)(rj / nrows);
-        h[((size_t)b * S + row0 + j) * d + k] = __bfloat162float(src[i]);
+        const uint4 r = tr_drop_words(dr, seed, b, row0 + j, c4);
+        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            float v = __bfloat162float(src[(size_t)rj * d + 4 * c4 + e]);
+            if (dr.keep < 1.f) v = v * car_keep_bit(rr[e], dr.keep) * dr.scale;
+            h[((size_t)b * S + row0 + j) * d + 4 * c4 + e] = v;
+        }
     }
 }
 
-// h[b][row0 + j][:] = table[index(b, j)][:] (fp32 gather): tok_embeddings(idx) (gpt_t2i.py:423, ld = n tokens) and
-// LabelEmbedder (gpt_t2i.py:78-97: index = drop ? num_classes : label; nrows = 1, drop / drop_to given)
+// h[b][row0 + j][:] = table[index(b, j)][:] * m * scale (fp32 gather through tok_dropout): tok_embeddings(idx) (gpt_t2i.py:423,
+// ld = n tokens) and LabelEmbedder (gpt_t2i.py:78-97: index = drop ? num_classes : label; nrows = 1, drop / drop_to given).
+// One CTA per row, four columns per thread; d % 4 == 0.
 __global__ void tr_embed_rows_kernel(const float* __restrict__ table, const int* __restrict__ idx, int ld, const unsigned char* __restrict__ drop,
-                                     int drop_to, float* __restrict__ h, int B, int nrows, int S, int row0, int d) {
+                                     int drop_to, float* __restrict__ h, int B, int nrows, int S, int row0, int d, TrDrop dr) {
+    const uint64_t seed = tr_drop_seed(dr);
     const int bj = blockIdx.x;
     const int b = bj / nrows, j = bj - b * nrows;
     int id = idx[(size_t)b * ld + j];
     if (drop != nullptr && drop[b]) id = drop_to;
     const float* src = table + (size_t)id * d;
     float* dst = h + ((size_t)b * S + row0 + j) * d;
-    for (int k = threadIdx.x; k < d; k += blockDim.x) dst[k] = src[k];
+    for (int c4 = threadIdx.x; c4 < d / 4; c4 += blockDim.x) {
+        const uint4 r = tr_drop_words(dr, seed, b, row0 + j, c4);
+        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            float v = src[4 * c4 + e];
+            if (dr.keep < 1.f) v = v * car_keep_bit(rr[e], dr.keep) * dr.scale;
+            dst[4 * c4 + e] = v;
+        }
+    }
 }
 
 // ConditionEmbedder.token_drop (gpt_t2i.py:110-120): rows of dropped samples become the all-zero uncond_embedding
@@ -56,16 +80,29 @@ __global__ void tr_zero_dropped_kernel(bf16* __restrict__ c, const unsigned char
         if (drop[i / per_sample]) c[i] = __float2bfloat16_rn(0.f);
 }
 
-// h[b][row0 + j][:] += add[b][j][:]  (fp32 += bf16): the residual adds (row0 = 0, nrows = S) and the control add
-// h[:, T-1:] += condition_layers[i](condition_token) (gpt_t2i.py:458-460; row0 = T - 1, nrows = n_img)
-__global__ void tr_add_rows_kernel(float* __restrict__ h, const bf16* __restrict__ add, int B, int nrows, int S, int row0, int d) {
-    const long long total = (long long)B * nrows * d;
+// h[b][row0 + j][:] += float(bf16(bf16(o * m * scale) * path)), o = add[b][j][:] bf16 (fp32 += bf16, every step skipped when its
+// site is off): the residual adds of the wo / w2 outputs through their dropout and drop path (gpt_t2i.py:305-306; row0 = 0,
+// nrows = S) and the control add h[:, T-1:] += condition_layers[i](condition_token) (gpt_t2i.py:458-460; row0 = T - 1,
+// nrows = n_img, TrDrop{}).  Four columns per thread (one generator call); d % 4 == 0.
+__global__ void tr_add_rows_kernel(float* __restrict__ h, const bf16* __restrict__ add, int B, int nrows, int S, int row0, int d, TrDrop dr) {
+    const uint64_t seed = tr_drop_seed(dr);
+    const int d4 = d / 4;
+    const long long total = (long long)B * nrows * d4;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int k = (int)(i % d);
-        const long long rj = i / d;
+        const int c4 = (int)(i % d4);
+        const long long rj = i / d4;
         const int j = (int)(rj % nrows), b = (int)(rj / nrows);
-        const size_t o = ((size_t)b * S + row0 + j) * d + k;
-        h[o] = h[o] + __bfloat162float(add[i]);
+        const uint4 r = tr_drop_words(dr, seed, b, row0 + j, c4);
+        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
+        const float pm = tr_path_mult(dr, seed, b);
+        const size_t o = ((size_t)b * S + row0 + j) * d + 4 * c4;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            float v = __bfloat162float(add[(size_t)rj * d + 4 * c4 + e]);
+            if (dr.keep < 1.f) v = rnd<bf16>(v * car_keep_bit(rr[e], dr.keep) * dr.scale);
+            if (dr.path_keep < 1.f) v = rnd<bf16>(v * pm);
+            h[o + e] = h[o + e] + v;
+        }
     }
 }
 

@@ -7,6 +7,7 @@
 // tensor-core kernels through explicit transposes, attention is two plain one-warp-per-row kernels; fusing is future work.
 #pragma once
 #include "common.cuh"
+#include "dropout.cuh"
 #include "train.cuh"
 
 // dst[c][r] = src[r][c] for r < rows, 0 for rows <= r < ldp: the K-major operand the [N][K] x [M][K]^T GEMM kernels want,
@@ -33,14 +34,34 @@ __global__ void tr_bf16_to_f32_2d_kernel(const bf16* __restrict__ src, int lds, 
         dst[i] = __bfloat162float(src[(i / cols) * lds + i % cols]);
 }
 
-// out[b][j][:] = bf16(h[b][row0 + j][:]) — the bf16 gradient a bf16 branch receives from the fp32 stream (fp32 + bf16 add)
-__global__ void tr_take_rows_bf16_kernel(const float* __restrict__ h, bf16* __restrict__ out, int B, int nrows, int S, int row0, int d) {
-    const long long total = (long long)B * nrows * d;
+// out[b][j][:] = bf16(dh[b][row0 + j][:]) — the bf16 gradient a bf16 branch receives from the fp32 stream (fp32 + bf16 add) —
+// through the branch's drop path and dropout, as autograd orders them: out = bf16(bf16(bf16(dh) * path) * m * scale), every step
+// skipped when its site is off.  Token site (the prefix rows of the caption MLP): out = bf16(dh * m * scale), fp32 product first.
+// Four columns per thread (one generator call); d % 4 == 0.
+__global__ void tr_take_rows_bf16_kernel(const float* __restrict__ dh, bf16* __restrict__ out, int B, int nrows, int S, int row0, int d, TrDrop dr) {
+    const uint64_t seed = tr_drop_seed(dr);
+    const int d4 = d / 4;
+    const long long total = (long long)B * nrows * d4;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int k = (int)(i % d);
-        const long long rj = i / d;
+        const int c4 = (int)(i % d4);
+        const long long rj = i / d4;
         const int j = (int)(rj % nrows), b = (int)(rj / nrows);
-        out[i] = __float2bfloat16_rn(h[((size_t)b * S + row0 + j) * d + k]);
+        const uint4 r = tr_drop_words(dr, seed, b, row0 + j, c4);
+        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
+        const float pm = tr_path_mult(dr, seed, b);
+        const float* src = dh + ((size_t)b * S + row0 + j) * d + 4 * c4;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            float g = src[e];
+            if (dr.site == CAR_DROP_TOKEN) {
+                if (dr.keep < 1.f) g = g * car_keep_bit(rr[e], dr.keep) * dr.scale;
+            } else {
+                g = rnd<bf16>(g);
+                if (dr.path_keep < 1.f) g = rnd<bf16>(g * pm);
+                if (dr.keep < 1.f) g = g * car_keep_bit(rr[e], dr.keep) * dr.scale;
+            }
+            out[(size_t)rj * d + 4 * c4 + e] = __float2bfloat16_rn(g);
+        }
     }
 }
 
@@ -362,15 +383,26 @@ __global__ void tr_rope_bwd_kernel(const bf16* __restrict__ dq, const bf16* __re
     }
 }
 
-// embedding-table gradients (tok_embeddings gpt_t2i.py:423, LabelEmbedder :78-97): grad[index(b, j)][:] += dh[b][row0 + j][:]
-// (fp32 atomics: rows that repeat an index accumulate in arrival order)
+// embedding-table gradients (tok_embeddings gpt_t2i.py:423, LabelEmbedder :78-97) through the token dropout:
+// grad[index(b, j)][:] += dh[b][row0 + j][:] * m * scale (fp32 atomics: rows that repeat an index accumulate in arrival order).
+// One CTA per row, four columns per thread; d % 4 == 0.
 __global__ void tr_embed_grad_kernel(const float* __restrict__ dh, const int* __restrict__ idx, int ld, const unsigned char* __restrict__ drop,
-                                     int drop_to, float* __restrict__ grad, int B, int nrows, int S, int row0, int d) {
+                                     int drop_to, float* __restrict__ grad, int B, int nrows, int S, int row0, int d, TrDrop dr) {
+    const uint64_t seed = tr_drop_seed(dr);
     const int bj = blockIdx.x;
     const int b = bj / nrows, j = bj - b * nrows;
     int id = idx[(size_t)b * ld + j];
     if (drop != nullptr && drop[b]) id = drop_to;
     const float* src = dh + ((size_t)b * S + row0 + j) * d;
     float* dst = grad + (size_t)id * d;
-    for (int k = threadIdx.x; k < d; k += blockDim.x) atomicAdd(dst + k, src[k]);
+    for (int c4 = threadIdx.x; c4 < d / 4; c4 += blockDim.x) {
+        const uint4 r = tr_drop_words(dr, seed, b, row0 + j, c4);
+        const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            float v = src[4 * c4 + e];
+            if (dr.keep < 1.f) v = v * car_keep_bit(rr[e], dr.keep) * dr.scale;
+            atomicAdd(dst + 4 * c4 + e, v);
+        }
+    }
 }
