@@ -61,6 +61,37 @@ class CarGemmDesc(C.Structure):
                 ("osy", C.c_int32), ("osx", C.c_int32), ("oay", C.c_int32), ("oax", C.c_int32), ("oH", C.c_int32), ("oW", C.c_int32)]
 
 
+class CarDinoDesc(C.Structure):
+    _fields_ = [("dtype", C.c_int32), ("hidden", C.c_int32), ("heads", C.c_int32), ("layers", C.c_int32),
+                ("patch", C.c_int32), ("pos_grid", C.c_int32), ("resize_mode", C.c_int32),
+                ("adapter_out_dim", C.c_int32), ("eps", C.c_float)]
+
+
+_DINO_ARRAYS = ["n1_w", "n1_b", "q_w", "q_b", "k_w", "k_b", "v_w", "v_b", "o_w", "o_b", "ls1", "n2_w", "n2_b",
+                "fc1_w", "fc1_b", "fc2_w", "fc2_b", "ls2"]
+
+
+class CarDinoWeights(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ["cls_token", "pos_emb", "patch_w", "patch_b", "ln_w", "ln_b"]] + \
+               [(n, C.POINTER(C.c_void_p)) for n in _DINO_ARRAYS] + \
+               [("adapter_fc1", C.c_void_p), ("adapter_fc2", C.c_void_p)]
+
+
+class CarVQDesc(C.Structure):
+    _fields_ = [("codebook_size", C.c_int32), ("embed_dim", C.c_int32), ("ch", C.c_int32), ("z_channels", C.c_int32),
+                ("n_levels", C.c_int32), ("num_res_blocks", C.c_int32), ("ch_mult", C.c_int32 * 8)]
+
+
+class CarT5Desc(C.Structure):
+    _fields_ = [("dtype", C.c_int32), ("d_model", C.c_int32), ("d_kv", C.c_int32), ("n_heads", C.c_int32), ("d_ff", C.c_int32),
+                ("n_layers", C.c_int32), ("vocab", C.c_int32), ("num_buckets", C.c_int32), ("max_distance", C.c_int32), ("eps", C.c_float)]
+
+
+class CarT5Weights(C.Structure):
+    _fields_ = [("embed", C.c_void_p), ("rel_bias", C.c_void_p), ("final_norm", C.c_void_p)] + \
+               [(n, C.POINTER(C.c_void_p)) for n in ("ln1", "q", "k", "v", "o", "ln2", "wi_0", "wi_1", "wo")]
+
+
 # name -> (restype, argtypes); every symbol declared in include/controlar_b200.h
 PROTOTYPES = {
     "car_last_error": (C.c_char_p, []),
@@ -111,6 +142,20 @@ PROTOTYPES = {
     "car_midas_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_midas_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_midas_destroy": (C.c_int, [C.c_void_p]),
+    "car_dino_create": (C.c_int, [C.POINTER(CarDinoDesc), C.POINTER(CarDinoWeights), C.c_void_p, C.POINTER(C.c_void_p)]),
+    "car_dino_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
+    "car_dino_destroy": (C.c_int, [C.c_void_p]),
+    "car_dino_train_create": (C.c_int, [C.POINTER(CarDinoDesc), C.POINTER(CarDinoWeights), C.c_void_p, C.POINTER(C.c_void_p)]),
+    "car_dino_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "car_dino_train_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(CarDinoWeights), C.c_void_p]),
+    "car_dino_train_destroy": (C.c_int, [C.c_void_p]),
+    "car_vq_create": (C.c_int, [C.POINTER(CarVQDesc), C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "car_vq_decode_code": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "car_vq_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "car_resize_bilinear_aa": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
+                                         C.c_void_p, C.c_void_p]),
+    "car_vq_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "car_vq_destroy": (C.c_int, [C.c_void_p]),
     "car_t5_create": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_t5_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_t5_destroy": (C.c_int, [C.c_void_p]),
@@ -265,4 +310,29 @@ def _ptr_array(ts):
     return arr
 
 
-from . import vision as _vision  # noqa: E402,F401  (registers the car_dino_* / car_vq_* prototypes in PROTOTYPES)
+def fill_struct(struct_type, entries, layers: int = 0):
+    """A `struct_type` pointing at the tensors of `entries`, and those tensors, which must stay alive while the library reads them.
+    An entry is (field, index, tensor or None); a dotted field ("w.wqkv") reaches into a nested struct.  The field's ctypes type
+    says what `index` is: ignored for a pointer, the slot of an inline array (`ctl_fc1[3]`), the layer of a per-layer
+    POINTER(c_void_p) array.  Per-layer arrays have `layers` entries and are kept alive by the struct.  Fields, slots and layers
+    that no entry names, or whose tensor is None, stay NULL."""
+    s, tensors, arrays = struct_type(), [], {}
+    for field, i, t in entries:
+        owner = s
+        *path, name = field.split(".")
+        for f in path:
+            owner = getattr(owner, f)
+        kind = dict(owner._fields_)[name]
+        p = _ptr(t)
+        if t is not None:
+            tensors.append(t)
+        if kind is C.c_void_p:
+            setattr(owner, name, p)
+        elif issubclass(kind, C.Array):
+            getattr(owner, name)[i] = p
+        else:
+            if field not in arrays:
+                arrays[field] = (C.c_void_p * layers)()
+                setattr(owner, name, C.cast(arrays[field], C.POINTER(C.c_void_p)))
+            arrays[field][i] = p
+    return s, tensors

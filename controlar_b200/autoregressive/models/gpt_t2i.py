@@ -307,8 +307,7 @@ class Transformer(nn.Module):
                                       "supported; token, residual and feed-forward dropout and drop_path_rate are")
         B, n = idx.shape
         th = getattr(self, "_car_train", None)
-        key = tuple(p.data_ptr() for p in self.parameters())
-        if th is None or th.key != key or th.max_batch < B or th.max_img_tokens < n + 1:
+        if th is None or th.key != _engine.train_key(self) or th.max_batch < B or th.max_img_tokens < n + 1:
             if th is not None:
                 th.close()
             th = self._car_train = _engine.ARTrainHandle(self, B, max(n + 1, self.block_size))

@@ -24,31 +24,44 @@ def _desc(m) -> CarModelDesc:
                         model_type=1 if t2i else 0, norm_eps=cfg.norm_eps, rope_base=cfg.rope_base)
 
 
-def _weights(m):
-    """CarWeights over the transformer's weights, and the tensors whose storage the library borrows through it (the per-layer
-    pointer arrays are kept alive by the CarWeights itself)."""
-    w = CarWeights()
-    ts = []
+_LAYER = [("attention_norm", "attention_norm"), ("wqkv", "attention.wqkv"), ("wo", "attention.wo"), ("ffn_norm", "ffn_norm"),
+          ("w1", "feed_forward.w1"), ("w3", "feed_forward.w3"), ("w2", "feed_forward.w2")]
 
-    def P(t):
-        t = t.detach()
-        ts.append(t)
-        return _ptr(t)
-    w.tok_embeddings, w.norm, w.output = P(m.tok_embeddings.weight), P(m.norm.weight), P(m.output.weight)
-    for name, get in [("attention_norm", lambda b: b.attention_norm.weight), ("wqkv", lambda b: b.attention.wqkv.weight),
-                      ("wo", lambda b: b.attention.wo.weight), ("ffn_norm", lambda b: b.ffn_norm.weight),
-                      ("w1", lambda b: b.feed_forward.w1.weight), ("w3", lambda b: b.feed_forward.w3.weight),
-                      ("w2", lambda b: b.feed_forward.w2.weight)]:
-        arr = (C.c_void_p * len(m.layers))(*[P(get(b)) for b in m.layers])
-        setattr(w, name, C.cast(arr, C.POINTER(C.c_void_p)))
+
+def _table(m):
+    """(state-dict name, CarTrainWeights field, index) of every transformer parameter the library reads, in the order of
+    `ARTrainHandle.grad_params`.  The "w." fields are the CarWeights of inference."""
+    t = [("tok_embeddings.weight", "w.tok_embeddings", None), ("norm.weight", "w.norm", None), ("output.weight", "w.output", None)]
+    for i in range(len(m.layers)):
+        t += [(f"layers.{i}.{k}.weight", "w." + f, i) for f, k in _LAYER]
     if m.model_type == "t2i":
-        w.cap_fc1, w.cap_fc2 = P(m.cls_embedding.cap_proj.fc1.weight), P(m.cls_embedding.cap_proj.fc2.weight)
+        t += [("cls_embedding.cap_proj.fc1.weight", "w.cap_fc1", None), ("cls_embedding.cap_proj.fc2.weight", "w.cap_fc2", None)]
     else:
-        w.label_table = P(m.cls_embedding.embedding_table.weight)
-    w.cond_fc1, w.cond_fc2 = P(m.condition_mlp.cap_proj.fc1.weight), P(m.condition_mlp.cap_proj.fc2.weight)
+        t += [("cls_embedding.embedding_table.weight", "w.label_table", None)]
+    t += [("condition_mlp.cap_proj.fc1.weight", "w.cond_fc1", None), ("condition_mlp.cap_proj.fc2.weight", "w.cond_fc2", None)]
     for j in range(3):
-        w.ctl_fc1[j], w.ctl_fc2[j] = P(m.condition_layers[j].fc1.weight), P(m.condition_layers[j].fc2.weight)
-    return w, ts
+        t += [(f"condition_layers.{j}.fc1.weight", "w.ctl_fc1", j), (f"condition_layers.{j}.fc2.weight", "w.ctl_fc2", j)]
+    return t + [("adapter_mlp.fc1.weight", "adapter_fc1", None), ("adapter_mlp.fc2.weight", "adapter_fc2", None)]
+
+
+def _param(m, name):
+    """`m.get_parameter(name)` without its per-level checks, which make it several times slower; every training step looks up
+    the whole table."""
+    *mods, p = name.split(".")
+    for k in mods:
+        m = m._modules[k]
+    return m._parameters[p]
+
+
+def _weights(m):
+    """CarWeights over the transformer's weights, and the tensors whose storage the library borrows through it."""
+    return _lib.fill_struct(CarWeights, [(f[2:], i, _param(m, k).detach()) for k, f, i in _table(m) if f.startswith("w.")],
+                            len(m.layers))
+
+
+def train_key(m) -> tuple:
+    """What an ARTrainHandle is created for: the storage of every parameter of the module."""
+    return tuple(p.data_ptr() for p in m.parameters())
 
 
 def _layout(m):
@@ -123,27 +136,21 @@ class ARTrainHandle(_lib.NativeHandle):
         self.device = m.tok_embeddings.weight.device
         self.max_batch, self.max_img_tokens = max_batch, max_img_tokens
         self.V, self.T = cfg.vocab_size, cfg.cls_token_num
-        self.key = tuple(p.data_ptr() for p in m.parameters())
+        self.key = train_key(m)
         self.generation = 0          # a backward belongs to the forward that produced its loss
         self._create(m)
 
     @on_own_device
     def _create(self, m):
-        w, keep = _weights(m)
-        tw = CarTrainWeights()
-        tw.w = w
-        tw.adapter_fc1 = _ptr(m.adapter_mlp.fc1.weight.detach()); tw.adapter_fc2 = _ptr(m.adapter_mlp.fc2.weight.detach())
+        entries = [(f, i, _param(m, k).detach()) for k, f, i in _table(m)]
+        if m.model_type == "t2i":
+            entries.append(("cap_uncond", None, m.cls_embedding.uncond_embedding.detach().to(torch.float32).contiguous()))
+        if not getattr(m, "zero_uncond_on_drop", False):       # a buffer, zeros unless a state dict says otherwise
+            entries.append(("cond_uncond", None, m.condition_mlp.uncond_embedding.detach().to(torch.float32).contiguous()))
+        # else: the legacy gpt.py class gives dropped samples literal zeros (gpt.py:118-119): NULL = zeros in the library
+        tw, keep = _lib.fill_struct(CarTrainWeights, entries, len(m.layers))
         tw.adapter_dim = m.adapter_mlp.fc1.weight.shape[1]
         tw.num_classes = m.config.num_classes
-        if m.model_type == "t2i":
-            unc = m.cls_embedding.uncond_embedding.detach().to(torch.float32).contiguous()
-            keep.append(unc)
-            tw.cap_uncond = _ptr(unc)
-        if not getattr(m, "zero_uncond_on_drop", False):
-            cunc = m.condition_mlp.uncond_embedding.detach().to(torch.float32).contiguous()   # buffer, zeros unless a state dict says otherwise
-            keep.append(cunc)
-            tw.cond_uncond = _ptr(cunc)
-        # else: the legacy gpt.py class gives dropped samples literal zeros (gpt.py:118-119): NULL = zeros in the library
         self.rope = m.freqs_cis.to(device=self.device, dtype=torch.float32).contiguous()
         check(self.lib.car_train_create(C.byref(_desc(m)), C.byref(tw), self.max_batch, self.max_img_tokens, _ptr(self.rope), cur_stream(),
                                         C.byref(self.handle)), "car_train_create")
@@ -194,25 +201,7 @@ class ARTrainHandle(_lib.NativeHandle):
     @staticmethod
     def grad_params(m):
         """The parameters `car_train_backward` produces gradients for, in a fixed order (name, parameter)."""
-        out = [("tok_embeddings.weight", m.tok_embeddings.weight), ("norm.weight", m.norm.weight), ("output.weight", m.output.weight)]
-        for i, b in enumerate(m.layers):
-            pre = f"layers.{i}."
-            out += [(pre + "attention_norm.weight", b.attention_norm.weight), (pre + "attention.wqkv.weight", b.attention.wqkv.weight),
-                    (pre + "attention.wo.weight", b.attention.wo.weight), (pre + "ffn_norm.weight", b.ffn_norm.weight),
-                    (pre + "feed_forward.w1.weight", b.feed_forward.w1.weight), (pre + "feed_forward.w3.weight", b.feed_forward.w3.weight),
-                    (pre + "feed_forward.w2.weight", b.feed_forward.w2.weight)]
-        if m.model_type == "t2i":
-            out += [("cls_embedding.cap_proj.fc1.weight", m.cls_embedding.cap_proj.fc1.weight),
-                    ("cls_embedding.cap_proj.fc2.weight", m.cls_embedding.cap_proj.fc2.weight)]
-        else:
-            out += [("cls_embedding.embedding_table.weight", m.cls_embedding.embedding_table.weight)]
-        out += [("condition_mlp.cap_proj.fc1.weight", m.condition_mlp.cap_proj.fc1.weight),
-                ("condition_mlp.cap_proj.fc2.weight", m.condition_mlp.cap_proj.fc2.weight)]
-        for j in range(3):
-            out += [(f"condition_layers.{j}.fc1.weight", m.condition_layers[j].fc1.weight),
-                    (f"condition_layers.{j}.fc2.weight", m.condition_layers[j].fc2.weight)]
-        out += [("adapter_mlp.fc1.weight", m.adapter_mlp.fc1.weight), ("adapter_mlp.fc2.weight", m.adapter_mlp.fc2.weight)]
-        return out
+        return [(k, _param(m, k)) for k, _, _ in _table(m)]
 
     @on_own_device
     def backward(self, module, loss_grad=None, want_feat_grad=True):
@@ -223,32 +212,11 @@ class ARTrainHandle(_lib.NativeHandle):
         idx, cond, feat, drop, m8, tg, vf, _seed = self._last
         if tg is None:
             raise RuntimeError("controlar_b200: the last training forward had no targets / loss")
-        names = self.grad_params(module)
+        table = _table(module)
         has_feat = feat is not None
         skip_wo_feat = ("condition_mlp.", "condition_layers.", "adapter_mlp.")
-        G = {k: torch.empty_like(p, dtype=torch.float32) for k, p in names if has_feat or not k.startswith(skip_wo_feat)}
-        L = len(module.layers)
-        gw = CarTrainWeights()
-        keep = []
-
-        def P(key):
-            t = G.get(key)
-            return None if t is None else _ptr(t)
-        gw.w.tok_embeddings = P("tok_embeddings.weight"); gw.w.norm = P("norm.weight"); gw.w.output = P("output.weight")
-        for field, suffix in [("attention_norm", "attention_norm.weight"), ("wqkv", "attention.wqkv.weight"), ("wo", "attention.wo.weight"),
-                              ("ffn_norm", "ffn_norm.weight"), ("w1", "feed_forward.w1.weight"), ("w3", "feed_forward.w3.weight"),
-                              ("w2", "feed_forward.w2.weight")]:
-            arr = _ptr_array([G[f"layers.{i}.{suffix}"] for i in range(L)])
-            keep.append(arr)
-            setattr(gw.w, field, C.cast(arr, C.POINTER(C.c_void_p)))
-        if module.model_type == "t2i":
-            gw.w.cap_fc1 = P("cls_embedding.cap_proj.fc1.weight"); gw.w.cap_fc2 = P("cls_embedding.cap_proj.fc2.weight")
-        else:
-            gw.w.label_table = P("cls_embedding.embedding_table.weight")
-        gw.w.cond_fc1 = P("condition_mlp.cap_proj.fc1.weight"); gw.w.cond_fc2 = P("condition_mlp.cap_proj.fc2.weight")
-        for j in range(3):
-            gw.w.ctl_fc1[j] = P(f"condition_layers.{j}.fc1.weight"); gw.w.ctl_fc2[j] = P(f"condition_layers.{j}.fc2.weight")
-        gw.adapter_fc1 = P("adapter_mlp.fc1.weight"); gw.adapter_fc2 = P("adapter_mlp.fc2.weight")
+        G = {k: torch.empty_like(_param(module, k), dtype=torch.float32) for k, _, _ in table if has_feat or not k.startswith(skip_wo_feat)}
+        gw, _ = _lib.fill_struct(CarTrainWeights, [(f, i, G.get(k)) for k, f, i in table], len(module.layers))
         dfeat = torch.empty_like(feat) if (has_feat and want_feat_grad) else None
         lg = None
         if loss_grad is not None:

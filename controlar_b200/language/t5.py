@@ -13,17 +13,7 @@ import ctypes as C
 import torch
 
 from .. import _lib
-from .._lib import CAR_BF16, check, cur_stream, on_own_device, _ptr, _ptr_array
-
-
-class CarT5Desc(C.Structure):
-    _fields_ = [("dtype", C.c_int32), ("d_model", C.c_int32), ("d_kv", C.c_int32), ("n_heads", C.c_int32), ("d_ff", C.c_int32),
-                ("n_layers", C.c_int32), ("vocab", C.c_int32), ("num_buckets", C.c_int32), ("max_distance", C.c_int32), ("eps", C.c_float)]
-
-
-class CarT5Weights(C.Structure):
-    _fields_ = [("embed", C.c_void_p), ("rel_bias", C.c_void_p), ("final_norm", C.c_void_p)] + \
-               [(n, C.POINTER(C.c_void_p)) for n in ("ln1", "q", "k", "v", "o", "ln2", "wi_0", "wi_1", "wo")]
+from .._lib import CAR_BF16, CarT5Desc, CarT5Weights, check, cur_stream, on_own_device, _ptr
 
 
 class T5EncoderB200:
@@ -44,13 +34,14 @@ class T5EncoderB200:
             return t.detach().to(device=dev, dtype=torch.bfloat16).contiguous()
         emb_key = "shared.weight" if "shared.weight" in sd else "encoder.embed_tokens.weight"
         # the library borrows these: they live as long as the encoder (a deep copy gets its own)
-        self._weights = {"embed": W(emb_key), "rel_bias": W("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"),
-                         "final_norm": W("encoder.final_layer_norm.weight")}
+        self._weights = [("embed", None, W(emb_key)),
+                         ("rel_bias", None, W("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight")),
+                         ("final_norm", None, W("encoder.final_layer_norm.weight"))]
         names = {"ln1": "layer.0.layer_norm", "q": "layer.0.SelfAttention.q", "k": "layer.0.SelfAttention.k", "v": "layer.0.SelfAttention.v",
                  "o": "layer.0.SelfAttention.o", "ln2": "layer.1.layer_norm", "wi_0": "layer.1.DenseReluDense.wi_0",
                  "wi_1": "layer.1.DenseReluDense.wi_1", "wo": "layer.1.DenseReluDense.wo"}
         for field, sub in names.items():
-            self._weights[field] = [W(f"encoder.block.{i}.{sub}.weight") for i in range(num_layers)]
+            self._weights += [(field, i, W(f"encoder.block.{i}.{sub}.weight")) for i in range(num_layers)]
         self.d_model = d_model
         self.max_rows = max_rows
         self._desc = CarT5Desc(CAR_BF16, d_model, d_kv, num_heads, d_ff, num_layers, vocab_size, num_buckets, max_distance, eps)
@@ -65,9 +56,7 @@ class T5EncoderB200:
         if not self._h.handle or rows > self.max_rows:
             self._h.close()
             max_rows = max(rows, self.max_rows)
-            w = CarT5Weights()
-            for field, t in self._weights.items():
-                setattr(w, field, _ptr(t) if torch.is_tensor(t) else C.cast(_ptr_array(t), C.POINTER(C.c_void_p)))
+            w, _ = _lib.fill_struct(CarT5Weights, self._weights, self._desc.n_layers)
             check(_lib.lib().car_t5_create(C.byref(self._desc), C.byref(w), max_rows, cur_stream(), C.byref(self._h.handle)), "car_t5_create")
             self.max_rows = max_rows
         return self._h.handle

@@ -7,47 +7,8 @@ from typing import List
 import torch
 
 from . import _lib
-from ._lib import check, cur_stream, dtype_code, on_own_device, param_signature, _ptr, _ptr_array
-
-
-class CarDinoDesc(C.Structure):
-    _fields_ = [("dtype", C.c_int32), ("hidden", C.c_int32), ("heads", C.c_int32), ("layers", C.c_int32),
-                ("patch", C.c_int32), ("pos_grid", C.c_int32), ("resize_mode", C.c_int32),
-                ("adapter_out_dim", C.c_int32), ("eps", C.c_float)]
-
-
-_DINO_ARRAYS = ["n1_w", "n1_b", "q_w", "q_b", "k_w", "k_b", "v_w", "v_b", "o_w", "o_b", "ls1", "n2_w", "n2_b",
-                "fc1_w", "fc1_b", "fc2_w", "fc2_b", "ls2"]
-
-
-class CarDinoWeights(C.Structure):
-    _fields_ = [(n, C.c_void_p) for n in ["cls_token", "pos_emb", "patch_w", "patch_b", "ln_w", "ln_b"]] + \
-               [(n, C.POINTER(C.c_void_p)) for n in _DINO_ARRAYS] + \
-               [("adapter_fc1", C.c_void_p), ("adapter_fc2", C.c_void_p)]
-
-
-class CarVQDesc(C.Structure):
-    _fields_ = [("codebook_size", C.c_int32), ("embed_dim", C.c_int32), ("ch", C.c_int32), ("z_channels", C.c_int32),
-                ("n_levels", C.c_int32), ("num_res_blocks", C.c_int32), ("ch_mult", C.c_int32 * 8)]
-
-
-_PROTOS = {
-    "car_dino_create": (C.c_int, [C.POINTER(CarDinoDesc), C.POINTER(CarDinoWeights), C.c_void_p, C.POINTER(C.c_void_p)]),
-    "car_dino_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
-    "car_dino_destroy": (C.c_int, [C.c_void_p]),
-    "car_dino_train_create": (C.c_int, [C.POINTER(CarDinoDesc), C.POINTER(CarDinoWeights), C.c_void_p, C.POINTER(C.c_void_p)]),
-    "car_dino_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
-    "car_dino_train_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(CarDinoWeights), C.c_void_p]),
-    "car_dino_train_destroy": (C.c_int, [C.c_void_p]),
-    "car_vq_create": (C.c_int, [C.POINTER(CarVQDesc), C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
-    "car_vq_decode_code": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
-    "car_vq_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
-    "car_resize_bilinear_aa": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
-                                         C.c_void_p, C.c_void_p]),
-    "car_vq_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "car_vq_destroy": (C.c_int, [C.c_void_p]),
-}
-_lib.PROTOTYPES.update(_PROTOS)
+from ._lib import CarDinoDesc, CarDinoWeights, CarVQDesc, check, cur_stream, dtype_code, on_own_device, _ptr, _ptr_array
+from ._lib import _DINO_ARRAYS  # noqa: F401  (callers that fill a CarDinoWeights by hand find its array names here)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -79,9 +40,12 @@ def _is_vit(m) -> bool:
     return hasattr(m.encoder.layer[0], "layernorm_before")      # HF ViTModel key names (vit_adapter.py) vs Dinov2Model
 
 
-def _resize_mode(adapter, is_vit: bool) -> int:
+def _dino_desc(adapter, dtype: int, adapter_out_dim: int) -> CarDinoDesc:
+    m = adapter.model
     # dinov2_adapter.py:20-24: nearest for canny / seg, bicubic otherwise; ViT_Adapter does not resize (nearest at P = 16 is the identity)
-    return 0 if (is_vit or adapter.condition_type in ("canny", "seg")) else 1
+    mode = 0 if (_is_vit(m) or adapter.condition_type in ("canny", "seg")) else 1
+    return CarDinoDesc(dtype=dtype, hidden=m.hidden, heads=m.heads, layers=m.n_layers, patch=m.patch, pos_grid=m.pos_grid,
+                       resize_mode=mode, adapter_out_dim=adapter_out_dim, eps=m.eps)
 
 
 class DinoHandle(_lib.ModuleHandle):
@@ -89,63 +53,37 @@ class DinoHandle(_lib.ModuleHandle):
         super().__init__("car_dino_destroy")
         self.lib = _lib.lib()
         self.adapter, self.adapter_mlp = adapter, adapter_mlp
-        self._build()
+        self._get()
 
     @property
     def device(self):
         return _dev_of(self.adapter)
 
-    def _params(self):
+    def _get(self):
         ps = list(self.adapter.model.parameters())
         if self.adapter_mlp is not None:
             ps += list(self.adapter_mlp.parameters())
-        return ps
+        return self.get(ps, self._create)
 
-    @on_own_device
-    def _build(self):
-        m = self.adapter.model
+    def _create(self, out):
+        m, mlp = self.adapter.model, self.adapter_mlp
         dt = m.layernorm.weight.dtype
-        keep = []
-
-        def P(t):
-            t = t.detach().contiguous()
-            keep.append(t)
-            return _ptr(t)
-        w = CarDinoWeights()
-        e = m.embeddings
-        w.cls_token, w.pos_emb = P(e.cls_token), P(e.position_embeddings)
-        w.patch_w, w.patch_b = P(e.patch_embeddings.projection.weight), P(e.patch_embeddings.projection.bias)
-        w.ln_w, w.ln_b = P(m.layernorm.weight), P(m.layernorm.bias)
-        layers = list(m.encoder.layer)
-        is_vit = _is_vit(m)
-        ones = None
-        if is_vit:
+        entries = encoder_train_params(m)
+        if _is_vit(m):
             ones = torch.ones(m.hidden, dtype=dt, device=m.layernorm.weight.device)     # no LayerScale in ViT: x 1 is exact
-            keep.append(ones)
-        for name in _DINO_ARRAYS:
-            ts = [_block_tensors(b, is_vit)[name] for b in layers]
-            ts = [(ones if t is None else t).detach().contiguous() for t in ts]
-            arr = _ptr_array(ts)
-            keep.extend(ts)
-            keep.append(arr)
-            setattr(w, name, C.cast(arr, C.POINTER(C.c_void_p)))
+            entries += [(f, i, ones) for f in ("ls1", "ls2") for i in range(m.n_layers)]
         out_dim = 0
-        if self.adapter_mlp is not None:
-            w.adapter_fc1, w.adapter_fc2 = P(self.adapter_mlp.fc1.weight), P(self.adapter_mlp.fc2.weight)
-            out_dim = self.adapter_mlp.fc2.weight.shape[0]
-        mode = _resize_mode(self.adapter, is_vit)
-        d = CarDinoDesc(dtype=dtype_code(dt), hidden=m.hidden, heads=m.heads, layers=m.n_layers, patch=m.patch,
-                        pos_grid=m.pos_grid, resize_mode=mode, adapter_out_dim=out_dim, eps=m.eps)
-        self.close()
-        check(self.lib.car_dino_create(C.byref(d), C.byref(w), cur_stream(), C.byref(self.handle)), "car_dino_create")
-        torch.cuda.current_stream().synchronize()     # conversions read `keep` tensors; safe to drop afterwards
+        if mlp is not None:
+            entries += [("adapter_fc1", None, mlp.fc1.weight), ("adapter_fc2", None, mlp.fc2.weight)]
+            out_dim = mlp.fc2.weight.shape[0]
+        w, keep = _lib.fill_struct(CarDinoWeights, [(f, i, t.detach().contiguous()) for f, i, t in entries], m.n_layers)
+        check(self.lib.car_dino_create(C.byref(_dino_desc(self.adapter, dtype_code(dt), out_dim)), C.byref(w), cur_stream(), C.byref(out)),
+              "car_dino_create")
         self.dtype, self.hidden, self.out_dim = dt, m.hidden, out_dim
-        self.sig = param_signature(self._params())
 
     @on_own_device
     def forward(self, x: torch.Tensor, apply_mlp: bool) -> torch.Tensor:
-        if param_signature(self._params()) != self.sig:
-            self._build()
+        self._get()
         B, _, H, W = x.shape
         x = x.to(self.dtype).contiguous()
         n = (H // 16) * (W // 16)
@@ -182,7 +120,6 @@ class DinoTrainHandle(_lib.NativeHandle):
         self.lib = _lib.lib()
         m = adapter.model
         self.params = encoder_train_params(m)
-        self.is_vit = _is_vit(m)
         self.key = self.key_of(adapter)
         self.device = m.layernorm.weight.device
         self.hidden, self.layers = m.hidden, m.n_layers
@@ -193,28 +130,11 @@ class DinoTrainHandle(_lib.NativeHandle):
     def key_of(adapter):
         return tuple(p.data_ptr() for _, _, p in encoder_train_params(adapter.model))
 
-    def _weights(self, tensors):
-        """CarDinoWeights over `tensors` (parallel to self.params; None = NULL) and the pointer arrays it needs kept alive"""
-        w, keep = CarDinoWeights(), []
-        per = {}
-        for (f, i, _), t in zip(self.params, tensors):
-            if i is None:
-                setattr(w, f, _ptr(t))
-            else:
-                per.setdefault(f, [None] * self.layers)[i] = t
-        for f, ts in per.items():
-            arr = (C.c_void_p * self.layers)(*[None if t is None else _ptr(t) for t in ts])
-            keep.append(arr)
-            setattr(w, f, C.cast(arr, C.POINTER(C.c_void_p)))
-        return w, keep
-
     @on_own_device
     def _create(self, adapter):
-        m = adapter.model
-        w, keep = self._weights([p.detach() for _, _, p in self.params])
-        d = CarDinoDesc(dtype=_lib.CAR_F32, hidden=m.hidden, heads=m.heads, layers=m.n_layers, patch=m.patch, pos_grid=m.pos_grid,
-                        resize_mode=_resize_mode(adapter, self.is_vit), adapter_out_dim=0, eps=m.eps)
-        check(self.lib.car_dino_train_create(C.byref(d), C.byref(w), cur_stream(), C.byref(self.handle)), "car_dino_train_create")
+        w, keep = _lib.fill_struct(CarDinoWeights, [(f, i, p.detach()) for f, i, p in self.params], self.layers)
+        check(self.lib.car_dino_train_create(C.byref(_dino_desc(adapter, _lib.CAR_F32, 0)), C.byref(w), cur_stream(), C.byref(self.handle)),
+              "car_dino_train_create")
 
     @on_own_device
     def forward(self, x: torch.Tensor) -> torch.Tensor:
@@ -230,7 +150,7 @@ class DinoTrainHandle(_lib.NativeHandle):
     def backward(self, dfeat: torch.Tensor, want):
         """fp32 gradients of the last forward for the parameters flagged in `want` (parallel to self.params; None elsewhere)"""
         grads = [torch.empty_like(p, dtype=torch.float32) if wnt else None for (_, _, p), wnt in zip(self.params, want)]
-        g, keep = self._weights(grads)
+        g, keep = _lib.fill_struct(CarDinoWeights, [(f, i, t) for (f, i, _), t in zip(self.params, grads)], self.layers)
         dfeat = dfeat.to(torch.float32).contiguous()
         check(self.lib.car_dino_train_backward(self.handle, _ptr(dfeat), C.byref(g), cur_stream()), "car_dino_train_backward")
         return grads
@@ -328,38 +248,32 @@ class VQHandle(_lib.ModuleHandle):
         super().__init__("car_vq_destroy")
         self.lib = _lib.lib()
         self.vq = vq
-        self._build()
+        cfg = vq.config
+        self.down = 2 ** (len(cfg.decoder_ch_mult) - 1)
+        self.e_dim = cfg.codebook_embed_dim
+        self._get()
 
     @property
     def device(self):
         return _dev_of(self.vq)
 
-    @on_own_device
-    def _build(self):
-        vq = self.vq
-        cfg = vq.config
-        ts = [t.detach().to(torch.float32).contiguous() for t in vq_tensor_order(vq)]
+    def _get(self):
+        return self.get(vq_tensor_order(self.vq), self._create)
+
+    def _create(self, out):
+        cfg = self.vq.config
+        ts = [t.detach().to(torch.float32).contiguous() for t in vq_tensor_order(self.vq)]
         arr = _ptr_array(ts)
         d = CarVQDesc(codebook_size=cfg.codebook_size, embed_dim=cfg.codebook_embed_dim, ch=128, z_channels=cfg.z_channels,
                       n_levels=len(cfg.decoder_ch_mult), num_res_blocks=2)
         assert list(cfg.encoder_ch_mult) == list(cfg.decoder_ch_mult)
         for i, v in enumerate(cfg.decoder_ch_mult):
             d.ch_mult[i] = int(v)
-        self.close()
-        check(self.lib.car_vq_create(C.byref(d), C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(self.handle)),
-              "car_vq_create")
-        torch.cuda.current_stream().synchronize()
-        self.sig = param_signature(vq_tensor_order(vq))
-        self.down = 2 ** (len(cfg.decoder_ch_mult) - 1)
-        self.e_dim = cfg.codebook_embed_dim
-
-    def _fresh(self):
-        if param_signature(vq_tensor_order(self.vq)) != self.sig:
-            self._build()
+        check(self.lib.car_vq_create(C.byref(d), C.cast(arr, C.POINTER(C.c_void_p)), len(ts), cur_stream(), C.byref(out)), "car_vq_create")
 
     @on_own_device
     def decode_code(self, codes: torch.Tensor, B: int, h: int, w: int) -> torch.Tensor:
-        self._fresh()
+        self._get()
         codes = codes.reshape(B, h * w).to(torch.int32).contiguous()
         out = torch.empty((B, 3, h * self.down, w * self.down), dtype=torch.float32, device=codes.device)
         check(self.lib.car_vq_decode_code(self.handle, _ptr(codes), B, h, w, _ptr(out), cur_stream()), "car_vq_decode_code")
@@ -368,7 +282,7 @@ class VQHandle(_lib.ModuleHandle):
 
     @on_own_device
     def decode(self, quant: torch.Tensor) -> torch.Tensor:
-        self._fresh()
+        self._get()
         B, e, h, w = quant.shape
         quant = quant.to(torch.float32).contiguous()
         out = torch.empty((B, 3, h * self.down, w * self.down), dtype=torch.float32, device=quant.device)
@@ -378,7 +292,7 @@ class VQHandle(_lib.ModuleHandle):
 
     @on_own_device
     def encode(self, img: torch.Tensor):
-        self._fresh()
+        self._get()
         B, _, H, W = img.shape
         img = img.to(torch.float32).contiguous()
         h, w = H // self.down, W // self.down

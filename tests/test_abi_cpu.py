@@ -34,6 +34,23 @@ def test_ctypes_prototypes_cover_header():
     assert b"null" in l.car_last_error()
 
 
+def test_fill_struct_places_each_entry_by_field_type(monkeypatch):
+    """A pointer field, a dotted field of a nested struct, an inline-array slot and a per-layer array entry each land where the field's
+    ctypes type says.  What no entry names, or names with None, stays NULL, and the struct keeps its per-layer arrays alive."""
+    import gc
+    import torch
+    from controlar_b200 import _lib
+    monkeypatch.setattr(_lib, "_ptr", lambda t: None if t is None else t.data_ptr())      # CPU tensors stand in for device ones
+    a, b, c, d = (torch.zeros(4) for _ in range(4))
+    s, ts = _lib.fill_struct(_lib.CarTrainWeights, [("adapter_fc1", None, a), ("w.norm", None, b), ("w.ctl_fc2", 2, c),
+                                                    ("w.wqkv", 1, d), ("w.wqkv", 0, None), ("cap_uncond", None, None)], 3)
+    gc.collect()
+    assert s.adapter_fc1 == a.data_ptr() and s.w.norm == b.data_ptr() and list(s.w.ctl_fc2) == [None, None, c.data_ptr()]
+    assert [s.w.wqkv[i] for i in range(3)] == [None, d.data_ptr(), None]
+    assert not s.w.wo and s.cap_uncond is None and s.w.output is None and list(s.w.ctl_fc1) == [None] * 3
+    assert [id(t) for t in ts] == [id(a), id(b), id(c), id(d)]
+
+
 def test_attention_ops_reject_bad_arguments_before_any_launch():
     """Each call differs from a valid one in one argument, which the op must refuse before it touches the device (the pointers are
     never dereferenced)."""
