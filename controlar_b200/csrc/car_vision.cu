@@ -10,6 +10,7 @@
 #include "lineart.cuh"
 #include "dpt.cuh"
 #include "midas.cuh"
+#include "groupnorm.cuh"
 
 template <typename... KArgs, typename... Args>
 static int launch_on(cudaStream_t st, void (*kernel)(KArgs...), unsigned grid, unsigned block, Args... args) {
@@ -564,7 +565,7 @@ extern "C" int car_vq_decode(CarVQ* m, const float* quant, int32_t B, int32_t h,
 // ---- VQModel.encode (vq_model.py:41-46) at fp32 grade: the split-bf16 ("x3") path of split3.cuh ----
 // fp32 NHWC activations; every convolution = one launch of the bf16 implicit-GEMM kernel over tripled K, fp32 output / bias / residual.
 struct ActF { float* p; int B, H, W, C; long long npix() const { return (long long)B * H * W; } long long n() const { return npix() * C; } };
-struct EncScratch { Buf<bf16> t3, x3; Buf<float> h1, sc; float* stats; Buf<float> qf, kf, vf, ctx; float *S, *P; Buf<bf16> q3, k3, P3, vT3; };
+struct EncScratch { Buf<bf16> t3, x3; Buf<float> h1, sc, gnp, stats; Buf<float> qf, kf, vf, ctx; float *S, *P; Buf<bf16> q3, k3, P3, vT3; };
 
 // fp32 rows x [M][N] -> S3 rows (mode X3_ROWS_A, X3_ROWS_A_GELU) or W3 rows (X3_ROWS_B) [M][3N]
 static int split3_rows(cudaStream_t st, const float* x, Buf<bf16> y, long long M, int N, int mode = X3_ROWS_A) {
@@ -593,20 +594,41 @@ static int x3_mma(cudaStream_t st, const X3W& w, const bf16* a3, int B, int Hs, 
     p.bias_f = w.b; p.C = out; p.ldc = w.n; p.out_mode = 1; p.resid_f = resid; p.ldr = w.n; p.act = act;
     return gemm(st, p);
 }
-static int gn_x3(cudaStream_t st, const NormF& nw, const ActF& x, Buf<bf16> y3, int swish, float* stats) {
-    const int G = 32;
-    CAR_TRY(car_fits(__func__, y3, (size_t)x.n() * 3));
-    CAR_LAUNCH(groupnorm_stats_f32_kernel, x.B * G, 512, 0, st, (const float*)x.p, stats, x.H * x.W, x.C, G);
-    CAR_LAUNCH(groupnorm_apply_split3_kernel, gsz(x.n()), 256, 0, st, (const float*)x.p, (const float*)stats, (const float*)nw.w, (const float*)nw.b, y3,
-               x.n(), x.H * x.W, x.C, G, swish);
+// fp32 GroupNorm statistics (groupnorm.cuh) of x [B][HW][C], cpg channels per group (InstanceNorm: 1) -> stats [B][C/cpg][2];
+// part holds the two [B][gn_nch(HW)][C] partial sums
+static int gn_stats(cudaStream_t st, const float* x, int B, int HW, int C, int cpg, float eps, Buf<float> part, Buf<float> stats) {
+    if (C % 32 || cpg < 1 || 32 % cpg) CAR_FAIL(CAR_ERR_STATE, "group statistics need C % 32 == 0 and cpg dividing 32");
+    const int nch = gn_nch(HW);
+    const size_t np = (size_t)B * nch * C;
+    CAR_TRY(car_fits(__func__, part, 2 * np));
+    CAR_TRY(car_fits(__func__, stats, (size_t)B * (C / cpg) * 2));
+    const dim3 grid(C / 32, B, nch);
+    CAR_LAUNCH(gn_partial_kernel<false>, grid, GN_THREADS, 0, st, x, nullptr, part, HW, C, cpg);
+    CAR_LAUNCH(gn_partial_kernel<true>, grid, GN_THREADS, 0, st, x, (const float*)part, part + np, HW, C, cpg);
+    CAR_LAUNCH(gn_finish_kernel, dim3(C / 32, B), 32, 0, st, (const float*)part, (const float*)(part + np), stats, HW, C, cpg, nch, eps);
     return CAR_OK;
+}
+// GroupNorm(32) of x [B][H][W][C] (+ resid, itself normalised when rn.stats) (act) (max-pool) -> S3 frame y, fp32 carrier when given
+static int gn_apply_s3(cudaStream_t st, const float* x, GnAffine gn, const float* resid, GnAffine rn, float* carrier, Buf<bf16> y, int B, int H, int W,
+                       int C, GnApply a) {
+    if (C % GN_GROUPS) CAR_FAIL(CAR_ERR_STATE, "GroupNorm(32) needs C % 32 == 0");
+    if (a.pool && a.act != GN_ACT_RELU) CAR_FAIL(CAR_ERR_STATE, "the GroupNorm max-pool follows ReLU only");
+    const long long n = (long long)B * a.Hp * a.Wp * C;
+    CAR_TRY(car_fits(__func__, y, (size_t)n * 3));
+    CAR_LAUNCH(gn_apply_s3_kernel, gsz(n), 256, 0, st, x, gn, resid, rn, carrier, y, B, H, W, C, a);
+    return CAR_OK;
+}
+// GroupNorm(32, eps 1e-6) (act) of an encoder activation -> S3 rows y3
+static int gn_x3(cudaStream_t st, const NormF& nw, const ActF& x, Buf<bf16> y3, int act, EncScratch& s) {
+    CAR_TRY(gn_stats(st, x.p, x.B, x.H * x.W, x.C, x.C / GN_GROUPS, 1e-6f, s.gnp, s.stats));
+    return gn_apply_s3(st, x.p, GnAffine{s.stats, nw.w, nw.b}, nullptr, GnAffine{}, nullptr, y3, x.B, x.H, x.W, x.C, GnApply{0, 0, x.H, x.W, act, 0});
 }
 // ResnetBlock.forward (vq_model.py:300-315)
 static int res_x3(cudaStream_t st, const ResX3& r, ActF& x, Buf<float> out, EncScratch& s) {
-    CAR_TRY(gn_x3(st, r.n1, x, s.t3, 1, s.stats));
+    CAR_TRY(gn_x3(st, r.n1, x, s.t3, GN_ACT_SWISH, s));
     CAR_TRY(x3_mma(st, r.c1, s.t3, x.B, x.H, x.W, 0, s.h1, nullptr, x.H, x.W));
     ActF h{s.h1, x.B, x.H, x.W, r.c1.n};
-    CAR_TRY(gn_x3(st, r.n2, h, s.t3, 1, s.stats));
+    CAR_TRY(gn_x3(st, r.n2, h, s.t3, GN_ACT_SWISH, s));
     const float* sc = x.p;
     if (r.has_nin) {
         CAR_TRY(split3_rows(st, x.p, s.x3, x.npix(), x.C));
@@ -622,7 +644,7 @@ static int attn_x3(cudaStream_t st, const AttnX3& a, ActF& x, Buf<float> out, En
     const int C = x.C, hw = x.H * x.W, B = x.B;
     const int hwp = (hw + 31) & ~31;
     const long long rows = (long long)B * hw;
-    CAR_TRY(gn_x3(st, a.n, x, s.t3, 0, s.stats));
+    CAR_TRY(gn_x3(st, a.n, x, s.t3, GN_ACT_NONE, s));
     CAR_TRY(x3_mma(st, a.q, s.t3, B, x.H, x.W, 0, s.qf, nullptr, x.H, x.W));
     CAR_TRY(x3_mma(st, a.k, s.t3, B, x.H, x.W, 0, s.kf, nullptr, x.H, x.W));
     CAR_TRY(x3_mma(st, a.v, s.t3, B, x.H, x.W, 0, s.vf, nullptr, x.H, x.W));
@@ -669,7 +691,8 @@ extern "C" int car_vq_encode(CarVQ* m, const float* img, int32_t B, int32_t H, i
         s.h1 = c.take<float>(actf); s.sc = c.take<float>(actf);
         s.t3 = c.take<bf16>(act3); s.x3 = c.take<bf16>(act3);
         img3 = c.take<bf16>((size_t)B * H * W * 32 * 3);
-        s.stats = c.take<float>((size_t)B * 32 * 2);
+        s.gnp = c.take<float>(2 * (size_t)B * GN_MAX_CHUNKS * Cmax);
+        s.stats = c.take<float>((size_t)B * GN_GROUPS * 2);
         s.qf = c.take<float>(af); s.kf = c.take<float>(af); s.vf = c.take<float>(af); s.ctx = c.take<float>(af);
         s.q3 = c.take<bf16>(a3); s.k3 = c.take<bf16>(a3);
         s.S = c.take<float>((size_t)B * hw * hwp); s.P = c.take<float>((size_t)B * hw * hwp);
@@ -696,7 +719,7 @@ extern "C" int car_vq_encode(CarVQ* m, const float* img, int32_t B, int32_t H, i
     CAR_TRY(res_x3(st, m->e_mid0, x, flip(x.p), s));
     CAR_TRY(attn_x3(st, m->e_mid1, x, flip(x.p), s));
     CAR_TRY(res_x3(st, m->e_mid2, x, flip(x.p), s));
-    CAR_TRY(gn_x3(st, m->e_norm_out, x, s.t3, 1, s.stats));
+    CAR_TRY(gn_x3(st, m->e_norm_out, x, s.t3, GN_ACT_SWISH, s));
     Buf<float> zc = flip(x.p);
     CAR_TRY(x3_mma(st, m->e_conv_out, s.t3, B, x.H, x.W, 0, zc, nullptr, x.H, x.W));               // [npix][z_channels]
     CAR_TRY(split3_rows(st, zc, s.x3, (long long)npix, d.z_channels));
@@ -916,7 +939,6 @@ static int x3_win(cudaStream_t st, const X3W& w, const bf16* a3, int B, int Hs, 
     p.osy = osy; p.osx = osx; p.oay = oay; p.oax = oax; p.oH = oH; p.oW = oW;
     return gemm(st, p);
 }
-static int la_nch(int HW) { return std::max(1, std::min(64, (HW + 2047) / 2048)); }
 
 // image fp32 NCHW [B][3][H][W] (values 0..255) -> map fp32 [B][1][Ho][Wo] in [0, 1], Ho = 4 ceil(ceil(H/2)/2) (likewise Wo)
 extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, int32_t H, int32_t W, float* out, void* stream) {
@@ -928,23 +950,19 @@ extern "C" int car_lineart_forward(CarLineArt* m, const float* img, int32_t B, i
     const size_t f_bytes = Bz * 4 * std::max({(size_t)H * W * 64, (size_t)H1 * W1 * 128, (size_t)H2 * W2 * 256, (size_t)H3 * W3 * 128, (size_t)Ho * Wo * 64});
     const size_t s_bytes = Bz * std::max({(size_t)(H + 6) * (W + 6) * 24 * 2, (size_t)(H + 2) * (W + 2) * 192 * 2, (size_t)(H1 + 2) * (W1 + 2) * 384 * 2,
                                           (size_t)(H2 + 2) * (W2 + 2) * 768 * 2, (size_t)(H3 + 1) * (W3 + 1) * 384 * 2, (size_t)(Ho + 6) * (Wo + 6) * 64 * 4});
-    const size_t x_bytes = Bz * H2 * W2 * 256 * 4, p_bytes = Bz * 64 * 256 * 4, st_bytes = Bz * 256 * 2 * 4;
-    Buf<float> F; Buf<char> S; float *X[2], *ps, *pq, *stats;   // S holds S3 (bf16) maps and, for the head, an fp32 map: carved in bytes
+    const size_t x_bytes = Bz * H2 * W2 * 256 * 4;
+    Buf<float> F, part, stats; Buf<char> S; float* X[2];   // S holds S3 (bf16) maps and, for the head, an fp32 map: carved in bytes
     CAR_TRY(m->ws.carve([&](Carve& c) {
         F = c.take<float>(f_bytes / 4);
         S = c.take<char>(s_bytes);
         X[0] = c.take<float>(x_bytes / 4); X[1] = c.take<float>(x_bytes / 4);
-        ps = c.take<float>(p_bytes / 4);
-        pq = c.take<float>(p_bytes / 4);
-        stats = c.take<float>(st_bytes / 4);
+        part = c.take<float>(2 * Bz * GN_MAX_CHUNKS * 256);
+        stats = c.take<float>(Bz * 256 * 2);
     }));
     bf16* S3 = (bf16*)S.p;
     // InstanceNorm of F [B][h][w][C] (+ resid) (ReLU) -> padded S, optional carrier
     auto inorm = [&](int h, int w, int C, const float* resid, float* carrier, InApply a) -> int {
-        const int nch = la_nch(h * w);
-        CAR_LAUNCH(instnorm_sum_kernel, dim3(C / 32, B, nch), IN_THREADS, 0, st, (const float*)F, ps, h * w, C);
-        CAR_LAUNCH(instnorm_sq_kernel, dim3(C / 32, B, nch), IN_THREADS, 0, st, (const float*)F, (const float*)ps, pq, h * w, C);
-        CAR_LAUNCH(instnorm_finish_kernel, (B * C + 255) / 256, 256, 0, st, (const float*)ps, (const float*)pq, stats, B, h * w, C, nch);
+        CAR_TRY(gn_stats(st, F, B, h * w, C, 1, 1e-5f, part, stats));
         const long long n = (long long)B * (h + a.pt + a.pb) * (w + a.pl + a.pr) * C;
         CAR_TRY(car_fits("inorm", S, (size_t)n * (a.s3 ? 6 : 4)));
         CAR_LAUNCH(instnorm_apply_pad_kernel, gsz(n), 256, 0, st, (const float*)F, (const float*)stats, resid, carrier, S, B, h, w, C, a);
@@ -1358,8 +1376,7 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
         const int rn_in[4] = {256, 512, MD_C, MD_C};
         for (int i = 0; i < 4; ++i) s3 = std::max(s3, Bz * x3_fh(sh[i]) * x3_fw(sw[i]) * 3 * std::max(rn_in[i], F));
     }
-    const size_t part = Bz * 64 * MD_GROUPS, stb = Bz * MD_GROUPS * 2;
-    Buf<float> X, X1, K[2], T0, T1, T2, Xa, Xb, Td, fe[4]; float *ps, *pq, *stats, *rstats; Buf<bf16> S;
+    Buf<float> X, X1, K[2], T0, T1, T2, Xa, Xb, Td, fe[4], part, stats, rstats; Buf<bf16> S;
     CAR_TRY(m->ws.carve([&](Carve& c) {
         X = c.take<float>((size_t)M * C);
         X1 = c.take<float>((size_t)M * C);
@@ -1371,36 +1388,26 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
         Xb = c.take<float>(car);
         Td = c.take<float>(car);
         for (int i = 0; i < 4; ++i) fe[i] = c.take<float>(Bz * sh[i] * sw[i] * F);
-        ps = c.take<float>(part);
-        pq = c.take<float>(part);
-        stats = c.take<float>(stb);
-        rstats = c.take<float>(stb);
+        part = c.take<float>(2 * Bz * GN_MAX_CHUNKS * MD_OUT[2]);
+        stats = c.take<float>(Bz * GN_GROUPS * 2);
+        rstats = c.take<float>(Bz * GN_GROUPS * 2);
         S = c.take<bf16>(s3);
     }));
 
-    // GroupNorm statistics of fp32 NHWC [B][hh][ww][Cc] -> stt [B][32][2]; chunks of about 4096 elements per (image, group)
-    auto gn_stats = [&](const float* src, int hh, int ww, int Cc, float* stt) -> int {
-        const int hw = hh * ww, nch = std::max(1, std::min(64, (hw * (Cc / MD_GROUPS) + 4095) / 4096));
-        CAR_LAUNCH(midas_gn_sum_kernel, dim3(MD_GROUPS, B, nch), MD_THREADS, 0, st, src, ps, hw, Cc);
-        CAR_LAUNCH(midas_gn_sq_kernel, dim3(MD_GROUPS, B, nch), MD_THREADS, 0, st, src, (const float*)ps, pq, hw, Cc);
-        CAR_LAUNCH(midas_gn_finish_kernel, (B * MD_GROUPS + 255) / 256, 256, 0, st, (const float*)ps, (const float*)pq, stt, B, hw, Cc, nch);
-        return CAR_OK;
-    };
+    // GroupNorm(32, eps 1e-5) statistics of fp32 NHWC [B][hh][ww][Cc] -> stt [B][32][2]
+    auto gstats = [&](const float* src, int hh, int ww, int Cc, Buf<float> stt) { return gn_stats(st, src, B, hh * ww, Cc, Cc / GN_GROUPS, 1e-5f, part, stt); };
     // GN(src) (+ resid, normalised by rn when rn.stats) (ReLU) (max-pool) -> S3 frame in S, fp32 carrier when given
-    auto gn_apply = [&](const float* src, const NormF& N, const float* resid, GnAffine rn, float* carrier, int hh, int ww, int Cc, GnApply a) -> int {
-        CAR_TRY(car_fits("gn_apply", S, (size_t)B * a.Hp * a.Wp * 3 * Cc));
-        CAR_LAUNCH(midas_gn_apply_kernel, gsz((long long)B * a.Hp * a.Wp * Cc), 256, 0, st, src, GnAffine{stats, N.w, N.b}, resid, rn, carrier, S, B, hh,
-                   ww, Cc, a);
-        return CAR_OK;
+    auto gn_apply = [&](const float* src, const NormF& N, const float* resid, GnAffine rn, float* carrier, int hh, int ww, int Cc, GnApply a) {
+        return gn_apply_s3(st, src, GnAffine{stats, N.w, N.b}, resid, rn, carrier, S, B, hh, ww, Cc, a);
     };
     const GnAffine none{nullptr, nullptr, nullptr};
 
     // ---- stem: conv 7x7/2 (SAME: 2 before, 3 after) -> GN + ReLU -> max-pool 3x3/2 (SAME: 0 before, 1 after) -> S3 rows
     CAR_TRY(image_split3(st, x, nullptr, S, X3Image{B, 3, H, W, 8, 2, 2, 3, 3, 0}));
     CAR_TRY(x3_win(st, m->stem, S, B, H + 5, W + 5, 2, H / 2, W / 2, T0, H / 2, W / 2));
-    CAR_TRY(gn_stats(T0, H / 2, W / 2, 64, stats));
+    CAR_TRY(gstats(T0, H / 2, W / 2, 64, stats));
     int hh = H / 4, ww = W / 4;
-    CAR_TRY(gn_apply(T0, m->stem_n, nullptr, none, nullptr, H / 2, W / 2, 64, GnApply{0, 0, hh, ww, 1, 1}));
+    CAR_TRY(gn_apply(T0, m->stem_n, nullptr, none, nullptr, H / 2, W / 2, 64, GnApply{0, 0, hh, ww, GN_ACT_RELU, 1}));
     // ---- stages: bottlenecks conv1 1x1 -> GN+ReLU -> conv2 3x3 (stride) -> GN+ReLU -> conv3 1x1 -> GN -> + shortcut -> ReLU.  S holds
     // the S3 rows of the block input; xin its fp32 carrier (the identity shortcut); the first block's shortcut is conv 1x1 (stride) + GN.
     float* xin = nullptr;
@@ -1413,25 +1420,25 @@ extern "C" int car_midas_forward(CarMidas* m, const float* x, int32_t B, int32_t
             if (b == 0) {
                 if (k.stride == 1) CAR_TRY(x3_gemm(st, k.dn, S, Min, Td, k.out));
                 else CAR_TRY(x3_win(st, k.dn, S, B, hh, ww, 2, ho, wo, Td, ho, wo));
-                CAR_TRY(gn_stats(Td, ho, wo, k.out, rstats));
+                CAR_TRY(gstats(Td, ho, wo, k.out, rstats));
                 rn = GnAffine{rstats, k.dnn.w, k.dnn.b};
             }
             CAR_TRY(x3_gemm(st, k.c1, S, Min, T0, k.mid));
-            CAR_TRY(gn_stats(T0, hh, ww, k.mid, stats));
+            CAR_TRY(gstats(T0, hh, ww, k.mid, stats));
             if (k.stride == 1) {
-                CAR_TRY(gn_apply(T0, k.n1, nullptr, none, nullptr, hh, ww, k.mid, GnApply{0, 0, x3_fh(hh), x3_fw(ww), 1, 0}));
+                CAR_TRY(gn_apply(T0, k.n1, nullptr, none, nullptr, hh, ww, k.mid, GnApply{0, 0, x3_fh(hh), x3_fw(ww), GN_ACT_RELU, 0}));
                 CAR_TRY(x3_conv3(st, k.c2, S, B, hh, ww, T1));
             } else {                                    // SAME for 3x3/2 on an even map: no padding before, one after
-                CAR_TRY(gn_apply(T0, k.n1, nullptr, none, nullptr, hh, ww, k.mid, GnApply{0, 0, hh + 1, ww + 1, 1, 0}));
+                CAR_TRY(gn_apply(T0, k.n1, nullptr, none, nullptr, hh, ww, k.mid, GnApply{0, 0, hh + 1, ww + 1, GN_ACT_RELU, 0}));
                 CAR_TRY(x3_win(st, k.c2, S, B, hh + 1, ww + 1, 2, ho, wo, T1, ho, wo));
             }
-            CAR_TRY(gn_stats(T1, ho, wo, k.mid, stats));
-            CAR_TRY(gn_apply(T1, k.n2, nullptr, none, nullptr, ho, wo, k.mid, GnApply{0, 0, ho, wo, 1, 0}));
+            CAR_TRY(gstats(T1, ho, wo, k.mid, stats));
+            CAR_TRY(gn_apply(T1, k.n2, nullptr, none, nullptr, ho, wo, k.mid, GnApply{0, 0, ho, wo, GN_ACT_RELU, 0}));
             CAR_TRY(x3_gemm(st, k.c3, S, Mo, T2, k.out));
-            CAR_TRY(gn_stats(T2, ho, wo, k.out, stats));
+            CAR_TRY(gstats(T2, ho, wo, k.out, stats));
             Buf<float> xo = xin == Xa ? Xb : Xa;
             CAR_TRY(car_fits("midas trunk carrier", xo, (size_t)Mo * k.out));
-            CAR_TRY(gn_apply(T2, k.n3, b == 0 ? Td : xin, rn, xo, ho, wo, k.out, GnApply{0, 0, ho, wo, 1, 0}));
+            CAR_TRY(gn_apply(T2, k.n3, b == 0 ? Td : xin, rn, xo, ho, wo, k.out, GnApply{0, 0, ho, wo, GN_ACT_RELU, 0}));
             xin = xo; hh = ho; ww = wo;
         }
         if (s < 2) {                                    // stage outputs 0 and 1 are features 1 and 2: scratch.layer{1,2}_rn

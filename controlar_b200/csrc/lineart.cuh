@@ -2,9 +2,9 @@
 // Every wide convolution is one A_WIN launch of the split-bf16 ("x3", split3.cuh) implicit GEMM over an S3 source whose padding was
 // written by the kernel that produced it (the stem's input: image_split3_kernel, reflect-pad 3, 8 channels per part); the kernels
 // below are the rest of that glue:
-//   instance norm  InstanceNorm2d defaults (affine=False, eps 1e-5, biased variance per (sample, channel)): deterministic two-pass
-//                  statistics over NHWC fp32, then one apply kernel that adds the residual, applies ReLU and writes the next
-//                  convolution's padded input (reflect or zero, S3 or fp32) plus, where asked, the fp32 carrier
+//   instance norm  InstanceNorm2d defaults (affine=False, eps 1e-5, biased variance per (sample, channel)): the statistics are
+//                  groupnorm.cuh's with one channel per group; the apply kernel here adds the residual, applies ReLU and writes the
+//                  next convolution's padded input (reflect or zero, S3 or fp32) plus, where asked, the fp32 carrier
 //   transposed     ConvTranspose2d(3, stride 2, pad 1, output_padding 1) as four sub-pixel stride-1 convolutions (parity class
 //   convolution    (a, b) of the output): along an axis even outputs 2i take tap 1 of input i, odd outputs 2i+1 take tap 2 of input
 //                  i and tap 0 of input i+1 (a zero row / column is appended at the bottom / right) -> windows of 1x1, 1x2, 2x1, 2x2
@@ -34,57 +34,6 @@ __global__ void convT_weight_pack_x3_kernel(const float* __restrict__ w, bf16* _
         const float v = c < Cin ? w[(((size_t)c * Cout + o) * 3 + ky) * 3 + kx] : 0.f;
         x3_put_w3(y + (i - c) * 3 + c, Cin_pad, v);     // (i - c) = index of this (class, o, tap) row times Cin_pad
     }
-}
-
-// ---- instance-norm statistics over NHWC fp32 [B][HW][C] (C % 32 == 0).  grid (C/32, B, nch), 256 threads = 32 channels x 8 pixel
-// lanes; pixel chunk j of nch covers [j*per, (j+1)*per).  Every sum has a fixed order that depends on (HW, C) only, never on B. ----
-constexpr int IN_THREADS = 256;
-__device__ __forceinline__ float in_chunk_sum(const float* __restrict__ xb, int HW, int C, int c, int nch, int j, float mean, bool centred,
-                                              float (*red)[32]) {
-    const int per = (HW + nch - 1) / nch;
-    const int p0 = j * per, p1 = min(HW, p0 + per);
-    const int lane = threadIdx.x & 31, row = threadIdx.x >> 5;
-    float s = 0.f;
-    for (int p = p0 + row; p < p1; p += IN_THREADS / 32) {
-        const float v = xb[(size_t)p * C + c];
-        if (centred) { const float d = v - mean; s = fmaf(d, d, s); } else s += v;
-    }
-    red[row][lane] = s;
-    __syncthreads();
-    float t = 0.f;
-    if (row == 0)
-        for (int k = 0; k < IN_THREADS / 32; ++k) t += red[k][lane];
-    return t;                                            // valid in row 0
-}
-__global__ void __launch_bounds__(IN_THREADS) instnorm_sum_kernel(const float* __restrict__ x, float* __restrict__ part_s /*[B][nch][C]*/, int HW, int C) {
-    __shared__ float red[IN_THREADS / 32][32];
-    const int c = blockIdx.x * 32 + (threadIdx.x & 31), b = blockIdx.y, j = blockIdx.z, nch = gridDim.z;
-    const float t = in_chunk_sum(x + (size_t)b * HW * C, HW, C, c, nch, j, 0.f, false, red);
-    if (threadIdx.x < 32) part_s[((size_t)b * nch + j) * C + c] = t;
-}
-__device__ __forceinline__ float in_mean(const float* __restrict__ part_s, int b, int nch, int C, int c, int HW) {
-    float s = 0.f;
-    for (int j = 0; j < nch; ++j) s += part_s[((size_t)b * nch + j) * C + c];
-    return s / (float)HW;
-}
-__global__ void __launch_bounds__(IN_THREADS) instnorm_sq_kernel(const float* __restrict__ x, const float* __restrict__ part_s, float* __restrict__ part_q,
-                                                                int HW, int C) {
-    __shared__ float red[IN_THREADS / 32][32];
-    const int c = blockIdx.x * 32 + (threadIdx.x & 31), b = blockIdx.y, j = blockIdx.z, nch = gridDim.z;
-    const float mean = in_mean(part_s, b, nch, C, c, HW);
-    const float t = in_chunk_sum(x + (size_t)b * HW * C, HW, C, c, nch, j, mean, true, red);
-    if (threadIdx.x < 32) part_q[((size_t)b * nch + j) * C + c] = t;
-}
-// stats [B][C][2] = (mean, 1 / sqrt(biased variance + 1e-5))
-__global__ void instnorm_finish_kernel(const float* __restrict__ part_s, const float* __restrict__ part_q, float* __restrict__ stats, int B, int HW,
-                                       int C, int nch) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= B * C) return;
-    const int b = i / C, c = i - b * C;
-    float q = 0.f;
-    for (int j = 0; j < nch; ++j) q += part_q[((size_t)b * nch + j) * C + c];
-    stats[2 * i] = in_mean(part_s, b, nch, C, c, HW);
-    stats[2 * i + 1] = 1.0f / sqrtf(q / (float)HW + 1e-5f);
 }
 
 // v = IN(x) (+ resid) (ReLU), in fp32, written as the next convolution's padded input y [B][H+pt+pb][W+pl+pr][C] (S3: 3C bf16 per

@@ -1,6 +1,6 @@
 // vision.cuh — normalisation / resampling / soft-max / quantiser kernels around the dense GEMM for the control
 // encoder (HF Dinov2Model as used by autoregressive/models/dinov2_adapter.py) and the VQGAN tokenizer
-// (tokenizer/tokenizer_image/vq_model.py).
+// (tokenizer/tokenizer_image/vq_model.py).  The fp32-grade encoder's GroupNorm is groupnorm.cuh's.
 #pragma once
 #include "common.cuh"
 #include "patch_embed.cuh"
@@ -352,37 +352,6 @@ __global__ void conv_weight_pack_x3_kernel(const float* __restrict__ w, bf16* __
         const int o = (int)(r / KH);
         const float v = c < Cin ? w[(((size_t)o * Cin + c) * KH + ky) * KW + kx] : 0.f;
         x3_put_w3(y + tapidx * 3 * Cin_pad + c, Cin_pad, v);
-    }
-}
-// GroupNorm(32, eps 1e-6) statistics over NHWC fp32 (two-pass mean / variance in fp64-free fp32: mean first, then centred squares)
-__global__ void groupnorm_stats_f32_kernel(const float* __restrict__ x, float* __restrict__ stats /*[B*G][2]*/, int HW, int C, int G) {
-    __shared__ float red[32];
-    const int b = blockIdx.x / G, g = blockIdx.x % G, cg = C / G;
-    const float* xb = x + (size_t)b * HW * C + g * cg;
-    const long long n = (long long)HW * cg;
-    float s = 0.f;
-    for (long long i = threadIdx.x; i < n; i += blockDim.x) s += xb[(i / cg) * C + (i % cg)];
-    s = block_sum(s, red);
-    __shared__ float s_mean;
-    if (threadIdx.x == 0) s_mean = s / n;
-    __syncthreads();
-    const float mean = s_mean;
-    float ss = 0.f;
-    for (long long i = threadIdx.x; i < n; i += blockDim.x) { const float d = xb[(i / cg) * C + (i % cg)] - mean; ss += d * d; }
-    ss = block_sum(ss, red);
-    if (threadIdx.x == 0) { stats[blockIdx.x * 2] = mean; stats[blockIdx.x * 2 + 1] = rsqrtf(ss / n + 1e-6f); }
-}
-// y = GN(x) (*swish) in fp32, written as S3
-__global__ void groupnorm_apply_split3_kernel(const float* __restrict__ x, const float* __restrict__ stats, const float* __restrict__ w,
-                                              const float* __restrict__ bsh, bf16* __restrict__ y3, long long total, int HW, int C, int G, int swish) {
-    const int cg = C / G;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const long long pix = i / C; const int c = (int)(i - pix * C);
-        const int b = (int)(pix / HW);
-        const float* st = stats + ((size_t)b * G + c / cg) * 2;
-        float v = (x[i] - st[0]) * st[1] * w[c] + bsh[c];
-        if (swish) v = v / (1.0f + expf(-v));
-        x3_put_s3(y3 + pix * 3 * C + c, C, v);
     }
 }
 // soft-max over rows of fp32 scores, fp32 out (columns >= n of the padded row are zeroed)
