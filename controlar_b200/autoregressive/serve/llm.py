@@ -95,7 +95,11 @@ class Scheduler:
 
 class LLM:
     """`LLM(model=<controlar_b200 GPT module>, vq=<VQ module or None>, cfg_scale=...)`; `generate(...)` as in the reference's
-    serve/sample_c2i.py:55-58, plus `add_request` / `step` for a queue that is fed while batches run."""
+    serve/sample_c2i.py:55-58, plus `add_request` / `step` for a queue that is fed while batches run.
+
+    `max_images_per_batch` (default 8) caps the images of one launch.  With CFG, up to 8 images (16 sequences) run on the
+    persistent decode kernel; 17 to 32 images (34 to 64 sequences) of a bf16 model run on the wide decode route, one tensor-core
+    pass over the weights per step (DESIGN.md §4.2); other sizes and fp32 models run on the per-kernel chain."""
 
     def __init__(self, args=None, model=None, vq=None, cfg_scale: Optional[float] = None, max_images_per_batch: int = 8, seed: int = 0,
                  runner: Optional[Callable[[List[Request], int], torch.Tensor]] = None, **unused):

@@ -68,6 +68,12 @@ struct CarState : CarOwned {
     unsigned int* pk_bar = nullptr; unsigned int pk_bar_count = 0, pk_tag_gen = 0;
     size_t pk_pkt_bytes = 0; void* pk_pkt_base = nullptr;
     long long* pk_step_ts = nullptr;   // caller-provided device buffer [N] for per-step timestamps (car_state_set_step_timer) or null
+    // wide decode route (bf16, 32 < b_eff <= 64): gemm_wide on the borrowed weights, RMSNorm into xn, one split-K workspace
+    bool wide = false;
+    void* xn = nullptr;                // [b_eff][dim] normalised rows
+    float* wide_part = nullptr; size_t wide_part_bytes = 0;
+    int* wide_tickets = nullptr; int wide_n_tickets = 0;
+    long long graph_launches = 0;      // launches in one replay of the decode graph
 
     // Releases the graph and the capture stream; the device memory goes with CarOwned.  It must not read `m`: a layout change
     // destroys the old CarModel (gpt_t2i.setup_caches) before the state built on it is closed.
@@ -343,6 +349,29 @@ static int pk_state_setup(CarState* s) {
     return CAR_OK;
 }
 
+// the wide decode route: every decode-step GEMM through gemm_wide (gemm.h) with one workspace sized for the largest of them.  Taken
+// above 32 rows: on an H100 at GPT-XL it is faster than the skinny chain at 50 and 64 rows and slower at 32, where its separate
+// RMSNorm launches and split-K partials cost more than the second weight pass of the chain's two 16-row tiles (DESIGN §4.2).
+static bool wide_route(const CarModelDesc& d, int b_eff) { return d.dtype == CAR_BF16 && b_eff > 32 && b_eff <= 64; }
+static int wide_state_setup(CarState* s) {
+    const CarModelDesc& d = s->m->d;
+    const int M = s->b_eff;
+    const WidePlan plans[5] = {gemm_wide_plan(M, 3 * d.dim, d.dim, false), gemm_wide_plan(M, d.dim, d.dim, false),
+                               gemm_wide_plan(M, d.ffn_dim, d.dim, true), gemm_wide_plan(M, d.dim, d.ffn_dim, false),
+                               gemm_wide_plan(M, d.vocab_size, d.dim, false)};
+    for (const WidePlan& w : plans) {
+        s->wide_part_bytes = std::max(s->wide_part_bytes, w.part_bytes);
+        s->wide_n_tickets = std::max(s->wide_n_tickets, w.tiles);
+    }
+    CAR_TRY(s->alloc(&s->xn, (size_t)M * d.dim * 2));
+    CAR_TRY(s->alloc(&s->wide_part, s->wide_part_bytes));
+    CAR_TRY(s->alloc(&s->wide_tickets, (size_t)s->wide_n_tickets * 4));
+    CAR_TRY(fill_u32(s->wide_tickets, 0u, (size_t)s->wide_n_tickets * 4, nullptr));
+    CAR_CUDA(cudaStreamSynchronize(nullptr));
+    s->wide = true;
+    return CAR_OK;
+}
+
 // key splits of the decode attention: about four CTAs per SM over all (b, h) rows, at most 16 per row
 static int attn_decode_nsplit(int bh) { return std::max(1, std::min(16, (4 * sm_count() + bh - 1) / bh)); }
 
@@ -374,6 +403,7 @@ static int state_init(CarState* s, void* const* k_cache, void* const* v_cache) {
     CAR_CUDA(cudaMemset(s->pos, 0, 16));
     s->done_ctr = s->pos + 1;
     s->pk_tag_gen = g_pk_tag_gen.load();
+    if (wide_route(d, b_eff)) CAR_TRY(wide_state_setup(s));
     return d.dtype == CAR_BF16 ? pk_state_setup(s) : CAR_OK;     // persistent decode kernel resources (bf16 only)
 }
 
@@ -487,6 +517,23 @@ static int enqueue_block_dense(CarState* s, int l, cudaStream_t st) {
     return CAR_OK;
 }
 
+// one GEMM of a block or of the head, RMSNorm `nw` in front when given.  Decode steps of the wide route: rmsnorm_rows_kernel then
+// gemm_wide on the borrowed [N][K] weights W (and W3 = w3 for SwiGLU); otherwise the skinny kernel on the packed copy Wp (N rows,
+// 2N when W3 is given: w1 / w3 interleaved) with the norm fused.
+static int block_linear(CarState* s, bool decode, cudaStream_t st, const void* A, int lda, const void* Wp, const void* W, const void* W3,
+                        const void* nw, int rows, int N, int K, const EpiParams& ep) {
+    const CarModelDesc& d = s->m->d;
+    if (decode && s->wide) {
+        if (nw) {
+            CAR_LAUNCH((rmsnorm_rows_kernel<bf16>), rows, 256, 0, st, (const bf16*)A, (const bf16*)nw, (bf16*)s->xn, K, d.norm_eps);
+            A = s->xn; lda = K;
+        }
+        return gemm_wide(st, (const bf16*)A, lda, (const bf16*)W, (const bf16*)W3, rows, N, K, ep, s->wide_part, s->wide_part_bytes,
+                         s->wide_tickets, s->wide_n_tickets);
+    }
+    return launch_skinny(st, d.dtype, A, lda, Wp, nw, nw ? d.norm_eps : 0.f, rows, W3 ? 2 * N : N, K, ep, nw != nullptr);
+}
+
 // one transformer block on `rows` rows; decode (rpb = 1, pos from device scalar) or prefill (rpb = T, pos = t)
 static int enqueue_block(CarState* s, int l, bool decode, cudaStream_t st) {
     CarModel* m = s->m;
@@ -503,7 +550,7 @@ static int enqueue_block(CarState* s, int l, bool decode, cudaStream_t st) {
     EpiParams e1 = epi_base(EPI_QKV);
     e1.rpb = rpb; e1.pos_ptr = posp; e1.rope = s->rope; e1.kc = s->kc[l]; e1.vc = s->vc[l]; e1.q = q; e1.S = s->S;
     e1.H = d.n_head; e1.d = dim;
-    CAR_TRY(launch_skinny(st, dt, h, dim, m->g_wqkv[l], m->attention_norm[l], d.norm_eps, rows, 3 * dim, dim, e1, true));
+    CAR_TRY(block_linear(s, decode, st, h, dim, m->g_wqkv[l], m->wqkv[l], nullptr, m->attention_norm[l], rows, 3 * dim, dim, e1));
 
     if (decode)
         CAR_TRY(launch_attn_decode(dt, st, s->q, s->kc[l], s->vc[l], s->emb_mask, s->T, s->pos, s->b_eff, d.n_head, s->S, s->T, s->nsplit,
@@ -513,11 +560,11 @@ static int enqueue_block(CarState* s, int l, bool decode, cudaStream_t st) {
 
     EpiParams e2 = epi_base(EPI_RESID);
     e2.rpb = rpb; e2.pos_ptr = posp; e2.h = h; e2.ldh = dim;
-    CAR_TRY(launch_skinny(st, dt, attn, dim, m->g_wo[l], nullptr, 0.f, rows, dim, dim, e2, false));
+    CAR_TRY(block_linear(s, decode, st, attn, dim, m->g_wo[l], m->wo[l], nullptr, nullptr, rows, dim, dim, e2));
 
     EpiParams e3 = epi_base(EPI_SWIGLU);
     e3.rpb = rpb; e3.out = act; e3.ldo = F;
-    CAR_TRY(launch_skinny(st, dt, h, dim, m->g_w13[l], m->ffn_norm[l], d.norm_eps, rows, 2 * F, dim, e3, true));
+    CAR_TRY(block_linear(s, decode, st, h, dim, m->g_w13[l], m->w1[l], m->w3[l], m->ffn_norm[l], rows, F, dim, e3));
 
     EpiParams e4 = epi_base(EPI_RESID);
     e4.rpb = rpb; e4.pos_ptr = posp; e4.h = h; e4.ldh = dim;
@@ -526,20 +573,20 @@ static int enqueue_block(CarState* s, int l, bool decode, cudaStream_t st) {
         // control add of the NEXT layer group fused here (gpt_t2i.py:466)
         e4.ctrl = s->ctrl[(l + 1) / step3]; e4.n_img = s->N; e4.T = s->T; e4.cs = s->cs;
     }
-    return launch_skinny(st, dt, act, F, m->g_w2[l], nullptr, 0.f, rows, dim, F, e4, false);
+    return block_linear(s, decode, st, act, F, m->g_w2[l], m->w2[l], nullptr, nullptr, rows, dim, F, e4);
 }
 
-static int enqueue_head(CarState* s, const void* hrows, int rows, float* logits, cudaStream_t st) {
+static int enqueue_head(CarState* s, const void* hrows, int rows, float* logits, bool decode, cudaStream_t st) {
     CarModel* m = s->m;
     const CarModelDesc& d = m->d;
     EpiParams e = epi_base(EPI_LOGITS);
     e.logits = logits; e.ldl = d.vocab_size;
-    return launch_skinny(st, d.dtype, hrows, d.dim, m->g_output, m->norm, d.norm_eps, rows, d.vocab_size, d.dim, e, true);
+    return block_linear(s, decode, st, hrows, d.dim, m->g_output, m->output, nullptr, m->norm, rows, d.vocab_size, d.dim, e);
 }
 
 static int enqueue_decode_layers(CarState* s, float* logits, cudaStream_t st) {
     for (int l = 0; l < s->m->d.n_layer; ++l) CAR_TRY(enqueue_block(s, l, true, st));
-    return enqueue_head(s, s->h, s->b_eff, logits, st);
+    return enqueue_head(s, s->h, s->b_eff, logits, true, st);
 }
 
 static int enqueue_mlp(CarState* s, const void* x, int rows, int K, const void* fc1, const void* fc2, const void* fc1_plain,
@@ -598,9 +645,9 @@ extern "C" int car_prefill(CarState* s, const void* cond, const void* condition,
     // 4. head: last prefix row always (feeds car_generate); all rows on request (forward() parity)
     if (d.dtype == CAR_BF16) CAR_LAUNCH((take_last_row_kernel<bf16>), s->b_eff, 256, 0, st, (const bf16*)s->hP, (bf16*)s->h, s->T, d.dim);
     else CAR_LAUNCH((take_last_row_kernel<float>), s->b_eff, 256, 0, st, (const float*)s->hP, (float*)s->h, s->T, d.dim);
-    CAR_TRY(enqueue_head(s, s->h, s->b_eff, s->logits, st));
+    CAR_TRY(enqueue_head(s, s->h, s->b_eff, s->logits, false, st));
     if (logits_out) {
-        if (all_rows) CAR_TRY(enqueue_head(s, s->hP, rows, logits_out, st));
+        if (all_rows) CAR_TRY(enqueue_head(s, s->hP, rows, logits_out, false, st));
         else CAR_CUDA(cudaMemcpyAsync(logits_out, s->logits, (size_t)s->b_eff * d.vocab_size * 4, cudaMemcpyDeviceToDevice, st));
     }
     CAR_LAUNCH(set_int_kernel, 1, 1, 0, st, s->pos, s->T - 1);
@@ -814,6 +861,7 @@ extern "C" int car_generate(CarState* s, const CarSampling* sp, int32_t n_tokens
             int r = enqueue_decode_layers(s, s->logits, s->cap_stream);
             if (r == CAR_OK) r = launch_sampler(a, s->cap_stream);
             cudaError_t ce = cudaStreamEndCapture(s->cap_stream, &g);
+            s->graph_launches = g_car_launches.load() - launched_before;
             g_car_launches.store(launched_before);
             if (r != CAR_OK) { if (g) cudaGraphDestroy(g); return r; }
             if (ce != cudaSuccess) CAR_FAIL(CAR_ERR_CUDA, std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
@@ -822,9 +870,8 @@ extern "C" int car_generate(CarState* s, const CarSampling* sp, int32_t n_tokens
             if (ce != cudaSuccess) CAR_FAIL(CAR_ERR_CUDA, std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ce));
             s->graph_ok = true; s->gsp = *sp; s->gnoise = noise; s->graph_pack_gen = s->m->pack_gen;
         }
-        const int per_step = s->m->d.n_layer * 5 + 2;
         for (int i = 1; i < n_tokens; ++i) CAR_CUDA(cudaGraphLaunch(s->gexec, st));
-        g_car_launches.fetch_add((long long)per_step * (n_tokens - 1), std::memory_order_relaxed);
+        g_car_launches.fetch_add(s->graph_launches * (n_tokens - 1), std::memory_order_relaxed);
     }
     const int B = a.B;
     CAR_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)n_tokens * 4, s->tokens, (size_t)s->N * 4, (size_t)n_tokens * 4, B,
@@ -833,20 +880,43 @@ extern "C" int car_generate(CarState* s, const CarSampling* sp, int32_t n_tokens
     return CAR_OK;
 }
 
-// teacher-forced run of the SAME device-side loop (parity tests): the token fed to step i + 1 is forced[b][i]; the sampler still
+// teacher forcing on the per-kernel chain: row r (image r mod B; a CFG pair shares its token) is fed forced[image][step]
+__global__ void forced_tokens_kernel(const int* __restrict__ forced, int ld, int step, int B, int b_eff, int* __restrict__ tok) {
+    for (int r = threadIdx.x; r < b_eff; r += blockDim.x) tok[r] = forced[(size_t)(r % B) * ld + step];
+}
+
+// the per-kernel chain's decode loop (wide route included), teacher-forced: per step the sampler (its fused tail advances the position), the forced token's
+// embedding (+ control add) in place of the sampled one, the layers and the head
+static int chain_forced_loop(CarState* s, const SampleArgs& a, int n_tokens, const int32_t* forced, float* trace, cudaStream_t st) {
+    const CarModelDesc& d = s->m->d;
+    const size_t row_bytes = (size_t)s->b_eff * d.vocab_size * 4;
+    if (trace) CAR_CUDA(cudaMemcpyAsync(trace, s->logits, row_bytes, cudaMemcpyDeviceToDevice, st));
+    for (int i = 0; i < n_tokens; ++i) {
+        CAR_TRY(launch_sampler(a, st));
+        if (i + 1 == n_tokens) break;
+        CAR_LAUNCH(forced_tokens_kernel, 1, 64, 0, st, (const int*)forced, n_tokens, i, a.B, s->b_eff, s->tok);
+        CAR_LAUNCH((gather_rows_kernel<bf16>), s->b_eff, 256, 0, st, (const bf16*)s->m->tok_emb, (const int*)s->tok, (bf16*)s->h, d.dim,
+                   (const bf16*)(s->has_ctrl ? s->ctrl[0] : nullptr), s->N, i + 1, s->cs);
+        CAR_TRY(enqueue_decode_layers(s, s->logits, st));
+        if (trace) CAR_CUDA(cudaMemcpyAsync(trace + (size_t)(i + 1) * s->b_eff * d.vocab_size, s->logits, row_bytes, cudaMemcpyDeviceToDevice, st));
+    }
+    return CAR_OK;
+}
+
+// teacher-forced run of the product decode loop (parity tests): the token fed to step i + 1 is forced[b][i]; the sampler still
 // runs and tokens_out holds what it would have chosen at every step given the forced prefix; logits_trace (optional) receives the
-// raw model logits of every step.
+// raw model logits of every step.  bf16: the persistent kernel where it runs, else the per-kernel chain (wide route above 32 rows).
 extern "C" int car_generate_forced(CarState* s, const CarSampling* sp, int32_t n_tokens, const float* noise, const int32_t* forced_tokens,
                                    float* logits_trace, int32_t* tokens_out, void* stream) {
     if (!s || !sp || !tokens_out || !forced_tokens) CAR_FAIL(CAR_ERR_ARG, "null argument");
     if (!s->prefilled) CAR_FAIL(CAR_ERR_STATE, "car_generate_forced must follow car_prefill on the same state");
     if (n_tokens < 1 || n_tokens > s->N) CAR_FAIL(CAR_ERR_ARG, "n_tokens must be in [1, N]");
-    if (!(s->m->d.dtype == CAR_BF16 && s->pk_ok))
-        CAR_FAIL(CAR_ERR_UNSUPPORTED, "teacher forcing through the device-side loop needs the persistent decode kernel (bf16); use car_decode_step");
+    if (s->m->d.dtype != CAR_BF16) CAR_FAIL(CAR_ERR_UNSUPPORTED, "teacher forcing through the device-side loop is bf16 only; use car_decode_step");
     cudaStream_t st = (cudaStream_t)stream;
     SampleArgs a;
     CAR_TRY(loop_sample_args(s, sp, noise, a));
-    CAR_TRY(launch_pk(s, a, n_tokens, st, forced_tokens, logits_trace));
+    if (s->pk_ok) CAR_TRY(launch_pk(s, a, n_tokens, st, forced_tokens, logits_trace));
+    else CAR_TRY(chain_forced_loop(s, a, n_tokens, forced_tokens, logits_trace, st));
     CAR_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)n_tokens * 4, s->tokens, (size_t)s->N * 4, (size_t)n_tokens * 4, a.B,
                                cudaMemcpyDeviceToDevice, st));
     CAR_LAUNCH(set_int_kernel, 1, 1, 0, st, s->pos, s->T - 1 + n_tokens);

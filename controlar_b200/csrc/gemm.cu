@@ -27,11 +27,11 @@ static int wg_encode(CUtensorMap* map, cuuint32_t rank, const void* base, const 
         CAR_FAIL(CAR_ERR_CUDA, "cuTensorMapEncodeTiled failed");
     return CAR_OK;
 }
-// row-major bf16 matrix [rows][cols] with row pitch ld elements; box = 64 columns x 128 rows
-static int wg_make_map(CUtensorMap* map, const void* base, int rows, int cols, int ld) {
+// row-major bf16 matrix [rows][cols] with row pitch ld elements; box = 64 columns x box_rows rows
+static int wg_make_map(CUtensorMap* map, const void* base, int rows, int cols, int ld, int box_rows = WG_BM) {
     const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
     const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-    const cuuint32_t box[2] = {WG_BK, WG_BM};
+    const cuuint32_t box[2] = {WG_BK, (cuuint32_t)box_rows};
     return wg_encode(map, 2, base, dims, strides, box);
 }
 // NHWC bf16 tensor [N][H][W][C] as a 4-D map {C, W, H, N}; box = {64 channels, 16 x, 8 y, 1 image}
@@ -178,6 +178,49 @@ int gemm_f32(cudaStream_t st, const bf16* A, const bf16* B, int M, int N, int K,
     memset(&q, 0, sizeof(q));
     q.M = M; q.N = N; q.K = K; q.bias_f = bias; q.resid_f = resid; q.ldr = ldc; q.C32 = out; q.ldc = ldc;
     return wg_plain<true>(st, q, A, K, B, K);
+}
+
+// one CTA per 64-column tile and K split; the fewest splits that give every SM a CTA (fewer fp32 partials to sum), each split
+// a whole number of k-blocks.  Depends on the SM count only, so a given card always reduces in the same order.
+WidePlan gemm_wide_plan(int M, int N, int K, bool dual) {
+    WidePlan w;
+    w.tiles = (N + WD_BN - 1) / WD_BN;
+    const int nkb = (K + WG_BK - 1) / WG_BK;
+    const int want = std::max(1, std::min(nkb, (sm_count() + w.tiles - 1) / w.tiles));
+    w.kper = (nkb + want - 1) / want;
+    w.splits = (nkb + w.kper - 1) / w.kper;
+    w.part_bytes = w.splits > 1 ? (size_t)w.tiles * w.splits * M * (dual ? 2 : 1) * WD_BN * 4 : 0;
+    return w;
+}
+
+int gemm_wide(cudaStream_t st, const bf16* A, int lda, const bf16* B, const bf16* B3, int M, int N, int K, const EpiParams& ep, float* part,
+              size_t part_bytes, int* tickets, int n_tickets) {
+    if (!A || !B) CAR_FAIL(CAR_ERR_ARG, "A and B must be non-null");
+    if (M < 1 || M > 64) CAR_FAIL(CAR_ERR_ARG, "M must be in [1, 64]");
+    if (N <= 0 || N % 8) CAR_FAIL(CAR_ERR_ARG, "N must be a positive multiple of 8");
+    if (K <= 0 || K % 8) CAR_FAIL(CAR_ERR_ARG, "K must be a positive multiple of 8");
+    if (lda < K || lda % 8) CAR_FAIL(CAR_ERR_ARG, "lda must be >= K and a multiple of 8");
+    if (!aligned16(A) || !aligned16(B) || (B3 && !aligned16(B3))) CAR_FAIL(CAR_ERR_ARG, "A, B and B3 must be 16-byte aligned");
+    if ((B3 != nullptr) != (ep.kind == EPI_SWIGLU)) CAR_FAIL(CAR_ERR_ARG, "B3 (w3) is given exactly for the SwiGLU epilogue");
+    const bool dual = B3 != nullptr;
+    const WidePlan w = gemm_wide_plan(M, N, K, dual);
+    if (w.splits > 1 && (!part || part_bytes < w.part_bytes || !tickets || n_tickets < w.tiles))
+        CAR_FAIL(CAR_ERR_ARG, "split-K workspace or tickets smaller than gemm_wide_plan asks");
+    alignas(64) CUtensorMap mapA, mapB, mapB3;
+    CAR_TRY(wg_make_map(&mapA, A, M, K, lda, 64));
+    CAR_TRY(wg_make_map(&mapB, B, N, K, K, WD_BN));
+    CAR_TRY(wg_make_map(&mapB3, dual ? B3 : B, N, K, K, WD_BN));
+    WdP q;
+    memset(&q, 0, sizeof(q));
+    q.M = M; q.N = N; q.K = K; q.splits = w.splits; q.kper = w.kper; q.part = part; q.tickets = tickets; q.ep = ep; q.ep.M = M;
+    static DevOnce once;
+    if (once.first()) {
+        CAR_CUDA(cudaFuncSetAttribute(gemm_wide_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wd_smem(false)));
+        CAR_CUDA(cudaFuncSetAttribute(gemm_wide_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wd_smem(true)));
+    }
+    if (dual) CAR_LAUNCH_PDL(gemm_wide_kernel<true>, dim3(w.tiles * w.splits), dim3(WD_THREADS), wd_smem(true), st, mapA, mapB, mapB3, q);
+    else CAR_LAUNCH_PDL(gemm_wide_kernel<false>, dim3(w.tiles * w.splits), dim3(WD_THREADS), wd_smem(false), st, mapA, mapB, mapB3, q);
+    return CAR_OK;
 }
 
 int gemm_f32_conv3(cudaStream_t st, const bf16* src, int fh, int fw, const bf16* B, int nimg, int H, int W, int cin, int N, const float* bias,

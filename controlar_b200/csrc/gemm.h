@@ -78,6 +78,19 @@ int gemm(cudaStream_t st, const DenseP& p, int batch = 1);
 // no rounding; bias and resid may be null.  M >= 0, N > 0 and N % 8 == 0, K > 0 and K % 8 == 0, ldc >= N and even; A and B
 // 16-byte aligned, out and resid 8-byte aligned.  Checked before any launch (CAR_ERR_ARG).
 int gemm_f32(cudaStream_t st, const bf16* A, const bf16* B, int M, int N, int K, const float* bias, const float* resid, float* out, int ldc);
+// Decode-step GEMM for 1 <= M <= 64 rows (the wide decode route, car_api.cu): A bf16 [M][lda] (one m64 wgmma tile) times the
+// weights B bf16 [N][K] (nn.Linear layout, read in place), fp32 accumulate, then the decode epilogue `ep` (EpiParams,
+// gemm_skinny.cuh: QKV + RoPE + KV append, residual (+ control add), SwiGLU, logits).  B3: the w3 weights of the SwiGLU epilogue
+// (given exactly when ep.kind == EPI_SWIGLU), over the same N columns as B = w1.  K is split over CTAs as gemm_wide_plan says;
+// with more than one split the fp32 partials go to `part` (part_bytes >= plan.part_bytes) and `tickets` (n_tickets >= plan.tiles,
+// zero before the first launch, left zero by every launch), and they are summed in split order: results do not depend on timing
+// and a row's result does not depend on the other rows.  N, K multiples of 8, lda >= K and a multiple of 8, A, B, B3 16-byte
+// aligned.  Checked before any launch (CAR_ERR_ARG).
+struct EpiParams;
+struct WidePlan { int tiles, splits, kper; size_t part_bytes; };
+WidePlan gemm_wide_plan(int M, int N, int K, bool dual);
+int gemm_wide(cudaStream_t st, const bf16* A, int lda, const bf16* B, const bf16* B3, int M, int N, int K, const EpiParams& ep, float* part,
+              size_t part_bytes, int* tickets, int n_tickets);
 // 3x3 / pad 1 / stride 1 convolution: src NHWC frame [nimg][fh][fw][cin] (fh >= max(H, 8), fw >= max(W, 16), zero outside the
 // H x W map; cin a positive multiple of WG_CBLK), B [N][9 cin] in (ky, kx, c) order -> out fp32 NHWC [nimg][H][W][N] = conv + bias
 // (+ resid, same shape).  nimg, H, W > 0, N > 0 and N % 8 == 0; src and B 16-byte aligned, out and resid 8-byte aligned.  Checked

@@ -20,6 +20,7 @@
 // layout 1 (128-byte swizzle) << 62; the k16 step inside a 128-byte swizzle atom advances the start address by 32 bytes.
 #pragma once
 #include "gemm.h"
+#include "gemm_skinny.cuh"
 #include <cuda.h>
 
 constexpr int WG_BM = 128, WG_BN = 128, WG_BK = WG_CBLK, WG_STAGES = 6, WG_THREADS = 384, WG_CONSUMERS = 2;
@@ -225,4 +226,177 @@ __global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_kernel(const __grid_
 __global__ void __launch_bounds__(WG_THREADS, 1) gemm_wgmma_f32_kernel(const __grid_constant__ CUtensorMap mapA,
                                                                        const __grid_constant__ CUtensorMap mapB, const WgP p) {
     gemm_wgmma_body<true>(mapA, mapB, p);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Wide decode GEMM (gemm_wide, gemm.h): one decode step's M <= 64 rows times the borrowed [N][K] weights, every weight read once
+// per step.  A is one m64 tile (rows M..63 zero-filled by TMA); CTA c = tile · splits + split owns 64 output columns and the
+// k-blocks [split · kper, +kper).  The fp32 partials of a column tile go to a workspace; the CTA that takes the last ticket of the
+// tile sums them in split order (the same order whichever CTA finishes last, so two runs give identical bits and every row is
+// reduced the same way), then runs the decode epilogue of gemm_skinny.cuh (run_epilogue<bf16>) on 16-row slabs.  One split: the
+// accumulators go to the epilogue directly.  DUAL (SwiGLU): a second weight map (w3) over the same columns, a second accumulator.
+// Roles: warps 0-3 (one warpgroup) issue wgmma.m64n64k16, warp 4 lane 0 is the TMA producer, all 8 warps reduce and store.
+// ---------------------------------------------------------------------------------------------------------
+constexpr int WD_BN = 64, WD_STAGES = 4, WD_THREADS = 256;
+constexpr int WD_A_BYTES = 64 * WG_BK * 2, WD_B_BYTES = WD_BN * WG_BK * 2;
+__host__ __device__ constexpr int wd_stage_bytes(bool dual) { return WD_A_BYTES + (dual ? 2 : 1) * WD_B_BYTES; }
+__host__ __device__ constexpr int wd_smem(bool dual) { return WD_STAGES * wd_stage_bytes(dual) + 1024; }
+static_assert(64 * 2 * WD_BN * 4 <= WD_STAGES * WD_A_BYTES, "the reduced [64][2 x 64] fp32 tile fits in the drained ring");
+
+struct WdP {
+    int M, N, K;
+    int splits, kper;     // K splits per column tile, k-blocks per split
+    float* part;          // [tiles · splits][M][(DUAL ? 2 : 1) · 64] fp32 partials (splits > 1)
+    int* tickets;         // [tiles], zero between launches: the last CTA of a tile resets its ticket
+    EpiParams ep;
+};
+
+// d[64 rows x 64 cols] (+)= A[64 x 16] · B[64 x 16]^T, both operands K-major in shared memory; scale_d = 0 overwrites d
+__device__ __forceinline__ void wg_mma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "
+        "%26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
+          "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]),
+          "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d)
+        : "memory");
+}
+
+// column c of the tile (w3 columns at 64 + c when DUAL) -> its place in the epilogue tile: run_epilogue's SwiGLU reads 8 w1
+// columns then the same 8 w3 columns (the packed interleave of the skinny kernel)
+template <bool DUAL>
+__device__ __forceinline__ int wd_tile_col(int c) {
+    if (!DUAL) return c;
+    const int u = c >> 6, cc = c & 63;
+    return (cc >> 3) * 16 + u * 8 + (cc & 7);
+}
+
+template <bool DUAL>
+__global__ void __launch_bounds__(WD_THREADS) gemm_wide_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                                                               const __grid_constant__ CUtensorMap mapB3, const WdP p) {
+    constexpr int STAGE = wd_stage_bytes(DUAL), W = (DUAL ? 2 : 1) * WD_BN;     // W: fp32 columns per row of a partial
+    extern __shared__ unsigned char wg_raw[];
+    __shared__ __align__(8) uint64_t bar_full[WD_STAGES], bar_empty[WD_STAGES];
+    __shared__ int s_last;
+    const uint32_t smem0 = (wg_smem(wg_raw) + 1023u) & ~1023u;
+    float* tileS = reinterpret_cast<float*>(wg_raw + (smem0 - wg_smem(wg_raw)));      // [64][W], over the drained ring
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tile = blockIdx.x / p.splits, split = blockIdx.x - tile * p.splits;
+    const int n0 = tile * WD_BN, kb0 = split * p.kper;
+    const int nk = min(p.kper, (p.K + WG_BK - 1) / WG_BK - kb0);
+
+    if (tid == 0) {
+        for (int s = 0; s < WD_STAGES; ++s) { wg_mbar_init(wg_smem(&bar_full[s]), 1); wg_mbar_init(wg_smem(&bar_empty[s]), 4); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
+        if (DUAL) asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB3) : "memory");
+    }
+    __syncthreads();
+    pdl_launch_dependents();
+
+    float acc[32], acc3[DUAL ? 32 : 1];
+    if (warp == 4) {
+        if (lane == 0) {
+            // ===== TMA producer: the first stages' weights are immutable and go in flight before the previous kernel has finished
+            const int pre = min(nk, WD_STAGES);
+            for (int i = 0; i < pre; ++i) {
+                const uint32_t sA = smem0 + i * STAGE, fb = wg_smem(&bar_full[i]);
+                wg_mbar_expect(fb, STAGE);
+                wg_tma_2d(sA + WD_A_BYTES, &mapB, (kb0 + i) * WG_BK, n0, fb);
+                if (DUAL) wg_tma_2d(sA + WD_A_BYTES + WD_B_BYTES, &mapB3, (kb0 + i) * WG_BK, n0, fb);
+            }
+            pdl_wait();
+            for (int i = 0; i < pre; ++i) wg_tma_2d(smem0 + i * STAGE, &mapA, (kb0 + i) * WG_BK, 0, wg_smem(&bar_full[i]));
+            for (int i = pre; i < nk; ++i) {
+                const uint32_t s = i % WD_STAGES, use = i / WD_STAGES;
+                wg_mbar_wait(wg_smem(&bar_empty[s]), (use - 1) & 1);
+                const uint32_t sA = smem0 + s * STAGE, fb = wg_smem(&bar_full[s]);
+                wg_mbar_expect(fb, STAGE);
+                wg_tma_2d(sA, &mapA, (kb0 + i) * WG_BK, 0, fb);
+                wg_tma_2d(sA + WD_A_BYTES, &mapB, (kb0 + i) * WG_BK, n0, fb);
+                if (DUAL) wg_tma_2d(sA + WD_A_BYTES + WD_B_BYTES, &mapB3, (kb0 + i) * WG_BK, n0, fb);
+            }
+        }
+        __syncwarp();
+    }
+    pdl_wait();
+    if (warp < 4) {
+        // ===== consumers: the warpgroup owns all 64 rows
+        for (int i = 0; i < nk; ++i) {
+            const uint32_t s = i % WD_STAGES, use = i / WD_STAGES;
+            wg_mbar_wait(wg_smem(&bar_full[s]), use & 1);
+            const uint32_t sA = smem0 + s * STAGE, sB = sA + WD_A_BYTES;
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+            for (int kk = 0; kk < WG_BK / 16; ++kk) {
+                const uint32_t sc = (i > 0 || kk > 0) ? 1u : 0u;
+                wg_mma_m64n64k16(acc, wg_desc_sw128(sA + kk * 32), wg_desc_sw128(sB + kk * 32), sc);
+                if constexpr (DUAL) wg_mma_m64n64k16(acc3, wg_desc_sw128(sA + kk * 32), wg_desc_sw128(sB + WD_B_BYTES + kk * 32), sc);
+            }
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+            if (i > 0) {                                    // the previous k-block's group has retired: its stage is free
+                __syncwarp();
+                if (lane == 0) wg_mbar_arrive(wg_smem(&bar_empty[(i - 1) % WD_STAGES]));
+            }
+        }
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    }
+    // accumulator fragment of m64nNk16: acc[4 j + 2 h + c] is row 16 warp + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + c
+    auto for_each_pair = [&](auto&& f) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = warp * 16 + (lane >> 2) + 8 * h;
+#pragma unroll
+            for (int j = 0; j < WD_BN / 8; ++j) {
+                const int c = 8 * j + 2 * (lane & 3);
+                f(row, c, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                if constexpr (DUAL) f(row, WD_BN + c, acc3[4 * j + 2 * h], acc3[4 * j + 2 * h + 1]);
+            }
+        }
+    };
+    if (p.splits == 1) {
+        __syncthreads();                                    // every stage consumed: the ring becomes the epilogue tile
+        if (warp < 4)
+            for_each_pair([&](int row, int c, float a0, float a1) {
+                *reinterpret_cast<float2*>(tileS + row * W + wd_tile_col<DUAL>(c)) = make_float2(a0, a1);
+            });
+    } else {
+        float* part = p.part + (size_t)blockIdx.x * p.M * W;
+        if (warp < 4)
+            for_each_pair([&](int row, int c, float a0, float a1) {
+                if (row < p.M) __stcg(reinterpret_cast<float2*>(part + (size_t)row * W + c), make_float2(a0, a1));
+            });
+        __threadfence();
+        __syncthreads();
+        if (tid == 0) {
+            const int old = atomicAdd(p.tickets + tile, 1);
+            s_last = old == p.splits - 1;
+            if (s_last) p.tickets[tile] = 0;                // every split has arrived: ready for the next launch
+        }
+        __syncthreads();
+        if (!s_last) return;
+        __threadfence();
+        // the last CTA of the tile: sum the splits in index order, four columns per thread
+        const float* base = p.part + (size_t)tile * p.splits * p.M * W;
+        for (int idx = tid; idx < p.M * (W / 4); idx += WD_THREADS) {
+            const int row = idx / (W / 4), c = (idx - row * (W / 4)) * 4;
+            float4 s = __ldcg(reinterpret_cast<const float4*>(base + (size_t)row * W + c));
+#pragma unroll 4
+            for (int sp = 1; sp < p.splits; ++sp) {
+                const float4 v = __ldcg(reinterpret_cast<const float4*>(base + ((size_t)sp * p.M + row) * W + c));
+                s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+            }
+            *reinterpret_cast<float4*>(tileS + row * W + wd_tile_col<DUAL>(c)) = s;
+        }
+    }
+    __syncthreads();
+    const int ncols = min(WD_BN, p.N - n0) * (DUAL ? 2 : 1);
+    for (int m0 = 0; m0 < p.M; m0 += 16)
+        run_epilogue<bf16>(p.ep, tileS + m0 * W, W, m0, (DUAL ? 2 : 1) * (n0 >> 3), ncols, tid, WD_THREADS);
 }

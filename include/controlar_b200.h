@@ -133,7 +133,8 @@ int car_sample(const float* logits, int32_t b_eff, int32_t V, const CarSampling*
 /* ---- device-side generation loop: generate()'s prefill-sample + decode_n_tokens (generate.py:113-131,
  * 195-204).  Must follow car_prefill(...) on the same state.  Runs n_tokens sampling steps (the first one on
  * the prefill logits) with no host synchronisation — bf16, B_eff <= 16: ONE persistent cooperative kernel
- * (csrc/decode_persistent.cuh); otherwise a replayed CUDA graph of the per-kernel chain.  tokens_out int32 [B, n_tokens].
+ * (csrc/decode_persistent.cuh); otherwise a replayed CUDA graph of the per-kernel chain, whose GEMMs are one wgmma weight pass
+ * per step (gemm_wide) for bf16 at 32 < B_eff <= 64.  tokens_out int32 [B, n_tokens].
  * noise: optional fp32 [n_tokens, B, V]. ---- */
 int car_generate(CarState* s, const CarSampling* sp, int32_t n_tokens, const float* noise,
                  int32_t* tokens_out, void* stream);
@@ -147,7 +148,8 @@ int car_state_set_step_timer(CarState* s, int64_t* step_ns_dev);
  * Transformer.forward(idx=forced[:, i], input_pos=[T+i]) step by step, gpt_t2i.py:444-470 / generate.py:97-110).
  * forced_tokens int32 [B, n_tokens] (device): the token fed to step i+1 is forced[b][i]; the sampler still runs and
  * tokens_out[b][i] is its choice given the forced prefix.  logits_trace (optional, device) fp32 [n_tokens, b_eff, V]
- * receives the raw model logits of every step (row 0 = the prefill logits).  bf16 persistent kernel only. */
+ * receives the raw model logits of every step (row 0 = the prefill logits).  bf16 only: the persistent kernel where it
+ * runs (B_eff <= 16), else the per-kernel chain step by step (the wide decode route for 32 < B_eff <= 64). */
 int car_generate_forced(CarState* s, const CarSampling* sp, int32_t n_tokens, const float* noise,
                         const int32_t* forced_tokens, float* logits_trace, int32_t* tokens_out, void* stream);
 
