@@ -44,6 +44,11 @@ class CarSampling(C.Structure):
                 ("seed", C.c_uint64)]
 
 
+class CarRowSampling(C.Structure):
+    _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float), ("sample_logits", C.c_int32),
+                ("seed", C.c_uint64), ("noise_row", C.c_uint32), ("control_strength", C.c_float)]
+
+
 class CarDptDesc(C.Structure):
     _fields_ = [("hidden", C.c_int32), ("n_layers", C.c_int32), ("n_heads", C.c_int32), ("mlp", C.c_int32),
                 ("out_indices", C.c_int32 * 4), ("neck", C.c_int32 * 4), ("fusion", C.c_int32), ("pos_grid", C.c_int32),
@@ -102,12 +107,15 @@ PROTOTYPES = {
     "car_state_create": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p),
                                    C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_void_p)]),
     "car_state_set_emb_mask": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "car_state_set_row_sampling": (C.c_int, [C.c_void_p, C.POINTER(CarRowSampling), C.c_int32]),
     "car_state_destroy": (C.c_int, [C.c_void_p]),
     "car_state_set_step_timer": (C.c_int, [C.c_void_p, C.c_void_p]),
     "car_prefill": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int32, C.c_void_p]),
     "car_decode_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "car_sample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(CarSampling), C.c_int32, C.c_int32,
                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "car_sample_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(CarRowSampling), C.c_int32, C.c_float, C.c_int32,
+                                  C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "car_generate": (C.c_int, [C.c_void_p, C.POINTER(CarSampling), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "car_generate_forced": (C.c_int, [C.c_void_p, C.POINTER(CarSampling), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),

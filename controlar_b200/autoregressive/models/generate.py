@@ -9,6 +9,9 @@ Deviations, on purpose and documented in DESIGN.md:
     greedy runs are deterministic.  Pass ``noise=`` ([N, B, V] Exp(1) draws) to fix the draws explicitly.
   * the per-step probability rows the reference keeps in Python lists (generate.py:127-128, never returned)
     are not materialised.
+
+Extension: ``temperature``, ``top_k``, ``top_p``, ``sample_logits``, ``seed`` and ``control_strength`` also take one value per
+image (a length-B sequence or tensor), all in one launch; see ``row_sampling``.  Scalars take the reference's path unchanged.
 """
 from __future__ import annotations
 
@@ -45,6 +48,59 @@ def sample(logits, temperature: float = 1.0, top_k: int = 2000, top_p: float = 1
     return idx.to(torch.int64).unsqueeze(-1), probs
 
 
+def _per_image(name, v, B):
+    if torch.is_tensor(v):
+        v = v.tolist()
+    if isinstance(v, (list, tuple)):
+        if len(v) != B:
+            raise ValueError(f"generate(): {name} has {len(v)} values for {B} images")
+        return list(v)
+    return [v] * B
+
+
+def _is_seq(v) -> bool:
+    return isinstance(v, (list, tuple)) or (torch.is_tensor(v) and v.dim() > 0)
+
+
+def row_sampling(model, B: int, use_cfg: bool, control_strength=1, seed=None, **sampling_kwargs):
+    """One CarRowSampling per image when any of temperature, top_k, top_p, sample_logits, seed or control_strength is a
+    sequence; None when all are scalars (generate() then takes the reference's path).  Scalars apply to every image.
+
+    A sequence of seeds gives image b the Philox key seed[b] and counter word 0, so its draws depend on its own seed alone, not on
+    its row or its neighbours.  A scalar seed keeps the rule of one seed per launch: key = seed, counter word = b.  As in the
+    scalar path, strengths are 1 without CFG (the reference's generate() does not pass them then), and the legacy gpt.py class,
+    which has no control_strength, refuses any other value."""
+    vals = {"temperature": sampling_kwargs.get("temperature", 1.0), "top_k": sampling_kwargs.get("top_k", 2000),
+            "top_p": sampling_kwargs.get("top_p", 1.0), "sample_logits": sampling_kwargs.get("sample_logits", True),
+            "control_strength": control_strength}
+    if not any(_is_seq(v) for v in vals.values()) and not _is_seq(seed):
+        return None
+    col = {k: _per_image(k, v, B) for k, v in vals.items()}
+    temps = [float(t) for t in col["temperature"]]
+    top_k = [int(k or 0) for k in col["top_k"]]
+    top_p = [float(p) for p in col["top_p"]]
+    greedy = [not bool(x) for x in col["sample_logits"]]
+    cs = [float(c) for c in col["control_strength"]] if use_cfg else [1.0] * B
+    for b in range(B):
+        if not (0.0 < temps[b] < float("inf")):
+            raise ValueError(f"generate(): image {b}: temperature must be > 0, got {temps[b]}")
+        if top_k[b] < 0:
+            raise ValueError(f"generate(): image {b}: top_k must be >= 0, got {top_k[b]}")
+        if not (0.0 < top_p[b] <= 1.0):
+            raise ValueError(f"generate(): image {b}: top_p must be in (0, 1], got {top_p[b]}")
+        if not (abs(cs[b]) < float("inf")):
+            raise ValueError(f"generate(): image {b}: control_strength must be finite, got {cs[b]}")
+    if not getattr(model, "has_control_strength", True) and any(c != 1.0 for c in cs):
+        raise TypeError("the legacy c2i class has no control_strength (gpt.py:400-409)")
+    if _is_seq(seed):
+        seeds, rows = [int(x) for x in _per_image("seed", seed, B)], [0] * B
+    else:
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if not all(greedy) else 0
+        seeds, rows = [int(seed)] * B, list(range(B))
+    return [_engine.make_row_sampling(temps[b], top_k[b], top_p[b], not greedy[b], seeds[b], rows[b], cs[b]) for b in range(B)]
+
+
 def logits_to_probs(logits, temperature: float = 1.0, top_p: float = 1.0, top_k: int = None, **kwargs):
     sp = _engine.make_sampling(temperature, top_k or 0, top_p, False, cfg_scale=1.0)
     return _engine.sample(logits, sp, return_probs=True)[1]
@@ -54,7 +110,9 @@ def logits_to_probs(logits, temperature: float = 1.0, top_p: float = 1.0, top_k:
 def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_interval=-1, condition=None,
              condition_null=None, condition_token_nums=0, control_strength=1, noise=None, seed=None,
              **sampling_kwargs):
-    """Reference generate.py:134-204."""
+    """Reference generate.py:134-204; per-image sampling parameters and strengths: `row_sampling`."""
+    use_cfg = cfg_scale > 1.0
+    rows = row_sampling(model, cond.shape[0], use_cfg, control_strength, seed, **sampling_kwargs)
     if condition is not None:
         if getattr(model.adapter, "forward", None) is not None and type(model.adapter).__name__ in ("Dinov2_Adapter", "ViT_Adapter") \
                 and "forward" not in vars(model.adapter) and "forward" not in vars(model.adapter_mlp):
@@ -68,7 +126,6 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
         else:
             condition = model.adapter(condition)                # generate.py:137
             condition = model.adapter_mlp(condition)            # generate.py:138
-    use_cfg = cfg_scale > 1.0
     if model.model_type == "c2i":
         cond_combined = torch.cat([cond, torch.ones_like(cond) * model.num_classes]) if use_cfg else cond
         T = 1 + condition_token_nums
@@ -102,6 +159,14 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
         st.set_emb_mask(None)
     model._mask_synced = True
 
+    if rows is not None:
+        sp = _engine.make_sampling(cfg_scale=cfg_scale, cfg_interval=cfg_interval)      # per launch; the rest comes from `rows`
+        st.set_row_sampling(rows)
+        try:
+            st.prefill(cond_combined, condition_combined, 1.0, all_rows=False)
+            return st.generate(sp, max_new_tokens, noise, cond.device)
+        finally:
+            st.set_row_sampling(None)
     # generate.py:92 does not forward control_strength when cfg_scale <= 1; forward() then resets it to 1
     cs = float(control_strength) if use_cfg else 1.0
     st.prefill(cond_combined, condition_combined, cs, all_rows=False)

@@ -57,6 +57,7 @@ class Transformer(_t.Transformer):
     # (gpt.py:118-119) instead of the `uncond_embedding` buffer — pinned against the reference's gpt.py in train mode by
     # tests/test_train_oracle_golden.py::test_legacy_gptpy_train_branch_is_the_same_arithmetic; forward / backward are inherited.
     zero_uncond_on_drop = True
+    has_control_strength = False      # generate() refuses per-image strengths other than 1, as forward() does below
 
     def __init__(self, config: ModelArgs):
         if config.condition_token_num != 0:

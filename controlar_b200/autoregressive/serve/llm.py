@@ -10,6 +10,8 @@ What is different from a text LLM server, and why the design is simpler than vLL
     indirection to the decode kernel's K/V stream.
   * CFG pairs (conditional row b, unconditional row b + B) live in the same launch and are combined inside the sampler
     (`csrc/sampler.cuh`), like the reference's `Sampler.forward` does on the split logits.
+  * with `mixed_sampling=True` the images of one launch each keep their own sampling parameters, seed and control strength, as
+    the reference's vLLM sampler lets every sequence group of a batch have its own; only cfg_scale is per engine.
 The scheduler below is plain host logic (CPU-tested); the GPU work is `generate()` + `decode_code()` of this package."""
 from __future__ import annotations
 
@@ -58,18 +60,43 @@ class Request:
     sampling: SamplingParams
     control_strength: float = 1.0
 
-    def group_key(self) -> Tuple:
+    def group_key(self, mixed: bool = False) -> Tuple:
+        """What the requests of one launch share: the grid (token count, control-map shape, whether there are caption masks) and,
+        unless the engine mixes sampling configurations, the sampling parameters and the control strength."""
         ctl = None if self.control is None else tuple(self.control.shape)
+        if mixed:
+            return (int(self.sampling.max_tokens), ctl, self.emb_mask is None)
         return (self.sampling.key(), ctl, float(self.control_strength), self.emb_mask is None)
 
 
-class Scheduler:
-    """FIFO admission with compatibility grouping: one launch of the decode kernel runs one sampling configuration and one grid
-    size, so a batch is the oldest waiting request plus the next waiting requests that share its group key, up to `max_images`."""
+def derived_seed(base_seed: int, request_id: int) -> int:
+    """The seed of a request that set none, in mixed mode: a function of the engine seed and the request id only (splitmix64), so
+    a request's image does not depend on when it was launched, on its row or on its neighbours."""
+    z = (int(base_seed) * 0x9E3779B97F4A7C15 + (int(request_id) + 1) * 0xBF58476D1CE4E5B9) & 0xFFFFFFFFFFFFFFFF
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & 0xFFFFFFFFFFFFFFFF
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & 0xFFFFFFFFFFFFFFFF
+    return (z ^ (z >> 31)) & 0x3FFFFFFFFFFFFFFF
 
-    def __init__(self, max_images: int = 8):
+
+def _check_mixed(sp: SamplingParams, control_strength) -> None:
+    """The per-image values generate() would refuse (models/generate.py:row_sampling), raised when the request is queued."""
+    t, p, c = float(sp.temperature), float(sp.top_p), float(control_strength)
+    if not (0.0 <= t < float("inf")):
+        raise ValueError(f"temperature must be >= 0 (0 = greedy), got {sp.temperature}")
+    if not (0.0 < p <= 1.0):
+        raise ValueError(f"top_p must be in (0, 1], got {sp.top_p}")
+    if not (abs(c) < float("inf")):
+        raise ValueError(f"control_strength must be finite, got {control_strength}")
+
+
+class Scheduler:
+    """FIFO admission with compatibility grouping: a batch is the oldest waiting request plus the next waiting requests that share
+    its group key, up to `max_images`.  One launch runs one grid size; it runs one sampling configuration unless `mixed`."""
+
+    def __init__(self, max_images: int = 8, mixed: bool = False):
         assert max_images >= 1
         self.max_images = max_images
+        self.mixed = mixed
         self.waiting: Deque[Request] = collections.deque()
 
     def add(self, req: Request) -> None:
@@ -81,11 +108,11 @@ class Scheduler:
     def next_batch(self) -> List[Request]:
         if not self.waiting:
             return []
-        key = self.waiting[0].group_key()
+        key = self.waiting[0].group_key(self.mixed)
         batch, rest = [], collections.deque()
         while self.waiting:
             r = self.waiting.popleft()
-            if len(batch) < self.max_images and r.group_key() == key:
+            if len(batch) < self.max_images and r.group_key(self.mixed) == key:
                 batch.append(r)
             else:
                 rest.append(r)
@@ -99,16 +126,28 @@ class LLM:
 
     `max_images_per_batch` (default 8) caps the images of one launch.  With CFG, up to 8 images (16 sequences) run on the
     persistent decode kernel; 17 to 32 images (34 to 64 sequences) of a bf16 model run on the wide decode route, one tensor-core
-    pass over the weights per step (DESIGN.md §4.2); other sizes and fp32 models run on the per-kernel chain."""
+    pass over the weights per step (DESIGN.md §4.2); other sizes and fp32 models run on the per-kernel chain.
+
+    `mixed_sampling` (default False) chooses how requests share a launch:
+      * False: a launch holds only requests with the same SamplingParams.key() (temperature, top-p, top-k, max_tokens) and control
+        strength, so a queue of 8 different configurations runs as 8 launches of one image.  The launch is seeded with the first
+        request's `seed`, or, when it has none, with `seed + <number of launches so far>`; the other requests' seeds are not used,
+        and an image depends on its row in the launch.  This stays the default because existing callers rely on exactly these
+        groups and seeds (tests/test_serve_cpu.py pins them).
+      * True: requests that differ only in sampling parameters or control strength share a launch (FIFO, up to
+        `max_images_per_batch`); each image is sampled with its own parameters and strength, and its noise is keyed by its own seed:
+        `SamplingParams.seed`, or `derived_seed(seed, request_id)` when unset, never the launch count or the row.  The runner then
+        receives the list of per-request seeds in place of one seed."""
 
     def __init__(self, args=None, model=None, vq=None, cfg_scale: Optional[float] = None, max_images_per_batch: int = 8, seed: int = 0,
-                 runner: Optional[Callable[[List[Request], int], torch.Tensor]] = None, **unused):
+                 runner: Optional[Callable[[List[Request], Any], torch.Tensor]] = None, mixed_sampling: bool = False, **unused):
         if model is None and runner is None:
             raise ValueError("LLM needs the GPT module (model=...): there are no checkpoints to locate by name without a network")
         self.model, self.vq = model, vq
         self.cfg_scale = float(cfg_scale if cfg_scale is not None else getattr(args, "cfg_scale", 1.0))
         self.num_classes = getattr(model, "num_classes", getattr(args, "num_classes", 1000))
-        self.scheduler = Scheduler(max_images_per_batch)
+        self.mixed_sampling = bool(mixed_sampling)
+        self.scheduler = Scheduler(max_images_per_batch, self.mixed_sampling)
         self.base_seed = int(seed)
         self._next_id = 0
         self._launches = 0
@@ -116,6 +155,8 @@ class LLM:
 
     # ---- queue interface
     def add_request(self, cond, sampling_params: SamplingParams, emb_mask=None, control=None, control_strength: float = 1.0) -> int:
+        if self.mixed_sampling:       # checked here: a bad request raised at launch time would take its batch-mates with it
+            _check_mixed(sampling_params, control_strength)
         rid = self._next_id
         self._next_id += 1
         self.scheduler.add(Request(rid, cond, emb_mask, control, sampling_params, control_strength))
@@ -129,7 +170,10 @@ class LLM:
         batch = self.scheduler.next_batch()
         if not batch:
             return []
-        seed = batch[0].sampling.seed if batch[0].sampling.seed is not None else self.base_seed + self._launches
+        if self.mixed_sampling:
+            seed = [r.sampling.seed if r.sampling.seed is not None else derived_seed(self.base_seed, r.request_id) for r in batch]
+        else:
+            seed = batch[0].sampling.seed if batch[0].sampling.seed is not None else self.base_seed + self._launches
         self._launches += 1
         tokens = self._runner(batch, seed)                   # int32 [len(batch), max_tokens]
         images = None
@@ -170,7 +214,8 @@ class LLM:
         return outs
 
     # ---- one batch on the GPU: generate() of this package (prefill + persistent decode kernel, CFG pairs inside)
-    def _run_batch(self, batch: List[Request], seed: int) -> torch.Tensor:
+    def _run_batch(self, batch: List[Request], seed) -> torch.Tensor:
+        """seed: one int for the launch, or (mixed sampling) one per request."""
         from ..models.generate import generate
         m = self.model
         dev = m.tok_embeddings.weight.device
@@ -182,6 +227,12 @@ class LLM:
             cond = torch.stack([r.cond for r in batch]).to(device=dev, dtype=m.tok_embeddings.weight.dtype)
             masks = None if batch[0].emb_mask is None else torch.stack([r.emb_mask for r in batch]).to(dev)
         control = None if batch[0].control is None else torch.stack([r.control for r in batch]).to(device=dev, dtype=m.tok_embeddings.weight.dtype)
+        if self.mixed_sampling:
+            sps = [r.sampling for r in batch]
+            return generate(m, cond, sp.max_tokens, emb_masks=masks, cfg_scale=self.cfg_scale, condition=control,
+                            control_strength=[r.control_strength for r in batch],
+                            temperature=[1.0 if p.temperature == 0 else p.temperature for p in sps], top_k=[max(int(p.top_k), 0) for p in sps],
+                            top_p=[p.top_p for p in sps], sample_logits=[p.temperature != 0 for p in sps], seed=list(seed))
         greedy = sp.temperature == 0
         return generate(m, cond, sp.max_tokens, emb_masks=masks, cfg_scale=self.cfg_scale, condition=control,
                         control_strength=batch[0].control_strength, temperature=1.0 if greedy else sp.temperature,

@@ -49,7 +49,12 @@ struct CarState : CarOwned {
     // control tokens [3][b_eff][N][d]
     void* ctrl[3];
     bool has_ctrl = false;
-    float cs = 1.f;
+    float cs = 1.f;                    // strength of every control add; 1 when car_prefill folded per-row strengths into ctrl
+    // per-image sampling (car_state_set_row_sampling); empty: the launch's CarSampling and car_prefill's control_strength
+    std::vector<CarRowSampling> row_sp;
+    std::vector<float> cs_rows;        // [b_eff] host staging of the per-row strengths
+    float* cs_dev = nullptr;           // [b_eff] the same on the device
+    SmpRow* smp_rows = nullptr;        // [b_eff] sampling parameters per image read by the sampler (the first B are used)
     // prefill scratch
     void *hP, *qP, *attnP, *actP, *t1, *t2;
     void *qkvP = nullptr, *gP = nullptr, *uP = nullptr;     // dense prefill path (bf16): qkv [rows][3d], w1 / w3 outputs [rows][F]
@@ -399,6 +404,8 @@ static int state_init(CarState* s, void* const* k_cache, void* const* v_cache) {
         CAR_TRY(s->alloc(&s->qkvP, MP * 3 * dd * es)); CAR_TRY(s->alloc(&s->gP, MP * F * es)); CAR_TRY(s->alloc(&s->uP, MP * F * es));
     }
     CAR_TRY(s->alloc(&s->emb_mask_store, MP * 4));
+    CAR_TRY(s->alloc(&s->cs_dev, (size_t)b_eff * 4)); CAR_TRY(s->alloc(&s->smp_rows, (size_t)b_eff * sizeof(SmpRow)));
+    s->cs_rows.assign(b_eff, 1.f);
     CAR_CUDA(cudaMemset(s->tickets, 0, (size_t)b_eff * d.n_head * 4));
     CAR_CUDA(cudaMemset(s->pos, 0, 16));
     s->done_ctr = s->pos + 1;
@@ -428,6 +435,27 @@ extern "C" int car_state_set_emb_mask(CarState* s, const int32_t* emb_mask_dev, 
     CAR_CUDA(cudaMemcpyAsync(s->emb_mask_store, emb_mask_dev, (size_t)s->b_eff * s->T * 4, cudaMemcpyDeviceToDevice,
                              (cudaStream_t)stream));
     s->emb_mask = s->emb_mask_store;
+    return CAR_OK;
+}
+
+// host checks of per-image parameters that arrive from outside the library
+static int check_rows(const CarRowSampling* rows, int B) {
+    for (int b = 0; b < B; ++b) {
+        const CarRowSampling& r = rows[b];
+        if (!(r.temperature > 0.f) || !std::isfinite(r.temperature)) CAR_FAIL(CAR_ERR_ARG, "row " + std::to_string(b) + ": need temperature > 0");
+        if (!(r.top_p > 0.f && r.top_p <= 1.f)) CAR_FAIL(CAR_ERR_ARG, "row " + std::to_string(b) + ": need 0 < top_p <= 1");
+        if (r.top_k < 0) CAR_FAIL(CAR_ERR_ARG, "row " + std::to_string(b) + ": need top_k >= 0");
+        if (!std::isfinite(r.control_strength)) CAR_FAIL(CAR_ERR_ARG, "row " + std::to_string(b) + ": control_strength must be finite");
+    }
+    return CAR_OK;
+}
+
+extern "C" int car_state_set_row_sampling(CarState* s, const CarRowSampling* rows, int32_t B) {
+    if (!s) CAR_FAIL(CAR_ERR_ARG, "null state");
+    if (!rows) { s->row_sp.clear(); return CAR_OK; }
+    if (B <= 0 || (B != s->b_eff && 2 * B != s->b_eff)) CAR_FAIL(CAR_ERR_ARG, "B must be the state's b_eff, or b_eff / 2 with CFG");
+    CAR_TRY(check_rows(rows, B));
+    s->row_sp.assign(rows, rows + B);
     return CAR_OK;
 }
 
@@ -620,7 +648,7 @@ extern "C" int car_prefill(CarState* s, const void* cond, const void* condition,
     CarModel* m = s->m;
     const CarModelDesc& d = m->d;
     const int rows = s->b_eff * s->T;
-    s->cs = control_strength;
+    s->cs = s->row_sp.empty() ? control_strength : 1.f;
     s->has_ctrl = condition != nullptr;
     s->graph_ok = false;
     // 1. prefix embeddings: CaptionEmbedder MLP (gpt_t2i.py:156-162) or LabelEmbedder gather (:89-97)
@@ -635,6 +663,17 @@ extern "C" int car_prefill(CarState* s, const void* cond, const void* condition,
         CAR_TRY(enqueue_mlp(s, condition, crow, d.dim, m->g_cond_fc1, m->g_cond_fc2, m->cond_fc1, m->cond_fc2, s->t1, s->t2, st));
         for (int j = 0; j < 3; ++j)
             CAR_TRY(enqueue_mlp(s, s->t2, crow, d.dim, m->g_ctl_fc1[j], m->g_ctl_fc2[j], m->ctl_fc1[j], m->ctl_fc2[j], s->t1, s->ctrl[j], st));
+        if (!s->row_sp.empty()) {
+            // per-row strengths (row r belongs to image r mod B: an unconditional row takes its partner's) folded into the tokens
+            const size_t nrs = s->row_sp.size();
+            for (int r = 0; r < s->b_eff; ++r) s->cs_rows[r] = s->row_sp[r % nrs].control_strength;
+            CAR_CUDA(cudaMemcpyAsync(s->cs_dev, s->cs_rows.data(), (size_t)s->b_eff * 4, cudaMemcpyHostToDevice, st));
+            const long long row_elems = (long long)s->N * d.dim, n = (long long)s->b_eff * row_elems;
+            for (int j = 0; j < 3; ++j) {
+                if (d.dtype == CAR_BF16) CAR_LAUNCH((scale_ctrl_rows_kernel<bf16>), gsz(n), 256, 0, st, (bf16*)s->ctrl[j], s->cs_dev, row_elems, n);
+                else CAR_LAUNCH((scale_ctrl_rows_kernel<float>), gsz(n), 256, 0, st, (float*)s->ctrl[j], s->cs_dev, row_elems, n);
+            }
+        }
     }
     // 3. blocks
     for (int l = 0; l < d.n_layer; ++l) {
@@ -681,10 +720,24 @@ static int fill_sample_args(SampleArgs& a, const CarSampling* sp, int b_eff, int
     if (a.use_cfg && (b_eff % 2)) CAR_FAIL(CAR_ERR_ARG, "cfg_scale > 1 needs an even number of rows");
     a.B = a.use_cfg ? b_eff / 2 : b_eff;
     a.cfg_on = 1; a.cfg_scale = sp->cfg_scale; a.cfg_interval = sp->cfg_interval;
-    a.inv_temp = 1.0f / fmaxf(sp->temperature, 1e-5f);
-    a.top_k = sp->top_k; a.top_p = sp->top_p; a.sample_logits = sp->sample_logits;
-    a.seed_lo = (uint32_t)(sp->seed & 0xffffffffu); a.seed_hi = (uint32_t)(sp->seed >> 32);
     return CAR_OK;
+}
+
+static SmpRow smp_row(float temperature, int top_k, float top_p, int sample_logits, uint64_t seed, uint32_t noise_row) {
+    SmpRow r;
+    r.inv_temp = 1.0f / fmaxf(temperature, 1e-5f);
+    r.top_k = top_k; r.top_p = top_p; r.sample_logits = sample_logits;
+    r.seed_lo = (uint32_t)(seed & 0xffffffffu); r.seed_hi = (uint32_t)(seed >> 32); r.noise_row = noise_row; r.pad = 0u;
+    return r;
+}
+
+// the sampler's parameters of B images: rows[b] when given, else every image from sp, its Philox counter word the image index
+static std::vector<SmpRow> smp_rows(const CarSampling* sp, const CarRowSampling* rows, int B) {
+    std::vector<SmpRow> out(B);
+    for (int b = 0; b < B; ++b)
+        out[b] = rows ? smp_row(rows[b].temperature, rows[b].top_k, rows[b].top_p, rows[b].sample_logits, rows[b].seed, rows[b].noise_row)
+                      : smp_row(sp->temperature, sp->top_k, sp->top_p, sp->sample_logits, sp->seed, (uint32_t)b);
+    return out;
 }
 
 static int launch_sampler(const SampleArgs& a, cudaStream_t st) {
@@ -693,14 +746,44 @@ static int launch_sampler(const SampleArgs& a, cudaStream_t st) {
     return CAR_OK;
 }
 
+// the standalone sampler: the per-image parameters go to a stream-ordered temporary
+static int launch_sampler_host_rows(SampleArgs& a, const std::vector<SmpRow>& rows, cudaStream_t st) {
+    void* d = nullptr;
+    CAR_CUDA(cudaMallocAsync(&d, rows.size() * sizeof(SmpRow), st));
+    const cudaError_t e = cudaMemcpyAsync(d, rows.data(), rows.size() * sizeof(SmpRow), cudaMemcpyHostToDevice, st);
+    int r = CAR_OK;
+    if (e != cudaSuccess) { g_car_err = std::string(__func__) + ": " + cudaGetErrorString(e); r = CAR_ERR_CUDA; }
+    else { a.rows = (const SmpRow*)d; r = launch_sampler(a, st); }
+    cudaFreeAsync(d, st);
+    return r;
+}
+
+static int standalone_sample_args(SampleArgs& a, const CarSampling* sp, const float* logits, int b_eff, int V, int cfg_on, int step,
+                                  const float* noise, int32_t* idx_out, float* probs_out, uint8_t* kept_out) {
+    CAR_TRY(fill_sample_args(a, sp, b_eff, V));
+    a.logits = logits; a.cfg_on = cfg_on; a.cfg_interval = -1; a.step = step; a.noise = noise;
+    a.idx_out = idx_out; a.tokens_ld = 0; a.probs_out = probs_out; a.kept_out = kept_out;
+    return CAR_OK;
+}
+
 extern "C" int car_sample(const float* logits, int32_t b_eff, int32_t V, const CarSampling* sp, int32_t cfg_on, int32_t step,
                           const float* noise, int32_t* idx_out, float* probs_out, uint8_t* kept_out, void* stream) {
     if (!logits || !sp || !idx_out) CAR_FAIL(CAR_ERR_ARG, "null argument");
     SampleArgs a;
-    CAR_TRY(fill_sample_args(a, sp, b_eff, V));
-    a.logits = logits; a.cfg_on = cfg_on; a.cfg_interval = -1; a.step = step; a.noise = noise;
-    a.idx_out = idx_out; a.tokens_ld = 0; a.probs_out = probs_out; a.kept_out = kept_out;
-    return launch_sampler(a, (cudaStream_t)stream);
+    CAR_TRY(standalone_sample_args(a, sp, logits, b_eff, V, cfg_on, step, noise, idx_out, probs_out, kept_out));
+    return launch_sampler_host_rows(a, smp_rows(sp, nullptr, a.B), (cudaStream_t)stream);
+}
+
+extern "C" int car_sample_rows(const float* logits, int32_t b_eff, int32_t V, const CarRowSampling* rows, int32_t B, float cfg_scale,
+                               int32_t cfg_on, int32_t step, const float* noise, int32_t* idx_out, float* probs_out, uint8_t* kept_out,
+                               void* stream) {
+    if (!logits || !rows || !idx_out) CAR_FAIL(CAR_ERR_ARG, "null argument");
+    if (b_eff <= 0 || B != (cfg_scale > 1.0f ? b_eff / 2 : b_eff)) CAR_FAIL(CAR_ERR_ARG, "B must be b_eff, or b_eff / 2 when cfg_scale > 1");
+    CAR_TRY(check_rows(rows, B));
+    CarSampling sp{1.0f, 0, 1.0f, 1, cfg_scale, -1, 0ull};
+    SampleArgs a;
+    CAR_TRY(standalone_sample_args(a, &sp, logits, b_eff, V, cfg_on, step, noise, idx_out, probs_out, kept_out));
+    return launch_sampler_host_rows(a, smp_rows(&sp, rows, B), (cudaStream_t)stream);
 }
 
 static bool same_sampling(const CarSampling& x, const CarSampling& y) {
@@ -708,9 +791,16 @@ static bool same_sampling(const CarSampling& x, const CarSampling& y) {
            x.cfg_scale == y.cfg_scale && x.cfg_interval == y.cfg_interval && x.seed == y.seed;
 }
 
-static int loop_sample_args(CarState* s, const CarSampling* sp, const float* noise, SampleArgs& a) {
+// the decode loop's sampler arguments; uploads the per-image parameters of this launch (car_state_set_row_sampling or sp)
+static int loop_sample_args(CarState* s, const CarSampling* sp, const float* noise, cudaStream_t st, SampleArgs& a) {
     const CarModelDesc& d = s->m->d;
     CAR_TRY(fill_sample_args(a, sp, s->b_eff, d.vocab_size));
+    if (!s->row_sp.empty() && (int)s->row_sp.size() != a.B)
+        CAR_FAIL(CAR_ERR_ARG, "the row sampling set on the state has " + std::to_string(s->row_sp.size()) + " images, the launch " +
+                              std::to_string(a.B) + " (cfg_scale decides whether b_eff counts the unconditional rows)");
+    const std::vector<SmpRow> rows = smp_rows(sp, s->row_sp.empty() ? nullptr : s->row_sp.data(), a.B);
+    CAR_CUDA(cudaMemcpyAsync(s->smp_rows, rows.data(), rows.size() * sizeof(SmpRow), cudaMemcpyHostToDevice, st));
+    a.rows = s->smp_rows;
     a.logits = s->logits; a.noise = noise; a.noise_per_step = noise ? 1 : 0;
     a.idx_out = s->tokens; a.tokens_ld = s->N; a.probs_out = nullptr;
     a.h_out = s->h; a.tok_emb = s->m->tok_emb; a.ctrl0 = s->has_ctrl ? s->ctrl[0] : nullptr; a.d = d.dim; a.n_img = s->N;
@@ -841,7 +931,7 @@ extern "C" int car_generate(CarState* s, const CarSampling* sp, int32_t n_tokens
     if (n_tokens < 1 || n_tokens > s->N) CAR_FAIL(CAR_ERR_ARG, "n_tokens must be in [1, N]");
     cudaStream_t st = (cudaStream_t)stream;
     SampleArgs a;
-    CAR_TRY(loop_sample_args(s, sp, noise, a));
+    CAR_TRY(loop_sample_args(s, sp, noise, st, a));
     if (s->m->d.dtype == CAR_BF16 && s->pk_ok) {
         CAR_TRY(launch_pk(s, a, n_tokens, st));
         CAR_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)n_tokens * 4, s->tokens, (size_t)s->N * 4, (size_t)n_tokens * 4, a.B,
@@ -914,7 +1004,7 @@ extern "C" int car_generate_forced(CarState* s, const CarSampling* sp, int32_t n
     if (s->m->d.dtype != CAR_BF16) CAR_FAIL(CAR_ERR_UNSUPPORTED, "teacher forcing through the device-side loop is bf16 only; use car_decode_step");
     cudaStream_t st = (cudaStream_t)stream;
     SampleArgs a;
-    CAR_TRY(loop_sample_args(s, sp, noise, a));
+    CAR_TRY(loop_sample_args(s, sp, noise, st, a));
     if (s->pk_ok) CAR_TRY(launch_pk(s, a, n_tokens, st, forced_tokens, logits_trace));
     else CAR_TRY(chain_forced_loop(s, a, n_tokens, forced_tokens, logits_trace, st));
     CAR_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)n_tokens * 4, s->tokens, (size_t)s->N * 4, (size_t)n_tokens * 4, a.B,

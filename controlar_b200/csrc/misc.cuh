@@ -51,6 +51,15 @@ __global__ void gather_rows_kernel(const T* __restrict__ table, const int* __res
     }
 }
 
+// per-row control strength folded into the control tokens of one layer group: ctrl[r] = rnd(cs[r] * ctrl[r]), r = row of
+// [rows][row_elems].  Every later add of these tokens then runs at strength 1 and gives rnd(h + rnd(1 * rnd(cs[r] * c))) =
+// rnd(h + rnd(cs[r] * c)) for bf16 (1 * x is exact): the bits of an add at strength cs[r], with the adds' code unchanged.
+template <typename T>
+__global__ void scale_ctrl_rows_kernel(T* __restrict__ ctrl, const float* __restrict__ cs, long long row_elems, long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        ctrl[i] = fromf<T>(cs[i / row_elems] * tof(ctrl[i]));
+}
+
 // prefill control add: h[b][T-1][:] += cs * ctrl[b][0][:]     gpt_t2i.py:463
 template <typename T>
 __global__ void prefill_ctrl_add_kernel(T* __restrict__ h, const T* __restrict__ ctrl, int Tq, int n_img, int d, float cs) {

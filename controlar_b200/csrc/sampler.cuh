@@ -7,7 +7,9 @@
 //   tok_embeddings(idx)         gpt_t2i.py:445     } fused tail: h for the next position
 //   h += cs*ctrl[0][:, p+1]     gpt_t2i.py:466     }
 // torch.multinomial(p, 1) == argmax(p / q), q ~ Exp(1) (SURVEY.md §7 hard-part 4).  q comes either from a
-// caller-provided buffer (parity tests) or from Philox4x32-10 keyed by (seed; step, row, index).
+// caller-provided buffer (parity tests) or from Philox4x32-10 keyed by (seed; step, noise_row, index).
+// Every image of a launch has its own temperature, top-k, top-p, greedy flag, Philox key and counter word (SmpRow); the scalar
+// entry points fill all rows alike.  The CFG combine pairs row b with row b + B and is the only cross-row arithmetic.
 #pragma once
 #include "common.cuh"
 
@@ -33,10 +35,10 @@ __device__ __forceinline__ void philox4x32_10(uint32_t k0, uint32_t k1, uint32_t
 }
 
 __device__ __forceinline__ float exp1_from_bits(uint32_t x);
-// Exp(1) draw of element i of row b at token `step` (kept out of line: it sits in a fully unrolled loop)
-__device__ __noinline__ float exp1_noise(uint32_t seed_lo, uint32_t seed_hi, int i, int b, int step) {
+// Exp(1) draw of element i at token `step` of the stream with counter word `row` (kept out of line: it sits in a fully unrolled loop)
+__device__ __noinline__ float exp1_noise(uint32_t seed_lo, uint32_t seed_hi, int i, uint32_t row, int step) {
     uint32_t r[4];
-    philox4x32_10(seed_lo, seed_hi, (uint32_t)(i >> 2), (uint32_t)b, (uint32_t)step, 0x43415231u, r);
+    philox4x32_10(seed_lo, seed_hi, (uint32_t)(i >> 2), row, (uint32_t)step, 0x43415231u, r);
     return exp1_from_bits(r[i & 3]);
 }
 __device__ __forceinline__ float exp1_from_bits(uint32_t x) {
@@ -45,14 +47,22 @@ __device__ __forceinline__ float exp1_from_bits(uint32_t x) {
     return -logf(u);
 }
 
+// sampling parameters of one image (32 bytes, read as two 16-byte loads)
+struct __align__(16) SmpRow {
+    float inv_temp; int top_k; float top_p; int sample_logits;
+    uint32_t seed_lo, seed_hi;  // Philox key
+    uint32_t noise_row;         // Philox counter word 1: the image's index under one seed per launch, 0 under a seed per image
+    uint32_t pad;
+};
+
 struct SampleArgs {
     const float* logits;    // [b_eff, V]
     int V; int B;           // B images; b_eff = 2B when cfg
     int use_cfg; int cfg_on; float cfg_scale;
-    float inv_temp; int top_k; float top_p; int sample_logits;
+    const SmpRow* rows;     // [B] (device)
     const float* noise;     // [B, V] (or [steps, B, V] when noise_per_step) or null
     int noise_per_step;
-    uint32_t seed_lo, seed_hi; int step;        // Philox sub-stream = index of the token being produced
+    int step;               // Philox sub-stream = index of the token being produced
     int cfg_interval;       // device-side cfg_flag: off when step-1 > cfg_interval >= 0  (generate.py:121-122)
     int* idx_out;           // [B] (or tokens_out + step when tokens_ld > 0)
     int tokens_ld;
@@ -139,14 +149,14 @@ constexpr float SMP_FIX = 1099511627776.0f;                              // 2^40
 
 // four consecutive elements of the CFG-combined, temperature-scaled row (generate.py:103-107, :60); separate sub / mul / add like
 // the eager reference (no FMA contraction), identical bits in every pass over the row
-__device__ __forceinline__ float4 smp_z4(const SampleArgs& a, const float* lc, const float* lu, int i4, bool cfg) {
+__device__ __forceinline__ float4 smp_z4(const SampleArgs& a, float inv_temp, const float* lc, const float* lu, int i4, bool cfg) {
     float4 v = __ldcg(reinterpret_cast<const float4*>(lc) + i4);
     if (cfg) {
         const float4 u = __ldcg(reinterpret_cast<const float4*>(lu) + i4);
         v.x = __fadd_rn(u.x, __fmul_rn(__fsub_rn(v.x, u.x), a.cfg_scale)); v.y = __fadd_rn(u.y, __fmul_rn(__fsub_rn(v.y, u.y), a.cfg_scale));
         v.z = __fadd_rn(u.z, __fmul_rn(__fsub_rn(v.z, u.z), a.cfg_scale)); v.w = __fadd_rn(u.w, __fmul_rn(__fsub_rn(v.w, u.w), a.cfg_scale));
     }
-    v.x = __fmul_rn(v.x, a.inv_temp); v.y = __fmul_rn(v.y, a.inv_temp); v.z = __fmul_rn(v.z, a.inv_temp); v.w = __fmul_rn(v.w, a.inv_temp);
+    v.x = __fmul_rn(v.x, inv_temp); v.y = __fmul_rn(v.y, inv_temp); v.z = __fmul_rn(v.z, inv_temp); v.w = __fmul_rn(v.w, inv_temp);
     return v;
 }
 
@@ -168,7 +178,7 @@ __device__ __forceinline__ float4 smp_z4(const SampleArgs& a, const float* lc, c
 
 // visit every kept element (index, value): the compacted list, or the whole row filtered by the threshold key
 template <int THREADS, typename F>
-__device__ __forceinline__ void smp_for_kept(const SampleArgs& a, const float* lc, const float* lu, bool cfg, bool use_list, const int* ki,
+__device__ __forceinline__ void smp_for_kept(const SampleArgs& a, float inv_temp, const float* lc, const float* lu, bool cfg, bool use_list, const int* ki,
                                              const float* kz, unsigned nk, bool has_thr, unsigned thr, F f) {
     if (use_list) {
         for (unsigned c = threadIdx.x; c < nk; c += THREADS) f(ki[c], kz[c]);
@@ -176,7 +186,7 @@ __device__ __forceinline__ void smp_for_kept(const SampleArgs& a, const float* l
         const int V4 = a.V >> 2;
 #pragma unroll 1
         for (int i4 = threadIdx.x; i4 < V4; i4 += THREADS) {   // (rare path: kept small, not fast)
-            const float4 z = smp_z4(a, lc, lu, i4, cfg);
+            const float4 z = smp_z4(a, inv_temp, lc, lu, i4, cfg);
             const float zz[4] = {z.x, z.y, z.z, z.w};
 #pragma unroll 1
             for (int q = 0; q < 4; ++q)
@@ -197,6 +207,12 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
     __shared__ unsigned s_cnt, s_nk, s_bin, s_krem, s_thr, s_over;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int V = a.V, V4 = V >> 2;                        // (host-checked: V % 4 == 0)
+    // the image's parameters in two 16-byte loads, issued together before the first pass over the row
+    const uint4 r0 = __ldg(reinterpret_cast<const uint4*>(a.rows + b)), r1 = __ldg(reinterpret_cast<const uint4*>(a.rows + b) + 1);
+    const float inv_temp = __uint_as_float(r0.x), top_p = __uint_as_float(r0.z);
+    const int top_k = (int)r0.y;
+    const bool sample_logits = r0.w != 0u;
+    const uint32_t seed_lo = r1.x, seed_hi = r1.y, noise_row = r1.z;
     const int pos = a.pos_ptr ? ld_cg(a.pos_ptr) : a.pos_val;
     const int step = a.pos_ptr ? (pos - a.T + 1) : a.step;   // index of the token being produced
     bool cfg_on = a.cfg_on != 0;
@@ -211,15 +227,15 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
     float* const s_kz = reinterpret_cast<float*>(scratch + SMP_NBIN * 4 + SMP_NCAND * 8 + SMP_CAP * 4);
 
     SMP_STAMP(0);
-    const bool has_thr = a.top_k > 0 && a.top_k < V;
-    bool use_list = has_thr && a.top_k + 64 <= SMP_CAP;   // room for ties at the threshold; else the stages run over the row
+    const bool has_thr = top_k > 0 && top_k < V;
+    bool use_list = has_thr && top_k + 64 <= SMP_CAP;   // room for ties at the threshold; else the stages run over the row
     unsigned thr = 0u, nk = 0u;
     if (has_thr) {
         // ---- level 1: value range, histogram, boundary bin
         float lo = INFINITY, hi = -INFINITY;
 #pragma unroll 2
         for (int i4 = tid; i4 < V4; i4 += THREADS) {
-            const float4 z = smp_z4(a, lc, lu, i4, cfg);
+            const float4 z = smp_z4(a, inv_temp, lc, lu, i4, cfg);
             lo = fminf(fminf(lo, z.x), fminf(z.y, fminf(z.z, z.w)));
             hi = fmaxf(fmaxf(hi, z.x), fmaxf(z.y, fmaxf(z.z, z.w)));
         }
@@ -227,12 +243,12 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
         lo = -smp_block_max<THREADS>(-lo, red_f);
         const float scale = (hi > lo && lo > -INFINITY) ? (float)(SMP_NBIN - 1) / (hi - lo) : 0.f;
         for (int i = tid; i < SMP_NBIN; i += THREADS) s_hist[i] = 0u;
-        if (tid == 0) { s_cnt = 0u; s_nk = 0u; s_thr = 0u; s_over = 0u; s_bin = 0u; s_krem = (unsigned)a.top_k; }
+        if (tid == 0) { s_cnt = 0u; s_nk = 0u; s_thr = 0u; s_over = 0u; s_bin = 0u; s_krem = (unsigned)top_k; }
         __syncthreads();
         SMP_STAMP(1);
 #pragma unroll 2
         for (int i4 = tid; i4 < V4; i4 += THREADS) {
-            const float4 z = smp_z4(a, lc, lu, i4, cfg);
+            const float4 z = smp_z4(a, inv_temp, lc, lu, i4, cfg);
             const float zz[4] = {z.x, z.y, z.z, z.w};
 #pragma unroll
             for (int q = 0; q < 4; ++q) atomicAdd(&s_hist[min(max((int)((zz[q] - lo) * scale), 0), SMP_NBIN - 1)], 1u);
@@ -251,7 +267,7 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
             __syncthreads();
             unsigned above = incl - mine;
             for (int w = warp + 1; w < NW; ++w) above += red_u[w];
-            const unsigned kk = (unsigned)a.top_k;
+            const unsigned kk = (unsigned)top_k;
 #pragma unroll
             for (int i = BPT - 1; i >= 0; --i) {
                 if (above < kk && kk <= above + loc[i]) { s_bin = (unsigned)(tid * BPT + i); s_krem = kk - above; }
@@ -267,7 +283,7 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
         for (int i0 = 0; i0 < V4; i0 += THREADS) {         // (warp-uniform trip count: the allocation below uses warp collectives)
             const int i4 = i0 + tid;
             const bool valid = i4 < V4;
-            const float4 z = smp_z4(a, lc, lu, valid ? i4 : 0, cfg);
+            const float4 z = smp_z4(a, inv_temp, lc, lu, valid ? i4 : 0, cfg);
             const float zz[4] = {z.x, z.y, z.z, z.w};
             int bin[4];
             unsigned mykeep = 0u;
@@ -325,13 +341,13 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
                 const unsigned t1 = thr | (1u << shift), t2 = thr | (2u << shift), t3 = thr | (3u << shift);
                 unsigned c1 = 0, c2 = 0, c3 = 0;
                 for (int i4 = tid; i4 < V4; i4 += THREADS) {
-                    const float4 z = smp_z4(a, lc, lu, i4, cfg);
+                    const float4 z = smp_z4(a, inv_temp, lc, lu, i4, cfg);
                     const float zz[4] = {z.x, z.y, z.z, z.w};
 #pragma unroll
                     for (int q = 0; q < 4; ++q) { const unsigned k = float_order_key(zz[q]); c1 += k >= t1 ? 1u : 0u; c2 += k >= t2 ? 1u : 0u; c3 += k >= t3 ? 1u : 0u; }
                 }
                 smp_block_count3<THREADS>(c1, c2, c3, red_c);
-                const unsigned kk = (unsigned)a.top_k;                 // counts are non-increasing in the threshold
+                const unsigned kk = (unsigned)top_k;                 // counts are non-increasing in the threshold
                 thr = c3 >= kk ? t3 : (c2 >= kk ? t2 : (c1 >= kk ? t1 : thr));
             }
             use_list = false;                              // (the list holds only the bins above; this rare path runs over the row)
@@ -340,7 +356,7 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
         if (nk > (unsigned)SMP_CAP) use_list = false;      // (CTA-uniform) more ties than the list holds
     }
     SMP_STAMP(2);
-    auto for_kept = [&](auto f) { smp_for_kept<THREADS>(a, lc, lu, cfg, use_list, s_ki, s_kz, nk, has_thr, thr, f); };
+    auto for_kept = [&](auto f) { smp_for_kept<THREADS>(a, inv_temp, lc, lu, cfg, use_list, s_ki, s_kz, nk, has_thr, thr, f); };
 
     // ---- soft-max over the kept elements
     float mx = -INFINITY;
@@ -358,8 +374,8 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
     // compared in 64-bit fixed point.  (torch.sort's order among exactly tied probabilities is unspecified; ties are kept together.)
     const float sum_pre = sum;                             // normaliser of the pre-nucleus probabilities
     unsigned p_key = 0u;                                   // elements whose pre-nucleus probability key is below p_key are dropped
-    if (a.top_p < 1.0f) {
-        const double budget = (double)a.top_p * (double)mass;
+    if (top_p < 1.0f) {
+        const double budget = (double)top_p * (double)mass;
         unsigned long long lo = 0ull, hi = 0xFFFFFFFFull;  // predicate(k): mass{key(p) > k} <= budget; true at hi, monotone in k
         while (lo < hi) {                                  // (CTA-uniform: every thread sees the same block sums)
             const unsigned mid = (unsigned)((lo + hi) >> 1);
@@ -395,7 +411,7 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, const int b, un
         const float e = expf(z - mx);
         if (float_order_key(e / sum_pre) >= p_key && e > 0.f) {
             float sv = e / sum;
-            if (a.sample_logits) sv = sv / (nz ? nz[i] : exp1_noise(a.seed_lo, a.seed_hi, i, b, step));
+            if (sample_logits) sv = sv / (nz ? nz[i] : exp1_noise(seed_lo, seed_hi, i, noise_row, step));
             if (sv > best || (sv == best && i < besti)) { best = sv; besti = i; }
         }
     });

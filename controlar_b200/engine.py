@@ -11,8 +11,8 @@ from typing import List, Optional
 import torch
 
 from . import _lib
-from ._lib import (CarGemmDesc, CarModelDesc, CarSampling, CarTrainWeights, CarWeights, check, cur_stream, dtype_code, on_own_device,
-                   param_signature, _ptr, _ptr_array)
+from ._lib import (CarGemmDesc, CarModelDesc, CarRowSampling, CarSampling, CarTrainWeights, CarWeights, check, cur_stream, dtype_code,
+                   on_own_device, param_signature, _ptr, _ptr_array)
 
 
 def _desc(m) -> CarModelDesc:
@@ -256,6 +256,16 @@ class ARStateHandle(_lib.NativeHandle):
         check(self.lib.car_state_set_emb_mask(self.handle, _ptr(em), cur_stream()), "car_state_set_emb_mask")
         self._mask_keep = em
 
+    def set_row_sampling(self, rows: Optional[List[CarRowSampling]]):
+        """Per-image sampling parameters and control strengths (car_state_set_row_sampling): one CarRowSampling per image (b_eff
+        or b_eff / 2 with CFG entries).  The next prefill takes the strengths, the next generate / generate_forced the sampling
+        parameters; their own scalar strength and CarSampling then only supply cfg_scale and cfg_interval.  None: scalar again."""
+        if rows is None:
+            check(self.lib.car_state_set_row_sampling(self.handle, None, 0), "car_state_set_row_sampling")
+            return
+        arr = (CarRowSampling * len(rows))(*rows)
+        check(self.lib.car_state_set_row_sampling(self.handle, arr, len(rows)), "car_state_set_row_sampling")
+
     @on_own_device
     def prefill(self, cond: torch.Tensor, condition: Optional[torch.Tensor], control_strength: float,
                 all_rows: bool) -> torch.Tensor:
@@ -335,6 +345,35 @@ def make_sampling(temperature=1.0, top_k=0, top_p=1.0, sample_logits=True, cfg_s
     return CarSampling(temperature=float(temperature), top_k=int(top_k or 0), top_p=float(top_p),
                        sample_logits=1 if sample_logits else 0, cfg_scale=float(cfg_scale),
                        cfg_interval=int(cfg_interval), seed=int(seed) & 0xFFFFFFFFFFFFFFFF)
+
+
+def make_row_sampling(temperature=1.0, top_k=0, top_p=1.0, sample_logits=True, seed=0, noise_row=0,
+                      control_strength=1.0) -> CarRowSampling:
+    """One image's CarRowSampling.  noise_row is the Philox counter word: 0 (the default) makes the image's draws depend on its
+    seed alone; the image index b reproduces what one CarSampling seed gives image b."""
+    return CarRowSampling(temperature=float(temperature), top_k=int(top_k or 0), top_p=float(top_p),
+                          sample_logits=1 if sample_logits else 0, seed=int(seed) & 0xFFFFFFFFFFFFFFFF,
+                          noise_row=int(noise_row) & 0xFFFFFFFF, control_strength=float(control_strength))
+
+
+def sample_rows(logits: torch.Tensor, rows: List[CarRowSampling], cfg_scale: float = 1.0, cfg_on: bool = True, step: int = 0,
+                noise: Optional[torch.Tensor] = None, return_probs: bool = False, return_kept: bool = False):
+    """`sample` with image b's parameters from rows[b] (car_sample_rows); B = len(rows) images, b_eff = 2B when cfg_scale > 1."""
+    lib = _lib.lib()
+    logits = logits.to(torch.float32).contiguous()
+    b_eff, V = logits.shape
+    B = len(rows)
+    idx = torch.empty((B,), dtype=torch.int32, device=logits.device)
+    probs = torch.empty((B, V), dtype=torch.float32, device=logits.device) if return_probs else None
+    kept = torch.empty((B, V), dtype=torch.uint8, device=logits.device) if return_kept else None
+    if noise is not None:
+        noise = noise.to(torch.float32).contiguous()
+    arr = (CarRowSampling * B)(*rows)
+    with torch.cuda.device(logits.device):
+        check(lib.car_sample_rows(_ptr(logits), b_eff, V, arr, B, float(cfg_scale), 1 if cfg_on else 0, int(step), _ptr(noise), _ptr(idx),
+                                  _ptr(probs), _ptr(kept), cur_stream()), "car_sample_rows")
+    out = (idx,) + ((probs,) if return_probs else ()) + ((kept.bool(),) if return_kept else ())
+    return out if len(out) > 1 else idx
 
 
 def sample(logits: torch.Tensor, sp: CarSampling, cfg_on: bool = True, step: int = 0,

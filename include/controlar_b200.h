@@ -92,6 +92,21 @@ typedef struct CarSampling {
     uint64_t seed;           /* Philox key for the in-kernel exponential noise */
 } CarSampling;
 
+/* Sampling parameters and control strength of ONE image of a launch (car_state_set_row_sampling, car_sample_rows).
+ * cfg_scale and cfg_interval stay per launch (CarSampling).  Checked on the host: temperature > 0, 0 < top_p <= 1, top_k >= 0. */
+typedef struct CarRowSampling {
+    float    temperature;
+    int32_t  top_k;            /* 0 = off */
+    float    top_p;            /* 1.0 = off */
+    int32_t  sample_logits;    /* 1 = multinomial (exponential race), 0 = arg-max */
+    uint64_t seed;             /* Philox key of this image's noise */
+    uint32_t noise_row;        /* Philox counter word of this image's noise: 0 makes the draws depend on `seed` alone; the image
+                                  index b reproduces the rule of CarSampling, whose one seed keys every image with counter b */
+    float    control_strength; /* strength of the control tokens on this image's rows (the unconditional partner's included);
+                                  car_prefill folds it into the image's control tokens, rnd(s * c), and every add then runs at
+                                  strength 1: for bf16 the bits of an add at strength s (fp32 checkpoints: DESIGN §4.1) */
+} CarRowSampling;
+
 const char* car_last_error(void);
 int car_version(void);
 
@@ -110,6 +125,11 @@ int car_model_destroy(CarModel* m);
 int car_state_create(CarModel* m, int32_t b_eff, int32_t max_seq /* S */, int32_t n_img_tokens /* N */,
                      void* const* k_cache, void* const* v_cache, const float* rope_table, CarState** out);
 int car_state_set_emb_mask(CarState* s, const int32_t* emb_mask_dev, void* stream);
+/* Per-image sampling: rows (host, B entries, copied) give image b its own CarRowSampling; B must be b_eff (no CFG) or b_eff / 2
+ * (CFG).  The following car_prefill takes each row's control strength (its control_strength argument is then unused) and the
+ * following car_generate / car_generate_forced take each row's sampling parameters, on every decode route; the CarSampling
+ * passed to them then only supplies cfg_scale and cfg_interval.  NULL returns to the scalar behaviour. */
+int car_state_set_row_sampling(CarState* s, const CarRowSampling* rows, int32_t B);
 int car_state_destroy(CarState* s);
 
 /* ---- prefill: Transformer.forward inference-prefill branch (gpt_t2i.py:433-442,455-470) ----
@@ -127,8 +147,14 @@ int car_decode_step(CarState* s, const int32_t* tok, int32_t pos, float* logits_
  * [b_eff, V] -> idx int32 [B] (B = b_eff/2 when cfg_scale > 1).  probs_out (fp32 [B, V]), kept_out (uint8 [B, V]:
  * 1 where the token survives top-k and top-p, also when its probability underflows to 0) and noise
  * (fp32 [B, V] Exp(1) draws; NULL = in-kernel Philox) are optional.  step is the Philox sub-stream index. */
+/* car_sample and car_sample_rows stage the per-image parameters in a stream-ordered temporary (cudaMallocAsync, a host-to-device
+ * copy, cudaFreeAsync around the launch), so neither can be captured into a CUDA graph; the decode loops do not use them. */
 int car_sample(const float* logits, int32_t b_eff, int32_t V, const CarSampling* sp, int32_t cfg_on, int32_t step,
                const float* noise, int32_t* idx_out, float* probs_out, uint8_t* kept_out, void* stream);
+/* The same sampler with image b's parameters from rows[b] (host, B entries; B = b_eff / 2 when cfg_scale > 1, else b_eff). */
+int car_sample_rows(const float* logits, int32_t b_eff, int32_t V, const CarRowSampling* rows, int32_t B, float cfg_scale,
+                    int32_t cfg_on, int32_t step, const float* noise, int32_t* idx_out, float* probs_out, uint8_t* kept_out,
+                    void* stream);
 
 /* ---- device-side generation loop: generate()'s prefill-sample + decode_n_tokens (generate.py:113-131,
  * 195-204).  Must follow car_prefill(...) on the same state.  Runs n_tokens sampling steps (the first one on
