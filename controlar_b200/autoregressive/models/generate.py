@@ -159,21 +159,20 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
         st.set_emb_mask(None)
     model._mask_synced = True
 
-    if rows is not None:
-        sp = _engine.make_sampling(cfg_scale=cfg_scale, cfg_interval=cfg_interval)      # per launch; the rest comes from `rows`
-        st.set_row_sampling(rows)
-        try:
-            st.prefill(cond_combined, condition_combined, 1.0, all_rows=False)
-            return st.generate(sp, max_new_tokens, noise, cond.device)
-        finally:
-            st.set_row_sampling(None)
-    # generate.py:92 does not forward control_strength when cfg_scale <= 1; forward() then resets it to 1
-    cs = float(control_strength) if use_cfg else 1.0
-    st.prefill(cond_combined, condition_combined, cs, all_rows=False)
-    sample_logits = sampling_kwargs.get("sample_logits", True)
-    if seed is None:
-        seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if sample_logits else 0
-    sp = _engine.make_sampling(temperature=sampling_kwargs.get("temperature", 1.0), top_k=sampling_kwargs.get("top_k", 2000),
-                               top_p=sampling_kwargs.get("top_p", 1.0), sample_logits=sample_logits,
-                               cfg_scale=cfg_scale, cfg_interval=cfg_interval, seed=seed)
-    return st.generate(sp, max_new_tokens, noise, cond.device)
+    if rows is None:
+        sample_logits = sampling_kwargs.get("sample_logits", True)
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if sample_logits else 0
+        sp = _engine.make_sampling(temperature=sampling_kwargs.get("temperature", 1.0), top_k=sampling_kwargs.get("top_k", 2000),
+                                   top_p=sampling_kwargs.get("top_p", 1.0), sample_logits=sample_logits,
+                                   cfg_scale=cfg_scale, cfg_interval=cfg_interval, seed=seed)
+        # generate.py:92 does not forward control_strength when cfg_scale <= 1; forward() then resets it to 1
+        cs = float(control_strength) if use_cfg else 1.0
+    else:       # per launch: cfg_scale and cfg_interval; sampling parameters and strengths come from `rows`
+        sp, cs = _engine.make_sampling(cfg_scale=cfg_scale, cfg_interval=cfg_interval), 1.0
+    st.set_row_sampling(rows)
+    try:
+        st.prefill(cond_combined, condition_combined, cs, all_rows=False)
+        return st.generate(sp, max_new_tokens, noise, cond.device)
+    finally:
+        st.set_row_sampling(None)

@@ -227,13 +227,10 @@ class LLM:
             cond = torch.stack([r.cond for r in batch]).to(device=dev, dtype=m.tok_embeddings.weight.dtype)
             masks = None if batch[0].emb_mask is None else torch.stack([r.emb_mask for r in batch]).to(dev)
         control = None if batch[0].control is None else torch.stack([r.control for r in batch]).to(device=dev, dtype=m.tok_embeddings.weight.dtype)
-        if self.mixed_sampling:
-            sps = [r.sampling for r in batch]
-            return generate(m, cond, sp.max_tokens, emb_masks=masks, cfg_scale=self.cfg_scale, condition=control,
-                            control_strength=[r.control_strength for r in batch],
-                            temperature=[1.0 if p.temperature == 0 else p.temperature for p in sps], top_k=[max(int(p.top_k), 0) for p in sps],
-                            top_p=[p.top_p for p in sps], sample_logits=[p.temperature != 0 for p in sps], seed=list(seed))
-        greedy = sp.temperature == 0
+        # per request in mixed mode, else the values the batch shares (its first request's); temperature 0 is greedy
+        per = (lambda f: [f(r) for r in batch]) if self.mixed_sampling else (lambda f: f(batch[0]))
         return generate(m, cond, sp.max_tokens, emb_masks=masks, cfg_scale=self.cfg_scale, condition=control,
-                        control_strength=batch[0].control_strength, temperature=1.0 if greedy else sp.temperature,
-                        top_k=max(int(sp.top_k), 0), top_p=sp.top_p, sample_logits=not greedy, seed=seed)
+                        control_strength=per(lambda r: r.control_strength),
+                        temperature=per(lambda r: 1.0 if r.sampling.temperature == 0 else r.sampling.temperature),
+                        top_k=per(lambda r: max(int(r.sampling.top_k), 0)), top_p=per(lambda r: r.sampling.top_p),
+                        sample_logits=per(lambda r: r.sampling.temperature != 0), seed=list(seed) if self.mixed_sampling else seed)

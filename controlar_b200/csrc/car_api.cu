@@ -49,11 +49,10 @@ struct CarState : CarOwned {
     // control tokens [3][b_eff][N][d]
     void* ctrl[3];
     bool has_ctrl = false;
-    float cs = 1.f;                    // strength of every control add; 1 when car_prefill folded per-row strengths into ctrl
     // per-image sampling (car_state_set_row_sampling); empty: the launch's CarSampling and car_prefill's control_strength
     std::vector<CarRowSampling> row_sp;
     std::vector<float> cs_rows;        // [b_eff] host staging of the per-row strengths
-    float* cs_dev = nullptr;           // [b_eff] the same on the device
+    float* cs_dev = nullptr;           // [b_eff] control strength of each row, read by every control add (set by car_prefill)
     SmpRow* smp_rows = nullptr;        // [b_eff] sampling parameters per image read by the sampler (the first B are used)
     // prefill scratch
     void *hP, *qP, *attnP, *actP, *t1, *t2;
@@ -62,8 +61,9 @@ struct CarState : CarOwned {
     // decode graph
     cudaGraphExec_t gexec = nullptr;
     cudaStream_t cap_stream = nullptr;   // capture happens on a private stream (the legacy default stream cannot capture)
+    // what the captured graph bakes in besides the state's buffers: the per-launch CFG parameters, the noise and the weight packing
     bool graph_ok = false; unsigned int graph_pack_gen = 0;
-    CarSampling gsp{};
+    float graph_cfg_scale = 0.f; int graph_cfg_interval = 0;
     const float* gnoise = nullptr;
     // persistent decode kernel (decode_persistent.cuh)
     void** pk_ptrs = nullptr;          // device arrays of per-layer pointers [8][L]
@@ -406,6 +406,7 @@ static int state_init(CarState* s, void* const* k_cache, void* const* v_cache) {
     CAR_TRY(s->alloc(&s->emb_mask_store, MP * 4));
     CAR_TRY(s->alloc(&s->cs_dev, (size_t)b_eff * 4)); CAR_TRY(s->alloc(&s->smp_rows, (size_t)b_eff * sizeof(SmpRow)));
     s->cs_rows.assign(b_eff, 1.f);
+    CAR_CUDA(cudaMemcpy(s->cs_dev, s->cs_rows.data(), (size_t)b_eff * 4, cudaMemcpyHostToDevice));
     CAR_CUDA(cudaMemset(s->tickets, 0, (size_t)b_eff * d.n_head * 4));
     CAR_CUDA(cudaMemset(s->pos, 0, 16));
     s->done_ctr = s->pos + 1;
@@ -599,7 +600,7 @@ static int enqueue_block(CarState* s, int l, bool decode, cudaStream_t st) {
     const int step3 = d.n_layer / 3;
     if (decode && s->has_ctrl && (l + 1) < d.n_layer && (l + 1) % step3 == 0) {
         // control add of the NEXT layer group fused here (gpt_t2i.py:466)
-        e4.ctrl = s->ctrl[(l + 1) / step3]; e4.n_img = s->N; e4.T = s->T; e4.cs = s->cs;
+        e4.ctrl = s->ctrl[(l + 1) / step3]; e4.n_img = s->N; e4.T = s->T; e4.cs = s->cs_dev;
     }
     return block_linear(s, decode, st, act, F, m->g_w2[l], m->w2[l], nullptr, nullptr, rows, dim, F, e4);
 }
@@ -637,7 +638,7 @@ static int prefill_small_kernels(CarState* s, int l, cudaStream_t st) {
     const CarModelDesc& d = s->m->d;
     const int step3 = d.n_layer / 3;
     if (s->has_ctrl && l % step3 == 0)
-        CAR_LAUNCH((prefill_ctrl_add_kernel<T>), s->b_eff, 256, 0, st, (T*)s->hP, (const T*)s->ctrl[l / step3], s->T, s->N, d.dim, s->cs);
+        CAR_LAUNCH((prefill_ctrl_add_kernel<T>), s->b_eff, 256, 0, st, (T*)s->hP, (const T*)s->ctrl[l / step3], s->T, s->N, d.dim, s->cs_dev);
     return CAR_OK;
 }
 
@@ -648,14 +649,18 @@ extern "C" int car_prefill(CarState* s, const void* cond, const void* condition,
     CarModel* m = s->m;
     const CarModelDesc& d = m->d;
     const int rows = s->b_eff * s->T;
-    s->cs = s->row_sp.empty() ? control_strength : 1.f;
+    // the control strength of every row, read by each control add of this prefill and of the decode that follows: image r mod B's
+    // when per-image sampling is set (an unconditional row takes its partner's), else control_strength
+    for (int r = 0; r < s->b_eff; ++r)
+        s->cs_rows[r] = s->row_sp.empty() ? control_strength : s->row_sp[r % s->row_sp.size()].control_strength;
+    CAR_CUDA(cudaMemcpyAsync(s->cs_dev, s->cs_rows.data(), (size_t)s->b_eff * 4, cudaMemcpyHostToDevice, st));
     s->has_ctrl = condition != nullptr;
     s->graph_ok = false;
     // 1. prefix embeddings: CaptionEmbedder MLP (gpt_t2i.py:156-162) or LabelEmbedder gather (:89-97)
     if (d.model_type == 1) CAR_TRY(enqueue_mlp(s, cond, rows, d.caption_dim, m->g_cap_fc1, m->g_cap_fc2, m->cap_fc1, m->cap_fc2, s->t1, s->hP, st));
     else {
-        if (d.dtype == CAR_BF16) CAR_LAUNCH((gather_rows_kernel<bf16>), rows, 256, 0, st, (const bf16*)m->label_table, (const int*)cond, (bf16*)s->hP, d.dim, (const bf16*)nullptr, 0, 0, 0.f);
-        else CAR_LAUNCH((gather_rows_kernel<float>), rows, 256, 0, st, (const float*)m->label_table, (const int*)cond, (float*)s->hP, d.dim, (const float*)nullptr, 0, 0, 0.f);
+        if (d.dtype == CAR_BF16) CAR_LAUNCH((gather_rows_kernel<bf16>), rows, 256, 0, st, (const bf16*)m->label_table, (const int*)cond, (bf16*)s->hP, d.dim, (const bf16*)nullptr, 0, 0, nullptr);
+        else CAR_LAUNCH((gather_rows_kernel<float>), rows, 256, 0, st, (const float*)m->label_table, (const int*)cond, (float*)s->hP, d.dim, (const float*)nullptr, 0, 0, nullptr);
     }
     // 2. control tokens: condition_mlp then the three condition_layers MLPs (gpt_t2i.py:438-442)
     if (condition) {
@@ -663,17 +668,6 @@ extern "C" int car_prefill(CarState* s, const void* cond, const void* condition,
         CAR_TRY(enqueue_mlp(s, condition, crow, d.dim, m->g_cond_fc1, m->g_cond_fc2, m->cond_fc1, m->cond_fc2, s->t1, s->t2, st));
         for (int j = 0; j < 3; ++j)
             CAR_TRY(enqueue_mlp(s, s->t2, crow, d.dim, m->g_ctl_fc1[j], m->g_ctl_fc2[j], m->ctl_fc1[j], m->ctl_fc2[j], s->t1, s->ctrl[j], st));
-        if (!s->row_sp.empty()) {
-            // per-row strengths (row r belongs to image r mod B: an unconditional row takes its partner's) folded into the tokens
-            const size_t nrs = s->row_sp.size();
-            for (int r = 0; r < s->b_eff; ++r) s->cs_rows[r] = s->row_sp[r % nrs].control_strength;
-            CAR_CUDA(cudaMemcpyAsync(s->cs_dev, s->cs_rows.data(), (size_t)s->b_eff * 4, cudaMemcpyHostToDevice, st));
-            const long long row_elems = (long long)s->N * d.dim, n = (long long)s->b_eff * row_elems;
-            for (int j = 0; j < 3; ++j) {
-                if (d.dtype == CAR_BF16) CAR_LAUNCH((scale_ctrl_rows_kernel<bf16>), gsz(n), 256, 0, st, (bf16*)s->ctrl[j], s->cs_dev, row_elems, n);
-                else CAR_LAUNCH((scale_ctrl_rows_kernel<float>), gsz(n), 256, 0, st, (float*)s->ctrl[j], s->cs_dev, row_elems, n);
-            }
-        }
     }
     // 3. blocks
     for (int l = 0; l < d.n_layer; ++l) {
@@ -703,10 +697,10 @@ extern "C" int car_decode_step(CarState* s, const int32_t* tok, int32_t pos, flo
     const int p = pos - s->T + 1;
     if (d.dtype == CAR_BF16)
         CAR_LAUNCH((gather_rows_kernel<bf16>), s->b_eff, 256, 0, st, (const bf16*)s->m->tok_emb, (const int*)tok, (bf16*)s->h, d.dim,
-                   (const bf16*)(s->has_ctrl ? s->ctrl[0] : nullptr), s->N, p, s->cs);
+                   (const bf16*)(s->has_ctrl ? s->ctrl[0] : nullptr), s->N, p, s->cs_dev);
     else
         CAR_LAUNCH((gather_rows_kernel<float>), s->b_eff, 256, 0, st, (const float*)s->m->tok_emb, (const int*)tok, (float*)s->h, d.dim,
-                   (const float*)(s->has_ctrl ? s->ctrl[0] : nullptr), s->N, p, s->cs);
+                   (const float*)(s->has_ctrl ? s->ctrl[0] : nullptr), s->N, p, s->cs_dev);
     return enqueue_decode_layers(s, logits_out, st);
 }
 
@@ -786,11 +780,6 @@ extern "C" int car_sample_rows(const float* logits, int32_t b_eff, int32_t V, co
     return launch_sampler_host_rows(a, smp_rows(&sp, rows, B), (cudaStream_t)stream);
 }
 
-static bool same_sampling(const CarSampling& x, const CarSampling& y) {
-    return x.temperature == y.temperature && x.top_k == y.top_k && x.top_p == y.top_p && x.sample_logits == y.sample_logits &&
-           x.cfg_scale == y.cfg_scale && x.cfg_interval == y.cfg_interval && x.seed == y.seed;
-}
-
 // the decode loop's sampler arguments; uploads the per-image parameters of this launch (car_state_set_row_sampling or sp)
 static int loop_sample_args(CarState* s, const CarSampling* sp, const float* noise, cudaStream_t st, SampleArgs& a) {
     const CarModelDesc& d = s->m->d;
@@ -804,7 +793,7 @@ static int loop_sample_args(CarState* s, const CarSampling* sp, const float* noi
     a.logits = s->logits; a.noise = noise; a.noise_per_step = noise ? 1 : 0;
     a.idx_out = s->tokens; a.tokens_ld = s->N; a.probs_out = nullptr;
     a.h_out = s->h; a.tok_emb = s->m->tok_emb; a.ctrl0 = s->has_ctrl ? s->ctrl[0] : nullptr; a.d = d.dim; a.n_img = s->N;
-    a.T = s->T; a.cs = s->cs; a.dtype = d.dtype; a.tok_buf = s->tok; a.pos_ptr = s->pos; a.done_ctr = s->done_ctr;
+    a.T = s->T; a.cs = s->cs_dev; a.dtype = d.dtype; a.tok_buf = s->tok; a.pos_ptr = s->pos; a.done_ctr = s->done_ctr;
     return CAR_OK;
 }
 
@@ -827,7 +816,7 @@ static int launch_pk(CarState* s, const SampleArgs& a, int n_tokens, cudaStream_
     PkParams P;
     memset(&P, 0, sizeof(P));
     P.dim = d.dim; P.F = d.ffn_dim; P.V = d.vocab_size; P.L = L; P.H = d.n_head; P.T = s->T; P.S = s->S; P.n_img = s->N;
-    P.b_eff = s->b_eff; P.B = a.B; P.eps = d.norm_eps; P.cs = s->cs;
+    P.b_eff = s->b_eff; P.B = a.B; P.eps = d.norm_eps; P.cs = s->cs_dev;
     P.tok_emb = (const bf16*)s->m->tok_emb; P.norm_w = (const bf16*)s->m->norm; P.w_out = (const uint4*)s->m->g_output;
     void** pp = s->pk_ptrs;
     P.wqkv = (const uint4* const*)(pp + 0 * L); P.wo = (const uint4* const*)(pp + 1 * L); P.w13 = (const uint4* const*)(pp + 2 * L);
@@ -943,7 +932,8 @@ extern "C" int car_generate(CarState* s, const CarSampling* sp, int32_t n_tokens
     // token 0 from the prefill logits (generate.py:198); its fused tail writes h for position T and bumps pos
     CAR_TRY(launch_sampler(a, st));
     if (n_tokens > 1) {
-        if (!s->graph_ok || !same_sampling(s->gsp, *sp) || s->gnoise != noise || s->graph_pack_gen != s->m->pack_gen) {
+        if (!s->graph_ok || s->graph_cfg_scale != sp->cfg_scale || s->graph_cfg_interval != sp->cfg_interval || s->gnoise != noise ||
+            s->graph_pack_gen != s->m->pack_gen) {
             if (s->gexec) { cudaGraphExecDestroy(s->gexec); s->gexec = nullptr; }
             cudaGraph_t g = nullptr;
             const long long launched_before = g_car_launches.load();   // captured nodes are not launches yet
@@ -958,7 +948,8 @@ extern "C" int car_generate(CarState* s, const CarSampling* sp, int32_t n_tokens
             ce = cudaGraphInstantiate(&s->gexec, g, 0);
             cudaGraphDestroy(g);
             if (ce != cudaSuccess) CAR_FAIL(CAR_ERR_CUDA, std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ce));
-            s->graph_ok = true; s->gsp = *sp; s->gnoise = noise; s->graph_pack_gen = s->m->pack_gen;
+            s->graph_ok = true; s->graph_cfg_scale = sp->cfg_scale; s->graph_cfg_interval = sp->cfg_interval; s->gnoise = noise;
+            s->graph_pack_gen = s->m->pack_gen;
         }
         for (int i = 1; i < n_tokens; ++i) CAR_CUDA(cudaGraphLaunch(s->gexec, st));
         g_car_launches.fetch_add(s->graph_launches * (n_tokens - 1), std::memory_order_relaxed);
@@ -986,7 +977,7 @@ static int chain_forced_loop(CarState* s, const SampleArgs& a, int n_tokens, con
         if (i + 1 == n_tokens) break;
         CAR_LAUNCH(forced_tokens_kernel, 1, 64, 0, st, (const int*)forced, n_tokens, i, a.B, s->b_eff, s->tok);
         CAR_LAUNCH((gather_rows_kernel<bf16>), s->b_eff, 256, 0, st, (const bf16*)s->m->tok_emb, (const int*)s->tok, (bf16*)s->h, d.dim,
-                   (const bf16*)(s->has_ctrl ? s->ctrl[0] : nullptr), s->N, i + 1, s->cs);
+                   (const bf16*)(s->has_ctrl ? s->ctrl[0] : nullptr), s->N, i + 1, s->cs_dev);
         CAR_TRY(enqueue_decode_layers(s, s->logits, st));
         if (trace) CAR_CUDA(cudaMemcpyAsync(trace + (size_t)(i + 1) * s->b_eff * d.vocab_size, s->logits, row_bytes, cudaMemcpyDeviceToDevice, st));
     }

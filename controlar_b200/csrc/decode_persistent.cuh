@@ -37,13 +37,14 @@ constexpr int PK_SMEM_RED = PK_WARPS * PK_NBMAX * PK_RED * 4;
 constexpr int PK_MAXA = 7;                           // k32-steps per warp (K <= 16 * 7 * 32 = 3584)
 constexpr int PK_MAXA_NORM = 3;                      // ... of the RMS-normalised GEMMs (K = dim <= 1536)
 constexpr int PK_MAXL = 64;                          // layers (shared-memory pointer tables)
-constexpr int PK_SMEM_MISC = 16 * 16 * 4 + 128 + 128 + 2 * 32 * 8 + 3 * 6 * 128     // ssq, mbarriers, stream cursor, residual pairs, q/k/v rows
+constexpr int PK_SMEM_MISC = 16 * 16 * 4 + 128 + 128 + 2 * 2 * 32 * 8 + 3 * 6 * 128     // ssq, mbarriers, stream cursor, residual and control pairs, q/k/v rows
                              + 1024 + 4 * PK_MAXL * 8 + PK_WARPS * PK_MAXA_NORM * 32 * 2;   // attention plan, pointer tables, norm weights
 constexpr int PK_SMEM_TOTAL = PK_SMEM_RING + PK_SMEM_RED + PK_SMEM_MISC;
 
 struct PkParams {
     int dim, F, V, L, H, T, S, n_img, b_eff, B;
-    float eps, cs;
+    float eps;
+    const float* cs;                   // [b_eff] control strength per row
     const bf16* tok_emb; const bf16* norm_w; const uint4* w_out;
     const uint4* const* wqkv; const uint4* const* wo; const uint4* const* w13; const uint4* const* w2;
     const bf16* const* attn_norm; const bf16* const* ffn_norm;
@@ -152,6 +153,7 @@ struct PkSmem {
     uint64_t* full;          // [PK_NSLOT]
     struct PkStream* st;     // weight-stream cursor (touched by the producer thread only)
     uint2* own;              // [2][32] residual-stream pairs of the d-column blocks this CTA owns {rows g, rows g + 8}
+    uint2* ctl;              // [2][32] the same pairs' control add of the next layer group, rnd(cs[r] * c)
     uint32_t* qrow;          // [3][PK_MAXSEG][32] q / newest k / newest v of the attention segments (bf16 pairs)
     PkAttnPlan* plan;        // this token's attention work split (pk_plan.h)
     const bf16** kvp;        // [L][2] K / V cache base of every layer (copied from the pointer arrays once per launch)
@@ -168,6 +170,7 @@ __device__ __forceinline__ PkSmem pk_smem_layout() {
     sm.full = reinterpret_cast<uint64_t*>(q); q += 128;
     sm.st = reinterpret_cast<PkStream*>(q); q += 128;
     sm.own = reinterpret_cast<uint2*>(q); q += 2 * 32 * 8;
+    sm.ctl = reinterpret_cast<uint2*>(q); q += 2 * 32 * 8;
     sm.qrow = reinterpret_cast<uint32_t*>(q); q += 3 * 6 * 128;
     sm.plan = reinterpret_cast<PkAttnPlan*>(q); q += 1024;
     sm.kvp = reinterpret_cast<const bf16**>(q); q += 2 * PK_MAXL * 8;
@@ -287,6 +290,15 @@ __device__ __forceinline__ void pk_prepoll(const uint2* buf, int K, unsigned int
 // ---------------------------------------------------------------------------------------------------------
 // GEMM phase.  kind: 0 qkv (+RoPE, KV append) | 1 wo (+residual) | 2 w1/w3 (+SwiGLU) | 3 w2 (+residual, control add)
 //              | 4 head (logits).  out[16, 8 nblk] = epi( norm?(A[16, K]) x Wp^T ), K split over the 16 warps.
+// rnd(s * c) of a bf16x2 control pair, repacked: each product rounded to bf16 as the control add rounds it, so the w2 epilogue's
+// rnd(h + that) is the add at strength s.  Formed when the pair is loaded and parked in shared memory (PkSmem::ctl), so the
+// per-row strength holds no register across the GEMM phase.
+__device__ __forceinline__ uint32_t pk_scaled_pair(float s, uint32_t c) {
+    float c0, c1;
+    unpack_bf16x2(c, c0, c1);
+    return pk_pack(rnd<bf16>(s * c0), rnd<bf16>(s * c1));
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Buffers by kind (l = layer, par = l & 1, tag = tag(step, l)):
 //   0 qkv : A = H2[par]            out = QKV[par]                 norm = attention_norm[l]
@@ -331,8 +343,7 @@ __device__ __forceinline__ unsigned int pk_gemm_phase(const PkParams& P, const i
 
     // epilogue identity of this thread (fixed across batches): block ej of the batch, row pair eg, column pair ecp
     const int ej = tid >> 7, eq = tid & 127, ei = eq >> 2, er = eq & 3, eg = ei >> 2, ecp = ei & 3;
-    // residual pairs / control pairs needed by the epilogue are requested before the A poll
-    uint32_t ctl_lo = 0, ctl_hi = 0;
+    // residual pairs / control pairs (scaled by their rows' strengths) needed by the epilogue are requested before the A poll
     if (kind == 1 && l == 0 && er == 0 && ej < 2 && blk_lo + ej < blk_hi) {
         const int n = (blk_lo + ej) * 8 + 2 * ecp;
         const uint2* pp = P.h2[0] + pk_a_index(eg, n);
@@ -346,8 +357,10 @@ __device__ __forceinline__ unsigned int pk_gemm_phase(const PkParams& P, const i
         const int n = (blk_lo + ej) * 8 + 2 * ecp;
         const int p = pos - P.T + 1;
         if (ctrl != nullptr && p >= 0 && p < P.n_img) {
-            if (eg < M) ctl_lo = __ldg(reinterpret_cast<const unsigned int*>(ctrl + ((size_t)eg * P.n_img + p) * P.dim + n));
-            if (eg + 8 < M) ctl_hi = __ldg(reinterpret_cast<const unsigned int*>(ctrl + ((size_t)(eg + 8) * P.n_img + p) * P.dim + n));
+            uint32_t lo = 0, hi = 0;
+            if (eg < M) lo = pk_scaled_pair(__ldg(P.cs + eg), __ldg(reinterpret_cast<const unsigned int*>(ctrl + ((size_t)eg * P.n_img + p) * P.dim + n)));
+            if (eg + 8 < M) hi = pk_scaled_pair(__ldg(P.cs + eg + 8), __ldg(reinterpret_cast<const unsigned int*>(ctrl + ((size_t)(eg + 8) * P.n_img + p) * P.dim + n)));
+            sm.ctl[(ej & 1) * 32 + ei] = make_uint2(lo, hi);
         }
     }
 
@@ -570,9 +583,10 @@ __device__ __forceinline__ unsigned int pk_gemm_phase(const PkParams& P, const i
                         const int p = pos - P.T + 1;
                         if (pk_ctrl_next(P, l) != nullptr && p >= 0 && p < P.n_img) {
                             float c0, c1, c2, c3;
-                            unpack_bf16x2(ctl_lo, c0, c1); unpack_bf16x2(ctl_hi, c2, c3);
-                            if (r_lo < M) { o0 = rnd<bf16>(o0 + rnd<bf16>(P.cs * c0)); o1 = rnd<bf16>(o1 + rnd<bf16>(P.cs * c1)); }
-                            if (r_hi < M) { o2 = rnd<bf16>(o2 + rnd<bf16>(P.cs * c2)); o3 = rnd<bf16>(o3 + rnd<bf16>(P.cs * c3)); }
+                            const uint2 cp = sm.ctl[(ej & 1) * 32 + ei];
+                            unpack_bf16x2(cp.x, c0, c1); unpack_bf16x2(cp.y, c2, c3);
+                            if (r_lo < M) { o0 = rnd<bf16>(o0 + c0); o1 = rnd<bf16>(o1 + c1); }
+                            if (r_hi < M) { o2 = rnd<bf16>(o2 + c2); o3 = rnd<bf16>(o3 + c3); }
                         }
                     }
                     const uint32_t p_lo = pk_pack(o0, o1), p_hi = pk_pack(o2, o3);
@@ -828,18 +842,19 @@ __device__ __forceinline__ void pk_attn_phase(const PkParams& P, int layer, int 
 // ---------------------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------------------
-// next-token input rows as H2 packets: h = tok_embeddings[tok] (+ cs * ctrl0[b][pos_next - T + 1])  gpt_t2i.py:445,466
+// next-token input rows as H2 packets: h = tok_embeddings[tok] (+ cs[b] * ctrl0[b][pos_next - T + 1])  gpt_t2i.py:445,466
 __device__ __forceinline__ void pk_write_embedding(const PkParams& P, uint2* h2, unsigned int tag, int row, int tok, int pos_next) {
     const bf16* e = P.tok_emb + (size_t)tok * P.dim;
     const int p = pos_next - P.T + 1;
     const bf16* c = (P.has_ctrl && p >= 0 && p < P.n_img) ? P.ctrl[0] + ((size_t)row * P.n_img + p) * P.dim : nullptr;
+    const float s = c ? __ldg(P.cs + row) : 0.f;
     for (int k2 = threadIdx.x; k2 < (P.dim >> 1); k2 += PK_THREADS) {
         float v0, v1;
         unpack_bf16x2(*reinterpret_cast<const uint32_t*>(e + 2 * k2), v0, v1);
         if (c) {
             float c0, c1;
             unpack_bf16x2(*reinterpret_cast<const uint32_t*>(c + 2 * k2), c0, c1);
-            v0 = rnd<bf16>(v0 + rnd<bf16>(P.cs * c0)); v1 = rnd<bf16>(v1 + rnd<bf16>(P.cs * c1));
+            v0 = rnd<bf16>(v0 + rnd<bf16>(s * c0)); v1 = rnd<bf16>(v1 + rnd<bf16>(s * c1));
         }
         pk_st64(h2 + pk_a_index(row, 2 * k2), pk_pack(v0, v1), tag);
     }

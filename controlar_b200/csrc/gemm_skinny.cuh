@@ -28,7 +28,7 @@ struct EpiParams {
     int out_reps; long long out_rep_stride;   // EPI_SWIGLU: extra replicas of the output (persistent kernel)
     // EPI_RESID (+ optional control add for the *next* layer group)
     void* h; int ldh;
-    const void* ctrl; int n_img; int T; float cs;
+    const void* ctrl; int n_img; int T; const float* cs;   // cs: control strength per batch element
     // EPI_QKV
     const float* rope; void* kc; void* vc; void* q; int S; int H; int d;
     // EPI_LOGITS
@@ -78,8 +78,9 @@ __device__ __forceinline__ void run_epilogue(const EpiParams& ep, const float* t
                     const int p = pos - ep.T + 1;
                     if (p >= 0 && p < ep.n_img) {
                         const T* cp_ = (const T*)ep.ctrl + ((size_t)b * ep.n_img + p) * ep.ldh + n;
-                        o0 = rnd<T>(o0 + rnd<T>(ep.cs * tof(cp_[0])));
-                        o1 = rnd<T>(o1 + rnd<T>(ep.cs * tof(cp_[1])));
+                        const float s = __ldg(ep.cs + b);
+                        o0 = rnd<T>(o0 + rnd<T>(s * tof(cp_[0])));
+                        o1 = rnd<T>(o1 + rnd<T>(s * tof(cp_[1])));
                     }
                 }
                 hp[0] = fromf<T>(o0); hp[1] = fromf<T>(o1);

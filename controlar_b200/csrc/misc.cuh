@@ -37,37 +37,30 @@ __global__ void interleave_rows_f32_kernel(const float* __restrict__ w1, const f
     }
 }
 
-// h[r] = table[idx[r]] (+ cs * ctrl[r][p]) — tok_embeddings / LabelEmbedder gather, gpt_t2i.py:445,89-97,466
+// h[r] = table[idx[r]] (+ cs[r] * ctrl[r][p]) — tok_embeddings / LabelEmbedder gather, gpt_t2i.py:445,89-97,466
 template <typename T>
 __global__ void gather_rows_kernel(const T* __restrict__ table, const int* __restrict__ idx, T* __restrict__ out,
-                                   int d, const T* __restrict__ ctrl, int n_img, int p, float cs) {
+                                   int d, const T* __restrict__ ctrl, int n_img, int p, const float* __restrict__ cs) {
     const int r = blockIdx.x;
     const T* src = table + (size_t)idx[r] * d;
     const T* c = (ctrl && p >= 0 && p < n_img) ? ctrl + ((size_t)r * n_img + p) * d : nullptr;
+    const float s = c ? cs[r] : 0.f;
     for (int k = threadIdx.x; k < d; k += blockDim.x) {
         float v = tof(src[k]);
-        if (c) v = rnd<T>(v + rnd<T>(cs * tof(c[k])));
+        if (c) v = rnd<T>(v + rnd<T>(s * tof(c[k])));
         out[(size_t)r * d + k] = fromf<T>(v);
     }
 }
 
-// per-row control strength folded into the control tokens of one layer group: ctrl[r] = rnd(cs[r] * ctrl[r]), r = row of
-// [rows][row_elems].  Every later add of these tokens then runs at strength 1 and gives rnd(h + rnd(1 * rnd(cs[r] * c))) =
-// rnd(h + rnd(cs[r] * c)) for bf16 (1 * x is exact): the bits of an add at strength cs[r], with the adds' code unchanged.
+// prefill control add: h[b][T-1][:] += cs[b] * ctrl[b][0][:]     gpt_t2i.py:463
 template <typename T>
-__global__ void scale_ctrl_rows_kernel(T* __restrict__ ctrl, const float* __restrict__ cs, long long row_elems, long long n) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        ctrl[i] = fromf<T>(cs[i / row_elems] * tof(ctrl[i]));
-}
-
-// prefill control add: h[b][T-1][:] += cs * ctrl[b][0][:]     gpt_t2i.py:463
-template <typename T>
-__global__ void prefill_ctrl_add_kernel(T* __restrict__ h, const T* __restrict__ ctrl, int Tq, int n_img, int d, float cs) {
+__global__ void prefill_ctrl_add_kernel(T* __restrict__ h, const T* __restrict__ ctrl, int Tq, int n_img, int d, const float* __restrict__ cs) {
     const int b = blockIdx.x;
     T* hp = h + ((size_t)b * Tq + (Tq - 1)) * d;
     const T* c = ctrl + (size_t)b * n_img * d;
+    const float s = cs[b];
     for (int k = threadIdx.x; k < d; k += blockDim.x)
-        hp[k] = fromf<T>(rnd<T>(tof(hp[k]) + rnd<T>(cs * tof(c[k]))));
+        hp[k] = fromf<T>(rnd<T>(tof(hp[k]) + rnd<T>(s * tof(c[k]))));
 }
 
 // copy row T-1 of every batch element: [B][Tq][d] -> [B][d]

@@ -69,7 +69,7 @@ struct SampleArgs {
     float* probs_out;       // [B, V] or null
     unsigned char* kept_out; // [B, V] or null: 1 where the token survives top-k and top-p (also when its probability underflows to 0)
     // fused next-step embedding (decode loop only; null => skip)
-    void* h_out; const void* tok_emb; const void* ctrl0; int d; int n_img; int T; float cs; int dtype;
+    void* h_out; const void* tok_emb; const void* ctrl0; int d; int n_img; int T; const float* cs; int dtype;   // cs: [b_eff] strengths
     int* tok_buf;           // [b_eff] int32 tokens consumed by teacher-free decode
     int* pos_ptr;           // device scalar: position of the token being produced is *pos_ptr + 1
     int* done_ctr;          // ticket: the last block to finish advances *pos_ptr
@@ -81,15 +81,16 @@ struct SampleArgs {
 
 template <typename T>
 __device__ __forceinline__ void write_next_h(const SampleArgs& a, int b_row, int tok, int pos_next, float* red32) {
-    // h = tok_embeddings[tok] (+ cs * ctrl0[b][pos_next - T + 1])    gpt_t2i.py:445,466
+    // h = tok_embeddings[tok] (+ cs[b] * ctrl0[b][pos_next - T + 1])    gpt_t2i.py:445,466
     const T* e = (const T*)a.tok_emb + (size_t)tok * a.d;
     T* h = (T*)a.h_out + (size_t)b_row * a.d;
     const int p = pos_next - a.T + 1;
     const T* c = (a.ctrl0 && p >= 0 && p < a.n_img) ? (const T*)a.ctrl0 + ((size_t)b_row * a.n_img + p) * a.d : nullptr;
+    const float s = c ? __ldg(a.cs + b_row) : 0.f;
     float ss = 0.f;
     for (int k = threadIdx.x; k < a.d; k += blockDim.x) {
         float v = tof(e[k]);
-        if (c) v = rnd<T>(v + rnd<T>(a.cs * tof(c[k])));
+        if (c) v = rnd<T>(v + rnd<T>(s * tof(c[k])));
         const T hv = fromf<T>(v);
         h[k] = hv;
         for (int rep = 1; rep < a.h_reps; ++rep) h[(size_t)rep * a.h_rep_stride + k] = hv;

@@ -102,9 +102,8 @@ typedef struct CarRowSampling {
     uint64_t seed;             /* Philox key of this image's noise */
     uint32_t noise_row;        /* Philox counter word of this image's noise: 0 makes the draws depend on `seed` alone; the image
                                   index b reproduces the rule of CarSampling, whose one seed keys every image with counter b */
-    float    control_strength; /* strength of the control tokens on this image's rows (the unconditional partner's included);
-                                  car_prefill folds it into the image's control tokens, rnd(s * c), and every add then runs at
-                                  strength 1: for bf16 the bits of an add at strength s (fp32 checkpoints: DESIGN §4.1) */
+    float    control_strength; /* strength of the control tokens on this image's rows (the unconditional partner's included),
+                                  applied by every control add of those rows, as a uniform launch at this strength applies it */
 } CarRowSampling;
 
 const char* car_last_error(void);
@@ -126,7 +125,8 @@ int car_state_create(CarModel* m, int32_t b_eff, int32_t max_seq /* S */, int32_
                      void* const* k_cache, void* const* v_cache, const float* rope_table, CarState** out);
 int car_state_set_emb_mask(CarState* s, const int32_t* emb_mask_dev, void* stream);
 /* Per-image sampling: rows (host, B entries, copied) give image b its own CarRowSampling; B must be b_eff (no CFG) or b_eff / 2
- * (CFG).  The following car_prefill takes each row's control strength (its control_strength argument is then unused) and the
+ * (CFG).  The following car_prefill takes each row's control strength (its control_strength argument is then unused), which every
+ * control add of that prefill and of the decode after it reads per row; the
  * following car_generate / car_generate_forced take each row's sampling parameters, on every decode route; the CarSampling
  * passed to them then only supplies cfg_scale and cfg_interval.  NULL returns to the scalar behaviour. */
 int car_state_set_row_sampling(CarState* s, const CarRowSampling* rows, int32_t B);

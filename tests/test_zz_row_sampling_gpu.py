@@ -7,6 +7,8 @@ The contract: row b of a mixed launch is bit-identical to row b of a uniform lau
   * the persistent kernel's sampler (pk_sample) against car_sample_rows, step by step;
   * the whole decode loop on every route: the persistent kernel at B_eff 16 (a small model and a GPT-XL-shaped one), the per-kernel
     chain at 24 and the wide route at 50, teacher-forced with mixed control strengths and free-running with mixed sampling;
+    mixed strengths also on an fp32 checkpoint (the chain at 24, teacher-forced through car_decode_step), where every control add
+    reads its row's strength exactly as a uniform launch reads it, so the compiler's fused multiply-add is the same in both;
   * the serving engine in mixed mode: 8 configurations in one launch."""
 import pytest
 import torch
@@ -145,10 +147,10 @@ XL = GPTSpec(dim=1280, n_layer=36, n_head=20, vocab_size=16384, cls_token_num=1,
 _MODELS = {}
 
 
-def _ctl_model(spec):
-    key = spec.dim
+def _ctl_model(spec, dtype=torch.bfloat16):
+    key = (spec.dim, dtype)
     if key not in _MODELS:
-        m, _ = build_product_gpt(spec, 8, torch.bfloat16)
+        m, _ = build_product_gpt(spec, 8, dtype)
         m.adapter.forward = lambda x: x              # control tokens given directly
         m.adapter_mlp.forward = lambda x: x
         _MODELS[key] = m
@@ -169,12 +171,14 @@ ROUTES = [pytest.param(SMALL, 8, id="persistent-b16"), pytest.param(XL, 8, id="p
           pytest.param(SMALL, 12, id="chain-b24"), pytest.param(SMALL, 25, id="wide-b50")]
 
 
-@pytest.mark.parametrize("spec,B", ROUTES)
-def test_mixed_strengths_teacher_forced_equal_uniform_launches(spec, B):
-    """car_generate_forced with strengths 0.3 / 0.6 / 1.0 cycling over the images: the logits trace of image b (its conditional and
-    unconditional row) equals, bit for bit, the trace of a uniform launch at image b's strength."""
+@pytest.mark.parametrize("spec,B,dtype", [pytest.param(*r.values, torch.bfloat16, id=r.id) for r in ROUTES] +
+                         [pytest.param(SMALL, 12, torch.float32, id="chain-b24-fp32")])
+def test_mixed_strengths_teacher_forced_equal_uniform_launches(spec, B, dtype):
+    """car_generate_forced (fp32: car_decode_step per token) with strengths 0.3 / 0.6 / 1.0 cycling over the images: the logits
+    trace of image b (its conditional and unconditional row) equals, bit for bit, the trace of a uniform launch at image b's
+    strength."""
     from controlar_b200 import engine
-    model = _ctl_model(spec)
+    model = _ctl_model(spec, dtype)
     cond, ctrl, forced, _ = _inputs(spec, B)
     cc = torch.cat([cond, torch.full_like(cond, spec.num_classes)])
     ctl = torch.cat([ctrl, torch.zeros_like(ctrl)])
@@ -182,12 +186,16 @@ def test_mixed_strengths_teacher_forced_equal_uniform_launches(spec, B):
     strength = [STRENGTHS[b % 3] for b in range(B)]
 
     def run(rows, cs):
-        model.setup_caches(2 * B, 1 + N_GEN, torch.bfloat16, n_img_tokens=N_GEN)
+        model.setup_caches(2 * B, 1 + N_GEN, dtype, n_img_tokens=N_GEN)
         st = model._car_state
         st.set_emb_mask(None)
         st.set_row_sampling(rows)
-        st.prefill(cc, ctl, cs, all_rows=False)
-        _, trace = st.generate_forced(sp, forced)
+        logits = st.prefill(cc, ctl, cs, all_rows=False)
+        if dtype == torch.bfloat16:
+            _, trace = st.generate_forced(sp, forced)
+        else:       # car_generate_forced is bf16 only: the same teacher-forced steps one at a time, the CFG pair sharing its token
+            tok = torch.cat([forced, forced])
+            trace = torch.stack([logits] + [st.decode_step(tok[:, i], st.T + i) for i in range(N_GEN - 1)])
         st.set_row_sampling(None)
         return trace.cpu()
     mixed = run([engine.make_row_sampling(sample_logits=False, control_strength=s) for s in strength], 1.0)
